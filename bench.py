@@ -5,6 +5,7 @@ for N > 1: every rank renders its own frames, one all-reduce of the shared featu
     python bench.py --gpus 1 --steps 20 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
     python bench.py --impl reference ...      # the CPU arm: the reference's algorithm (oracle port) on the host cores
+    python bench.py ... --dump-outputs DIR    # also write what the last timed step computed, as DIR/<name>.npy
 
 One "step" = SMPL pose -> feature net -> LBS -> rasterize B frames -> L1+SSIM loss -> backward -> Adam (train.py:66-97).
 Rank 0 prints ONE JSON line.  Timing: CUDA events on the launching stream, barrier + synchronize on both sides, max over
@@ -32,9 +33,8 @@ UNIT = "frames/s"
 
 # ---------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md clocks line), in-process through NVML
-    (`pynvml`, three cheap queries every 50 ms from a daemon thread).  An external `nvidia-smi -lms 100` loop was measured to
-    stall kernel launches on some boxes of this pool (the same graph-replayed step took 5.2 .. 15 ms while it ran); it is only the
+    """SM clock / throttle reasons sampled DURING the timed region, in-process through NVML (`pynvml`, three cheap queries every
+    50 ms from a daemon thread).  An external `nvidia-smi -lms 100` loop can stall kernel launches while it runs; it is only the
     fallback when pynvml is unavailable."""
     REASONS = (("hw_slowdown", 0x8), ("hw_thermal_slowdown", 0x40), ("sw_thermal_slowdown", 0x20), ("sw_power_cap", 0x4))
 
@@ -108,7 +108,7 @@ def measured_peaks() -> dict:
         d = json.load(open(p))
         d["_source"] = "measured (MEASURED_PEAKS.json)"
         return d
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "_source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "_source": "H100 SXM data sheet (700 W), not measured"}
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -200,6 +200,26 @@ def run_reference_arm(args):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+def dump_outputs(out_dir: str, trainer, loss, batch, iteration: int, start_params) -> None:
+    """What the last timed step computed from the seeded parameters: its loss (float64, [1]), the gradients it left on the feature
+    net (`net_grad`, the flat buffer) and on geo_feature (`geo_feature_grad`), and the frames it rendered (`images`, [B,3,H,W]; the
+    step keeps no copy of them, so the same forward runs again, untimed, on the step's inputs).  Gradients carry the run-to-run
+    scatter of float-atomic reduction order: compare them with a tolerance."""
+    import numpy as np
+    import torch
+    m = trainer.model
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().double().reshape(1).cpu().numpy())
+    np.save(os.path.join(out_dir, "net_grad.npy"), m.net.flat.grad.detach().float().cpu().numpy())
+    np.save(os.path.join(out_dir, "geo_feature_grad.npy"), m.geo_feature.grad.detach().float().cpu().numpy())
+    with torch.no_grad():
+        m.net.flat.copy_(start_params[0])
+        m.geo_feature.copy_(start_params[1])
+        _, image = trainer.loss(batch, iteration, epoch=1)
+    np.save(os.path.join(out_dir, "images.npy"), image.detach().float().cpu().numpy())
+
+
 def algorithmic_cost(N, S, side, R, B):
     """Per-launch algorithmic bytes / flops of the kernels we report rooflines for (DESIGN.md §6; SURVEY.md §8d)."""
     M = S * S
@@ -225,6 +245,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the config-4 (1 frame/GPU) and config-5 (novel-pose) side measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (loss, gradients, rendered frames) as DIR/<name>.npy; "
+                         "that step starts from the seeded initial parameters, so its inputs are the same on every run")
     args = ap.parse_args()
     args.warmup = max(3, args.warmup) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
@@ -255,6 +278,10 @@ def main():
     wl = Stage1Workload(args.config, B, device=dev)
     wl.make_ground_truth()
     trainer = Stage1Trainer(wl.model, fused_adam=True)
+    # The backward accumulates per-Gaussian and per-weight gradients with float atomics whose order varies from run to run, and Adam
+    # carries that into the parameters of every later step.  With --dump-outputs the last timed step therefore starts from the seeded
+    # initial parameters (two small device copies inside the timed region), so that its inputs are identical on every run.
+    start_params = (wl.model.net.flat.detach().clone(), wl.model.geo_feature.detach().clone()) if args.dump_outputs else None
     iteration0 = 5000      # >= 1000: no scale ramp (SURVEY.md §8d)
 
     def barrier():
@@ -275,7 +302,8 @@ def main():
         for b in dev_batches.values():
             b["original_image"] = b["original_image"].clone()
 
-    def run_value(n, start):
+    def run_value(n, start, restore_last=False):
+        loss = None
         t0 = time.perf_counter()
         trainer.host_wait_s = trainer.host_enqueue_s = 0.0
         diag_ev = [] if (os.environ.get("GA_BENCH_DIAG") == "1" and rank == 0 and n > 2) else None
@@ -283,7 +311,11 @@ def main():
             batch = dev_batches[tuple(wl.frame_ids(start + i, rank, world))]
             if _sleep_ms:
                 time.sleep(_sleep_ms * 1e-3)
-            trainer.step(batch, iteration0 + start + i, epoch=1)
+            if restore_last and i == n - 1:
+                with torch.no_grad():
+                    wl.model.net.flat.copy_(start_params[0])
+                    wl.model.geo_feature.copy_(start_params[1])
+            loss = trainer.step(batch, iteration0 + start + i, epoch=1)
             if diag_ev is not None:
                 e = torch.cuda.Event(enable_timing=True); e.record(); diag_ev.append(e)
         if os.environ.get("GA_BENCH_DIAG") == "1" and rank == 0 and n > 2:
@@ -294,6 +326,7 @@ def main():
             print("value diag per-step ms:", " ".join(f"{a.elapsed_time(b):.2f}" for a, b in zip(diag_ev[:-1], diag_ev[1:])), file=sys.stderr, flush=True)
         if os.environ.get("GA_BENCH_DIAG") == "1" and rank == 0 and n > 2:
             print(f"value diag (rank 0): host enqueue loop {1e3 * (time.perf_counter() - t0) / n:.2f} ms per step", file=sys.stderr, flush=True)
+        return loss
 
     h2d_bytes = [0]
     copy_stream = torch.cuda.Stream(device=dev)
@@ -345,11 +378,13 @@ def main():
             print(f"e2e diag (rank 0, per step): fetch {1e3 * t_fetch / n:.2f} ms, enqueue {1e3 * t_step / n:.2f} ms, wait {1e3 * t_wait / n:.2f} ms", file=sys.stderr, flush=True)
         return last
 
+    last_out = [None]
+
     def timed(fn, n, start):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        fn(n, start)
+        last_out[0] = fn(n, start)
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1)
@@ -361,9 +396,9 @@ def main():
 
     # ---- launch-mode calibration (untimed, part of the warm-up) ----------------------------------------------------------
     # The step runs either as ~120 eager launches or as ONE replayed CUDA graph (+ the optimizer launches).  Which is faster depends
-    # on the box: the replayed graph costs the device ~0.4 ms more per step than back-to-back stream launches (measured: 5.2-5.5 vs
-    # 4.7-4.9 ms), but a slow host cannot keep 120 launches per step ahead of the GPU (6.9 ms of enqueueing per step on one box of
-    # this pool).  Both compute the same thing (tests/test_train_gpu.py::test_graphed_step_matches_eager_step), so measure and pick.
+    # on the machine: a replayed graph can cost the device more per step than back-to-back stream launches, but a slow host cannot
+    # keep 120 launches per step ahead of the GPU.  Both compute the same thing (tests/test_train_gpu.py::test_graphed_step_matches_eager_step),
+    # so measure and pick.
     calib = None
     if os.environ.get("GA_STEP_GRAPH") is None and world == 1:
         def ms_per_step(n, start):
@@ -387,10 +422,16 @@ def main():
     run_value(args.warmup, 0)
     clocks.rows.clear()                    # keep only samples taken during the timed region
     l0 = _lib.launch_count() + trainer.replayed_launches
-    ms_value = timed(run_value, args.steps, args.warmup)
+    ms_value = timed(lambda n, start: run_value(n, start, restore_last=start_params is not None), args.steps, args.warmup)
     launches = _lib.launch_count() + trainer.replayed_launches - l0      # eager launches + the kernels inside the replayed step graphs
     clk = clocks.stop() if rank == 0 else {}
     fps = world * B * args.steps / (ms_value * 1e-3)
+    if args.dump_outputs:
+        trainer.finish()                   # settle the last step: it is run again if its binning buffer overflowed
+        if rank == 0:
+            last = args.warmup + args.steps - 1
+            dump_outputs(args.dump_outputs, trainer, last_out[0], dev_batches[tuple(wl.frame_ids(last, rank, world))], iteration0 + last,
+                         start_params)
 
     # ---- end to end through the public API with host batches ----------------------------------------------------------
     e2e = None
@@ -441,32 +482,18 @@ def main():
     mlp_ms = kms("mlp_tc_fwd", "mlp_tc_bwd") + sum(v[1] for k, v in per_step.items() if k.startswith("mlp_") and not k.startswith("mlp_tc"))
     dominant = max(per_step.items(), key=lambda kv: kv[1][1])[0] if per_step else None
 
-    # dram__bytes_read.sum + dram__bytes_write.sum of ONE launch, from committed `ncu --set full` captures: profiles/ncu_traffic.json names
-    # the kernel source hash each capture was taken at; a capture whose source has changed since is stale and reported as null
-    ncu_traffic = {}
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath) and (wl.S, wl.side) == (512, 1024):
-        import hashlib
-        for kname, rec in json.load(open(tpath)).get("kernels", {}).items():
-            src = os.path.join(ROOT, rec["source"])
-            if os.path.exists(src) and hashlib.sha256(open(src, "rb").read()).hexdigest() == rec["source_sha256"]:
-                ncu_traffic[kname] = (rec["dram_bytes"], rec["algorithmic_bytes"], rec["profile"])
-
     def hbm_roof(name, nbytes, label):
         ms = kms(name)
         n = per_step[name][0] if name in per_step else 0
         gbs = nbytes / (ms * 1e-3) / 1e9 if ms > 0 else None
-        tr = ncu_traffic.get(name)
         return {"kernel": label, "bound": "hbm", "achieved": gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": gbs / peaks["hbm_gbs"] if gbs else None, "traffic": tr[0] if tr else None,
-                "traffic_note": (f"ncu dram bytes of one 128->128 layer launch ({tr[2]}); algorithmic bytes of that launch: {tr[1]:.0f}" if tr
-                                 else "no ncu capture of the current kernel source committed (profiles/ncu_traffic.json)"),
+                "frac": gbs / peaks["hbm_gbs"] if gbs else None, "traffic": None,
                 "launches_per_step": n, "ms_per_step": ms,
                 "avg_launch_ms": ms / n if n else None, "algorithmic_bytes_per_step": nbytes,
                 "share_of_kernel_time": ms / total_kernel_ms if total_kernel_ms else None, "peak_source": peaks["_source"]}
 
     if dominant in ("mlp_tc_bwd", "mlp_tc_fwd"):
-        roofline = hbm_roof("mlp_tc_bwd", tc_bwd_bytes, "tc_bwd_kernel (fused dgrad+wgrad of one decoder layer, tcgen05 TF32): all launches of one step")
+        roofline = hbm_roof("mlp_tc_bwd", tc_bwd_bytes, "tc_bwd_kernel (fused dgrad+wgrad of one decoder layer, TF32 tensor cores): all launches of one step")
         roofline["tensor_tflops_all_mlp"] = tc_flops / (mlp_ms * 1e-3) / 1e12 if mlp_ms > 0 else None
     else:
         mlp_tflops = tc_flops / (mlp_ms * 1e-3) / 1e12 if mlp_ms > 0 else None
@@ -475,7 +502,7 @@ def main():
                     "unit": "TFLOP/s", "frac": (mlp_tflops / tf32_peak) if mlp_tflops else None, "traffic": None,
                     "peak_source": peaks["_source"] + "; tf32 dense = 1/2 x bf16 sustained", "ms_per_step": mlp_ms,
                     "share_of_kernel_time": mlp_ms / total_kernel_ms if total_kernel_ms else None}
-    fwd_roofline = hbm_roof("mlp_tc_fwd", tc_fwd_bytes, "tc_fwd_kernel (one decoder layer forward, tcgen05 TF32): all launches of one step")
+    fwd_roofline = hbm_roof("mlp_tc_fwd", tc_fwd_bytes, "tc_fwd_kernel (one decoder layer forward, TF32 tensor cores): all launches of one step")
     raster_fwd_names = ["preprocess_fwd_kernel", "tile_scan_kernel", "bucket_scatter_kernel", "tile_sort_kernel", "render_fwd_kernel"]
     raster_fwd_ms = kms(*raster_fwd_names) / B          # per frame
     raster_bwd_ms = kms("render_bwd_kernel", "preprocess_bwd_kernel") / B
@@ -631,7 +658,7 @@ def main():
                 "dtype": "tf32" if wl.model.net.tensor_cores else "f32", "data": "synthetic",
                 "config": {"workload": f"config{args.config}: {wl.N} Gaussians, UV {wl.S}^2, {wl.side}x{wl.side}, stage-1 train step (feature net + "
                                        f"L1/SSIM), {B} frames/GPU/step, global batch {B * world}", "poses": wl.pose_source,
-                           "l2_policy": "inputs and activations (>1.5 GB/step) exceed the 126 MB L2; no explicit flush",
+                           "l2_policy": "inputs and activations (>1.5 GB/step) exceed the 50 MB L2; no explicit flush",
                            "parallelism": f"dp{world} (frames sharded, 1 all-reduce of 1.56M fp32 grads)",
                            "step_graph": step_graph_used, "step_mode_calibration": calib},
                 "clocks": clk, "e2e": e2e, "gpu_launches": int(launches), "roofline": roofline, "mlp_fwd_roofline": fwd_roofline, "raster_roofline": raster_roofline,

@@ -1,4 +1,4 @@
-"""ctypes binding of libgavatar_sm100.so (the C ABI declared in include/gavatar.h).
+"""ctypes binding of libgavatar_sm90.so (the C ABI declared in include/gavatar.h).
 
 There is no CPU fallback and no alternative backend: if the library is missing or a call fails, a RuntimeError is
 raised.  The library is built in-tree by ``gaussianavatar_b200.build.build_library()`` (``__graft_entry__.build()``).
@@ -10,7 +10,7 @@ import os
 
 from .build import LIB_PATH
 
-# developer override used by tools/variants.py to time / test experiment builds of the same library (same C ABI)
+# developer override: load an experiment build of the same library (same C ABI) instead of the in-tree one
 LIB_PATH = os.environ.get("GA_LIB_PATH", LIB_PATH)
 
 c_f32p = ctypes.POINTER(ctypes.c_float)
@@ -103,7 +103,7 @@ def lib() -> ctypes.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
-                f"{LIB_PATH} is missing: the sm_100a CUDA library has not been built. Run "
+                f"{LIB_PATH} is missing: the sm_90a CUDA library has not been built. Run "
                 "`python -c 'import __graft_entry__ as g; g.build()'` (needs nvcc). There is no CPU fallback.")
         L = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():

@@ -1,5 +1,5 @@
 """`AvatarModel` with the reference's public surface (/root/reference model/avatar_model.py:19-649) over the fused
-sm_100a kernels: SMPL pose -> cano2live (one kernel), feature net (once per step), fused LBS + attribute assembly,
+sm_90a kernels: SMPL pose -> cano2live (one kernel), feature net (once per step), fused LBS + attribute assembly,
 tile rasterizer per frame.
 
 Same methods / attributes as the reference: train_stage1, render_free_stage1, training_setup, zero_grad, step, save,

@@ -1,4 +1,4 @@
-"""In-tree nvcc build of libgavatar_sm100.so (sm_100a only; no JIT cache, no multi-arch)."""
+"""In-tree nvcc build of libgavatar_sm90.so (sm_90a only; no JIT cache, no multi-arch)."""
 from __future__ import annotations
 
 import glob
@@ -10,9 +10,9 @@ from concurrent.futures import ThreadPoolExecutor
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_PKG, "csrc")
 _OBJ = os.path.join(_PKG, "build")
-LIB_PATH = os.path.join(_PKG, "libgavatar_sm100.so")
+LIB_PATH = os.path.join(_PKG, "libgavatar_sm90.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -20,7 +20,7 @@ def _nvcc() -> str:
     for cand in (shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found; libgavatar_sm100.so cannot be built")
+    raise RuntimeError("nvcc not found; libgavatar_sm90.so cannot be built")
 
 
 def _deps_mtime() -> float:
@@ -30,7 +30,7 @@ def _deps_mtime() -> float:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Compile every csrc/*.cu for sm_100a and link the shared library.  Incremental per translation unit."""
+    """Compile every csrc/*.cu for sm_90a and link the shared library.  Incremental per translation unit."""
     nvcc = _nvcc()
     os.makedirs(_OBJ, exist_ok=True)
     srcs = sorted(glob.glob(os.path.join(_CSRC, "*.cu")))
@@ -55,7 +55,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(run, jobs))
     if jobs or not os.path.exists(LIB_PATH) or any(os.path.getmtime(o) > os.path.getmtime(LIB_PATH) for o in objs):
-        run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH, *objs, "-lcudart"])
+        run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB_PATH, *objs, "-lcudart"])
     return LIB_PATH
 
 

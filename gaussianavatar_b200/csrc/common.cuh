@@ -1,4 +1,4 @@
-// Shared helpers for libgavatar_sm100.so (sm_100a only).
+// Shared helpers for libgavatar_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -81,15 +81,14 @@ struct PerDeviceOnce {
     }
 };
 
-constexpr int kNumSMs = 148;  // B200 (compile-time grid constants of the tensor-core kernels)
+constexpr int kNumSMs = 132;  // H100 SXM (compile-time grid constants of the heads / split-K kernels)
 int num_sms();                // multiProcessorCount of the current device, queried once per device
 
 // ---- programmatic dependent launch -------------------------------------------------------------------------------------------
 // Every kernel of this library is launched with the programmatic-stream-serialization attribute and begins with pdl_wait():
 // the grid may be scheduled (and run anything placed BEFORE the wait: barrier / tensor-memory setup) while its predecessor in the
 // stream is still draining, and reads or writes global memory only after the predecessor has completed and flushed.  A step is
-// ~120 dependent launches.  Measured on the captured step graph (B200, config 3): 5.20 ms without, 5.22 ms with — no gain, so it is OFF
-// unless GA_PDL=1 (the waits are then the only cost: one instruction per kernel).
+// ~120 dependent launches.  It is OFF unless GA_PDL=1 (the waits are then the only cost: one instruction per kernel).
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 #endif
@@ -110,6 +109,11 @@ inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t sme
 __device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d)
 {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+// the same for two consecutive floats (8-byte aligned address)
+__device__ __forceinline__ void red_add_v2(float *addr, float a, float b)
+{
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 }  // namespace ga

@@ -1,5 +1,5 @@
 // The geometry net's 5x5 convolutions (GeomConvLayers, model/modules.py:122-137: three 64->64 convs, padding 2, no bias, no
-// activation) as implicit GEMMs on the 5th-generation tensor cores (tcgen05 kind::tf32, accumulator in TMEM).
+// activation) as implicit GEMMs on the tensor cores (mma.sync m16n8k8 TF32, fp32 accumulators in registers; tc_common.cuh).
 //
 //   mode 0  forward        Y [px][co]      = sum_{tap,ci} X [px + tap][ci] * W[tap][ci][co]
 //   mode 1  data gradient  dX[px][ci]      = sum_{tap,co} dY[px - tap][co] * W[tap][ci][co]
@@ -7,13 +7,13 @@
 //
 // Feature maps are NHWC [P = Hf*Hf][64] fp32 whose values are already rounded to TF32 (round_tf32_kernel, or the
 // producing conv's epilogue), so operands can travel global -> shared memory with cp.async (16-byte pieces, zero-fill for the
-// padding, no registers) straight into the UMMA layouts:
+// padding, no registers) straight into the swizzled images the fragments are read from:
 //   modes 0/1: one CTA per 128 consecutive pixels; 50 K-steps (tap x 32-channel half); A = im2col rows, K-major 128 B swizzle;
-//              B = W[tap][ci half][64 co] consumed MN-major (mode 0) or W[tap][64 ci][co half] K-major (mode 1)
+//              B = W[tap][ci half][64 co] pixel-major (mode 0) or W[tap][64 ci][co half] K-major (mode 1)
 //   mode 2   : one CTA per (pair of taps, pixel split); K = pixel (32 per step); A = the two taps' shifted X (M = 2 x 64 ci),
-//              B = dY, both MN-major -- the pixel-major images are consumed as they lie (layout: tc_bwd_kernel / DESIGN.md §4)
-// Pipeline: 8 producer warps keep kDepth cp.async groups in flight over an 8-stage ring; one MMA warp issues 4 tcgen05.mma
-// (M128 N64 K8) per step and frees the stage with tcgen05.commit; 4 epilogue warps drain TMEM once at the end.
+//              B = dY, both pixel-major, consumed as they lie
+// Pipeline: every one of the 8 warps copies its pieces kDepth steps ahead over an 8-stage ring, then multiplies its 16 rows of the
+// 128 x 64 output tile; one block barrier per step.  The accumulators leave the registers once at the end.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -25,9 +25,10 @@ using namespace tc;
 constexpr int kC = 64, kTaps = 25;
 constexpr int kCStages = 8;
 constexpr int kABytes = 16384, kBBytes = 8192, kCStageBytes = kABytes + kBBytes;
-constexpr int kDepth = 5;                       // cp.async groups in flight per producer thread
-constexpr int kConvThreads = 13 * 32;           // 8 producer warps, 1 MMA warp, 4 epilogue warps
+constexpr int kDepth = 6;                       // steps of cp.async groups in flight (a stage is refilled 2 steps after it was read)
+constexpr int kConvThreads = 8 * 32;
 constexpr int kTapPairs = 13;
+static_assert(kDepth + 2 <= kCStages, "a stage must not be refilled while a warp may still read it");
 
 struct ConvParams {
     const float *in;       // modes 0, 2: X; mode 1: dY          [P][64], TF32-rounded
@@ -38,14 +39,9 @@ struct ConvParams {
 
 struct alignas(1024) ConvSmem {
     unsigned char st[kCStages][kCStageBytes];
-    uint64_t full[kCStages], empty[kCStages], done;
-    uint32_t tmem_base;
 };
 
 __device__ __forceinline__ float round_tf32(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
-
-// byte offset of 16-byte unit v (0..7) of row r inside a [rows][128 B] MN-major chunk (32-byte-base 128 B swizzle)
-__device__ __forceinline__ uint32_t mn_unit(int r, int v) { return (uint32_t)r * 128u + (uint32_t)((((v >> 1) ^ (r & 3)) << 5) | ((v & 1) << 4)); }
 
 template <int MODE>
 __global__ void __launch_bounds__(kConvThreads, 1)
@@ -55,6 +51,7 @@ conv_tc_kernel(const ConvParams p)
     extern __shared__ unsigned char smem_raw[];
     ConvSmem &sm = *reinterpret_cast<ConvSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int g = lane >> 2, t4 = lane & 3;
     const int Hf = p.Hf, P = p.P;
 
     // work of this CTA
@@ -63,43 +60,30 @@ conv_tc_kernel(const ConvParams p)
         tpair = blockIdx.x % kTapPairs; z = blockIdx.x / kTapPairs;
         const int nchunk = (P + 31) / 32;
         nst = z < nchunk ? (nchunk - z + p.nsplit - 1) / p.nsplit : 0;
-        if (nst == 0) return;                                    // uniform for the CTA, before any barrier / TMEM use
+        if (nst == 0) return;                                    // uniform for the CTA, before any barrier
     } else {
         m0 = blockIdx.x * 128;
         nst = 2 * kTaps;
     }
 
-    if (tid == 0) {
-        for (int s = 0; s < kCStages; ++s) { mbar_init(&sm.full[s], 8); mbar_init(&sm.empty[s], 1); }
-        mbar_init(&sm.done, 1);
-        fence_barrier_init();
-    }
-    if (warp == 8) tmem_alloc(&sm.tmem_base, 64);
-    tc_fence_before_sync();
-    __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = sm.tmem_base;
-
-    if (warp < 8) {
-        // ================================ producers ================================
-        const int u = tid & 7, rg = tid >> 3;                    // 16-byte unit, row group (0..31)
-        int py[4], px[4]; bool pv[4];
-        if (MODE != 2) {
+    // ================================ copies ================================
+    const int u = tid & 7, rg = tid >> 3;                        // 16-byte unit, row group (0..31)
+    int py[4], px[4]; bool pv[4];
+    if (MODE != 2) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i) { const int m = m0 + rg + 32 * i; pv[i] = m < P; py[i] = m / Hf; px[i] = m % Hf; }
-        }
-        const uint32_t a_off = (uint32_t)rg * 128u + (uint32_t)((u ^ (rg & 7)) << 4);          // K-major A: + i * 4096  (modes 0, 1)
-        const uint32_t a_off_mn = mn_unit(rg, u);                                                 // MN-major A: + chunk * 4096 (mode 2)
-        // B tile: unit v (0..15) of row kk = tid >> 4 (+16 per pass) for the 256-byte rows, or unit u of row rg (+32) for 128-byte rows
-        const int v = tid & 15, kk = tid >> 4;
-        const uint32_t b_off_mn = (uint32_t)(v >> 3) * 4096u + mn_unit(kk, v & 7);              // + i2 * 16 * 128 (kk & 3 unchanged)
-        const uint32_t b_off_k = (uint32_t)rg * 128u + (uint32_t)((u ^ (rg & 7)) << 4);         // + i2 * 4096
-        const uint32_t st0 = smem_u32(sm.st[0]);
+        for (int i = 0; i < 4; ++i) { const int m = m0 + rg + 32 * i; pv[i] = m < P; py[i] = m / Hf; px[i] = m % Hf; }
+    }
+    const uint32_t a_off = (uint32_t)rg * 128u + (uint32_t)((u ^ (rg & 7)) << 4);          // K-major A: + i * 4096  (modes 0, 1)
+    const uint32_t a_off_mn = mn_unit(rg, u);                                                 // pixel-major A: + chunk * 4096 (mode 2)
+    // B tile: unit v (0..15) of row kk = tid >> 4 (+16 per pass) for the 256-byte rows, or unit u of row rg (+32) for 128-byte rows
+    const int v = tid & 15, kk = tid >> 4;
+    const uint32_t b_off_mn = (uint32_t)(v >> 3) * 4096u + mn_unit(kk, v & 7);              // + i2 * 16 * 128 (kk & 3 unchanged)
+    const uint32_t b_off_k = (uint32_t)rg * 128u + (uint32_t)((u ^ (rg & 7)) << 4);         // + i2 * 4096
+    const uint32_t st0 = smem_u32(sm.st[0]);
 
-        for (int q = 0; q < nst; ++q) {
-            const int s = q % kCStages;
-            warp_wait(&sm.empty[s], ((q / kCStages) & 1) ^ 1, lane);
-            const uint32_t sa = st0 + (uint32_t)s * kCStageBytes, sb = sa + kABytes;
+    auto issue = [&](int q) {
+        if (q < nst) {
+            const uint32_t sa = st0 + (uint32_t)(q % kCStages) * kCStageBytes, sb = sa + kABytes;
             if (MODE != 2) {
                 const int t = q >> 1, h = q & 1;
                 const int dy = (MODE == 0 ? 1 : -1) * (t / 5 - 2), dx = (MODE == 0 ? 1 : -1) * (t % 5 - 2);
@@ -113,11 +97,11 @@ conv_tc_kernel(const ConvParams p)
                 if (MODE == 0) {
 #pragma unroll
                     for (int i2 = 0; i2 < 2; ++i2)
-                        cp_async16(sb + b_off_mn + i2 * 2048u, p.w + ((size_t)(t * kC + h * 32 + kk + 16 * i2) * kC + v * 4), true);
+                        cp_async16_full(sb + b_off_mn + i2 * 2048u, p.w + ((size_t)(t * kC + h * 32 + kk + 16 * i2) * kC + v * 4));
                 } else {
 #pragma unroll
                     for (int i2 = 0; i2 < 2; ++i2)
-                        cp_async16(sb + b_off_k + i2 * 4096u, p.w + ((size_t)(t * kC + rg + 32 * i2) * kC + h * 32 + u * 4), true);
+                        cp_async16_full(sb + b_off_k + i2 * 4096u, p.w + ((size_t)(t * kC + rg + 32 * i2) * kC + h * 32 + u * 4));
                 }
             } else {
                 const int pxl0 = (z + q * p.nsplit) * 32;                 // first pixel of this step's 32-pixel chunk
@@ -139,73 +123,66 @@ conv_tc_kernel(const ConvParams p)
                     cp_async16(sb + b_off_mn + i2 * 2048u, p.w + ((size_t)(ok ? mb : 0) * kC + v * 4), ok);
                 }
             }
-            cp_async_commit();
-            if (q >= kDepth) {
-                cp_async_wait<kDepth>();
-                fence_proxy_async_smem();
-                warp_arrive(&sm.full[(q - kDepth) % kCStages], lane);
-            }
         }
-        cp_async_wait<0>();
-        fence_proxy_async_smem();
-        for (int q = (nst > kDepth ? nst - kDepth : 0); q < nst; ++q) warp_arrive(&sm.full[q % kCStages], lane);
-    } else if (warp == 8) {
-        // ================================ MMA issuer ================================
-        constexpr uint32_t idesc = make_idesc_tf32(128, 64, MODE == 2, MODE != 1);
-        constexpr uint32_t hi_k = desc_hi(1024);                                   // K-major, 128 B swizzle
-        constexpr uint32_t hi_mn = (512u >> 4) | (1u << 14) | (1u << 29);           // MN-major, 32-byte-base 128 B swizzle
-        for (int q = 0; q < nst; ++q) {
-            const int s = q % kCStages;
-            warp_wait(&sm.full[s], (q / kCStages) & 1, lane);
-            tc_fence_after_sync();
-            if (lane == 0) {
-                const uint32_t sa = smem_u32(sm.st[s]), sb = sa + kABytes;
+        cp_async_commit();                                      // one group per step, empty past the end: the wait count stays uniform
+    };
+
+    for (int q = 0; q < kDepth; ++q) issue(q);
+    float acc[8][4];
 #pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const uint64_t da = MODE == 2 ? (((uint64_t)hi_mn << 32) | desc_lo(sa + j * 1024u, 4096))
-                                                  : (((uint64_t)hi_k << 32) | (desc_lo(sa, 16) + (uint32_t)j * 2u));
-                    const uint64_t db = MODE == 1 ? (((uint64_t)hi_k << 32) | (desc_lo(sb, 16) + (uint32_t)j * 2u))
-                                                  : (((uint64_t)hi_mn << 32) | desc_lo(sb + j * 1024u, 4096));
-                    mma_tf32(tmem_base, da, db, idesc, q > 0 || j > 0);
-                }
-                mma_commit(&sm.empty[s]);
-                if (q == nst - 1) mma_commit(&sm.done);
-            }
-            __syncwarp();
-        }
-    } else {
-        // ================================ epilogue ================================
-        const int qd = warp & 3;
-        const int row = qd * 32 + lane;
-        warp_wait(&sm.done, 0, lane);
-        tc_fence_after_sync();
-#pragma unroll 1
-        for (int cc = 0; cc < 4; ++cc) {
-            float v[16];
-            tmem_ld_32x16(tmem_base + ((uint32_t)(qd * 32) << 16) + cc * 16, v);
-            if (MODE != 2) {
-                const int m = m0 + row;
-                if (m < P) {
+    for (int nt = 0; nt < 8; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+    const int mr = 16 * warp + g;                                // this lane's output rows: mr, mr + 8
+    for (int q = 0; q < nst; ++q) {
+        cp_async_wait<kDepth - 1>();                             // this thread's pieces of step q have landed ...
+        __syncthreads();                                         // ... and everybody's; every warp is done with step q - 1
+        issue(q + kDepth);
+        const uint32_t sa = st0 + (uint32_t)(q % kCStages) * kCStageBytes, sb = sa + kABytes;
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        float4 o = make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-                        if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); o.z = round_tf32(o.z); o.w = round_tf32(o.w); }
-                        *reinterpret_cast<float4 *>(p.out + (size_t)m * kC + cc * 16 + g * 4) = o;
-                    }
-                }
+        for (int ks = 0; ks < 4; ++ks) {
+            const int k = 8 * ks + t4;
+            uint32_t a[4];
+            if (MODE == 2) {
+                a[0] = lds32(sa + mnmajor_off(k, mr, 4096)); a[1] = lds32(sa + mnmajor_off(k, mr + 8, 4096));
+                a[2] = lds32(sa + mnmajor_off(k + 4, mr, 4096)); a[3] = lds32(sa + mnmajor_off(k + 4, mr + 8, 4096));
             } else {
-                const int t = 2 * tpair + (row >> 6), ci = row & 63;
-                if (t < kTaps) {
+                a[0] = lds32(sa + kmajor_off(mr, k, 0)); a[1] = lds32(sa + kmajor_off(mr + 8, k, 0));
+                a[2] = lds32(sa + kmajor_off(mr, k + 4, 0)); a[3] = lds32(sa + kmajor_off(mr + 8, k + 4, 0));
+            }
 #pragma unroll
-                    for (int g = 0; g < 4; ++g)
-                        red_add_v4(p.out + ((size_t)(t * kC + ci) * kC + cc * 16 + g * 4), v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-                }
+            for (int nt = 0; nt < 8; ++nt) {
+                const int n = 8 * nt + g;
+                uint32_t b0, b1;
+                if (MODE == 1) { b0 = lds32(sb + kmajor_off(n, k, 0)); b1 = lds32(sb + kmajor_off(n, k + 4, 0)); }
+                else { b0 = lds32(sb + mnmajor_off(k, n, 4096)); b1 = lds32(sb + mnmajor_off(k + 4, n, 4096)); }
+                mma_tf32(acc[nt], a, b0, b1);
             }
         }
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 8) tmem_dealloc(tmem_base, 64);
+    cp_async_wait<0>();
+
+    // ================================ epilogue: rows mr, mr + 8; columns 8 nt + 2 t4, + 1 ================================
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int row = mr + 8 * h;
+        if (MODE != 2) {
+            const int m = m0 + row;
+            if (m < P) {
+#pragma unroll
+                for (int nt = 0; nt < 8; ++nt) {
+                    float2 o = make_float2(acc[nt][2 * h], acc[nt][2 * h + 1]);
+                    if (p.round_out) { o.x = round_tf32(o.x); o.y = round_tf32(o.y); }
+                    *reinterpret_cast<float2 *>(p.out + (size_t)m * kC + 8 * nt + 2 * t4) = o;
+                }
+            }
+        } else {
+            const int t = 2 * tpair + (row >> 6), ci = row & 63;
+            if (t < kTaps) {
+#pragma unroll
+                for (int nt = 0; nt < 8; ++nt)
+                    red_add_v2(p.out + ((size_t)(t * kC + ci) * kC + 8 * nt + 2 * t4), acc[nt][2 * h], acc[nt][2 * h + 1]);
+            }
+        }
+    }
 }
 
 __global__ void __launch_bounds__(256) round_tf32_kernel(const float *__restrict__ in, float *__restrict__ out, size_t n4)
@@ -251,12 +228,13 @@ int launch_round_tf32(const float *in, float *out, size_t n, cudaStream_t st)
 // mode 0: out[P][64] = conv(in, w); mode 1: out = conv_transpose-style data gradient of `in` = dY; mode 2: out (dW) += wgrad(in = X, w = dY)
 int launch_conv_tc(int mode, const float *in, const float *w, float *out, int Hf, int round_out, cudaStream_t st)
 {
-    GA_REQUIRE(mode >= 0 && mode <= 2 && in && w && out && Hf > 0, "tcgen05 conv: bad arguments");
+    GA_REQUIRE(mode >= 0 && mode <= 2 && in && w && out && Hf > 0, "tensor-core conv: bad arguments");
     const int P = Hf * Hf;
     ConvParams p{in, w, out, Hf, P, round_out, 1};
     if (mode == 2) {
         const int nchunk = cdiv(P, 32);
-        p.nsplit = nchunk < 11 ? nchunk : 11;                    // 13 tap pairs x 11 pixel splits = 143 CTAs on 148 SMs
+        const int split = num_sms() / kTapPairs;                 // 13 tap pairs x 10 pixel splits = 130 CTAs on 132 SMs
+        p.nsplit = nchunk < split ? nchunk : split;
         return launch_mode<2>(p, kTapPairs * p.nsplit, "geom_conv_tc_wgrad", st);
     }
     const int tiles = cdiv(P, 128);

@@ -617,7 +617,7 @@ extern "C" int ga_decoder_forward(const GaDecoderDesc *d, const float *params, c
     }
     GA_CHECK_LAUNCH("chw_to_hwc_kernel");
     if (d->flags & GA_DECODER_TENSOR_CORES) {
-        // tcgen05 implicit GEMMs on TF32-rounded operands (what cuDNN computes for the reference's Conv2d): round the input and the
+        // tensor-core implicit GEMMs on TF32-rounded operands (what cuDNN computes for the reference's Conv2d): round the input and the
         // weights once; every conv but the last writes its output already rounded (it is only ever read as an MMA operand again)
         if (int rc = launch_round_tf32(w.F[0], w.F[0], (size_t)P * kCg, st)) return rc;
         for (int i = 0; i < 3; ++i)
@@ -661,7 +661,7 @@ extern "C" int ga_decoder_forward(const GaDecoderDesc *d, const float *params, c
         return GA_OK;
     };
     if (d->flags & GA_DECODER_TENSOR_CORES) {
-        // ---- tcgen05 / TF32 path: one persistent warp-specialised launch per 128-wide layer (mlp_tc.cu) ----
+        // ---- tensor-core / TF32 path: one persistent launch per 128-wide layer (mlp_tc.cu) ----
         if (int rc = launch_tc_fwd(w.feat, kFeatLd, kFeatLd, nullptr, nullptr, params + L.w[0], kFeatLd, params + L.b[0], w.Y[0], kH, 0,
                                    sum + kBnOff[0], sumsq + kBnOff[0], M, st)) return rc;
         if (int rc = finalize(0, kH)) return rc;
@@ -800,7 +800,7 @@ extern "C" int ga_decoder_backward(const GaDecoderDesc *d, const float *params, 
     }
     float *cur = nullptr, *nxt = nullptr;
     if (d->flags & GA_DECODER_TENSOR_CORES) {
-        // ---- tcgen05 / TF32 path: data + weight gradient of a layer in one fused launch (mlp_tc.cu: tc_bwd_kernel) ----
+        // ---- tensor-core / TF32 path: data + weight gradient of a layer in one fused launch (mlp_tc.cu: tc_bwd_kernel) ----
         auto tc = [&](const float *dZl, const float *Yl, int ldg, int ol, const float *Yp, int ldp, int op, const float *Wl, int ldw, float *dWl,
                       float *dZp, int ldo, int mode) -> int {
             return launch_tc_bwd(dZl, Yl, ldg, cf.ga + ol, cf.m1 + ol, cf.m2 + ol, cf.mean + ol, cf.rstd + ol, Yp, ldp, cf.a + op, cf.b + op,

@@ -6,7 +6,7 @@
 // accumulator tile (bias + per-channel statistics, activation backward, split-K atomics, ...).
 //
 // This is the reference-accuracy path of the decoder MLP / geometry convs (every product is an FP32 FMA); the
-// tcgen05 TF32 tensor-core path (mlp_tc.cu) shares the same loaders' semantics and is checked against this one.
+// TF32 tensor-core path (mlp_tc.cu) shares the same loaders' semantics and is checked against this one.
 #pragma once
 #include "common.cuh"
 

@@ -1,58 +1,32 @@
-// Decoder-MLP layers on the 5th-generation tensor cores (tcgen05, kind::tf32, accumulators in TMEM).
+// Decoder-MLP layers on the tensor cores (mma.sync m16n8k8 TF32, fp32 accumulators in registers; tc_common.cuh says why not wgmma).
 //
-// Forward: one persistent, warp-specialised CTA per SM computes  Y[M,128] (+)= act(bn(X))[M,K] * W[128,K]^T + bias  for its share
-// of 64-pixel tiles, as the TRANSPOSED product  Y^T[out, px] = W[out, K] * act(bn(X))[px, K]^T  (17 warps):
-//   warps 0-7   converters: the raw (pre-BatchNorm) input rows travel global -> shared with 16-byte cp.async, each piece straight to
-//                           its place in the 128-byte-swizzled K-major UMMA image, up to three tiles ahead (four 32 KB stages); the thread
-//                           that copied a piece converts it IN PLACE (BatchNorm + Softplus in the log2 domain, TF32 rounding), then
-//                           fence.proxy.async, mbarrier
-//   warp  8     MMA issuer: one elected lane issues K/8 tcgen05.mma (M = 128 output channels, N = 64 pixels, K = 8) per tile into one of
-//                           four 64-column TMEM accumulators, tcgen05.commit -> mbarrier (which also frees the input stage)
-//   warps 9-16  epilogue  : two warps per TMEM lane quarter, 32 pixels each; a TMEM lane is an OUTPUT CHANNEL, so bias and the layer's
-//                           BatchNorm sum / sum-of-squares are thread-local, and Y leaves straight from the registers: a warp
-//                           instruction writes 32 channels of one pixel = one whole 128-byte line (no staging pass, no named barrier)
-// The layer moves 1 KiB per pixel against 32.8 kFLOP: HBM is the bound.  Round 1 computed Y (not Y^T) in 128-pixel tiles with two
-// 64 KB stages, register loads and a shared-memory staging pass for coalesced row stores: 0.57 of the HBM peak; this form 0.69
-// (0.863 -> 0.714 ms per step at config 3; lookahead 1 / 2 / 3 tiles: 0.93 / 0.73 / 0.71 ms).
+// Forward: one persistent CTA per SM (8 warps) computes  Y[M,128] (+)= act(bn(X))[M,K] * W[128,K]^T + bias  for its share of 64-pixel
+// tiles, as the TRANSPOSED product  Y^T[out, px] = W[out, K] * act(bn(X))[px, K]^T:
+//   copies   : the raw (pre-BatchNorm) input rows travel global -> shared with 16-byte cp.async, each piece straight to its place in the
+//              128-byte-swizzled K-major tile image, up to three tiles ahead over four 32 KB stages; the thread that copied a piece
+//              converts it IN PLACE (BatchNorm + Softplus in the log2 domain, TF32 rounding) once it has landed
+//   MMA      : warp w owns output channels 16 w .. 16 w + 15 for every tile: its slice of W lives in registers as A fragments for the
+//              whole launch, the tile supplies the B fragments (K/8 x 8 MMAs per warp and tile)
+//   epilogue : straight from the accumulators: bias, the fan-in's existing Y, the layer's BatchNorm sum / sum-of-squares (per channel,
+//              reduced over the four lanes that share a channel), Y stored as 32-byte row pieces
+// One block barrier per tile separates "every piece converted" from the MMAs; it also proves the stage refilled next was read.
 //
 // TF32 is what the reference computes these 1x1 convolutions in on any Ampere+ GPU (cuDNN allow_tf32 default,
 // SURVEY.md §8 a-4); the strict-FP32 CUDA-core path (gemm.cuh) remains selectable and is the GPU-side reference.
 #include "gemm.cuh"
 #include "tc_common.cuh"
-#include <type_traits>
-
-// timing-ablation switches for tools/variants.py (never set in the product build): 1 no global loads in the producers, 2 no activation
-// math, 4 no MMA issue, 8 no epilogue math, 16 no epilogue global traffic
-#ifndef GA_ABLATE
-#define GA_ABLATE 0
-#endif
-// GA_TC_TIMING=1: every warp of CTA 0 prints the cycles it spent inside mbarrier waits (tools/variants.py; never set in the product build)
-#ifndef GA_TC_TIMING
-#define GA_TC_TIMING 0
-#endif
-#if GA_TC_TIMING
-#define TWAIT(slot, call) do { const long long t0_ = clock64(); call; tw_[slot] += clock64() - t0_; } while (0)
-#else
-#define TWAIT(slot, call) call
-#endif
-#if GA_TC_TIMING
-#define TMARK(var) const long long var = clock64()
-#define TADD(slot, var) tw_[slot] += clock64() - var
-#else
-#define TMARK(var)
-#define TADD(slot, var)
-#endif
 
 namespace ga {
 namespace {
 
 using namespace tc;
 
-constexpr int kBM = 128, kBN = 128;
-constexpr int kChunkBytes = kBM * 128;          // one 32-channel chunk of a 128-row tile: 16 KB
-constexpr int kMaxChunks = 4;                    // K <= 128
-constexpr int kStageBytes = kMaxChunks * kChunkBytes;   // 64 KB
-constexpr uint32_t kTmemCols = 256;
+constexpr int kTPx = 64, kTStages = 4;
+constexpr int kTLook = 3;                            // tiles of copies in flight (a stage is refilled one tile after it was read)
+constexpr int kTChunk = kTPx * 128;                  // 8 KB: [64 px rows][32 channels]
+constexpr int kTStageBytes = 4 * kTChunk;            // 32 KB: K <= 128
+constexpr int kTThreads = 8 * 32;
+static_assert(kTLook < kTStages, "lookahead must leave the stage being read alone");
 
 struct TcFwdParams {
     const float *X; int ldx; int K;
@@ -64,82 +38,61 @@ struct TcFwdParams {
     int M;
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Forward layer (see the file header).  Operand images: A = W [4 chunks][128 out rows][128 B], B = the X tile [4 chunks][64 px rows]
-// [128 B], both K-major with the 128-byte swizzle (16-byte units XOR row % 8); a chunk is 32 input channels.
-constexpr int kTPx = 64, kTStages = 4;
-constexpr int kTChunk = kTPx * 128;                 // 8 KB: [64 px rows][32 channels]
-constexpr int kTStageBytes = kMaxChunks * kTChunk;   // 32 KB
-constexpr int kTThreads = 17 * 32;
-constexpr int kTMmaWarp = 8, kTEpiWarp0 = 9;
-#ifndef GA_FWDT_LOOK
-#define GA_FWDT_LOOK 3
-#endif
-constexpr int kTLook = GA_FWDT_LOOK;                 // tiles of copies in flight per converter thread (1..3)
-
-struct alignas(1024) TcFwdTSmem {
-    unsigned char w[kStageBytes];                    // W: [4 chunks][128 out rows][128 B], K-major, 128-byte swizzle
-    unsigned char x[kTStages][kTStageBytes];         // X tile: [4 chunks][64 px rows][128 B]
-    float sa[kBN], sb[kBN], sbias[kBN];
-    double red[2][kBN];
-    uint64_t full[kTStages], mma_done[kTStages], tmem_empty[kTStages];
-    uint32_t tmem_base;
+struct alignas(1024) TcFwdSmem {
+    unsigned char x[kTStages][kTStageBytes];         // X tile: [4 chunks][64 px rows][128 B], K-major, 128-byte swizzle
+    float sa[128], sb[128];
 };
 
 __global__ void __launch_bounds__(kTThreads, 1)
 tc_fwd_kernel(const TcFwdParams p)
 {
     extern __shared__ unsigned char smem_raw[];
-    TcFwdTSmem &sm = *reinterpret_cast<TcFwdTSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
+    TcFwdSmem &sm = *reinterpret_cast<TcFwdSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int g = lane >> 2, t4 = lane & 3;
     const int num_tiles = (p.M + kTPx - 1) / kTPx;
     const int gstep = gridDim.x;
-
-    if (tid == 0) {
-        for (int s = 0; s < kTStages; ++s) {
-            mbar_init(&sm.full[s], 8 * kArrivalsPerWarp); mbar_init(&sm.mma_done[s], 1); mbar_init(&sm.tmem_empty[s], 8 * kArrivalsPerWarp);
-        }
-        fence_barrier_init();
-    }
-    if (warp == kTMmaWarp) tmem_alloc(&sm.tmem_base, kTmemCols);
+    const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
+    const int nk = p.K / 8;                                                  // 16 (K = 128) or 9 (K = 72)
     pdl_wait();
-    for (int i = tid; i < kBN * (p.K / 4); i += kTThreads) {          // weights -> shared, K-major, 128-byte swizzle
-        const int n = i / (p.K / 4), q = i % (p.K / 4);
-        const float4 v = *reinterpret_cast<const float4 *>(p.W + (size_t)n * p.ldw + q * 4);
-        *reinterpret_cast<float4 *>(sm.w + (q >> 3) * kChunkBytes + sw128_offset(n, q & 7)) = to_tf32(v);
-    }
-    for (int i = tid; i < kBN; i += kTThreads) {
-        sm.sbias[i] = p.bias ? p.bias[i] : 0.f;
-        if (i < p.K) { sm.sa[i] = p.a ? p.a[i] : 1.f; sm.sb[i] = p.a ? p.b[i] : 0.f; }
-    }
-    fence_proxy_async_smem();
-    tc_fence_before_sync();
-    __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = sm.tmem_base;
 
-    if (warp < kTMmaWarp) {
-        // ================================ converters ================================
-        // warp w owns channel chunk c = w & 3 and pixel rows r0 + 8 i (i = 0..7): a warp instruction covers 4 rows x 128 B.
-        const int rl = lane >> 3, u = lane & 7;
-        const int c = warp & 3, r0 = (warp >> 2) * 4 + rl;
-        const int k = c * 32 + u * 4;
-        const bool kin = k < p.K, chunk_used = c * 32 < p.K;
-        float4 av = make_float4(1.f, 1.f, 1.f, 1.f), bv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (kin) { av = *reinterpret_cast<const float4 *>(&sm.sa[k]); bv = *reinterpret_cast<const float4 *>(&sm.sb[k]); }
-        const bool act = p.a != nullptr && !(GA_ABLATE & 2);
-        {   // log2 domain: z * log2(e) comes straight out of the FMA
-            const float L2E = 1.44269504089f;
-            av.x *= L2E; av.y *= L2E; av.z *= L2E; av.w *= L2E; bv.x *= L2E; bv.y *= L2E; bv.z *= L2E; bv.w *= L2E;
-        }
-        const int M = p.M, ldx = p.ldx;
-        const uint32_t soff = (uint32_t)c * kTChunk + sw128_offset(r0, u);      // + i * 1024
-        const float *x0 = p.X + (size_t)r0 * ldx + k;
-        auto issue = [&](int t, int st) {
-            if (!chunk_used || (GA_ABLATE & 1)) return;
-            const uint32_t dst = smem_u32(sm.x[st]) + soff;
+    // W slice of this warp as A fragments: rows (output channels) oc, oc + 8; K columns 8 ks + t4, + 4
+    const int oc = 16 * warp + g;
+    uint32_t wa[16][4];
+#pragma unroll
+    for (int ks = 0; ks < 16; ++ks) {
+        const int k = 8 * ks + t4;
+        const bool ok = ks < nk;
+        wa[ks][0] = __float_as_uint(ok ? to_tf32(p.W[(size_t)oc * p.ldw + k]) : 0.f);
+        wa[ks][1] = __float_as_uint(ok ? to_tf32(p.W[(size_t)(oc + 8) * p.ldw + k]) : 0.f);
+        wa[ks][2] = __float_as_uint(ok ? to_tf32(p.W[(size_t)oc * p.ldw + k + 4]) : 0.f);
+        wa[ks][3] = __float_as_uint(ok ? to_tf32(p.W[(size_t)(oc + 8) * p.ldw + k + 4]) : 0.f);
+    }
+    const float bias0 = p.bias ? p.bias[oc] : 0.f, bias1 = p.bias ? p.bias[oc + 8] : 0.f;
+    for (int i = tid; i < p.K; i += kTThreads) { sm.sa[i] = p.a ? p.a[i] : 1.f; sm.sb[i] = p.a ? p.b[i] : 0.f; }
+    __syncthreads();
+
+    // ---- copies / conversion: warp w owns channel chunk c = w & 3 and pixel rows r0 + 8 i (i = 0..7); a warp instruction covers
+    // 4 rows x 128 B
+    const int rl = lane >> 3, u = lane & 7;
+    const int c = warp & 3, r0 = (warp >> 2) * 4 + rl;
+    const int k = c * 32 + u * 4;
+    const bool kin = k < p.K, chunk_used = c * 32 < p.K;
+    float4 av = make_float4(1.f, 1.f, 1.f, 1.f), bv = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (kin) { av = *reinterpret_cast<const float4 *>(&sm.sa[k]); bv = *reinterpret_cast<const float4 *>(&sm.sb[k]); }
+    const bool act = p.a != nullptr;
+    {   // log2 domain: z * log2(e) comes straight out of the FMA
+        const float L2E = 1.44269504089f;
+        av.x *= L2E; av.y *= L2E; av.z *= L2E; av.w *= L2E; bv.x *= L2E; bv.y *= L2E; bv.z *= L2E; bv.w *= L2E;
+    }
+    const int M = p.M, ldx = p.ldx;
+    const uint32_t soff = (uint32_t)c * kTChunk + sw128_offset(r0, u);      // + i * 1024
+    const uint32_t x0s = smem_u32(sm.x[0]);
+    const float *x0 = p.X + (size_t)r0 * ldx + k;
+    auto issue = [&](int j) {
+        if (j < ntl && chunk_used) {
+            const int t = blockIdx.x + j * gstep;
+            const uint32_t dst = x0s + (uint32_t)(j % kTStages) * kTStageBytes + soff;
             const float *src = x0 + (size_t)t * kTPx * ldx;
             const bool whole = (t + 1) * kTPx <= M;
 #pragma unroll
@@ -147,126 +100,81 @@ tc_fwd_kernel(const TcFwdParams p)
                 const bool ok = kin && (whole || t * kTPx + r0 + 8 * i < M);      // rows >= M and channels >= K are zero-filled, never read
                 cp_async16(dst + i * 1024, ok ? src + (size_t)(8 * i) * ldx : p.X, ok);
             }
-        };
-        // the stage of tile t + kTStages is free once the tensor core has read tile t (mma_done): the first refill blocks, the others only probe
-        int tl = blockIdx.x, sl = 0, nl = 0, ahead = 0;
-        auto refill = [&]() {
-            while (ahead < kTLook && tl < num_tiles) {
-                if (ahead == 0) warp_wait(&sm.mma_done[sl], (nl & 1) ^ 1, lane);
-                else if (!warp_test(&sm.mma_done[sl], (nl & 1) ^ 1, lane)) break;
-                issue(tl, sl);
-                cp_async_commit();                         // one group per tile
-                ++ahead; tl += gstep; if (++sl == kTStages) { sl = 0; ++nl; }
-            }
-        };
-        refill();
-        int s = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gstep) {
-            if (ahead >= 3) cp_async_wait<2>(); else if (ahead == 2) cp_async_wait<1>(); else cp_async_wait<0>();
-            if (chunk_used) {
-                unsigned char *xs = sm.x[s] + soff;
+        }
+        cp_async_commit();                             // one group per tile (empty past the end): the wait count stays uniform
+    };
+    for (int j = 0; j < kTLook; ++j) issue(j);
+
+    const int ldy = p.ldy;
+    double dsum[2] = {0.0, 0.0}, dsq[2] = {0.0, 0.0};
+    for (int j = 0; j < ntl; ++j) {
+        const int tile = blockIdx.x + j * gstep;
+        const uint32_t xs_u = x0s + (uint32_t)(j % kTStages) * kTStageBytes;
+        cp_async_wait<kTLook - 1>();
+        if (chunk_used) {
+            unsigned char *xs = sm.x[j % kTStages] + soff;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    float4 x = (GA_ABLATE & 1) ? make_float4(0.5f, 0.25f, 0.125f, 1.f) : *reinterpret_cast<const float4 *>(xs + i * 1024);
-                    if (act) {
-                        x.x = softplus_log2(fmaf(x.x, av.x, bv.x)); x.y = softplus_log2(fmaf(x.y, av.y, bv.y));
-                        x.z = softplus_log2(fmaf(x.z, av.z, bv.z)); x.w = softplus_log2(fmaf(x.w, av.w, bv.w));
-                    }
-                    *reinterpret_cast<float4 *>(xs + i * 1024) = to_tf32(x);       // rows >= M hold act(bn(0)): their columns are never stored
+            for (int i = 0; i < 8; ++i) {
+                float4 x = *reinterpret_cast<const float4 *>(xs + i * 1024);
+                if (act) {
+                    x.x = softplus_log2(fmaf(x.x, av.x, bv.x)); x.y = softplus_log2(fmaf(x.y, av.y, bv.y));
+                    x.z = softplus_log2(fmaf(x.z, av.z, bv.z)); x.w = softplus_log2(fmaf(x.w, av.w, bv.w));
+                }
+                *reinterpret_cast<float4 *>(xs + i * 1024) = to_tf32(x);       // rows >= M hold act(bn(0)): their columns are never stored
+            }
+        }
+        __syncthreads();                               // the tile is complete; every warp has finished the previous one
+        issue(j + kTLook);                             // refills the stage of tile j - 1
+
+        float acc[8][4];
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < 16; ++ks) {
+            if (ks < nk) {
+                const int kk = 8 * ks + t4;
+#pragma unroll
+                for (int nt = 0; nt < 8; ++nt) {
+                    const int n = 8 * nt + g;
+                    mma_tf32(acc[nt], wa[ks], lds32(xs_u + kmajor_off(n, kk, kTChunk)), lds32(xs_u + kmajor_off(n, kk + 4, kTChunk)));
                 }
             }
-            fence_proxy_async_smem();
-            warp_arrive(&sm.full[s], lane);
-            if (++s == kTStages) s = 0;
-            --ahead;
-            refill();
         }
-    } else if (warp == kTMmaWarp) {
-        // ================================ MMA issuer ================================
-        constexpr uint32_t idesc = make_idesc_tf32(128, kTPx, false, false);
-        const uint32_t w_lo = desc_lo(smem_u32(sm.w), 16);
-        const int nk = (GA_ABLATE & 4) ? 0 : p.K / 8;               // 16 (K = 128) or 9 (K = 72)
-        int s = 0, n = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gstep) {
-            warp_wait(&sm.full[s], n & 1, lane);
-            warp_wait(&sm.tmem_empty[s], (n & 1) ^ 1, lane);
-            tc_fence_after_sync();
-            if (lane == 0) {
-                constexpr uint32_t hi = desc_hi(1024);
-                const uint32_t x_lo = desc_lo(smem_u32(sm.x[s]), 16);
-                const uint32_t d = tmem_base + (uint32_t)s * kTPx;
+
+        // ---- epilogue: acc[nt] = {Y^T(oc, px), Y^T(oc, px + 1), Y^T(oc + 8, px), Y^T(oc + 8, px + 1)}, px = 8 nt + 2 t4
+        float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
+        const int rows = M - tile * kTPx;              // valid pixels of this tile
+        float *yt = p.Y + (size_t)tile * kTPx * ldy;
 #pragma unroll
-                for (int k = 0; k < 16; ++k)
-                    if (k < nk)
-                        mma_tf32_lohi(d, w_lo + (uint32_t)(k >> 2) * (kChunkBytes >> 4) + (uint32_t)(k & 3) * 2u,
-                                      x_lo + (uint32_t)(k >> 2) * (kTChunk >> 4) + (uint32_t)(k & 3) * 2u, hi, idesc, k > 0);
-                mma_commit(&sm.mma_done[s]);
-            }
-            __syncwarp();
-            if (++s == kTStages) { s = 0; ++n; }
-        }
-    } else {
-        // ================================ epilogue: one output channel per thread ================================
-        const int ew = warp - kTEpiWarp0, q = warp & 3, half = ew >> 2;
-        const int c = q * 32 + lane;                 // TMEM lane == output channel
-        const float bias = sm.sbias[c];
-        const int ldy = p.ldy;
-        const bool accumulate = p.accumulate && !(GA_ABLATE & 16);
-        const size_t ystep = (size_t)gstep * kTPx * ldy;
-        float *yp = p.Y + ((size_t)blockIdx.x * kTPx + half * 32) * ldy + c;        // this thread's column, first of its 32 rows
-        double dsum = 0.0, dsq = 0.0;
-        int s = 0, n = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gstep, yp += ystep) {
-            const int rows = p.M - (tile * kTPx + half * 32);                       // valid rows of this warp's slice (may be <= 0 or >= 32)
-            float ev[16];
-            auto ldev = [&](int ph) {                // existing Y (the fan-in's other half): fetched before the accumulator is needed
+        for (int nt = 0; nt < 8; ++nt) {
 #pragma unroll
-                for (int j = 0; j < 16; ++j) ev[j] = (ph * 16 + j < rows) ? yp[(ph * 16 + j) * ldy] : 0.f;
-            };
-            if (accumulate) ldev(0);
-            warp_wait(&sm.mma_done[s], n & 1, lane);
-            tc_fence_after_sync();
-            float cs = 0.f, cq = 0.f;
-#pragma unroll 1
-            for (int ph = 0; ph < 2; ++ph) {
-                float v[16];
-                tmem_ld_32x16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)s * kTPx + half * 32 + ph * 16, v);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] += bias;
-                if (accumulate) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] += ev[j];
-                    if (ph == 0) ldev(1);
-                }
-                if (rows >= (ph + 1) * 16) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        if (!(GA_ABLATE & 16)) yp[(ph * 16 + j) * ldy] = v[j];
-                        if (!(GA_ABLATE & 8)) { cs += v[j]; cq = fmaf(v[j], v[j], cq); }
-                    }
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j)
-                        if (ph * 16 + j < rows) {
-                            if (!(GA_ABLATE & 16)) yp[(ph * 16 + j) * ldy] = v[j];
-                            if (!(GA_ABLATE & 8)) { cs += v[j]; cq = fmaf(v[j], v[j], cq); }
-                        }
+            for (int e = 0; e < 2; ++e) {
+                const int px = 8 * nt + 2 * t4 + e;
+                if (px < rows) {
+                    float *yp = yt + (size_t)px * ldy + oc;
+                    float v0 = acc[nt][e] + bias0, v1 = acc[nt][2 + e] + bias1;
+                    if (p.accumulate) { v0 += yp[0]; v1 += yp[8]; }
+                    yp[0] = v0; yp[8] = v1;
+                    cs[0] += v0; cq[0] = fmaf(v0, v0, cq[0]);
+                    cs[1] += v1; cq[1] = fmaf(v1, v1, cq[1]);
                 }
             }
-            tc_fence_before_sync();
-            warp_arrive(&sm.tmem_empty[s], lane);          // accumulator drained
-            dsum += (double)cs; dsq += (double)cq;
-            if (++s == kTStages) { s = 0; ++n; }
         }
-        if (p.sum) {                                 // the two pixel halves of a channel meet in shared memory: 2 atomics per channel per CTA
-            if (half == 1) { sm.red[0][c] = dsum; sm.red[1][c] = dsq; }
-            named_bar_sync(1, 8 * 32);
-            if (half == 0) { atomicAdd(&p.sum[c], dsum + sm.red[0][c]); atomicAdd(&p.sumsq[c], dsq + sm.red[1][c]); }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) { dsum[h] += (double)cs[h]; dsq[h] += (double)cq[h]; }
+    }
+    cp_async_wait<0>();
+    if (p.sum) {                                       // the four lanes of a channel meet by shuffles: 2 atomics per channel per CTA
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int o = 1; o < 4; o <<= 1) {
+                dsum[h] += __shfl_xor_sync(0xffffffffu, dsum[h], o);
+                dsq[h] += __shfl_xor_sync(0xffffffffu, dsq[h], o);
+            }
+            if (t4 == 0) { atomicAdd(&p.sum[oc + 8 * h], dsum[h]); atomicAdd(&p.sumsq[oc + 8 * h], dsq[h]); }
         }
     }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == kTMmaWarp) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 }  // namespace
@@ -275,18 +183,18 @@ tc_fwd_kernel(const TcFwdParams p)
 int launch_tc_fwd(const float *X, int ldx, int K, const float *a, const float *b, const float *W, int ldw, const float *bias, float *Y,
                   int ldy, int accumulate, double *sum, double *sumsq, int M, cudaStream_t st)
 {
-    GA_REQUIRE(K % 8 == 0 && K >= 8 && K <= 128, "tcgen05 layer: K=%d must be a multiple of 8 in [8,128]", K);
-    GA_REQUIRE(ldx % 4 == 0 && ldw % 4 == 0 && ldy % 4 == 0, "tcgen05 layer: leading dimensions must be multiples of 4");
+    GA_REQUIRE(K % 8 == 0 && K >= 8 && K <= 128, "tensor-core layer: K=%d must be a multiple of 8 in [8,128]", K);
+    GA_REQUIRE(ldx % 4 == 0 && ldw % 4 == 0 && ldy % 4 == 0, "tensor-core layer: leading dimensions must be multiples of 4");
     TcFwdParams p{X, ldx, K, a, b, W, ldw, bias, Y, ldy, accumulate, sum, sumsq, M};
     static PerDeviceOnce attr_t_set;
     if (attr_t_set.first()) {
-        GA_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcFwdTSmem) + 1024));
+        GA_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcFwdSmem) + 1024));
     }
-    const int tiles = cdiv(M, kTPx);
-    const int grid = tiles < kNumSMs ? tiles : kNumSMs;
+    const int tiles = cdiv(M, kTPx), sms = num_sms();
+    const int grid = tiles < sms ? tiles : sms;
     {
         ProfScope _ps("mlp_tc_fwd", st);
-        launch_k(tc_fwd_kernel, grid, kTThreads, sizeof(TcFwdTSmem) + 1024, st, p);
+        launch_k(tc_fwd_kernel, grid, kTThreads, sizeof(TcFwdSmem) + 1024, st, p);
     }
     GA_CHECK_LAUNCH("tc_fwd_kernel");
     return GA_OK;
@@ -308,56 +216,25 @@ extern "C" int ga_tc_linear_forward(int32_t M, int32_t K, const float *X, int32_
 //
 //   G  = dY_l      [px, out] = ga (dZ_l - m1 - xhat_l m2)          BatchNorm backward applied while loading (dZ_l, Y_l)
 //   X  = x_l       [px, in ] = softplus(a Y_{l-1} + b)             recomputed while loading Y_{l-1}
-//   dW_l [out,in] += G^T X      K = pixel: A = G and B = X are consumed MN-major straight from their pixel-major images
-//                               (128-byte swizzle with a 32-byte base, UMMA layout type 1); the accumulator lives in TMEM for
-//                               the whole kernel, one flush (16-byte vector reductions) at the end
-//   dX^T [in, px]  = W_l^T G^T  A = W_l^T [in rows][out] (transposed once per CTA), B = G [px rows][out] K-major; computed
-//                               TRANSPOSED so that a TMEM lane is an input channel: the epilogue thread's BatchNorm
-//                               scalars are constants and sum(dZ), sum(dZ xhat) need no cross-thread reduction
+//   dW_l [out,in] += G^T X      K = pixel: warp w accumulates output rows 16 w .. 16 w + 15 x all 128 input columns in registers for
+//                               the whole launch (A fragments from the K-major G image, B fragments from the pixel-major X image),
+//                               one flush (8-byte vector reductions) at the end
+//   dX^T [in, px]  = W_l^T G^T  computed TRANSPOSED: warp w owns input channels 16 w .. 16 w + 15, whose W^T slice lives in registers
+//                               as A fragments for the whole launch; a thread's BatchNorm scalars are constants
 //   dZ_{l-1} = dX * sigmoid(z_{l-1})   (sigmoid(z_{l-1}) and xhat_{l-1} recovered from x = softplus(z) in the X tile: no re-read)
-// G is stored in two swizzles of the same [px][channel] image (K-major operands reject layout type 1), X once.  The raw operands
-// travel global -> shared with 16-byte cp.async (no register behind a load in flight) and are converted IN PLACE; dZ_{l-1} leaves
-// straight from the epilogue registers (one whole 128-byte line per warp instruction).  32-pixel tiles, three stages, 25 warps:
-// 8 converters for G, 8 for X, 1 MMA issuer, 8 epilogue (two per TMEM lane quarter, 16 pixels each).
-// Round-2 log (tools/variants.py on the device, profiles/r2_tc_bwd_ncu.md): register loads one tile ahead -> cp.async in place
-// 1.97 -> 1.63 ms per step; shared-memory staging + named barrier + row stores -> direct stores 1.63 -> 1.55 ms.  What did NOT pay:
-// bulk L2 prefetch from the MMA warp (3.1 ms: 128 small TMA requests per tile), dedicated copy warps / copies issued by the
-// epilogue warps with mbarrier completion (1.8 / 1.7 ms: one more parked wait per tile on the ring), spinning instead of
-// suspended mbarrier waits (1.8 ms), "arrive before prefetch" (2.0 ms).  With every load, store, MMA and activation ablated the
-// skeleton (waits, converter LDS/STS, tcgen05.ld) still takes 58 us of the 129 us per launch: the kernel is bound by the per-tile
-// hand-offs of its 32-pixel tiles, which the 227 KB of shared memory do not allow to grow (64 KB W^T + 3 x 48 KB stages).
+// The raw operands travel global -> shared with 16-byte cp.async (no register behind a load in flight), three 32-pixel tiles ahead
+// over four 48 KB stages, and are converted IN PLACE by the thread that copied them; one block barrier per tile.
 // =====================================================================================================================
 namespace ga {
 namespace {
 
-#ifndef GA_BWD_PX
-#define GA_BWD_PX 32
-#endif
-constexpr int kPx = GA_BWD_PX;            // pixels per tile: 32, or 64 (two stages) when W^T lives in tensor memory
-constexpr int kBlk = kPx / 8, kPh = kPx / 16;
-static_assert(kPx == 32 || kPx == 64, "tc_bwd tile: 32 pixels (default) or 64; 48 was measured (no gain) and is not supported");
-#ifndef GA_BWD_WT_TMEM
-#define GA_BWD_WT_TMEM 1
-#endif
-constexpr int kBStages = GA_BWD_PX == 64 ? 2 : GA_BWD_WT_TMEM ? 4 : 3;   // W^T in tensor memory frees 64 KB of shared memory: a fourth 48 KB stage
+constexpr int kPx = 32, kBlk = kPx / 8;
+constexpr int kBStages = 4, kLook = 3;    // tiles of raw operand copies in flight (a stage is refilled one tile after it was read)
 constexpr int kGkChunk = kPx * 128;       // 4 KB: [32 px rows][32 channels]
 constexpr int kGkTile = 4 * kGkChunk;     // 16 KB
-constexpr int kMnTile = 4 * kGkChunk;     // 16 KB: MN-major image [4 x 32-channel chunks][32 px][128 B] (32-byte-base swizzle)
-#ifndef GA_BWD_EWARPS
-#define GA_BWD_EWARPS 8
-#endif
-#ifndef GA_BWD_G_MMADONE
-#define GA_BWD_G_MMADONE 1
-#endif
-#ifndef GA_BWD_LOOK
-#define GA_BWD_LOOK (GA_BWD_PX == 64 ? 1 : GA_BWD_WT_TMEM ? 3 : 2)
-#endif
-constexpr int kLook = GA_BWD_LOOK;               // tiles of raw operand copies in flight per producer thread (1 or 2; < kBStages)
-constexpr int kBwdEWarps = GA_BWD_EWARPS;  // epilogue warps: 4 (each 2 x 16 pixels) or 8 (two per TMEM lane quarter, 16 pixels each)
-constexpr int kBwdThreads = (17 + kBwdEWarps) * 32;      // 8 G-producer warps, 8 X-producer warps, 1 MMA warp, epilogue warps
-constexpr int kBwdMmaWarp = 16, kBwdEpiWarp0 = 17;
-constexpr uint32_t kBwdTmemCols = GA_BWD_WT_TMEM ? 512 : 256;    // [0,128): dW accumulator; 128 + 32 s: dX^T accumulator of stage s; [256,384): W^T
-constexpr uint32_t kWtCol = 256;
+constexpr int kMnTile = 4 * kGkChunk;     // 16 KB: pixel-major image [4 x 32-channel chunks][32 px][128 B] (32-byte pieces XOR px % 4)
+constexpr int kBwdThreads = 8 * 32;
+static_assert(kLook < kBStages, "lookahead must leave the stage being read alone");
 
 struct TcBwdParams {
     const float *dZ, *Y; int ldg;                      // layer l: [M][ldg], 128 output channels from the pointer
@@ -375,16 +252,11 @@ struct TcBwdParams {
 };
 
 struct alignas(1024) TcBwdSmem {
-#if !GA_BWD_WT_TMEM
-    unsigned char wt[4 * 128 * 128];                   // 64 KB: W^T, rows = input channel, K = output channel
-#endif
-    unsigned char gk[kBStages][kGkTile];               // G   rows = pixel,          K = output channel   (dgrad B operand)
-    unsigned char gm[kBStages][kMnTile];               // G   MN-major: M = output channel, K = pixel     (wgrad A operand)
-    unsigned char xm[kBStages][kMnTile];               // X   MN-major: N = input channel,  K = pixel     (wgrad B operand)
+    unsigned char gk[kBStages][kGkTile];               // G   rows = pixel, K = output channel (K-major); dZ lands here
+    unsigned char ym[kBStages][kMnTile];               // raw Y_l, pixel-major: only read by the G conversion
+    unsigned char xm[kBStages][kMnTile];               // X   pixel-major: rows = pixel, 128 input channels
     float gA[128], gB[128], gC[128];                   // dY = gA dZ + gB Y + gC  (BatchNorm backward folded to two FMAs)
     float pa[128], pb[128], pbeta[128], pinvg[128];    // layer l-1: z log2e = y pa + pb ; xhat = (z - pbeta) * pinvg
-    uint64_t full[kBStages], empty[kBStages], mma_done[kBStages], tmem_empty[kBStages];
-    uint32_t tmem_base;
 };
 
 __global__ void __launch_bounds__(kBwdThreads, 1)
@@ -393,34 +265,24 @@ tc_bwd_kernel(const TcBwdParams p)
     extern __shared__ unsigned char smem_raw[];
     TcBwdSmem &sm = *reinterpret_cast<TcBwdSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int num_tiles = (p.M + kPx - 1) / kPx;
-#if GA_TC_TIMING
-    long long tw_[4] = {0, 0, 0, 0};
-    const long long tstart_ = clock64();
-#endif
+    const int g = lane >> 2, t4 = lane & 3;
+    const int M = p.M;
+    const int num_tiles = (M + kPx - 1) / kPx;
+    const int gstep = gridDim.x;
+    const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
+    pdl_wait();
 
-    if (tid == 0) {
-        for (int s = 0; s < kBStages; ++s) {
-            mbar_init(&sm.full[s], 16 * kArrivalsPerWarp); mbar_init(&sm.empty[s], kBwdEWarps * kArrivalsPerWarp);        // arrivals are per WARP (warp_arrive)
-            mbar_init(&sm.mma_done[s], 1); mbar_init(&sm.tmem_empty[s], kBwdEWarps * kArrivalsPerWarp);
-        }
-        fence_barrier_init();
+    // W^T slice of this warp as A fragments: rows (input channels) ic, ic + 8; K columns (output channels) 8 ks + t4, + 4
+    const int ic = 16 * warp + g;
+    uint32_t wa[16][4];
+#pragma unroll
+    for (int ks = 0; ks < 16; ++ks) {
+        const int o = 8 * ks + t4;
+        wa[ks][0] = __float_as_uint(ic < p.kin ? to_tf32(p.W[(size_t)o * p.ldw + ic]) : 0.f);
+        wa[ks][1] = __float_as_uint(ic + 8 < p.kin ? to_tf32(p.W[(size_t)o * p.ldw + ic + 8]) : 0.f);
+        wa[ks][2] = __float_as_uint(ic < p.kin ? to_tf32(p.W[(size_t)(o + 4) * p.ldw + ic]) : 0.f);
+        wa[ks][3] = __float_as_uint(ic + 8 < p.kin ? to_tf32(p.W[(size_t)(o + 4) * p.ldw + ic + 8]) : 0.f);
     }
-    if (warp == kBwdMmaWarp) tmem_alloc(&sm.tmem_base, kBwdTmemCols);
-    pdl_wait();            // barrier init and TMEM allocation above overlap the previous kernel's tail
-#if !GA_BWD_WT_TMEM
-    // W^T -> shared (K-major over the OUTPUT channel): element (in, out) <- W[out][in]
-    // thread = (input channel, group of 4 output channels): four coalesced row reads of W, ONE 16-byte store of the transposed quad
-    // (the 8 lanes of a store phase have 8 different `in & 7`, hence 8 different 16-byte units: conflict-free)
-    for (int i = tid; i < 128 * 32; i += kBwdThreads) {
-        const int in = i & 127, o = (i >> 7) * 4;
-        if (in < p.kin) {
-            const float *wp = p.W + (size_t)o * p.ldw + in;
-            const float4 v = to_tf32(make_float4(wp[0], wp[p.ldw], wp[2 * p.ldw], wp[3 * p.ldw]));
-            *reinterpret_cast<float4 *>(sm.wt + (o >> 5) * (128 * 128) + in * 128 + ((((o & 31) >> 2) ^ (in & 7)) << 4)) = v;
-        }
-    }
-#endif
     for (int i = tid; i < 128; i += kBwdThreads) {
         if (p.ga) {   // ga (dZ - m1 - (Y - mu) rstd m2)
             const float ga = p.ga[i], k = p.rstd[i] * p.m2[i];
@@ -435,351 +297,174 @@ tc_bwd_kernel(const TcBwdParams p)
             sm.pbeta[i] = b + p.pmu[i] * a; sm.pinvg[i] = p.prstd[i] / a;
         }
     }
-    fence_proxy_async_smem();
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = sm.tmem_base;
-#if GA_BWD_WT_TMEM
-    // W^T -> TENSOR MEMORY: the dgrad's A operand (rows = input channel = TMEM lane, one column per output channel) is read by the
-    // tensor core from there, so it costs neither shared memory (64 KB) nor shared-memory bandwidth (it was re-read for every tile).
-    // Four warps, one per lane quarter: lanes read W[out][in] coalesced over `in`.
-    if (warp >= kBwdEpiWarp0 && warp < kBwdEpiWarp0 + 4) {
-        const int in = (warp & 3) * 32 + lane;
-        const float *wp = p.W + in;
-#pragma unroll 1
-        for (int cc = 0; cc < 8; ++cc) {
-            float v[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = in < p.kin ? to_tf32(wp[(size_t)(cc * 16 + j) * p.ldw]) : 0.f;
-            tmem_st_32x16(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + kWtCol + cc * 16, v);
-        }
-    }
-    tc_fence_before_sync();
-    __syncthreads();
-    tc_fence_after_sync();
-#endif
-#if GA_TC_TIMING
-    const long long tpro_ = clock64() - tstart_;
-    long long tloop_ = 0;
-#endif
 
-    // ================================ converters: warps 0-7 build G (two swizzles), warps 8-15 build X =================
-    // Both wgrad operands are consumed MN-major (pixel = K index), which for 32-bit elements means the 128-byte swizzle with a
-    // 32-byte base (layout type 1; the physical layout was decoded with tools/exp_umma_probe.cu):
-    //     byte(px, c) = (c / 32) * LBO + (px / 4) * SBO + (px % 4) * 128 + ((((c % 32) / 8) ^ (px % 4)) * 32) + (c % 8) * 4
-    // so a pixel's 32 channels stay one permuted 128-byte row, exactly like the K-major image the dgrad needs (16-byte units
-    // XOR px % 8): the two images differ only by a permutation of the 16-byte pieces inside each 128-byte row.  A warp instruction
-    // covers 4 pixels x 128 B (full-line global requests) and every quarter-warp touches one whole row (conflict-free).
-    // Warp w owns the 32-channel chunk j = w & 3 (its BatchNorm coefficients are thread constants) and pixel rows p0 + 8 e.
-    const int M = p.M;
-    if (warp < kBwdMmaWarp) {
-        const int c16 = lane & 7, pxl = lane >> 3;
-        const int pw = warp & 7;
-        const int j = pw & 3, p0 = (pw >> 2) * 4 + pxl;                      // block e is pixel p0 + 8 e:  px & 7 == p0, px & 3 == pxl
-        const int ch = j * 32 + c16 * 4;                                     // this thread's 4 channels (all tiles, all blocks)
-        const uint32_t k_off = (uint32_t)j * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((c16 ^ p0) << 4);                       // + e * 1024
-        const uint32_t mn_off = (uint32_t)j * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((((c16 >> 1) ^ pxl) << 5) | ((c16 & 1) << 4));
-        int s = 0, n = 0;
-        const int gstep = gridDim.x;
-        int tile = blockIdx.x;
-        if (warp < 8) {
-            const float4 cA = *reinterpret_cast<const float4 *>(&sm.gA[ch]), cB = *reinterpret_cast<const float4 *>(&sm.gB[ch]),
-                         cC = *reinterpret_cast<const float4 *>(&sm.gC[ch]);
-            const int ldg = p.ldg;
-            const bool has_y = p.ga != nullptr;
-            const float *dz0 = p.dZ + (size_t)p0 * ldg + ch, *y0 = (has_y ? p.Y : p.dZ) + (size_t)p0 * ldg + ch;   // block e adds 8 e rows
-            const size_t tile_stride = (size_t)kPx * ldg;
-            // The raw dZ / Y pieces travel global -> shared with 16-byte cp.async, each straight to the address its converted value will
-            // occupy (dZ: the K-major image, Y: the MN-major image), kLook tiles ahead and without a register; once a tile has landed, the
-            // thread that copied a piece reads it back, folds the BatchNorm backward and overwrites both images IN PLACE -- every piece is
-            // private to one thread, so the conversion needs no synchronisation beyond cp.async.wait_group.
-            const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            const int row8 = 8 * ldg;
-            const ptrdiff_t ydelta = y0 - dz0;
-            // running source pointer of the NEXT tile to copy, stage addresses as base + stage * size: a whole tile (every tile but possibly
-            // the last) is 8 plain copies with no predicate or select -- this bookkeeping used to be 15 % of the kernel's instructions
-            const float *pz = dz0 + (size_t)tile * tile_stride;
-            const size_t pstep = (size_t)gstep * tile_stride;
-            const uint32_t dk0 = smem_u32(sm.gk[0]) + k_off, dm0 = smem_u32(sm.gm[0]) + mn_off;
-            auto issue = [&](int t, int st) {
-                if (!(GA_ABLATE & 1)) {
-                    const uint32_t dk = dk0 + (uint32_t)st * kGkTile, dm = dm0 + (uint32_t)st * kMnTile;
-                    if ((t + 1) * kPx <= M) {
+    // ---- copies / conversion.  The pixel-major image (32-byte pieces XOR px % 4):
+    //     byte(px, c) = (c / 32) * kGkChunk + px * 128 + ((((c % 32) / 8) ^ (px % 4)) * 32) + (c % 8) * 4
+    // keeps a pixel's 32 channels one permuted 128-byte row, exactly like the K-major image (16-byte units XOR px % 8): a warp
+    // instruction covers 4 pixels x 128 B (full-line global requests).  Warp w owns the 32-channel chunk j = w & 3 (its BatchNorm
+    // coefficients are thread constants) and pixel rows p0 + 8 e, for G and for X.
+    const int c16 = lane & 7, pxl = lane >> 3;
+    const int jc = warp & 3, p0 = (warp >> 2) * 4 + pxl;                     // block e is pixel p0 + 8 e:  px & 7 == p0, px & 3 == pxl
+    const int ch = jc * 32 + c16 * 4;                                        // this thread's 4 channels (all tiles, all blocks)
+    const uint32_t k_off = (uint32_t)jc * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((c16 ^ p0) << 4);                       // + e * 1024
+    const uint32_t mn_off = (uint32_t)jc * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((((c16 >> 1) ^ pxl) << 5) | ((c16 & 1) << 4));
+    const float4 cA = *reinterpret_cast<const float4 *>(&sm.gA[ch]), cB = *reinterpret_cast<const float4 *>(&sm.gB[ch]),
+                 cC = *reinterpret_cast<const float4 *>(&sm.gC[ch]);
+    const float4 av = *reinterpret_cast<const float4 *>(&sm.pa[ch]), bv = *reinterpret_cast<const float4 *>(&sm.pb[ch]);
+    const bool has_y = p.ga != nullptr, raw = p.x_raw != 0, okc = ch < p.kin;
+    const int ldg = p.ldg, ldp = p.ldp;
+    const float *dz0 = p.dZ + (size_t)p0 * ldg + ch, *y0 = (has_y ? p.Y : p.dZ) + (size_t)p0 * ldg + ch;   // block e adds 8 e rows
+    const float *x0 = p.Yprev + (size_t)p0 * ldp + ch;
+    const uint32_t gk0 = smem_u32(sm.gk[0]), ym0 = smem_u32(sm.ym[0]), xm0 = smem_u32(sm.xm[0]);
+    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    auto issue = [&](int jt) {
+        if (jt < ntl) {
+            const int t = blockIdx.x + jt * gstep, st = jt % kBStages;
+            const uint32_t dk = gk0 + (uint32_t)st * kGkTile + k_off, dy = ym0 + (uint32_t)st * kMnTile + mn_off,
+                           dx = xm0 + (uint32_t)st * kMnTile + mn_off;
+            const float *pz = dz0 + (size_t)t * kPx * ldg, *py = y0 + (size_t)t * kPx * ldg, *px = x0 + (size_t)t * kPx * ldp;
 #pragma unroll
-                        for (int e = 0; e < kBlk; ++e) cp_async16_full(dk + e * 1024, pz + e * row8);
-                        if (has_y) {
-#pragma unroll
-                            for (int e = 0; e < kBlk; ++e) cp_async16_full(dm + e * 1024, pz + ydelta + e * row8);
-                        }
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < kBlk; ++e) {
-                            const bool ok = t * kPx + e * 8 + p0 < M;          // rows >= M are zero-filled
-                            cp_async16(dk + e * 1024, ok ? pz + e * row8 : dz0, ok);
-                            if (has_y) cp_async16(dm + e * 1024, ok ? pz + ydelta + e * row8 : dz0, ok);
-                        }
-                    }
-                }
-                pz += pstep;
-            };
-            // Copies run up to two tiles ahead.  The stage of the tile after next is the one the epilogue frees LAST, so it is only probed:
-            // if it is still busy the copy is issued one iteration later (blocking then would serialise conversion behind the epilogue).
-            int tl = tile, sl = 0, nl = 0, ahead = 0;      // next tile to copy, its stage / round; tiles copied but not yet converted
-            auto refill = [&]() {
-                while (ahead < kLook && tl < num_tiles) {
-                    uint64_t *freed = GA_BWD_G_MMADONE ? &sm.mma_done[sl] : &sm.empty[sl];   // the epilogue never touches the G images
-                    if (ahead == 0) TWAIT(0, warp_wait(freed, (nl & 1) ^ 1, lane));
-                    else if (!warp_test(freed, (nl & 1) ^ 1, lane)) break;
-                    issue(tl, sl);
-                    cp_async_commit();                     // one group per tile
-                    ++ahead; tl += gstep; if (++sl == kBStages) { sl = 0; ++nl; }
-                }
-            };
-            refill();
-            for (; tile < num_tiles; tile += gstep) {
-                if (ahead >= 3) cp_async_wait<2>(); else if (ahead == 2) cp_async_wait<1>(); else cp_async_wait<0>();      // this tile's pieces have landed (younger groups stay in flight)
-                unsigned char *gk = sm.gk[s] + k_off, *gm = sm.gm[s] + mn_off;
-                const bool ragged = (tile + 1) * kPx > M;
-#pragma unroll
-                for (int e = 0; e < kBlk; ++e) {
-                    float4 za, ya;
-                    if (GA_ABLATE & 1) { za = ya = make_float4(0.5f, 0.25f, 0.125f, 1.f); }
-                    else {
-                        za = *reinterpret_cast<const float4 *>(gk + e * 1024);
-                        ya = has_y ? *reinterpret_cast<const float4 *>(gm + e * 1024) : za;
-                    }
-                    float4 o;
-                    o.x = fmaf(cA.x, za.x, fmaf(cB.x, ya.x, cC.x)); o.y = fmaf(cA.y, za.y, fmaf(cB.y, ya.y, cC.y));
-                    o.z = fmaf(cA.z, za.z, fmaf(cB.z, ya.z, cC.z)); o.w = fmaf(cA.w, za.w, fmaf(cB.w, ya.w, cC.w));
-                    if (ragged && tile * kPx + e * 8 + p0 >= M) o = zero4;       // rows >= M carry zeros (gC alone would not be zero)
-                    o = to_tf32(o);
-                    *reinterpret_cast<float4 *>(gk + e * 1024) = o;
-                    *reinterpret_cast<float4 *>(gm + e * 1024) = o;
-                }
-                fence_proxy_async_smem();
-                warp_arrive(&sm.full[s], lane);
-                if (++s == kBStages) { s = 0; ++n; }
-                --ahead;
-                refill();
-            }
-        } else {
-            const int ldp = p.ldp;
-            const bool raw = p.x_raw != 0 || (GA_ABLATE & 2);
-            const bool x_read_by_epilogue = (p.mode == 0 || p.mode == 3) && !(GA_ABLATE & 8);      // final modes recover sigmoid / xhat from the X tile
-            const float4 av = *reinterpret_cast<const float4 *>(&sm.pa[ch]), bv = *reinterpret_cast<const float4 *>(&sm.pb[ch]);
-            const bool okc = ch < p.kin;
-            const float *x0 = p.Yprev + (size_t)p0 * ldp + ch;
-            const size_t tile_stride = (size_t)kPx * ldp;
-            const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            const int row8 = 8 * ldp;
-            const float *px = x0 + (size_t)tile * tile_stride;
-            const size_t pstep = (size_t)gstep * tile_stride;
-            const uint32_t dm0 = smem_u32(sm.xm[0]) + mn_off;
-            auto issue = [&](int t, int st) {
-                if (!(GA_ABLATE & 1)) {
-                    const uint32_t dm = dm0 + (uint32_t)st * kMnTile;
-                    if (okc && (t + 1) * kPx <= M) {
-#pragma unroll
-                        for (int e = 0; e < kBlk; ++e) cp_async16_full(dm + e * 1024, px + e * row8);
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < kBlk; ++e) {
-                            const bool ok = okc && t * kPx + e * 8 + p0 < M;     // channels past kin (the 72-wide input layer) are never read
-                            cp_async16(dm + e * 1024, ok ? px + e * row8 : p.Yprev, ok);
-                        }
-                    }
-                }
-                px += pstep;
-            };
-            int tl = tile, sl = 0, nl = 0, ahead = 0;
-            auto refill = [&]() {
-                while (ahead < kLook && tl < num_tiles) {
-                    uint64_t *freed = (GA_BWD_G_MMADONE && !x_read_by_epilogue) ? &sm.mma_done[sl] : &sm.empty[sl];
-                    if (ahead == 0) TWAIT(0, warp_wait(freed, (nl & 1) ^ 1, lane));
-                    else if (!warp_test(freed, (nl & 1) ^ 1, lane)) break;
-                    issue(tl, sl);
-                    cp_async_commit();
-                    ++ahead; tl += gstep; if (++sl == kBStages) { sl = 0; ++nl; }
-                }
-            };
-            refill();
-            for (; tile < num_tiles; tile += gstep) {
-                if (ahead >= 3) cp_async_wait<2>(); else if (ahead == 2) cp_async_wait<1>(); else cp_async_wait<0>();
-                unsigned char *xm = sm.xm[s] + mn_off;
-                const bool ragged = (tile + 1) * kPx > M;
-#pragma unroll
-                for (int e = 0; e < kBlk; ++e) {
-                    float4 o = (GA_ABLATE & 1) ? make_float4(0.5f, 0.25f, 0.125f, 1.f) : *reinterpret_cast<const float4 *>(xm + e * 1024);
-                    if (!raw) {
-                        o.x = softplus_log2(fmaf(o.x, av.x, bv.x)); o.y = softplus_log2(fmaf(o.y, av.y, bv.y));
-                        o.z = softplus_log2(fmaf(o.z, av.z, bv.z)); o.w = softplus_log2(fmaf(o.w, av.w, bv.w));
-                    }
-                    if (!okc || (ragged && tile * kPx + e * 8 + p0 >= M)) o = zero4;      // softplus(bn(0)) is not 0: rows >= M must be
-                    *reinterpret_cast<float4 *>(xm + e * 1024) = to_tf32(o);
-                }
-                fence_proxy_async_smem();
-                warp_arrive(&sm.full[s], lane);
-                if (++s == kBStages) { s = 0; ++n; }
-                --ahead;
-                refill();
+            for (int e = 0; e < kBlk; ++e) {
+                const bool ok = t * kPx + e * 8 + p0 < M;                        // rows >= M are zero-filled
+                cp_async16(dk + e * 1024, ok ? pz + (size_t)e * 8 * ldg : p.dZ, ok);
+                if (has_y) cp_async16(dy + e * 1024, ok ? py + (size_t)e * 8 * ldg : p.dZ, ok);
+                cp_async16(dx + e * 1024, ok && okc ? px + (size_t)e * 8 * ldp : p.Yprev, ok && okc);    // channels past kin are never read
             }
         }
-    } else if (warp == kBwdMmaWarp) {
-        // ================================ MMA issuer ================================
-        constexpr uint32_t idesc_dgrad = make_idesc_tf32(128, kPx, false, false);
-        constexpr uint32_t idesc_wgrad = make_idesc_tf32(128, 128, true, true);      // both operands MN-major (K = pixel)
-#if !GA_BWD_WT_TMEM
-        const uint32_t wt_addr = smem_u32(sm.wt);
-#endif
-        int it = 0, s = 0, n = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-            TWAIT(0, warp_wait(&sm.full[s], n & 1, lane));
-            TWAIT(1, warp_wait(&sm.tmem_empty[s], (n & 1) ^ 1, lane));
-            tc_fence_after_sync();
-            TMARK(tm_);
-            if (lane == 0 && (GA_ABLATE & 4)) mma_commit(&sm.mma_done[s]);
-            if (lane == 0 && !(GA_ABLATE & 4)) {
-                constexpr uint32_t hi = desc_hi(1024);
-                // MN-major images: 32-channel chunks kGkChunk apart (LBO), 4-pixel swizzle atoms 512 B apart (SBO), layout type 1
-                constexpr uint32_t hi_mn = (512u >> 4) | (1u << 14) | (1u << 29);
-#if !GA_BWD_WT_TMEM
-                const uint32_t wt_lo = desc_lo(wt_addr, 16);
-#endif
-                const uint32_t gk_lo = desc_lo(smem_u32(sm.gk[s]), 16), gm_lo = desc_lo(smem_u32(sm.gm[s]), kGkChunk),
-                               xm_lo = desc_lo(smem_u32(sm.xm[s]), kGkChunk);
-                const uint32_t d_dx = tmem_base + 128 + (uint32_t)s * kPx;
-                // dX^T[in, px] = sum_out W^T[in, out] G[px, out]: 16 steps of 8 output channels
+        cp_async_commit();                             // one group per tile (empty past the end): the wait count stays uniform
+    };
+    for (int jt = 0; jt < kLook; ++jt) issue(jt);
+
+    // ---- per-thread constants of the epilogue: input channels ic + 8 h
+    const bool final_mode = p.mode == 0 || p.mode == 3;
+    const bool add_existing = p.mode >= 2;
+    float cinvg[2], cbg[2], cl2g[2];
 #pragma unroll
-                for (int k = 0; k < 16; ++k)
-#if GA_BWD_WT_TMEM
-                    mma_tf32_ts(d_dx, tmem_base + kWtCol + (uint32_t)k * 8u, gk_lo + (uint32_t)(k >> 2) * (kGkChunk >> 4) + (uint32_t)(k & 3) * 2u, hi, idesc_dgrad, k > 0);
-#else
-                    mma_tf32_lohi(d_dx, wt_lo + (uint32_t)(k >> 2) * ((128 * 128) >> 4) + (uint32_t)(k & 3) * 2u,
-                                  gk_lo + (uint32_t)(k >> 2) * (kGkChunk >> 4) + (uint32_t)(k & 3) * 2u, hi, idesc_dgrad, k > 0);
-#endif
-                // dW[out, in] += sum_px G^T[out, px] X^T[in, px]: 4 steps of 8 pixels
-#pragma unroll
-                for (int j = 0; j < kPx / 8; ++j)
-                    mma_tf32_lohi(tmem_base, gm_lo + (uint32_t)j * (1024u >> 4), xm_lo + (uint32_t)j * (1024u >> 4), hi_mn, idesc_wgrad, (it > 0) || (j > 0));
-                mma_commit(&sm.mma_done[s]);
-            }
-            __syncwarp();
-            TADD(2, tm_);
-            if (++s == kBStages) { s = 0; ++n; }
-        }
-    } else {
-        // ================================ epilogue: one input channel per thread ================================
-        // 4 warps (TMEM lane quarter = warp & 3).  A thread's BatchNorm scalars are constants; sigmoid(z_{l-1}) and
-        // xhat_{l-1} are recovered from x = softplus(z) in the X^T tile (no global re-read); 2 x 16 pixels per tile.
-        const int ew = warp - kBwdEpiWarp0;          // 0..kBwdEWarps-1
-        constexpr int kPhStep = kBwdEWarps / 4;
-        const int q = warp & 3;
-        const int c = q * 32 + lane;                 // TMEM lane == input channel
+    for (int h = 0; h < 2; ++h) {
         // xhat = (z - beta) / gamma with z = x + ln2 * log2(sigmoid):  xhat = ln2/gamma * ls + (x / gamma - beta / gamma)
-        const float cinvg = sm.pinvg[c], cbg = sm.pbeta[c] * cinvg, cl2g = 0.69314718056f * cinvg;
-        const bool final_mode = (p.mode == 0 || p.mode == 3) && !(GA_ABLATE & 8);
-        const bool add_existing = p.mode >= 2 && c < p.kin && !(GA_ABLATE & 16);     // uniform per warp when kin is a multiple of 32
-        uint32_t xoff[4];                            // this channel's word inside the row of a pixel with px % 4 == i (MN-major image of X)
+        const int c = ic + 8 * h;
+        cinvg[h] = sm.pinvg[c]; cbg[h] = sm.pbeta[c] * cinvg[h]; cl2g[h] = 0.69314718056f * cinvg[h];
+    }
+    const int ldo = p.ldo;
+    float dw[16][4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) xoff[i] = (uint32_t)(c >> 5) * kGkChunk + (uint32_t)((((lane >> 3) ^ i) << 5) + (lane & 7) * 4);
-        const int ldo = p.ldo;
-        double d1 = 0.0, d2 = 0.0;
-        int s = 0, n = 0;
-        // running pointers (advanced by one grid round of tiles): the channel column this thread accumulates into, and the rows this warp stores
-        const size_t ostep = (size_t)gridDim.x * kPx * ldo;
-        const float *evp = p.dZprev + (size_t)blockIdx.x * kPx * ldo + c;
-        const bool store_col = c < p.kin && !(GA_ABLATE & 16);
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, evp += ostep) {
-            const int m0 = tile * kPx;
-            const bool full = m0 + kPx <= p.M;            // only the last tile can be ragged: one uniform branch instead of a test per row
-            // raw dX already accumulated by an earlier layer of this fan-in: fetched BEFORE waiting for the tensor core, and the second
-            // half while the first is being processed, so the latency hides behind the MMA and the sigmoid math (rows >= M are never read)
-            float ev[16];
-            auto ldev = [&](int ph) {
-                const float *ep = evp + ph * 16 * ldo;
-                if (full) {
+    for (int nt = 0; nt < 16; ++nt) dw[nt][0] = dw[nt][1] = dw[nt][2] = dw[nt][3] = 0.f;
+    double d1[2] = {0.0, 0.0}, d2[2] = {0.0, 0.0};
+
+    for (int jt = 0; jt < ntl; ++jt) {
+        const int tile = blockIdx.x + jt * gstep, st = jt % kBStages;
+        const int m0 = tile * kPx;
+        const bool ragged = m0 + kPx > M;
+        cp_async_wait<kLook - 1>();
+        {   // G = gA dZ + gB Y + gC -> K-major image (in place over dZ); X = softplus(bn(Yprev)) in place
+            unsigned char *gk = sm.gk[st] + k_off, *ym = sm.ym[st] + mn_off, *xm = sm.xm[st] + mn_off;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) ev[j] = ep[j * ldo];
-                } else {
-                    const int rows = p.M - (m0 + ph * 16);
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) ev[j] = (j < rows) ? ep[j * ldo] : 0.f;
+            for (int e = 0; e < kBlk; ++e) {
+                const bool row_ok = !ragged || m0 + e * 8 + p0 < M;
+                const float4 za = *reinterpret_cast<const float4 *>(gk + e * 1024);
+                const float4 ya = has_y ? *reinterpret_cast<const float4 *>(ym + e * 1024) : za;
+                float4 o;
+                o.x = fmaf(cA.x, za.x, fmaf(cB.x, ya.x, cC.x)); o.y = fmaf(cA.y, za.y, fmaf(cB.y, ya.y, cC.y));
+                o.z = fmaf(cA.z, za.z, fmaf(cB.z, ya.z, cC.z)); o.w = fmaf(cA.w, za.w, fmaf(cB.w, ya.w, cC.w));
+                if (!row_ok) o = zero4;                                   // rows >= M carry zeros (gC alone would not be zero)
+                *reinterpret_cast<float4 *>(gk + e * 1024) = to_tf32(o);
+                float4 x = *reinterpret_cast<const float4 *>(xm + e * 1024);
+                if (!raw) {
+                    x.x = softplus_log2(fmaf(x.x, av.x, bv.x)); x.y = softplus_log2(fmaf(x.y, av.y, bv.y));
+                    x.z = softplus_log2(fmaf(x.z, av.z, bv.z)); x.w = softplus_log2(fmaf(x.w, av.w, bv.w));
                 }
-            };
-            if (add_existing) ldev(ew >> 2);
-            TWAIT(0, warp_wait(&sm.mma_done[s], n & 1, lane));
-            tc_fence_after_sync();
-            TMARK(te_);
-            float t1 = 0.f, t2 = 0.f;
-#pragma unroll 1
-            for (int ph = ew >> 2; ph < kPh; ph += kPhStep) {
-                float v[16];
-                tmem_ld_32x16(tmem_base + ((uint32_t)(q * 32) << 16) + 128 + (uint32_t)s * kPx + ph * 16, v);
-                if (add_existing) {
+                if (!okc || !row_ok) x = zero4;                           // softplus(bn(0)) is not 0: rows >= M must be
+                *reinterpret_cast<float4 *>(xm + e * 1024) = to_tf32(x);
+            }
+        }
+        __syncthreads();                               // the tile is complete; every warp has finished the previous one
+        issue(jt + kLook);                             // refills the stage of tile jt - 1
+
+        const uint32_t gks = gk0 + (uint32_t)st * kGkTile, xms = xm0 + (uint32_t)st * kMnTile;
+        // dX^T[in, px] = sum_out W^T[in, out] G[px, out]: 16 steps of 8 output channels x 4 pixel columns of 8
+        float dx[4][4];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] += ev[j];
-                    if (ph + kPhStep < kPh) ldev(ph + kPhStep);
-                }
-                if (final_mode) {
-                    const unsigned char *xr = sm.xm[s] + ph * (16 * 128);
+        for (int nt = 0; nt < 4; ++nt) dx[nt][0] = dx[nt][1] = dx[nt][2] = dx[nt][3] = 0.f;
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        // the producers stored x + half a TF32 ulp (bit pattern + 0x1000, nothing truncated): undo it -> exact fp32 x
-                        const float x = __uint_as_float(*reinterpret_cast<const uint32_t *>(xr + j * 128 + xoff[j & 3]) - 0x1000u);
+        for (int ks = 0; ks < 16; ++ks) {
+            const int o = 8 * ks + t4;
+#pragma unroll
+            for (int nt = 0; nt < 4; ++nt) {
+                const int n = 8 * nt + g;
+                mma_tf32(dx[nt], wa[ks], lds32(gks + kmajor_off(n, o, kGkChunk)), lds32(gks + kmajor_off(n, o + 4, kGkChunk)));
+            }
+        }
+        // dW[out, in] += sum_px G^T[out, px] X[px, in]: 4 steps of 8 pixels x 16 input columns of 8
+#pragma unroll
+        for (int ks = 0; ks < kPx / 8; ++ks) {
+            const int q = 8 * ks + t4;
+            const int oc = 16 * warp + g;
+            const uint32_t a[4] = {lds32(gks + kmajor_off(q, oc, kGkChunk)), lds32(gks + kmajor_off(q, oc + 8, kGkChunk)),
+                                   lds32(gks + kmajor_off(q + 4, oc, kGkChunk)), lds32(gks + kmajor_off(q + 4, oc + 8, kGkChunk))};
+#pragma unroll
+            for (int nt = 0; nt < 16; ++nt) {
+                const int n = 8 * nt + g;
+                mma_tf32(dw[nt], a, lds32(xms + mnmajor_off(q, n, kGkChunk)), lds32(xms + mnmajor_off(q + 4, n, kGkChunk)));
+            }
+        }
+
+        // ---- epilogue: dx[nt] = {dX^T(ic, px), dX^T(ic, px + 1), dX^T(ic + 8, px), dX^T(ic + 8, px + 1)}, px = 8 nt + 2 t4
+        const int rows = M - m0;
+        float t1[2] = {0.f, 0.f}, t2[2] = {0.f, 0.f};
+        float *ot = p.dZprev + (size_t)m0 * ldo;
+#pragma unroll
+        for (int nt = 0; nt < 4; ++nt) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int px = 8 * nt + 2 * t4 + e;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int c = ic + 8 * h;
+                    float v = dx[nt][2 * h + e];
+                    float *op = ot + (size_t)px * ldo + c;
+                    const bool store = px < rows && c < p.kin;
+                    if (add_existing && store) v += *op;
+                    if (final_mode) {
+                        // the conversion stored x + half a TF32 ulp (bit pattern + 0x1000, nothing truncated): undo it -> exact fp32 x
+                        const float x = __uint_as_float(lds32(xms + mnmajor_off(px, c, kGkChunk)) - 0x1000u);
                         float em, ls;
                         asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(em) : "f"(-1.44269504089f * x));
                         const float sg = 1.f - em;                                  // sigmoid(z) = 1 - exp(-softplus(z))
                         asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(ls) : "f"(fmaxf(sg, 1e-30f)));
-                        const float dx = v[j] * sg;                                 // 0 for pixels >= M (G and X are zero there)
-                        v[j] = dx;
-                        t1 += dx;
-                        t2 = fmaf(dx, fmaf(ls, cl2g, fmaf(x, cinvg, -cbg)), t2);
+                        v *= sg;                                                    // 0 for pixels >= M (G and X are zero there)
+                        t1[h] += v;
+                        t2[h] = fmaf(v, fmaf(ls, cl2g[h], fmaf(x, cinvg[h], -cbg[h])), t2[h]);
                     }
-                }
-                // straight from the registers: a warp instruction writes 32 consecutive channels of one pixel = one whole 128-byte line
-                if (store_col) {
-                    float *oc = const_cast<float *>(evp) + ph * 16 * ldo;
-                    if (full) {
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) oc[j * ldo] = v[j];
-                    } else {
-                        const int rows = p.M - (m0 + ph * 16);
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) if (j < rows) oc[j * ldo] = v[j];
-                    }
+                    if (store) *op = v;
                 }
             }
-            tc_fence_before_sync();
-            warp_arrive(&sm.tmem_empty[s], lane);
-            d1 += (double)t1; d2 += (double)t2;
-            TADD(2, te_);
-            TMARK(ts_);
-            warp_arrive(&sm.empty[s], lane);               // the X tile has been read: nothing of this stage is needed any more
-            TADD(3, ts_);
-            if (++s == kBStages) { s = 0; ++n; }
         }
-#if GA_TC_TIMING
-        tloop_ = clock64() - tstart_;
-#endif
-        if (final_mode && p.s1) { atomicAdd(&p.s1[c], d1); atomicAdd(&p.s2[c], d2); }
-        // flush the weight-gradient accumulator: lane == output channel; every MMA was covered by the last mma_done wait
-        tc_fence_after_sync();
-#pragma unroll 1
-        for (int cc = (ew >> 2) * (8 / kPhStep); cc < ((ew >> 2) + 1) * (8 / kPhStep); ++cc) {      // with 8 warps each pair splits the columns
-            float v[16];
-            tmem_ld_32x16(tmem_base + ((uint32_t)(q * 32) << 16) + cc * 16, v);
 #pragma unroll
-            for (int g = 0; g < 4; ++g)          // kin and lddw are multiples of 4: 16-byte vector reductions
-                if (cc * 16 + g * 4 < p.kin) red_add_v4(p.dW + (size_t)c * p.lddw + cc * 16 + g * 4, v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
+        for (int h = 0; h < 2; ++h) { d1[h] += (double)t1[h]; d2[h] += (double)t2[h]; }
+    }
+    cp_async_wait<0>();
+    if (final_mode && p.s1) {                          // the four lanes of a channel meet by shuffles
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int o = 1; o < 4; o <<= 1) {
+                d1[h] += __shfl_xor_sync(0xffffffffu, d1[h], o);
+                d2[h] += __shfl_xor_sync(0xffffffffu, d2[h], o);
+            }
+            if (t4 == 0) { atomicAdd(&p.s1[ic + 8 * h], d1[h]); atomicAdd(&p.s2[ic + 8 * h], d2[h]); }
         }
     }
-#if GA_TC_TIMING
-    if (blockIdx.x == 0 && lane == 0) printf("TCT bwd pro %lld loopend %lld mode=%d kin=%d warp %d total %lld wait0 %lld wait1 %lld ph2 %lld ph3 %lld tiles %d\n", tpro_, tloop_, p.mode, p.kin, warp, clock64() - tstart_, tw_[0], tw_[1], tw_[2], tw_[3], (num_tiles + (int)gridDim.x - 1) / (int)gridDim.x);
-#endif
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == kBwdMmaWarp) tmem_dealloc(tmem_base, kBwdTmemCols);
+    // flush the weight-gradient accumulators: rows (output channels) 16 w + g (+ 8), columns 8 nt + 2 t4 (+ 1)
+    const int oc = 16 * warp + g;
+#pragma unroll
+    for (int nt = 0; nt < 16; ++nt) {
+        const int in = 8 * nt + 2 * t4;
+        if (in < p.kin) {                              // kin is a multiple of 4: a column pair is inside or outside as a whole
+            red_add_v2(p.dW + (size_t)oc * p.lddw + in, dw[nt][0], dw[nt][1]);
+            red_add_v2(p.dW + (size_t)(oc + 8) * p.lddw + in, dw[nt][2], dw[nt][3]);
+        }
+    }
 }
 
 }  // namespace
@@ -788,16 +473,16 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
                   const float *Yprev, int ldp, const float *pa, const float *pb, const float *pmu, const float *prstd, const float *W, int ldw,
                   float *dW, int lddw, float *dZprev, int ldo, int mode, double *s1, double *s2, int M, int kin, int x_raw, cudaStream_t st)
 {
-    GA_REQUIRE(kin % 4 == 0 && kin >= 4 && kin <= 128 && (!x_raw || mode == 1 || mode == 2), "tcgen05 backward: bad kin / mode");
-    GA_REQUIRE(ldg % 4 == 0 && ldp % 4 == 0 && ldw % 4 == 0 && ldo % 4 == 0, "tcgen05 backward: leading dimensions must be multiples of 4");
-    GA_REQUIRE(lddw % 4 == 0 && (reinterpret_cast<uintptr_t>(dW) & 15) == 0, "tcgen05 backward: dW must be 16-byte aligned with lddw a multiple of 4");
+    GA_REQUIRE(kin % 4 == 0 && kin >= 4 && kin <= 128 && (!x_raw || mode == 1 || mode == 2), "tensor-core backward: bad kin / mode");
+    GA_REQUIRE(ldg % 4 == 0 && ldp % 4 == 0 && ldw % 4 == 0 && ldo % 4 == 0, "tensor-core backward: leading dimensions must be multiples of 4");
+    GA_REQUIRE(lddw % 4 == 0 && (reinterpret_cast<uintptr_t>(dW) & 15) == 0, "tensor-core backward: dW must be 16-byte aligned with lddw a multiple of 4");
     static PerDeviceOnce attr_set;
     if (attr_set.first()) {
         GA_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcBwdSmem) + 1024));
     }
     TcBwdParams p{dZ, Y, ldg, ga, m1, m2, mu, rstd, Yprev, ldp, pa, pb, pmu, prstd, W, ldw, dW, lddw, dZprev, ldo, mode, s1, s2, M, kin, x_raw};
-    const int tiles = cdiv(M, kPx);
-    const int grid = tiles < kNumSMs ? tiles : kNumSMs;
+    const int tiles = cdiv(M, kPx), sms = num_sms();
+    const int grid = tiles < sms ? tiles : sms;
     {
         ProfScope _ps("mlp_tc_bwd", st);
         launch_k(tc_bwd_kernel, grid, kBwdThreads, sizeof(TcBwdSmem) + 1024, st, p);

@@ -1,4 +1,4 @@
-// Differentiable 3D-Gaussian tile rasterizer for sm_100a — forward (K1..K6) and backward (K7, fused K8/K9), for one frame or
+// Differentiable 3D-Gaussian tile rasterizer for sm_90a — forward (K1..K6) and backward (K7, fused K8/K9), for one frame or
 // for all frames of a training step in one set of launches.
 //
 // Replaces what the reference reaches through `GaussianRasterizer(raster_settings)(...)`

@@ -1,6 +1,11 @@
-// Blackwell (sm_100a) tensor-core plumbing written directly in PTX: mbarrier, tcgen05 alloc / mma / commit / ld, UMMA
-// shared-memory and instruction descriptors for kind::tf32.  Bit layouts follow the CUTLASS reference definitions
-// (cute/arch/mma_sm100_desc.hpp: SmemDescriptor, InstrDescriptor); nothing from CUTLASS is compiled in.
+// Hopper (sm_90a) tensor-core plumbing written directly in PTX: cp.async staging and the warp-level TF32 MMA
+// (mma.sync m16n8k8, fp32 accumulators in registers), with fragment loads out of the 128-byte-swizzled shared-memory images.
+//
+// Why mma.sync and not wgmma: TF32 wgmma reads both shared-memory operands K-major only (the transpose bits exist for 16-bit types
+// alone), while the backward layer and the convolution weight gradient consume pixel-major images as they lie.  mma.sync takes its
+// fragments from registers, so every image is read in whichever layout the producers wrote it.  The decoder layers move ~1 KiB per
+// pixel against ~33 kFLOP (HBM bound on H100: 3.35 TB/s x 33 FLOP/B is a fraction of the TF32 rate), so the instruction's peak is
+// not the limit.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -10,62 +15,6 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// ---- mbarrier --------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void fence_barrier_init()
-{
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n"      // %2: suspend-time hint -> the poll parks in hardware
-        "@p bra DONE_%=;\n"
-        "bra WAIT_%=;\n"
-        "DONE_%=:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity), "r"(0x989680u) : "memory");
-}
-// Warp-granular handshakes: ONE lane polls / arrives, the rest of the warp parks on the warp barrier.  With per-thread
-// try_wait loops the ~500 waiting threads of a CTA flood the shared-memory pipe with barrier polls (7.4 M polls per launch in
-// the ncu profile) and every full/empty handoff is hundreds of serialised shared-memory atomics.
-#ifndef GA_TC_THREAD_SYNC
-#define GA_TC_THREAD_SYNC 0
-#endif
-#if GA_TC_THREAD_SYNC
-constexpr int kArrivalsPerWarp = 32;
-__device__ __forceinline__ void warp_wait(uint64_t *bar, uint32_t parity, int) { mbar_wait(bar, parity); }
-__device__ __forceinline__ void warp_arrive(uint64_t *bar, int) { mbar_arrive(bar); }
-#else
-constexpr int kArrivalsPerWarp = 1;
-__device__ __forceinline__ void warp_wait(uint64_t *bar, uint32_t parity, int lane)
-{
-    if (lane == 0) mbar_wait(bar, parity);
-    __syncwarp();
-}
-__device__ __forceinline__ void warp_arrive(uint64_t *bar, int lane)
-{
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar);
-}
-#endif
-// Non-blocking probe of a phase (warp-uniform result): lane 0 tests, the answer is broadcast.
-__device__ __forceinline__ bool warp_test(uint64_t *bar, uint32_t parity, int lane)
-{
-    uint32_t ok = 0;
-    if (lane == 0)
-        asm volatile("{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    return __shfl_sync(0xffffffffu, ok, 0) != 0;
-}
 // 16-byte asynchronous global -> shared copy (L2 only); !valid: the 16 bytes are zero-filled and nothing is read
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid)
 {
@@ -77,152 +26,43 @@ __device__ __forceinline__ void cp_async16_full(uint32_t dst, const void *src)
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-// generic-proxy writes to shared memory -> visible to the async proxy (tensor core / TMA reads)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---- tensor memory ---------------------------------------------------------------------------------------------------
-// One full warp allocates `ncols` (power of two >= 32) columns; the base address lands in *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32, issued by ONE thread
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// Same, with the two descriptors given as (low word, shared high word): inside an unrolled issue loop only the 14-bit
-// address field of the low word changes, so each MMA costs two integer adds instead of a 64-bit descriptor rebuild
-// (the issuing thread is a serial resource: ~20 MMAs per 32-pixel tile in the backward kernel).
-__device__ __forceinline__ void mma_tf32_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc, bool accumulate)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        ".reg .b64 da, db;\n"
-        "setp.ne.b32 p, %5, 0;\n"
-        "mov.b64 da, {%1, %3};\n"
-        "mov.b64 db, {%2, %3};\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %4, p;\n"
-        "}\n" ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// low / high words of a SWIZZLE_128B descriptor (see make_smem_desc)
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo_bytes) { return ((smem_addr >> 4) & 0x3FFFu) | ((lbo_bytes >> 4) << 16); }
-constexpr uint32_t desc_hi(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (1u << 14) | (2u << 29); }
-
-// A operand in TENSOR MEMORY (rows = TMEM lanes, one 32-bit column per K element), B through a shared-memory descriptor
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint32_t b_lo, uint32_t hi, uint32_t idesc, bool accumulate)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        ".reg .b64 db;\n"
-        "setp.ne.b32 p, %5, 0;\n"
-        "mov.b64 db, {%2, %3};\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], db, %4, p;\n"
-        "}\n" ::"r"(d_tmem), "r"(a_tmem), "r"(b_lo), "r"(hi), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once every previously issued MMA of this thread has completed
-__device__ __forceinline__ void mma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 columns of fp32: thread i of the warp receives row (lane_base + i), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float (&v)[32])
-{
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, "
-        "%27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-          "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// store 32 lanes x 16 columns: thread i of the warp writes row (lane_base + i), columns [col, col+16)
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const float (&v)[16])
-{
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])),
-        "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])),
-        "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])),
-        "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15]))
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float (&v)[16])
-{
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// fp32 -> tf32 with round-to-nearest (the tensor core itself would truncate the low 13 mantissa bits)
-// cvt.rna.tf32.f32 == add half an ulp of the 10-bit mantissa, then drop 13 bits; the tensor core does the dropping
-// itself when it reads the operand, so one integer add per element is all that is needed.
+// fp32 -> tf32 with round-to-nearest: add half an ulp of the 10-bit mantissa; the tensor core drops the low 13 bits itself when it
+// reads the operand, so one integer add per element is all that is needed.
 __device__ __forceinline__ float to_tf32(float x) { return __uint_as_float(__float_as_uint(x) + 0x1000u); }
 __device__ __forceinline__ float4 to_tf32(float4 v) { return make_float4(to_tf32(v.x), to_tf32(v.y), to_tf32(v.z), to_tf32(v.w)); }
 
-// ---- descriptors -----------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle (LayoutType::SWIZZLE_128B = 2), version 1 (Blackwell).
-//   K-major  operand: rows of 128 B (32 fp32 of K), 8-row swizzle atoms 1024 B apart            -> SBO = 1024 B, LBO unused (1)
-//   MN-major operand: rows of 128 B (32 fp32 of M/N) per K index, 8 K-rows per atom; the next 32 M/N elements start
-//                     `lbo_bytes` further                                                        -> LBO = group stride, SBO = 1024 B
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
+// D[16x8] += A[16x8] * B[8x8], TF32 in, fp32 accumulate.  With g = lane / 4, t = lane % 4:
+//   a = {A(g, t), A(g+8, t), A(g, t+4), A(g+8, t+4)},  b = {B(t, g), B(t+4, g)},  d = {D(g, 2t), D(g, 2t+1), D(g+8, 2t), D(g+8, 2t+1)}
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
 {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;   // version
-    d |= (uint64_t)2 << 61;   // SWIZZLE_128B
-    return d;
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-// Instruction descriptor for kind::tf32 with fp32 accumulation (InstrDescriptor bit fields).
-constexpr uint32_t make_idesc_tf32(int M, int N, bool a_mn_major, bool b_mn_major)
+__device__ __forceinline__ uint32_t lds32(uint32_t addr)
 {
-    return (1u << 4)                          // c_format = F32
-           | (2u << 7) | (2u << 10)           // a_format = b_format = TF32
-           | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16)
-           | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
 }
 
-// Byte offset of element (row r, 16-byte unit u) inside a [rows][32 fp32] chunk stored with the 128-byte swizzle.
-// The chunk base must be 1024-byte aligned.
+// ---- image layouts -----------------------------------------------------------------------------------------------------
+// K-major image: rows of 128 B (32 fp32 of K) with the 128-byte swizzle (16-byte unit XOR row % 8); a 32-wide K chunk of `rows`
+// rows is one block, the next chunk follows `chunk_bytes` further.
 __device__ __forceinline__ uint32_t sw128_offset(int r, int u) { return (uint32_t)r * 128u + (uint32_t)((u ^ (r & 7)) << 4); }
+__device__ __forceinline__ uint32_t kmajor_off(int r, int k, uint32_t chunk_bytes)
+{
+    return (uint32_t)(k >> 5) * chunk_bytes + sw128_offset(r, (k & 31) >> 2) + (uint32_t)(k & 3) * 4u;
+}
+// Pixel-major ("MN-major") image: one 128-byte row per K index (pixel) holding 32 fp32 of M/N, the 32-byte pieces XOR row % 4;
+// the next 32 M/N elements follow `chunk_bytes` further.
+__device__ __forceinline__ uint32_t mn_unit(int r, int v) { return (uint32_t)r * 128u + (uint32_t)((((v >> 1) ^ (r & 3)) << 5) | ((v & 1) << 4)); }
+__device__ __forceinline__ uint32_t mnmajor_off(int k, int mn, uint32_t chunk_bytes)
+{
+    return (uint32_t)(mn >> 5) * chunk_bytes + (uint32_t)k * 128u + (uint32_t)(((((mn & 31) >> 3) ^ (k & 3)) << 5) + (mn & 7) * 4);
+}
 
 }  // namespace tc
 }  // namespace ga

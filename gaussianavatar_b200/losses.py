@@ -1,5 +1,5 @@
 """Image losses with the reference's names and semantics (/root/reference utils/loss_utils.py:7-8,23-53) over the fused
-sm_100a kernel, plus the combined form train.py:74-77 uses."""
+sm_90a kernel, plus the combined form train.py:74-77 uses."""
 from __future__ import annotations
 
 import torch

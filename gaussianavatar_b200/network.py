@@ -1,4 +1,4 @@
-"""`POP_no_unet`-compatible feature net over the fused sm_100a decoder (reference: /root/reference model/network.py:9-83).
+"""`POP_no_unet`-compatible feature net over the fused sm_90a decoder (reference: /root/reference model/network.py:9-83).
 
 All trainable tensors live in ONE flat fp32 buffer (`self.flat`, kernel-friendly packing described in
 include/gavatar.h) so that the optimizer step and the data-parallel gradient all-reduce are each a single operation;
@@ -64,7 +64,7 @@ class POP_no_unet(nn.Module):
             raise NotImplementedError("only c_geom=64, hsize=128, uv_feat_dim=2 (arguments/__init__.py:101-111) are built")
         self.geom_layer_type = geom_layer_type
         self.c_geom, self.hsize = c_geom, hsize
-        # MLP math: tcgen05 TF32 tensor cores (what the reference's cuDNN convs use on Ampere+) or strict FP32 CUDA cores
+        # MLP math: TF32 tensor cores (mma.sync) (what the reference's cuDNN convs use on Ampere+) or strict FP32 CUDA cores
         self.tensor_cores = os.environ.get("GA_DECODER_FP32", "0") != "1"
         self.layout = decoder_layout(c_geom, hsize)
         self.flat = nn.Parameter(torch.zeros(int(self.layout.total)))

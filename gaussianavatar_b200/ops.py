@@ -1,6 +1,6 @@
 """torch.autograd bridges over the C ABI for the non-rasterizer stages of the hot path.
 
-Each Function only moves pointers: all device work happens inside libgavatar_sm100.so on the current CUDA stream.
+Each Function only moves pointers: all device work happens inside libgavatar_sm90.so on the current CUDA stream.
 There is no CPU implementation behind these — CPU tensors raise.
 """
 from __future__ import annotations

@@ -16,7 +16,7 @@ tests/golden/unet5ds_nf8_s32.npz through oracle/avatar_oracle.py:unet5ds_forward
 
 Scope note: at 1.2 GFLOP per frame (the decoder behind it: 95 GFLOP per frame) these ten convolutions run on cuDNN — library kernels,
 in TF32 like the reference's — not on hand-written ones; what this package hand-writes of stage 2 is everything downstream: the
-per-frame decoder on tcgen05 (`POP_no_unet.forward_packed_frames`), per-frame LBS / assembly and the batched rasterizer.
+per-frame decoder on the tensor cores (`POP_no_unet.forward_packed_frames`), per-frame LBS / assembly and the batched rasterizer.
 BatchNorm here is written out (sums -> mean / variance -> normalise) so that the data-parallel variant is the same code with the
 two sums all-reduced over the ranks (`sync_group`): exact global-batch statistics, as SURVEY.md §8e asks for stage 2."""
 from __future__ import annotations

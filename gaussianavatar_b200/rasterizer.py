@@ -1,4 +1,4 @@
-"""`diff_gaussian_rasterization`-compatible Python surface over the sm_100a rasterizer.
+"""`diff_gaussian_rasterization`-compatible Python surface over the sm_90a rasterizer.
 
 Mirrors the API generation the reference binds at /root/reference gaussian_renderer/__init__.py:6,21-48:
 ``GaussianRasterizationSettings`` (12-field NamedTuple), ``GaussianRasterizer(raster_settings)(means3D=, means2D=, shs=,

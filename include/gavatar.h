@@ -1,5 +1,5 @@
 /*
- * gavatar.h — C ABI of libgavatar_sm100.so, the B200-native (sm_100a) implementation of GaussianAvatar's per-frame
+ * gavatar.h — C ABI of libgavatar_sm90.so, the H100-native (sm_90a) implementation of GaussianAvatar's per-frame
  * render hot path.  Flat extern "C" surface: plain device/host pointers, sizes, a CUDA stream handle passed as
  * void*.  No torch types.  Every function returns 0 (GA_OK) or a negative GaStatus; ga_last_error() gives the
  * message of the last failure on the calling thread.  The library never allocates persistent device memory: the
@@ -181,7 +181,7 @@ int ga_lbs_backward(int32_t N, int32_t B, int32_t num_pixels, float scale_mul, i
 typedef struct GaDecoderDesc {
     int32_t S, feat_res, batch, c_geom, hsize;
     float bn_eps, bn_momentum;
-    int32_t flags;   /* GA_DECODER_TENSOR_CORES: MLP layers on tcgen05 (TF32, the reference's cuDNN numerics); 0: strict FP32 */
+    int32_t flags;   /* GA_DECODER_TENSOR_CORES: MLP layers on the tensor cores (TF32, the reference's cuDNN numerics); 0: strict FP32 */
     int32_t frames;  /* distinct input maps = decoder row blocks: 0 / 1 = stage 1 (one map shared by the batch), B = stage 2 (one
                       * pose_featmap per frame, model/avatar_model.py:401-405): rows, dec_out and d_dec_out are then [frames*S*S, .] */
 } GaDecoderDesc;

@@ -66,6 +66,37 @@ def gen_dataset_items():
     np.savez_compressed(os.path.join(OUT, "dataset_items.npz"), **out)
 
 
+def gen_dataset_items_all():
+    """EVERY item of the reference's dataset classes on the stage-1 synthetic folder (no position maps; image values sampled): the
+    vectors tests/test_dataset_cpu.py::test_items_match_reference_classes_directly compares against."""
+    import tempfile
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from dataset_fixture import write_synthetic_dataset
+    from scene import dataset_mono as ref
+    _orig = ref.getProjectionMatrix
+    ref.getProjectionMatrix = lambda **kw: _orig(**{**kw, "K": np.asarray(kw["K"]).astype(np.float64)})
+    fields = ("original_image", "world_view_transform", "projection_matrix", "full_proj_transform", "camera_center")
+    out = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        mp = write_synthetic_dataset(tmp)
+        mp.no_mask = 1
+        sets = dict(train=ref.MonoDataset_train(mp, device="cpu"), test=ref.MonoDataset_test(mp, device="cpu"),
+                    novel_pose=ref.MonoDataset_novel_pose(mp, device="cpu"))
+        for name, dset in sets.items():
+            out[f"{name}/len"] = np.array(len(dset))
+            for i in range(len(dset)):
+                item = dset[i]
+                for k in fields + ("pose_data", "transl_data", "inp_pos_map"):
+                    if k in item:
+                        out[f"{name}/{i}/{k}"] = np.asarray(item[k], dtype=np.float64)
+                # images: a fixed seeded sample of 64 values keeps the fixture small
+                if "original_image" in item:
+                    img = np.asarray(item["original_image"], dtype=np.float32).reshape(-1)
+                    out[f"{name}/{i}/original_image"] = img[np.random.default_rng(i).choice(img.size, 64, replace=False)]
+                out[f"{name}/{i}/scalars"] = np.array([item["FovX"], item["FovY"], item["width"], item["height"], item["pose_idx"]], dtype=np.float64)
+    np.savez_compressed(os.path.join(OUT, "dataset_items_all.npz"), **out)
+
+
 def gen_smpl_A():
     body = syn.make_body(0)
     d = np.load(os.path.join(OUT, "test_pose_subset.npz"))
@@ -220,5 +251,6 @@ if __name__ == "__main__":
     gen_unet()
     gen_unet_full_size()
     gen_dataset_items()
+    gen_dataset_items_all()
     for f in sorted(os.listdir(OUT)):
         print(f, os.path.getsize(os.path.join(OUT, f)))

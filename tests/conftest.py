@@ -9,8 +9,8 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
-    config.addinivalue_line("markers", "tf32: run the decoder MLP on the tcgen05 TF32 path (default in tests: strict-FP32 path)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
+    config.addinivalue_line("markers", "tf32: run the decoder MLP on the tensor-core TF32 path (default in tests: strict-FP32 path)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -30,7 +30,7 @@ def pytest_collection_modifyitems(config, items):
 @pytest.fixture(autouse=True)
 def _decoder_math_mode(request, monkeypatch):
     """Parity tests with tight tolerances run the decoder MLP on the strict-FP32 CUDA-core path; tests marked `tf32`
-    exercise the production tcgen05 TF32 path with the (looser) tolerances SURVEY.md Appendix C assigns to it."""
+    exercise the production tensor-core TF32 path with the (looser) tolerances SURVEY.md Appendix C assigns to it."""
     if "tf32" in request.keywords:
         monkeypatch.delenv("GA_DECODER_FP32", raising=False)
     else:

@@ -90,7 +90,7 @@ LAYOUT_HARNESS = r"""
 #define __device__
 #define __forceinline__ inline
 %(functions)s
-// decoded on the device (profiles/r1_umma_mn_major_probe.md): byte offset of element (k, m) of an MN-major kind::tf32 operand
+// byte offset of element (k, m) of the pixel-major image: 32-element chunks lbo apart, 4-row atoms sbo apart, 32-byte pieces XOR k %% 4
 static uint32_t probe_byte(int k, int m, uint32_t lbo, uint32_t sbo)
 { return (uint32_t)(m / 32) * lbo + (uint32_t)(k / 4) * sbo + (uint32_t)(k %% 4) * 128u + (uint32_t)((((m %% 32) / 8) ^ (k %% 4)) * 32) + (uint32_t)(m %% 8) * 4u; }
 int main()
@@ -113,6 +113,11 @@ int main()
             seen.insert(off);
         }
     bad += seen.size() != 1024;
+    for (int r = 0; r < 32; ++r)                 // element offsets the MMA fragments are read with: the same images, word by word
+        for (int c = 0; c < 128; ++c) {
+            bad += mnmajor_off(r, c, 4096) != probe_byte(r, c, 4096, 512);
+            bad += kmajor_off(r, c, 4096) != (uint32_t)(c / 32) * 4096u + sw128_offset(r, (c %% 32) / 4) + (uint32_t)(c %% 4) * 4u;
+        }
     std::printf("%%d\n", bad);
     return 0;
 }
@@ -120,15 +125,14 @@ int main()
 
 
 def test_umma_layout_helpers_match_the_decoded_hardware_layout(tmp_path):
-    """`mn_unit` (conv_tc.cu) and `sw128_offset` (tc_common.cuh), lifted from the product sources and compiled for the host: the
-    MN-major helper must reproduce the layout decoded on the device word by word, and both must be bijections onto their tiles."""
-    conv = open(os.path.join(ROOT, "gaussianavatar_b200", "csrc", "conv_tc.cu")).read()
+    """`mn_unit`, `sw128_offset`, `kmajor_off` and `mnmajor_off` (tc_common.cuh), lifted from the product source and compiled for the
+    host: the pixel-major helpers must reproduce that layout word by word, the K-major ones the 128-byte swizzle, and the piece helpers
+    must be bijections onto their tiles."""
     tcc = open(os.path.join(ROOT, "gaussianavatar_b200", "csrc", "tc_common.cuh")).read()
-    f1 = re.search(r"__device__ __forceinline__ uint32_t mn_unit\(.*?\}\n", conv, re.S)
-    f2 = re.search(r"__device__ __forceinline__ uint32_t sw128_offset\(.*?\}\n", tcc, re.S)
-    assert f1 and f2
+    fs = [re.search(r"__device__ __forceinline__ uint32_t " + n + r"\(.*?\}\n", tcc, re.S) for n in ("sw128_offset", "kmajor_off", "mn_unit", "mnmajor_off")]
+    assert all(fs)
     cpp, exe = tmp_path / "layout.cpp", tmp_path / "layout"
-    cpp.write_text(LAYOUT_HARNESS % {"functions": f1.group(0) + "\n" + f2.group(0)})
+    cpp.write_text(LAYOUT_HARNESS % {"functions": "\n".join(f.group(0) for f in fs)})
     cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
     r = subprocess.run([cxx, "-std=c++17", "-O1", "-o", str(exe), str(cpp)], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
@@ -146,15 +150,19 @@ def _c_expr(src: str, pattern: str) -> str:
 
 
 def test_tc_bwd_piece_addresses_are_the_umma_images():
-    """mlp_tc.cu, backward layer: the cp.async destinations / in-place conversion addresses of the 16 converter warps (`k_off`, `mn_off`)
-    and the epilogue's read-back of x (`xoff`), lifted from the kernel source as written, against the two operand layouts the tensor
-    core consumes: K-major with the 128-byte swizzle (16-byte units XOR px % 8) and MN-major with the 32-byte-base swizzle decoded on the
-    device (tools/exp_umma_probe.cu; formula in the kernel's comment).  Every thread must own whole 16-byte pieces, the pieces of one
-    array must tile the 32-pixel x 128-channel image exactly once, and the epilogue thread of channel c must read element (px, c)."""
+    """mlp_tc.cu, backward layer: the cp.async destinations / in-place conversion addresses of the converter threads (`k_off`, `mn_off`),
+    lifted from the kernel source as written, and the element offsets the MMA fragments and the epilogue's read-back of x use
+    (`kmajor_off`, `mnmajor_off`, lifted from tc_common.cuh), against the two image layouts: K-major with the 128-byte swizzle (16-byte
+    units XOR px % 8) and pixel-major with 32-byte pieces XOR px % 4 (formula in the kernel's comment).  Every thread must own whole
+    16-byte pieces, the pieces of one array must tile the 32-pixel x 128-channel image exactly once, and a read of element (px, c) must
+    land where the conversion wrote it."""
     src = open(os.path.join(ROOT, "gaussianavatar_b200", "csrc", "mlp_tc.cu")).read()
     k_off = _c_expr(src, r"const uint32_t k_off = (.*?);\s")
     mn_off = _c_expr(src, r"const uint32_t mn_off = (.*?);\n")
-    xoff = _c_expr(src, r"xoff\[i\] = (.*?);\n")
+    tcc = open(os.path.join(ROOT, "gaussianavatar_b200", "csrc", "tc_common.cuh")).read()
+    kmaj = _c_expr(tcc, r"uint32_t kmajor_off\(int r, int k, uint32_t chunk_bytes\)\n\{\n\s*return (.*?);\n").replace("chunk_bytes", "kGkChunk")
+    mnmaj = _c_expr(tcc, r"uint32_t mnmajor_off\(int k, int mn, uint32_t chunk_bytes\)\n\{\n\s*return (.*?);\n").replace("chunk_bytes", "kGkChunk")
+    kmaj = kmaj.replace("sw128_offset(r, (k & 31) >> 2)", "(r * 128 + ((((k & 31) >> 2) ^ (r & 7)) << 4))")
     kPx = 32
     kGkChunk = kPx * 128
 
@@ -165,13 +173,12 @@ def test_tc_bwd_piece_addresses_are_the_umma_images():
         return (c // 32) * kGkChunk + (px // 4) * 512 + (px % 4) * 128 + ((((c % 32) // 8) ^ (px % 4)) * 32) + (c % 8) * 4
 
     seen_k, seen_mn = set(), set()
-    for warp in range(8):                       # G converters; the X converters (warps 8-15) use pw = warp & 7 -> the same mapping
+    for warp in range(8):                       # every warp converts the same pieces of G and of X
         for lane in range(32):
             c16, pxl = lane & 7, lane >> 3
-            pw = warp & 7
-            j, p0 = pw & 3, (pw >> 2) * 4 + pxl
-            ch = j * 32 + c16 * 4
-            env = dict(j=j, p0=p0, c16=c16, pxl=pxl, kGkChunk=kGkChunk)
+            jc, p0 = warp & 3, (warp >> 2) * 4 + pxl
+            ch = jc * 32 + c16 * 4
+            env = dict(jc=jc, p0=p0, c16=c16, pxl=pxl, kGkChunk=kGkChunk)
             ko, mo = eval(k_off, {}, env), eval(mn_off, {}, env)
             for e in range(kPx // 8):
                 px = p0 + 8 * e
@@ -181,15 +188,10 @@ def test_tc_bwd_piece_addresses_are_the_umma_images():
                 seen_k.add(ko + e * 1024); seen_mn.add(mo + e * 1024)
     assert seen_k == set(range(0, 4 * kGkChunk, 16)) and seen_mn == set(range(0, 4 * kGkChunk, 16))      # each image tiled exactly once
 
-    for q in range(4):                          # epilogue: thread = input channel c, reads x(px, c) from the MN-major X image
-        for lane in range(32):
-            c = q * 32 + lane
-            for i in range(4):
-                xo = eval(xoff, {}, dict(c=c, lane=lane, i=i, kGkChunk=kGkChunk))
-                for ph in range(kPx // 16):
-                    for jj in range(i, 16, 4):  # the kernel indexes xoff[j & 3]
-                        px = ph * 16 + jj
-                        assert ph * 16 * 128 + jj * 128 + xo == byte_mn(px, c), (q, lane, ph, jj)
+    for px in range(kPx):                       # fragment / epilogue reads: element (px, c) of either image
+        for c in range(128):
+            assert eval(kmaj, {}, dict(r=px, k=c, kGkChunk=kGkChunk)) == byte_k(px, c), (px, c)
+            assert eval(mnmaj, {}, dict(k=px, mn=c, kGkChunk=kGkChunk)) == byte_mn(px, c), (px, c)
 
 
 def test_tc_fwd_piece_addresses_are_the_umma_image():

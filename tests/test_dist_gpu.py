@@ -1,6 +1,6 @@
 """NCCL correctness of the data-parallel path (needs >= 2 GPUs; skipped otherwise): two ranks x 2 frames produce the same
 averaged gradients and the same updated parameters as one rank x 4 frames (SURVEY.md §8e, App. C "DP" row).  Runs the
-production configuration (TF32 decoder, frame streams).  `gpurun --gpus 2 -- python -m pytest tests/test_dist_gpu.py -m gpu`."""
+production configuration (TF32 decoder, frame streams).  Needs two GPUs: `python -m pytest tests/test_dist_gpu.py -m gpu`."""
 import os
 import tempfile
 

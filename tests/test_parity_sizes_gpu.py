@@ -1,6 +1,6 @@
 """GPU parity of the PRODUCTION path at BASELINE.json sizes (VERDICT r1 "next round" item 1).
 
-Production path = what bench.py times: decoder MLP on the tcgen05 TF32 kernels, frames of a batch rendered on the
+Production path = what bench.py times: decoder MLP on the TF32 tensor-core kernels, frames of a batch rendered on the
 two alternating streams, sub-tile culling in the compositing kernels.  Every test here is marked `tf32`, which makes
 tests/conftest.py leave GA_DECODER_FP32 unset.
 

@@ -1,4 +1,4 @@
-"""GPU parity: sm_100a rasterizer (through the C ABI) vs the CPU oracle on the same seeded inputs.
+"""GPU parity: sm_90a rasterizer (through the C ABI) vs the CPU oracle on the same seeded inputs.
 
 Bars (SURVEY.md Appendix C): radii / tiles / rect / offsets / sort keys / sorted values / ranges bit-exact; depth bits
 exact; image mean-L1 <= 1e-4 per pixel; gradients rel-L2 <= 1e-4 vs the fp32 oracle... (float atomics order noise).
@@ -271,51 +271,3 @@ def test_equal_depths_keep_upstream_tie_order(kind):
     np.testing.assert_array_equal(v["keys_sorted"].numpy().view(np.uint64), k)
     np.testing.assert_array_equal(v["vals_sorted"].numpy().view(np.uint32), o.get("vals"))
     assert np.abs(color.cpu().numpy().astype(np.float64) - o.image).mean() <= 1e-4
-
-
-def _upstream_extension():
-    """The compiled upstream extension (graphdeco-inria/diff-gaussian-rasterization), if this box happens to have it — NOT this repo's
-    drop-in of the same name (gaussianavatar_b200/dropin/, only importable when a caller puts that folder on PYTHONPATH)."""
-    import importlib
-    import importlib.util
-    spec = importlib.util.find_spec("diff_gaussian_rasterization")
-    if spec is None or "gaussianavatar_b200" in (spec.origin or ""):
-        return None
-    try:
-        mod = importlib.import_module("diff_gaussian_rasterization")
-        return mod if hasattr(mod, "_C") or importlib.util.find_spec("diff_gaussian_rasterization._C") else None
-    except Exception:
-        return None
-
-
-def test_differential_against_upstream_extension_if_present():
-    """VERDICT r1 'parity unpinned': the reference neither vendors nor pins the rasterizer, so the oracle cannot be pinned to it here.
-    If a box ever carries the upstream CUDA extension, this compares the two GPU implementations directly on one scene (image and the
-    gradients the reference consumes) at the tolerances the oracle tests use; otherwise it skips."""
-    up = _upstream_extension()
-    if up is None:
-        pytest.skip("upstream diff_gaussian_rasterization is not installed on this box (it is not in the image; no network)")
-    from gaussianavatar_b200.rasterizer import GaussianRasterizationSettings, GaussianRasterizer
-    sc = random_scene(P=3000, H=160, W=144, seed=61, scale_mean=0.02, aniso=True)
-    dev = torch.device("cuda:0")
-    cam = sc["cam"].to(dev)
-    kw = dict(image_height=cam.height, image_width=cam.width, tanfovx=math.tan(cam.FovX / 2), tanfovy=math.tan(cam.FovY / 2),
-              bg=sc["bg"].to(dev), scale_modifier=1.0, viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform, sh_degree=0,
-              campos=cam.camera_center, prefiltered=False, debug=False)
-    gw = torch.randn(3, cam.height, cam.width, generator=torch.Generator().manual_seed(5)).to(dev)
-    out = []
-    for Settings, Rasterizer in ((GaussianRasterizationSettings, GaussianRasterizer),
-                                 (up.GaussianRasterizationSettings, up.GaussianRasterizer)):
-        leaves = {k: sc[k].to(dev).clone().requires_grad_(True) for k in ("means3D", "colors", "scales", "rotations", "opacities")}
-        means2D = torch.zeros_like(leaves["means3D"], requires_grad=True)
-        res = Rasterizer(Settings(**kw))(means3D=leaves["means3D"], means2D=means2D, shs=None, colors_precomp=leaves["colors"],
-                                         opacities=leaves["opacities"], scales=leaves["scales"], rotations=leaves["rotations"], cov3D_precomp=None)
-        img, radii = res[0], res[1]
-        (img * gw).sum().backward()
-        out.append((img.detach(), radii, {k: v.grad.detach() for k, v in leaves.items()}))
-    (img_a, rad_a, g_a), (img_b, rad_b, g_b) = out
-    assert torch.equal(rad_a.int().cpu(), rad_b.int().cpu())
-    assert (img_a - img_b).abs().mean().item() <= 1e-4
-    for k in g_a:
-        a, b = g_a[k].double(), g_b[k].double()
-        assert ((a - b).norm() / (b.norm() + 1e-30)).item() < 5e-4, k

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (TF32) decoder layer against fp64 torch math, and the whole TF32 decoder against the reference fixtures."""
+"""GPU: the tensor-core (TF32) decoder layer against fp64 torch math, and the whole TF32 decoder against the reference fixtures."""
 import os
 
 import numpy as np
@@ -32,7 +32,7 @@ def tf32_trunc(t):
 @pytest.mark.parametrize("M,K,act,acc", [(128, 128, False, False), (1024, 128, True, False), (5000, 72, False, False),
                                          (128 * 300, 128, True, True), (2304, 128, True, False),
                                          (1000, 128, True, True),      # ragged last 64-pixel tile (40 rows: the second pixel half has 8) + fan-in accumulate
-                                         (40, 72, True, True), (64 * 148 * 5 + 33, 128, False, False)])      # less than one tile; > 4 stage rounds per CTA
+                                         (40, 72, True, True), (47393, 128, False, False)])      # less than one tile; > 4 stage rounds per CTA on 132 SMs
 def test_tc_linear_forward(M, K, act, acc):
     g = torch.Generator().manual_seed(M + K)
     X = torch.randn(M, K, generator=g).to(DEV)
@@ -153,7 +153,7 @@ def test_decoder_tf32_backward_vs_reference_fixture(name):
 
 @pytest.mark.parametrize("Hf", [16, 40, 128])
 def test_tc_conv5x5_all_modes(Hf):
-    """tcgen05 implicit-GEMM 5x5 conv (forward, data gradient, weight gradient) vs fp64 torch conv2d on the same TF32-rounded
+    """tensor-core implicit-GEMM 5x5 conv (forward, data gradient, weight gradient) vs fp64 torch conv2d on the same TF32-rounded
     operands: only the accumulation order differs, so the tolerance is fp32 round-off (rel 1e-5)."""
     import torch.nn.functional as F
     from gaussianavatar_b200 import _lib

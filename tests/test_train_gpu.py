@@ -86,7 +86,7 @@ def test_fused_adam_matches_torch_adam():
 def test_train_step_gradients_vs_oracle_chain(mode):
     """d loss / d (net params, geo_feature, pose, transl) of one stage-1 step: CUDA chain vs the CPU oracle chain
     (torch autograd for the net / SMPL / LBS / losses + the C oracle's rasterizer backward).  Runs on the strict-FP32 decoder
-    path (tight tolerance) and on the production tcgen05 TF32 path (the tolerance SURVEY.md App. C assigns to TF32)."""
+    path (tight tolerance) and on the production tensor-core TF32 path (the tolerance SURVEY.md App. C assigns to TF32)."""
     tol = 5e-3 if mode == "fp32" else 3e-2
     from gaussianavatar_b200.trainer import Stage1Trainer
     from gaussianavatar_b200.workload import Stage1Workload

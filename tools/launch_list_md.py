@@ -24,7 +24,7 @@ for k, v in step:
     agg[k][0] += 1; agg[k][1] += v
 tot = sum(v for _, v in agg.values())
 with open(out, "w") as f:
-    f.write("# ncu launch list of ONE stage-1 train step (config 3, B=2 frames), B200\n\n")
+    f.write("# ncu launch list of ONE stage-1 train step (config 3, B=2 frames)\n\n")
     f.write(f"Command (under gpurun): `{cmd}`\n\nTimes under ncu are cold-cache and serialised: compare SHARES with bench.py's live CUDA-event numbers "
             "(`kernel_ms_per_step`), not absolutes.\n\n")
     f.write(f"Launches in the step: {len(step)}; summed duration {tot / 1e3:.3f} ms\n\n| kernel | launches | total us | share |\n|---|---:|---:|---:|\n")

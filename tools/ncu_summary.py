@@ -1,4 +1,4 @@
-"""Summarise an ncu report (raw + source pages) into a small markdown file for profiles/.
+"""Summarise an ncu report (raw + source pages) into a small markdown file.
 usage: python tools/ncu_summary.py <report.ncu-rep> <out.md> "<title / command>" """
 import csv, subprocess, sys
 from collections import Counter

@@ -1,5 +1,5 @@
 """Rasterizer micro-benchmark on the synthetic avatar scene (SURVEY.md §8d "Raster micro-bench").  Run on the GPU box:
-    python tools/time_raster.py --config 3 --iters 50 > gpurun_out/raster_c3.json
+    python tools/time_raster.py --config 3 --iters 50 > raster_c3.json
 """
 import argparse
 import json
