@@ -1,15 +1,18 @@
-// Decoder-MLP layers on the tensor cores (mma.sync m16n8k8 TF32, fp32 accumulators in registers; tc_common.cuh says why not wgmma).
+// Decoder-MLP layers on the tensor cores (wgmma.mma_async TF32, fp32 accumulators in registers), warp-specialised.
 //
-// Forward: one persistent CTA per SM (8 warps) computes  Y[M,128] (+)= act(bn(X))[M,K] * W[128,K]^T + bias  for its share of 64-pixel
-// tiles, as the TRANSPOSED product  Y^T[out, px] = W[out, K] * act(bn(X))[px, K]^T:
-//   copies   : the raw (pre-BatchNorm) input rows travel global -> shared with 16-byte cp.async, each piece straight to its place in the
-//              128-byte-swizzled K-major tile image, up to three tiles ahead over four 32 KB stages; the thread that copied a piece
-//              converts it IN PLACE (BatchNorm + Softplus in the log2 domain, TF32 rounding) once it has landed
-//   MMA      : warp w owns output channels 16 w .. 16 w + 15 for every tile: its slice of W lives in registers as A fragments for the
-//              whole launch, the tile supplies the B fragments (K/8 x 8 MMAs per warp and tile)
-//   epilogue : straight from the accumulators: bias, the fan-in's existing Y, the layer's BatchNorm sum / sum-of-squares (per channel,
-//              reduced over the four lanes that share a channel), Y stored as 32-byte row pieces
-// One block barrier per tile separates "every piece converted" from the MMAs; it also proves the stage refilled next was read.
+// Forward: one persistent CTA per SM computes  Y[M,128] (+)= act(bn(X))[M,K] * W[128,K]^T + bias  for its share of 64-pixel tiles,
+// as the TRANSPOSED product  Y^T[out, px] = W[out, K] * act(bn(X))[px, K]^T, with three warpgroups:
+//   producer  (warpgroup 0): the raw (pre-BatchNorm) input rows travel global -> shared with 16-byte cp.async, each piece straight to
+//              its place in the 128-byte-swizzled K-major tile image, up to four tiles ahead over six 32 KB stages; the thread that
+//              copied a piece converts it IN PLACE (BatchNorm + Softplus in the log2 domain, TF32 rounding) once it has landed and
+//              hands the stage to the consumers through the stage's `full` mbarrier
+//   consumers (warpgroups 1, 2): warpgroup c owns output channels 64 c .. 64 c + 63; its slice of W lives in registers as wgmma A
+//              fragments for the whole launch (zero past K), the tile image is the B operand (16 wgmma m64n64k8 per tile, a uniform
+//              sequence the compiler does not have to fence one by one; channels past K are zero-filled); the stage goes back to
+//              the producer through its `empty` mbarrier as soon as the MMAs have retired, then the epilogue works from the
+//              accumulators: bias, the fan-in's existing Y, the layer's BatchNorm sum / sum-of-squares (per channel, reduced over the
+//              four lanes that share a channel), Y stored as 32-byte row pieces
+// setmaxnreg moves registers from the producer (a few per element in flight) to the consumers (W fragments + accumulators).
 //
 // TF32 is what the reference computes these 1x1 convolutions in on any Ampere+ GPU (cuDNN allow_tf32 default,
 // SURVEY.md §8 a-4); the strict-FP32 CUDA-core path (gemm.cuh) remains selectable and is the GPU-side reference.
@@ -21,12 +24,15 @@ namespace {
 
 using namespace tc;
 
-constexpr int kTPx = 64, kTStages = 4;
-constexpr int kTLook = 3;                            // tiles of copies in flight (a stage is refilled one tile after it was read)
+constexpr int kTcThreads = 3 * 128;                  // producer warpgroup + two consumer warpgroups
+constexpr int kProdRegs = 80, kConsRegs = 208;       // setmaxnreg split: 128 x 80 + 256 x 208 <= 384 x 168 (the launch allocation)
+static_assert(128 * kProdRegs + 256 * kConsRegs <= kTcThreads * 168, "the consumers' registers must come from the producer's");
+
+constexpr int kTPx = 64, kTStages = 6;
+constexpr int kTLook = 4;                            // tiles of copies in flight (a stage is refilled two tiles after it was read)
 constexpr int kTChunk = kTPx * 128;                  // 8 KB: [64 px rows][32 channels]
 constexpr int kTStageBytes = 4 * kTChunk;            // 32 KB: K <= 128
-constexpr int kTThreads = 8 * 32;
-static_assert(kTLook < kTStages, "lookahead must leave the stage being read alone");
+static_assert(kTLook <= kTStages - 2, "lookahead must leave the stages being converted and read alone");
 
 struct TcFwdParams {
     const float *X; int ldx; int K;
@@ -41,105 +47,129 @@ struct TcFwdParams {
 struct alignas(1024) TcFwdSmem {
     unsigned char x[kTStages][kTStageBytes];         // X tile: [4 chunks][64 px rows][128 B], K-major, 128-byte swizzle
     float sa[128], sb[128];
+    uint64_t full[kTStages], empty[kTStages];        // producer -> consumers (128 arrivals), consumers -> producer (256 arrivals)
 };
 
-__global__ void __launch_bounds__(kTThreads, 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
 tc_fwd_kernel(const TcFwdParams p)
 {
     extern __shared__ unsigned char smem_raw[];
     TcFwdSmem &sm = *reinterpret_cast<TcFwdSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = lane >> 2, t4 = lane & 3;
     const int num_tiles = (p.M + kTPx - 1) / kTPx;
     const int gstep = gridDim.x;
     const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
-    const int nk = p.K / 8;                                                  // 16 (K = 128) or 9 (K = 72)
+    const int M = p.M;
+    if (tid < kTStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
     pdl_wait();
+    for (int i = tid; i < p.K; i += kTcThreads) { sm.sa[i] = p.a ? p.a[i] : 1.f; sm.sb[i] = p.a ? p.b[i] : 0.f; }
+    __syncthreads();
+    const uint32_t x0s = smem_u32(sm.x[0]);
 
-    // W slice of this warp as A fragments: rows (output channels) oc, oc + 8; K columns 8 ks + t4, + 4
-    const int oc = 16 * warp + g;
+    if (warp < 4) {
+        // ---- producer: warp w owns channel chunk c = w and pixel rows r0 + 8 i (i = 0..7) for r0 = 4 h + lane / 8, h = 0, 1; a warp
+        // instruction covers 4 rows x 128 B
+        setmaxnreg_dec<kProdRegs>();
+        const int rl = lane >> 3, u = lane & 7;
+        const int c = warp;
+        const int k = c * 32 + u * 4;
+        const bool kin = k < p.K;
+        float4 av = make_float4(1.f, 1.f, 1.f, 1.f), bv = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (kin) { av = *reinterpret_cast<const float4 *>(&sm.sa[k]); bv = *reinterpret_cast<const float4 *>(&sm.sb[k]); }
+        const bool act = p.a != nullptr;
+        {   // log2 domain: z * log2(e) comes straight out of the FMA
+            const float L2E = 1.44269504089f;
+            av.x *= L2E; av.y *= L2E; av.z *= L2E; av.w *= L2E; bv.x *= L2E; bv.y *= L2E; bv.z *= L2E; bv.w *= L2E;
+        }
+        const int ldx = p.ldx;
+        uint32_t soffs[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r0 = 4 * h + rl;
+            const uint32_t soff = (uint32_t)c * kTChunk + sw128_offset(r0, u);   // + i * 1024
+            soffs[h] = soff;
+        }
+        const float *x0 = p.X + (size_t)rl * ldx + k;
+        auto issue = [&](int j) {
+            const int st = j % kTStages;
+            // every producer thread waits (also those without copies): none may arrive on a stage's `full` barrier a round early
+            if (j < ntl && j >= kTStages) mbar_wait(smem_u32(&sm.empty[st]), ((j / kTStages) & 1) ^ 1);   // tile j - kTStages is read
+            if (j < ntl) {
+                const int t = blockIdx.x + j * gstep;
+                const uint32_t dst = x0s + (uint32_t)st * kTStageBytes;
+                const float *src = x0 + (size_t)t * kTPx * ldx;
+                const bool whole = (t + 1) * kTPx <= M;
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const int r = 4 * h + rl + 8 * i;
+                        const bool ok = kin && (whole || t * kTPx + r < M);      // rows >= M and channels >= K are zero-filled
+                        cp_async16(dst + soffs[h] + i * 1024, ok ? src + (size_t)(4 * h + 8 * i) * ldx : p.X, ok);
+                    }
+            }
+            cp_async_commit();                             // one group per tile (empty past the end): the wait count stays uniform
+        };
+        for (int j = 0; j < kTLook; ++j) issue(j);
+        for (int j = 0; j < ntl; ++j) {
+            const int st = j % kTStages;
+            cp_async_wait<kTLook - 1>();
+            if (kin) {                                     // channels >= K stay zero: the MMAs multiply them by zero weights
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    unsigned char *xs = sm.x[st] + soffs[h];
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        float4 x = *reinterpret_cast<const float4 *>(xs + i * 1024);
+                        if (act) {
+                            x.x = softplus_log2(fmaf(x.x, av.x, bv.x)); x.y = softplus_log2(fmaf(x.y, av.y, bv.y));
+                            x.z = softplus_log2(fmaf(x.z, av.z, bv.z)); x.w = softplus_log2(fmaf(x.w, av.w, bv.w));
+                        }
+                        *reinterpret_cast<float4 *>(xs + i * 1024) = to_tf32(x);   // rows >= M hold act(bn(0)): their columns are never stored
+                    }
+                }
+            }
+            fence_proxy_async();                           // the converted pieces are read by the tensor cores (async proxy)
+            mbar_arrive(smem_u32(&sm.full[st]));
+            issue(j + kTLook);
+        }
+        cp_async_wait<0>();
+        return;
+    }
+
+    // ---- consumers
+    setmaxnreg_inc<kConsRegs>();
+    const int g = lane >> 2, t4 = lane & 3;
+    // W slice of this warp as A fragments: rows (output channels) oc, oc + 8; K columns 8 ks + t4, + 4 (zero past K)
+    const int oc = 16 * (warp - 4) + g;                                      // warpgroup c = (warp - 4) / 4: channels 64 c .. 64 c + 63
     uint32_t wa[16][4];
 #pragma unroll
     for (int ks = 0; ks < 16; ++ks) {
         const int k = 8 * ks + t4;
-        const bool ok = ks < nk;
+        const bool ok = 8 * ks < p.K;
         wa[ks][0] = __float_as_uint(ok ? to_tf32(p.W[(size_t)oc * p.ldw + k]) : 0.f);
         wa[ks][1] = __float_as_uint(ok ? to_tf32(p.W[(size_t)(oc + 8) * p.ldw + k]) : 0.f);
         wa[ks][2] = __float_as_uint(ok ? to_tf32(p.W[(size_t)oc * p.ldw + k + 4]) : 0.f);
         wa[ks][3] = __float_as_uint(ok ? to_tf32(p.W[(size_t)(oc + 8) * p.ldw + k + 4]) : 0.f);
     }
     const float bias0 = p.bias ? p.bias[oc] : 0.f, bias1 = p.bias ? p.bias[oc + 8] : 0.f;
-    for (int i = tid; i < p.K; i += kTThreads) { sm.sa[i] = p.a ? p.a[i] : 1.f; sm.sb[i] = p.a ? p.b[i] : 0.f; }
-    __syncthreads();
-
-    // ---- copies / conversion: warp w owns channel chunk c = w & 3 and pixel rows r0 + 8 i (i = 0..7); a warp instruction covers
-    // 4 rows x 128 B
-    const int rl = lane >> 3, u = lane & 7;
-    const int c = warp & 3, r0 = (warp >> 2) * 4 + rl;
-    const int k = c * 32 + u * 4;
-    const bool kin = k < p.K, chunk_used = c * 32 < p.K;
-    float4 av = make_float4(1.f, 1.f, 1.f, 1.f), bv = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (kin) { av = *reinterpret_cast<const float4 *>(&sm.sa[k]); bv = *reinterpret_cast<const float4 *>(&sm.sb[k]); }
-    const bool act = p.a != nullptr;
-    {   // log2 domain: z * log2(e) comes straight out of the FMA
-        const float L2E = 1.44269504089f;
-        av.x *= L2E; av.y *= L2E; av.z *= L2E; av.w *= L2E; bv.x *= L2E; bv.y *= L2E; bv.z *= L2E; bv.w *= L2E;
-    }
-    const int M = p.M, ldx = p.ldx;
-    const uint32_t soff = (uint32_t)c * kTChunk + sw128_offset(r0, u);      // + i * 1024
-    const uint32_t x0s = smem_u32(sm.x[0]);
-    const float *x0 = p.X + (size_t)r0 * ldx + k;
-    auto issue = [&](int j) {
-        if (j < ntl && chunk_used) {
-            const int t = blockIdx.x + j * gstep;
-            const uint32_t dst = x0s + (uint32_t)(j % kTStages) * kTStageBytes + soff;
-            const float *src = x0 + (size_t)t * kTPx * ldx;
-            const bool whole = (t + 1) * kTPx <= M;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const bool ok = kin && (whole || t * kTPx + r0 + 8 * i < M);      // rows >= M and channels >= K are zero-filled, never read
-                cp_async16(dst + i * 1024, ok ? src + (size_t)(8 * i) * ldx : p.X, ok);
-            }
-        }
-        cp_async_commit();                             // one group per tile (empty past the end): the wait count stays uniform
-    };
-    for (int j = 0; j < kTLook; ++j) issue(j);
-
     const int ldy = p.ldy;
     double dsum[2] = {0.0, 0.0}, dsq[2] = {0.0, 0.0};
     for (int j = 0; j < ntl; ++j) {
-        const int tile = blockIdx.x + j * gstep;
-        const uint32_t xs_u = x0s + (uint32_t)(j % kTStages) * kTStageBytes;
-        cp_async_wait<kTLook - 1>();
-        if (chunk_used) {
-            unsigned char *xs = sm.x[j % kTStages] + soff;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                float4 x = *reinterpret_cast<const float4 *>(xs + i * 1024);
-                if (act) {
-                    x.x = softplus_log2(fmaf(x.x, av.x, bv.x)); x.y = softplus_log2(fmaf(x.y, av.y, bv.y));
-                    x.z = softplus_log2(fmaf(x.z, av.z, bv.z)); x.w = softplus_log2(fmaf(x.w, av.w, bv.w));
-                }
-                *reinterpret_cast<float4 *>(xs + i * 1024) = to_tf32(x);       // rows >= M hold act(bn(0)): their columns are never stored
-            }
-        }
-        __syncthreads();                               // the tile is complete; every warp has finished the previous one
-        issue(j + kTLook);                             // refills the stage of tile j - 1
+        const int tile = blockIdx.x + j * gstep, st = j % kTStages;
+        const uint32_t xs_u = x0s + (uint32_t)st * kTStageBytes;
+        mbar_wait(smem_u32(&sm.full[st]), (j / kTStages) & 1);
 
         float acc[8][4];
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
+        wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < 16; ++ks) {
-            if (ks < nk) {
-                const int kk = 8 * ks + t4;
-#pragma unroll
-                for (int nt = 0; nt < 8; ++nt) {
-                    const int n = 8 * nt + g;
-                    mma_tf32(acc[nt], wa[ks], lds32(xs_u + kmajor_off(n, kk, kTChunk)), lds32(xs_u + kmajor_off(n, kk + 4, kTChunk)));
-                }
-            }
-        }
+        for (int ks = 0; ks < 16; ++ks) wgmma_tf32_n64(acc, wa[ks], wgmma_desc(kstep_addr(xs_u, ks, kTChunk)));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operand(acc);
+        mbar_arrive(smem_u32(&sm.empty[st]));
 
         // ---- epilogue: acc[nt] = {Y^T(oc, px), Y^T(oc, px + 1), Y^T(oc + 8, px), Y^T(oc + 8, px + 1)}, px = 8 nt + 2 t4
         float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
@@ -163,7 +193,6 @@ tc_fwd_kernel(const TcFwdParams p)
 #pragma unroll
         for (int h = 0; h < 2; ++h) { dsum[h] += (double)cs[h]; dsq[h] += (double)cq[h]; }
     }
-    cp_async_wait<0>();
     if (p.sum) {                                       // the four lanes of a channel meet by shuffles: 2 atomics per channel per CTA
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -194,7 +223,7 @@ int launch_tc_fwd(const float *X, int ldx, int K, const float *a, const float *b
     const int grid = tiles < sms ? tiles : sms;
     {
         ProfScope _ps("mlp_tc_fwd", st);
-        launch_k(tc_fwd_kernel, grid, kTThreads, sizeof(TcFwdSmem) + 1024, st, p);
+        launch_k(tc_fwd_kernel, grid, kTcThreads, sizeof(TcFwdSmem) + 1024, st, p);
     }
     GA_CHECK_LAUNCH("tc_fwd_kernel");
     return GA_OK;
@@ -216,25 +245,28 @@ extern "C" int ga_tc_linear_forward(int32_t M, int32_t K, const float *X, int32_
 //
 //   G  = dY_l      [px, out] = ga (dZ_l - m1 - xhat_l m2)          BatchNorm backward applied while loading (dZ_l, Y_l)
 //   X  = x_l       [px, in ] = softplus(a Y_{l-1} + b)             recomputed while loading Y_{l-1}
-//   dW_l [out,in] += G^T X      K = pixel: warp w accumulates output rows 16 w .. 16 w + 15 x all 128 input columns in registers for
-//                               the whole launch (A fragments from the K-major G image, B fragments from the pixel-major X image),
-//                               one flush (8-byte vector reductions) at the end
-//   dX^T [in, px]  = W_l^T G^T  computed TRANSPOSED: warp w owns input channels 16 w .. 16 w + 15, whose W^T slice lives in registers
-//                               as A fragments for the whole launch; a thread's BatchNorm scalars are constants
+//   dX^T [in, px]  = W_l^T G^T  computed TRANSPOSED: consumer warpgroup c owns input channels 64 c .. 64 c + 63, whose W^T slice lives
+//                               in registers as wgmma A fragments for the whole launch; B = the G image (K-major in the output channel)
+//   dW_l [out,in] += G^T X      K = pixel: consumer warpgroup c accumulates output rows 64 c .. 64 c + 63 x all 128 input columns in
+//                               registers for the whole launch (A = G^T fragments read from the G image, B = the TRANSPOSED X image
+//                               [in][px], K-major in the pixel), one flush (8-byte vector reductions) at the end
 //   dZ_{l-1} = dX * sigmoid(z_{l-1})   (sigmoid(z_{l-1}) and xhat_{l-1} recovered from x = softplus(z) in the X tile: no re-read)
-// The raw operands travel global -> shared with 16-byte cp.async (no register behind a load in flight), three 32-pixel tiles ahead
-// over four 48 KB stages, and are converted IN PLACE by the thread that copied them; one block barrier per tile.
+// Warp-specialised like the forward: the producer warpgroup copies the raw operands global -> shared with 16-byte cp.async (no
+// register behind a load in flight), two 32-pixel tiles ahead over four 48 KB stages, converts them (G in place; X, after a
+// producer-only barrier, from the landed Y_{l-1} pieces of any producer thread, written transposed over the raw Y_l) and hands each
+// stage over through mbarriers; the consumers run the data-gradient MMAs, then the weight-gradient MMAs, whose completion they only wait for after the
+// epilogue.
 // =====================================================================================================================
 namespace ga {
 namespace {
 
-constexpr int kPx = 32, kBlk = kPx / 8;
-constexpr int kBStages = 4, kLook = 3;    // tiles of raw operand copies in flight (a stage is refilled one tile after it was read)
+constexpr int kPx = 32;
+constexpr int kBStages = 4, kLook = 2;    // tiles of raw operand copies in flight (a stage is refilled two tiles after it was read)
 constexpr int kGkChunk = kPx * 128;       // 4 KB: [32 px rows][32 channels]
 constexpr int kGkTile = 4 * kGkChunk;     // 16 KB
-constexpr int kMnTile = 4 * kGkChunk;     // 16 KB: pixel-major image [4 x 32-channel chunks][32 px][128 B] (32-byte pieces XOR px % 4)
-constexpr int kBwdThreads = 8 * 32;
-static_assert(kLook < kBStages, "lookahead must leave the stage being read alone");
+constexpr int kXtTile = 128 * 128;        // 16 KB: transposed X [128 input channels][32 px], K-major in the pixel
+static_assert(kXtTile == kGkTile, "X is written over the raw Y_l");
+static_assert(kLook <= kBStages - 2, "lookahead must leave the stages being converted and read alone");
 
 struct TcBwdParams {
     const float *dZ, *Y; int ldg;                      // layer l: [M][ldg], 128 output channels from the pointer
@@ -253,37 +285,26 @@ struct TcBwdParams {
 
 struct alignas(1024) TcBwdSmem {
     unsigned char gk[kBStages][kGkTile];               // G   rows = pixel, K = output channel (K-major); dZ lands here
-    unsigned char ym[kBStages][kMnTile];               // raw Y_l, pixel-major: only read by the G conversion
-    unsigned char xm[kBStages][kMnTile];               // X   pixel-major: rows = pixel, 128 input channels
+    unsigned char yx[kBStages][kXtTile];               // raw Y_l (gk's layout) for the G conversion, then X: rows = input channel, K = pixel
+    unsigned char xm[kBStages][kXtTile];               // raw Y_{l-1}, pixel-major: rows = pixel, 32-byte pieces XOR px % 4
     float gA[128], gB[128], gC[128];                   // dY = gA dZ + gB Y + gC  (BatchNorm backward folded to two FMAs)
     float pa[128], pb[128], pbeta[128], pinvg[128];    // layer l-1: z log2e = y pa + pb ; xhat = (z - pbeta) * pinvg
+    uint64_t full[kBStages], empty[kBStages];          // producer -> consumers (128 arrivals), consumers -> producer (256 arrivals)
 };
 
-__global__ void __launch_bounds__(kBwdThreads, 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
 tc_bwd_kernel(const TcBwdParams p)
 {
     extern __shared__ unsigned char smem_raw[];
     TcBwdSmem &sm = *reinterpret_cast<TcBwdSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int g = lane >> 2, t4 = lane & 3;
     const int M = p.M;
     const int num_tiles = (M + kPx - 1) / kPx;
     const int gstep = gridDim.x;
     const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
+    if (tid < kBStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
     pdl_wait();
-
-    // W^T slice of this warp as A fragments: rows (input channels) ic, ic + 8; K columns (output channels) 8 ks + t4, + 4
-    const int ic = 16 * warp + g;
-    uint32_t wa[16][4];
-#pragma unroll
-    for (int ks = 0; ks < 16; ++ks) {
-        const int o = 8 * ks + t4;
-        wa[ks][0] = __float_as_uint(ic < p.kin ? to_tf32(p.W[(size_t)o * p.ldw + ic]) : 0.f);
-        wa[ks][1] = __float_as_uint(ic + 8 < p.kin ? to_tf32(p.W[(size_t)o * p.ldw + ic + 8]) : 0.f);
-        wa[ks][2] = __float_as_uint(ic < p.kin ? to_tf32(p.W[(size_t)(o + 4) * p.ldw + ic]) : 0.f);
-        wa[ks][3] = __float_as_uint(ic + 8 < p.kin ? to_tf32(p.W[(size_t)(o + 4) * p.ldw + ic + 8]) : 0.f);
-    }
-    for (int i = tid; i < 128; i += kBwdThreads) {
+    for (int i = tid; i < 128; i += kTcThreads) {
         if (p.ga) {   // ga (dZ - m1 - (Y - mu) rstd m2)
             const float ga = p.ga[i], k = p.rstd[i] * p.m2[i];
             sm.gA[i] = ga; sm.gB[i] = -ga * k; sm.gC[i] = ga * (k * p.mu[i] - p.m1[i]);
@@ -298,44 +319,130 @@ tc_bwd_kernel(const TcBwdParams p)
         }
     }
     __syncthreads();
+    const uint32_t gk0 = smem_u32(sm.gk[0]), yx0 = smem_u32(sm.yx[0]), xm0 = smem_u32(sm.xm[0]);
 
-    // ---- copies / conversion.  The pixel-major image (32-byte pieces XOR px % 4):
-    //     byte(px, c) = (c / 32) * kGkChunk + px * 128 + ((((c % 32) / 8) ^ (px % 4)) * 32) + (c % 8) * 4
-    // keeps a pixel's 32 channels one permuted 128-byte row, exactly like the K-major image (16-byte units XOR px % 8): a warp
-    // instruction covers 4 pixels x 128 B (full-line global requests).  Warp w owns the 32-channel chunk j = w & 3 (its BatchNorm
-    // coefficients are thread constants) and pixel rows p0 + 8 e, for G and for X.
-    const int c16 = lane & 7, pxl = lane >> 3;
-    const int jc = warp & 3, p0 = (warp >> 2) * 4 + pxl;                     // block e is pixel p0 + 8 e:  px & 7 == p0, px & 3 == pxl
-    const int ch = jc * 32 + c16 * 4;                                        // this thread's 4 channels (all tiles, all blocks)
-    const uint32_t k_off = (uint32_t)jc * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((c16 ^ p0) << 4);                       // + e * 1024
-    const uint32_t mn_off = (uint32_t)jc * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((((c16 >> 1) ^ pxl) << 5) | ((c16 & 1) << 4));
-    const float4 cA = *reinterpret_cast<const float4 *>(&sm.gA[ch]), cB = *reinterpret_cast<const float4 *>(&sm.gB[ch]),
-                 cC = *reinterpret_cast<const float4 *>(&sm.gC[ch]);
-    const float4 av = *reinterpret_cast<const float4 *>(&sm.pa[ch]), bv = *reinterpret_cast<const float4 *>(&sm.pb[ch]);
-    const bool has_y = p.ga != nullptr, raw = p.x_raw != 0, okc = ch < p.kin;
-    const int ldg = p.ldg, ldp = p.ldp;
-    const float *dz0 = p.dZ + (size_t)p0 * ldg + ch, *y0 = (has_y ? p.Y : p.dZ) + (size_t)p0 * ldg + ch;   // block e adds 8 e rows
-    const float *x0 = p.Yprev + (size_t)p0 * ldp + ch;
-    const uint32_t gk0 = smem_u32(sm.gk[0]), ym0 = smem_u32(sm.ym[0]), xm0 = smem_u32(sm.xm[0]);
-    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    auto issue = [&](int jt) {
-        if (jt < ntl) {
-            const int t = blockIdx.x + jt * gstep, st = jt % kBStages;
-            const uint32_t dk = gk0 + (uint32_t)st * kGkTile + k_off, dy = ym0 + (uint32_t)st * kMnTile + mn_off,
-                           dx = xm0 + (uint32_t)st * kMnTile + mn_off;
-            const float *pz = dz0 + (size_t)t * kPx * ldg, *py = y0 + (size_t)t * kPx * ldg, *px = x0 + (size_t)t * kPx * ldp;
+    if (warp < 4) {
+        // ---- producer.  Copies: warp w owns the 32-channel chunk jc = w (its BatchNorm coefficients are thread constants) and pixel
+        // rows p0 + 8 e for p0 = 4 h + lane / 8, h = 0, 1, of dZ, Y_l and Y_{l-1}; a warp instruction covers 4 pixels x 128 B
+        // (full-line global requests).  The pixel-major image of Y_{l-1} (32-byte pieces XOR px % 4):
+        //     byte(px, c) = (c / 32) * kGkChunk + px * 128 + ((((c % 32) / 8) ^ (px % 4)) * 32) + (c % 8) * 4
+        // keeps a pixel's 32 channels one permuted 128-byte row, like the K-major image (16-byte units XOR px % 8).
+        // X conversion: lane owns pixels 4 q .. 4 q + 3 (q = lane / 4) of channel groups cg = 4 (2 w + b) + lane % 4, b = 0, 1
+        // (16-byte pieces of 4 channels): a 4 x 4 block per b that it writes transposed as four 16-byte pieces of the X image.
+        setmaxnreg_dec<kProdRegs>();
+        const int c16 = lane & 7, pxl = lane >> 3, jc = warp;
+        const int ch = jc * 32 + c16 * 4;                                    // this thread's 4 channels of G
+        uint32_t k_offs[2], mn_offs[2];                                      // + e * 1024
 #pragma unroll
-            for (int e = 0; e < kBlk; ++e) {
-                const bool ok = t * kPx + e * 8 + p0 < M;                        // rows >= M are zero-filled
-                cp_async16(dk + e * 1024, ok ? pz + (size_t)e * 8 * ldg : p.dZ, ok);
-                if (has_y) cp_async16(dy + e * 1024, ok ? py + (size_t)e * 8 * ldg : p.dZ, ok);
-                cp_async16(dx + e * 1024, ok && okc ? px + (size_t)e * 8 * ldp : p.Yprev, ok && okc);    // channels past kin are never read
-            }
+        for (int h = 0; h < 2; ++h) {
+            const int p0 = 4 * h + pxl;                                      // p0 % 4 == pxl
+            const uint32_t k_off = (uint32_t)jc * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((c16 ^ p0) << 4);
+            const uint32_t mn_off = (uint32_t)jc * kGkChunk + (uint32_t)p0 * 128u + (uint32_t)((((c16 >> 1) ^ pxl) << 5) | ((c16 & 1) << 4));
+            k_offs[h] = k_off; mn_offs[h] = mn_off;
         }
-        cp_async_commit();                             // one group per tile (empty past the end): the wait count stays uniform
-    };
-    for (int jt = 0; jt < kLook; ++jt) issue(jt);
+        const int q = lane >> 2;
+        int cgs[2];
+#pragma unroll
+        for (int b = 0; b < 2; ++b) cgs[b] = 4 * (2 * warp + b) + (lane & 3);
+        const bool has_y = p.ga != nullptr, raw = p.x_raw != 0, okc = ch < p.kin;
+        const int ldg = p.ldg, ldp = p.ldp;
+        const float *dz0 = p.dZ + (size_t)pxl * ldg + ch, *y0 = (has_y ? p.Y : p.dZ) + (size_t)pxl * ldg + ch;
+        const float *x0 = p.Yprev + (size_t)pxl * ldp + ch;
+        const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        auto issue = [&](int jt) {
+            if (jt < ntl) {
+                const int t = blockIdx.x + jt * gstep, st = jt % kBStages;
+                if (jt >= kBStages) mbar_wait(smem_u32(&sm.empty[st]), ((jt / kBStages) & 1) ^ 1);   // tile jt - kBStages is read
+                const uint32_t dk = gk0 + (uint32_t)st * kGkTile, dy = yx0 + (uint32_t)st * kXtTile, dx = xm0 + (uint32_t)st * kXtTile;
+                const float *pz = dz0 + (size_t)t * kPx * ldg, *py = y0 + (size_t)t * kPx * ldg, *px = x0 + (size_t)t * kPx * ldp;
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < kPx / 8; ++e) {
+                        const int r = 4 * h + 8 * e;                             // + pxl
+                        const bool ok = t * kPx + r + pxl < M;                   // rows >= M are zero-filled
+                        cp_async16(dk + k_offs[h] + e * 1024, ok ? pz + (size_t)r * ldg : p.dZ, ok);
+                        if (has_y) cp_async16(dy + k_offs[h] + e * 1024, ok ? py + (size_t)r * ldg : p.dZ, ok);
+                        cp_async16(dx + mn_offs[h] + e * 1024, ok && okc ? px + (size_t)r * ldp : p.Yprev, ok && okc);   // channels past kin are never read
+                    }
+            }
+            cp_async_commit();                             // one group per tile (empty past the end): the wait count stays uniform
+        };
+        for (int jt = 0; jt < kLook; ++jt) issue(jt);
 
+        for (int jt = 0; jt < ntl; ++jt) {
+            const int st = jt % kBStages;
+            const int m0 = (blockIdx.x + jt * gstep) * kPx;
+            const bool ragged = m0 + kPx > M;
+            cp_async_wait<kLook - 1>();
+            {   // G = gA dZ + gB Y + gC -> K-major image, in place over dZ
+                const float4 cA = *reinterpret_cast<const float4 *>(&sm.gA[ch]), cB = *reinterpret_cast<const float4 *>(&sm.gB[ch]),
+                             cC = *reinterpret_cast<const float4 *>(&sm.gC[ch]);
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    unsigned char *gk = sm.gk[st] + k_offs[h], *ym = sm.yx[st] + k_offs[h];
+#pragma unroll
+                    for (int e = 0; e < kPx / 8; ++e) {
+                        const bool row_ok = !ragged || m0 + 4 * h + 8 * e + pxl < M;
+                        const float4 za = *reinterpret_cast<const float4 *>(gk + e * 1024);
+                        const float4 ya = has_y ? *reinterpret_cast<const float4 *>(ym + e * 1024) : za;
+                        float4 o;
+                        o.x = fmaf(cA.x, za.x, fmaf(cB.x, ya.x, cC.x)); o.y = fmaf(cA.y, za.y, fmaf(cB.y, ya.y, cC.y));
+                        o.z = fmaf(cA.z, za.z, fmaf(cB.z, ya.z, cC.z)); o.w = fmaf(cA.w, za.w, fmaf(cB.w, ya.w, cC.w));
+                        if (!row_ok) o = zero4;                               // rows >= M carry zeros (gC alone would not be zero)
+                        *reinterpret_cast<float4 *>(gk + e * 1024) = to_tf32(o);
+                    }
+                }
+            }
+            // every raw Y_l piece of the tile has been read (X may overwrite them), and every producer thread's Y_{l-1} copies have landed
+            warpgroup_bar(1);
+            // X = softplus(bn(Y_{l-1})) written transposed: channel c's pixels 4 q .. 4 q + 3 are the 16-byte unit q of row c of the
+            // K-major image
+#pragma unroll
+            for (int b = 0; b < 2; ++b) {
+                const int c0 = 4 * cgs[b];
+                const float4 av = *reinterpret_cast<const float4 *>(&sm.pa[c0]), bv = *reinterpret_cast<const float4 *>(&sm.pb[c0]);
+                const bool okc = c0 < p.kin;
+                float4 xv[4];
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    float4 x = *reinterpret_cast<const float4 *>(sm.xm[st] + mnmajor_off(4 * q + r, c0, kGkChunk));
+                    if (!raw) {
+                        x.x = softplus_log2(fmaf(x.x, av.x, bv.x)); x.y = softplus_log2(fmaf(x.y, av.y, bv.y));
+                        x.z = softplus_log2(fmaf(x.z, av.z, bv.z)); x.w = softplus_log2(fmaf(x.w, av.w, bv.w));
+                    }
+                    if (!okc || (ragged && m0 + 4 * q + r >= M)) x = zero4;   // softplus(bn(0)) is not 0: rows >= M must be
+                    xv[r] = to_tf32(x);
+                }
+                unsigned char *xt = sm.yx[st];
+                *reinterpret_cast<float4 *>(xt + sw128_offset(c0 + 0, q)) = make_float4(xv[0].x, xv[1].x, xv[2].x, xv[3].x);
+                *reinterpret_cast<float4 *>(xt + sw128_offset(c0 + 1, q)) = make_float4(xv[0].y, xv[1].y, xv[2].y, xv[3].y);
+                *reinterpret_cast<float4 *>(xt + sw128_offset(c0 + 2, q)) = make_float4(xv[0].z, xv[1].z, xv[2].z, xv[3].z);
+                *reinterpret_cast<float4 *>(xt + sw128_offset(c0 + 3, q)) = make_float4(xv[0].w, xv[1].w, xv[2].w, xv[3].w);
+            }
+            fence_proxy_async();                           // the converted images are read by the tensor cores (async proxy)
+            mbar_arrive(smem_u32(&sm.full[st]));
+            issue(jt + kLook);
+        }
+        cp_async_wait<0>();
+        return;
+    }
+
+    // ---- consumers
+    setmaxnreg_inc<kConsRegs>();
+    const int g = lane >> 2, t4 = lane & 3;
+    // W^T slice of this warp as A fragments: rows (input channels) ic, ic + 8; K columns (output channels) 8 ks + t4, + 4.  The same
+    // index is the output channel of this thread's weight-gradient rows.
+    const int ic = 16 * (warp - 4) + g;
+    uint32_t wa[16][4];
+#pragma unroll
+    for (int ks = 0; ks < 16; ++ks) {
+        const int o = 8 * ks + t4;
+        wa[ks][0] = __float_as_uint(ic < p.kin ? to_tf32(p.W[(size_t)o * p.ldw + ic]) : 0.f);
+        wa[ks][1] = __float_as_uint(ic + 8 < p.kin ? to_tf32(p.W[(size_t)o * p.ldw + ic + 8]) : 0.f);
+        wa[ks][2] = __float_as_uint(ic < p.kin ? to_tf32(p.W[(size_t)(o + 4) * p.ldw + ic]) : 0.f);
+        wa[ks][3] = __float_as_uint(ic + 8 < p.kin ? to_tf32(p.W[(size_t)(o + 4) * p.ldw + ic + 8]) : 0.f);
+    }
     // ---- per-thread constants of the epilogue: input channels ic + 8 h
     const bool final_mode = p.mode == 0 || p.mode == 3;
     const bool add_existing = p.mode >= 2;
@@ -355,59 +462,30 @@ tc_bwd_kernel(const TcBwdParams p)
     for (int jt = 0; jt < ntl; ++jt) {
         const int tile = blockIdx.x + jt * gstep, st = jt % kBStages;
         const int m0 = tile * kPx;
-        const bool ragged = m0 + kPx > M;
-        cp_async_wait<kLook - 1>();
-        {   // G = gA dZ + gB Y + gC -> K-major image (in place over dZ); X = softplus(bn(Yprev)) in place
-            unsigned char *gk = sm.gk[st] + k_off, *ym = sm.ym[st] + mn_off, *xm = sm.xm[st] + mn_off;
-#pragma unroll
-            for (int e = 0; e < kBlk; ++e) {
-                const bool row_ok = !ragged || m0 + e * 8 + p0 < M;
-                const float4 za = *reinterpret_cast<const float4 *>(gk + e * 1024);
-                const float4 ya = has_y ? *reinterpret_cast<const float4 *>(ym + e * 1024) : za;
-                float4 o;
-                o.x = fmaf(cA.x, za.x, fmaf(cB.x, ya.x, cC.x)); o.y = fmaf(cA.y, za.y, fmaf(cB.y, ya.y, cC.y));
-                o.z = fmaf(cA.z, za.z, fmaf(cB.z, ya.z, cC.z)); o.w = fmaf(cA.w, za.w, fmaf(cB.w, ya.w, cC.w));
-                if (!row_ok) o = zero4;                                   // rows >= M carry zeros (gC alone would not be zero)
-                *reinterpret_cast<float4 *>(gk + e * 1024) = to_tf32(o);
-                float4 x = *reinterpret_cast<const float4 *>(xm + e * 1024);
-                if (!raw) {
-                    x.x = softplus_log2(fmaf(x.x, av.x, bv.x)); x.y = softplus_log2(fmaf(x.y, av.y, bv.y));
-                    x.z = softplus_log2(fmaf(x.z, av.z, bv.z)); x.w = softplus_log2(fmaf(x.w, av.w, bv.w));
-                }
-                if (!okc || !row_ok) x = zero4;                           // softplus(bn(0)) is not 0: rows >= M must be
-                *reinterpret_cast<float4 *>(xm + e * 1024) = to_tf32(x);
-            }
-        }
-        __syncthreads();                               // the tile is complete; every warp has finished the previous one
-        issue(jt + kLook);                             // refills the stage of tile jt - 1
+        const uint32_t gks = gk0 + (uint32_t)st * kGkTile, xts = yx0 + (uint32_t)st * kXtTile;
+        mbar_wait(smem_u32(&sm.full[st]), (jt / kBStages) & 1);
 
-        const uint32_t gks = gk0 + (uint32_t)st * kGkTile, xms = xm0 + (uint32_t)st * kMnTile;
-        // dX^T[in, px] = sum_out W^T[in, out] G[px, out]: 16 steps of 8 output channels x 4 pixel columns of 8
+        // dX^T[in, px] = sum_out W^T[in, out] G[px, out]: 16 k-steps of 8 output channels, N = 32 pixels
         float dx[4][4];
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) dx[nt][0] = dx[nt][1] = dx[nt][2] = dx[nt][3] = 0.f;
-#pragma unroll
-        for (int ks = 0; ks < 16; ++ks) {
-            const int o = 8 * ks + t4;
-#pragma unroll
-            for (int nt = 0; nt < 4; ++nt) {
-                const int n = 8 * nt + g;
-                mma_tf32(dx[nt], wa[ks], lds32(gks + kmajor_off(n, o, kGkChunk)), lds32(gks + kmajor_off(n, o + 4, kGkChunk)));
-            }
-        }
-        // dW[out, in] += sum_px G^T[out, px] X[px, in]: 4 steps of 8 pixels x 16 input columns of 8
+        // dW[out, in] += sum_px G^T[out, px] X[px, in]: 4 k-steps of 8 pixels, N = 128 input channels; A = G^T rows ic, ic + 8
+        uint32_t a[4][4];
 #pragma unroll
         for (int ks = 0; ks < kPx / 8; ++ks) {
             const int q = 8 * ks + t4;
-            const int oc = 16 * warp + g;
-            const uint32_t a[4] = {lds32(gks + kmajor_off(q, oc, kGkChunk)), lds32(gks + kmajor_off(q, oc + 8, kGkChunk)),
-                                   lds32(gks + kmajor_off(q + 4, oc, kGkChunk)), lds32(gks + kmajor_off(q + 4, oc + 8, kGkChunk))};
-#pragma unroll
-            for (int nt = 0; nt < 16; ++nt) {
-                const int n = 8 * nt + g;
-                mma_tf32(dw[nt], a, lds32(xms + mnmajor_off(q, n, kGkChunk)), lds32(xms + mnmajor_off(q + 4, n, kGkChunk)));
-            }
+            a[ks][0] = lds32(gks + kmajor_off(q, ic, kGkChunk)); a[ks][1] = lds32(gks + kmajor_off(q, ic + 8, kGkChunk));
+            a[ks][2] = lds32(gks + kmajor_off(q + 4, ic, kGkChunk)); a[ks][3] = lds32(gks + kmajor_off(q + 4, ic + 8, kGkChunk));
         }
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 16; ++ks) wgmma_tf32_n32(dx, wa[ks], wgmma_desc(kstep_addr(gks, ks, kGkChunk)));
+        wgmma_commit();
+#pragma unroll
+        for (int ks = 0; ks < kPx / 8; ++ks) wgmma_tf32_n128(dw, a[ks], wgmma_desc(kstep_addr(xts, ks, 0)));
+        wgmma_commit();
+        wgmma_wait<1>();                               // the data gradient; the weight-gradient MMAs run on under the epilogue
+        wgmma_fence_operand(dx);
 
         // ---- epilogue: dx[nt] = {dX^T(ic, px), dX^T(ic, px + 1), dX^T(ic + 8, px), dX^T(ic + 8, px + 1)}, px = 8 nt + 2 t4
         const int rows = M - m0;
@@ -427,7 +505,7 @@ tc_bwd_kernel(const TcBwdParams p)
                     if (add_existing && store) v += *op;
                     if (final_mode) {
                         // the conversion stored x + half a TF32 ulp (bit pattern + 0x1000, nothing truncated): undo it -> exact fp32 x
-                        const float x = __uint_as_float(lds32(xms + mnmajor_off(px, c, kGkChunk)) - 0x1000u);
+                        const float x = __uint_as_float(lds32(xts + kmajor_off(c, px, 0)) - 0x1000u);
                         float em, ls;
                         asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(em) : "f"(-1.44269504089f * x));
                         const float sg = 1.f - em;                                  // sigmoid(z) = 1 - exp(-softplus(z))
@@ -442,8 +520,11 @@ tc_bwd_kernel(const TcBwdParams p)
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) { d1[h] += (double)t1[h]; d2[h] += (double)t2[h]; }
+        wgmma_wait<0>();
+        wgmma_fence_operand(a);
+        wgmma_fence_operand(dw);
+        mbar_arrive(smem_u32(&sm.empty[st]));
     }
-    cp_async_wait<0>();
     if (final_mode && p.s1) {                          // the four lanes of a channel meet by shuffles
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -455,14 +536,13 @@ tc_bwd_kernel(const TcBwdParams p)
             if (t4 == 0) { atomicAdd(&p.s1[ic + 8 * h], d1[h]); atomicAdd(&p.s2[ic + 8 * h], d2[h]); }
         }
     }
-    // flush the weight-gradient accumulators: rows (output channels) 16 w + g (+ 8), columns 8 nt + 2 t4 (+ 1)
-    const int oc = 16 * warp + g;
+    // flush the weight-gradient accumulators: rows (output channels) ic (+ 8), columns 8 nt + 2 t4 (+ 1)
 #pragma unroll
     for (int nt = 0; nt < 16; ++nt) {
         const int in = 8 * nt + 2 * t4;
         if (in < p.kin) {                              // kin is a multiple of 4: a column pair is inside or outside as a whole
-            red_add_v2(p.dW + (size_t)oc * p.lddw + in, dw[nt][0], dw[nt][1]);
-            red_add_v2(p.dW + (size_t)(oc + 8) * p.lddw + in, dw[nt][2], dw[nt][3]);
+            red_add_v2(p.dW + (size_t)ic * p.lddw + in, dw[nt][0], dw[nt][1]);
+            red_add_v2(p.dW + (size_t)(ic + 8) * p.lddw + in, dw[nt][2], dw[nt][3]);
         }
     }
 }
@@ -485,7 +565,7 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
     const int grid = tiles < sms ? tiles : sms;
     {
         ProfScope _ps("mlp_tc_bwd", st);
-        launch_k(tc_bwd_kernel, grid, kBwdThreads, sizeof(TcBwdSmem) + 1024, st, p);
+        launch_k(tc_bwd_kernel, grid, kTcThreads, sizeof(TcBwdSmem) + 1024, st, p);
     }
     GA_CHECK_LAUNCH("tc_bwd_kernel");
     return GA_OK;

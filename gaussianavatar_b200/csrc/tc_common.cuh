@@ -1,11 +1,11 @@
-// Hopper (sm_90a) tensor-core plumbing written directly in PTX: cp.async staging and the warp-level TF32 MMA
-// (mma.sync m16n8k8, fp32 accumulators in registers), with fragment loads out of the 128-byte-swizzled shared-memory images.
-//
-// Why mma.sync and not wgmma: TF32 wgmma reads both shared-memory operands K-major only (the transpose bits exist for 16-bit types
-// alone), while the backward layer and the convolution weight gradient consume pixel-major images as they lie.  mma.sync takes its
-// fragments from registers, so every image is read in whichever layout the producers wrote it.  The decoder layers move ~1 KiB per
-// pixel against ~33 kFLOP (HBM bound on H100: 3.35 TB/s x 33 FLOP/B is a fraction of the TF32 rate), so the instruction's peak is
-// not the limit.
+// Hopper (sm_90a) tensor-core plumbing written directly in PTX: cp.async staging, the 128-byte-swizzled shared-memory images and
+// their address helpers, and two ways of multiplying them:
+//   * wgmma.mma_async (TF32 in, fp32 accumulate, one warpgroup per m64 slab), used by the decoder-MLP layers (mlp_tc.cu): A in
+//     registers, B read by the tensor cores through a shared-memory matrix descriptor.  TF32 wgmma reads shared-memory operands
+//     K-major only, so every image a descriptor points at is K-major (the backward layer writes its X tile transposed for that);
+//     the mbarrier / setmaxnreg wrappers serve the warp-specialised pipeline around it.
+//   * mma.sync m16n8k8 with fragments from ld.shared, kept only by the convolutions (conv_tc.cu): their weight gradient reads the
+//     pixel-major images as they lie, which TF32 wgmma cannot.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -63,6 +63,117 @@ __device__ __forceinline__ uint32_t mnmajor_off(int k, int mn, uint32_t chunk_by
 {
     return (uint32_t)(mn >> 5) * chunk_bytes + (uint32_t)k * 128u + (uint32_t)(((((mn & 31) >> 3) ^ (k & 3)) << 5) + (mn & 7) * 4);
 }
+
+// ---- wgmma (warpgroup MMA) ---------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor of a K-major operand in the 128-byte-swizzled layout above (rows of 128 B = 32 TF32 along K,
+// 8-row atoms of 1024 B): start address >> 4 (bits 0-13), leading byte offset 1 (unused by swizzled K-major layouts: one k-step
+// never leaves the 128-byte row), stride byte offset 1024 >> 4 (bits 32-45: the next 8 rows of M/N), base offset 0, swizzle mode
+// 1 = 128 B (bits 62-63).  The hardware applies the swizzle to address bits 4-6 from bits 7-9, so images start on 1024-byte
+// boundaries and a k-step inside the atom simply advances the start address (kstep_addr).
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr)
+{
+    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024u >> 4) << 32) | ((uint64_t)1 << 62);
+}
+// start address of k-step ks (8 TF32 = 32 bytes of K) of a K-major image whose 32-wide K chunks lie chunk_bytes apart
+__device__ __forceinline__ uint32_t kstep_addr(uint32_t base, int ks, uint32_t chunk_bytes)
+{
+    return base + (uint32_t)(ks >> 2) * chunk_bytes + (uint32_t)(ks & 3) * 32u;
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving a register read by / written by an in-flight wgmma across the wait that retires it
+template <int R, int C> __device__ __forceinline__ void wgmma_fence_operand(float (&d)[R][C])
+{
+#pragma unroll
+    for (int i = 0; i < R; ++i)
+#pragma unroll
+        for (int j = 0; j < C; ++j) asm volatile("" : "+f"(d[i][j])::"memory");
+}
+template <int R, int C> __device__ __forceinline__ void wgmma_fence_operand(uint32_t (&d)[R][C])
+{
+#pragma unroll
+    for (int i = 0; i < R; ++i)
+#pragma unroll
+        for (int j = 0; j < C; ++j) asm volatile("" : "+r"(d[i][j])::"memory");
+}
+
+// D[64 x N] += A[64 x 8] * B[8 x N] for one warpgroup, TF32 in, fp32 accumulate.  A comes from registers: warp w % 4 of the group
+// holds rows 16 (w % 4) .. + 15 as the m16n8k8 A fragment (mma_tf32 above).  B is read through a descriptor (wgmma_desc).  d[nt]
+// is the m16n8k8 accumulator fragment of columns 8 nt .. 8 nt + 7 of the warp's 16 rows.
+__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[4][4], const uint32_t (&a)[4], uint64_t b)
+{
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n}\n"
+                 : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]),
+                   "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]),
+                   "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]),
+                   "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[8][4], const uint32_t (&a)[4], uint64_t b)
+{
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n}\n"
+                 : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]),
+                   "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]),
+                   "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]),
+                   "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]),
+                   "+f"(d[4][0]), "+f"(d[4][1]), "+f"(d[4][2]), "+f"(d[4][3]),
+                   "+f"(d[5][0]), "+f"(d[5][1]), "+f"(d[5][2]), "+f"(d[5][3]),
+                   "+f"(d[6][0]), "+f"(d[6][1]), "+f"(d[6][2]), "+f"(d[6][3]),
+                   "+f"(d[7][0]), "+f"(d[7][1]), "+f"(d[7][2]), "+f"(d[7][3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1));
+}
+__device__ __forceinline__ void wgmma_tf32_n128(float (&d)[16][4], const uint32_t (&a)[4], uint64_t b)
+{
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n}\n"
+                 : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]),
+                   "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]),
+                   "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]),
+                   "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]),
+                   "+f"(d[4][0]), "+f"(d[4][1]), "+f"(d[4][2]), "+f"(d[4][3]),
+                   "+f"(d[5][0]), "+f"(d[5][1]), "+f"(d[5][2]), "+f"(d[5][3]),
+                   "+f"(d[6][0]), "+f"(d[6][1]), "+f"(d[6][2]), "+f"(d[6][3]),
+                   "+f"(d[7][0]), "+f"(d[7][1]), "+f"(d[7][2]), "+f"(d[7][3]),
+                   "+f"(d[8][0]), "+f"(d[8][1]), "+f"(d[8][2]), "+f"(d[8][3]),
+                   "+f"(d[9][0]), "+f"(d[9][1]), "+f"(d[9][2]), "+f"(d[9][3]),
+                   "+f"(d[10][0]), "+f"(d[10][1]), "+f"(d[10][2]), "+f"(d[10][3]),
+                   "+f"(d[11][0]), "+f"(d[11][1]), "+f"(d[11][2]), "+f"(d[11][3]),
+                   "+f"(d[12][0]), "+f"(d[12][1]), "+f"(d[12][2]), "+f"(d[12][3]),
+                   "+f"(d[13][0]), "+f"(d[13][1]), "+f"(d[13][2]), "+f"(d[13][3]),
+                   "+f"(d[14][0]), "+f"(d[14][1]), "+f"(d[14][2]), "+f"(d[14][3]),
+                   "+f"(d[15][0]), "+f"(d[15][1]), "+f"(d[15][2]), "+f"(d[15][3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1));
+}
+
+// ---- mbarrier / warpgroup register split -------------------------------------------------------------------------------
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
+{
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// waits for the completion of the barrier phase with this parity (phase k of a barrier has parity k & 1)
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
+{
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "WAIT_%=:\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+        "@p bra DONE_%=;\n"
+        "bra WAIT_%=;\n"
+        "DONE_%=:\n"
+        "}\n" ::"r"(bar), "r"(parity) : "memory");
+}
+// generic-proxy shared-memory writes (st.shared) made visible to the async proxy (wgmma operand reads)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// barrier of the 128 threads of one warpgroup (id 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 }  // namespace tc
 }  // namespace ga
