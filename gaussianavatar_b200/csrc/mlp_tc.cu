@@ -11,11 +11,15 @@
 //              sequence the compiler does not have to fence one by one; channels past K are zero-filled); the stage goes back to
 //              the producer through its `empty` mbarrier as soon as the MMAs have retired, then the epilogue works from the
 //              accumulators: bias, the fan-in's existing Y, the layer's BatchNorm sum / sum-of-squares (per channel, reduced over the
-//              four lanes that share a channel), Y stored as 32-byte row pieces
+//              four lanes that share a channel); the values go to the warpgroup's own 16 KB staging half (its two 32-channel chunks,
+//              laid out like the X image, which is the TMA SWIZZLE_128B box) and one thread stores the half with two TMA tensor
+//              stores, which drain while the warpgroup runs the next tile's MMAs (the half is rewritten once the stores have read it)
 // setmaxnreg moves registers from the producer (a few per element in flight) to the consumers (W fragments + accumulators).
 //
 // TF32 is what the reference computes these 1x1 convolutions in on any Ampere+ GPU (cuDNN allow_tf32 default,
 // SURVEY.md §8 a-4); the strict-FP32 CUDA-core path (gemm.cuh) remains selectable and is the GPU-side reference.
+#include <cudaTypedefs.h>
+
 #include "gemm.cuh"
 #include "tc_common.cuh"
 
@@ -23,6 +27,32 @@ namespace ga {
 namespace {
 
 using namespace tc;
+
+constexpr size_t kMaxSmemPerBlock = 232448;          // sm_90 opt-in limit of dynamic shared memory per block (227 KB)
+
+// Tensor map of the fp32 matrix [rows][cols] (leading dimension ld floats) in 128-byte-swizzled boxes of 32 columns x box_rows rows,
+// the K-major image layout of tc_common.cuh.  cuTensorMapEncodeTiled is a driver function; it is reached through the runtime's
+// entry-point query so that the library links the runtime only.
+int make_tmap(CUtensorMap *m, const float *base, int cols, int rows, int ld, int box_rows)
+{
+    static PFN_cuTensorMapEncodeTiled_v12000 encode = [] {
+        void *fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            fn = nullptr;
+        return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+    }();
+    GA_REQUIRE(encode, "cuTensorMapEncodeTiled is not available from the driver");
+    GA_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "tensor-core layer: the output must be 16-byte aligned");
+    const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows}, strides[1] = {(cuuint64_t)ld * sizeof(float)};
+    const cuuint32_t box[2] = {32, (cuuint32_t)box_rows}, estr[2] = {1, 1};
+    const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    GA_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d): cols %d rows %d ld %d", (int)r, cols, rows, ld);
+    return GA_OK;
+}
 
 constexpr int kTcThreads = 3 * 128;                  // producer warpgroup + two consumer warpgroups
 constexpr int kProdRegs = 80, kConsRegs = 208;       // setmaxnreg split: 128 x 80 + 256 x 208 <= 384 x 168 (the launch allocation)
@@ -35,23 +65,27 @@ constexpr int kTStageBytes = 4 * kTChunk;            // 32 KB: K <= 128
 static_assert(kTLook <= kTStages - 2, "lookahead must leave the stages being converted and read alone");
 
 struct TcFwdParams {
+    CUtensorMap ymap;              // Y [M][128] (leading dimension ldy) in boxes of 32 channels x 64 pixels
     const float *X; int ldx; int K;
     const float *a, *b;            // folded BatchNorm of the producer layer (nullptr: raw input, no activation)
     const float *W; int ldw;       // [128][K] row-major
     const float *bias;             // nullable
-    float *Y; int ldy; int accumulate;
+    int accumulate;
     double *sum, *sumsq;           // nullable
     int M;
 };
 
 struct alignas(1024) TcFwdSmem {
     unsigned char x[kTStages][kTStageBytes];         // X tile: [4 chunks][64 px rows][128 B], K-major, 128-byte swizzle
+    unsigned char ys[2][2 * kTChunk];                // Y staging of consumer warpgroup c: its 2 chunks of 32 channels, the X tile's layout
     float sa[128], sb[128];
     uint64_t full[kTStages], empty[kTStages];        // producer -> consumers (128 arrivals), consumers -> producer (256 arrivals)
+    uint64_t yload[2];                               // accumulate: the existing Y of the tile has landed in ys[c] (TMA load)
 };
+static_assert(sizeof(TcFwdSmem) + 1024 <= kMaxSmemPerBlock, "forward shared memory");
 
 __global__ void __launch_bounds__(kTcThreads, 1)
-tc_fwd_kernel(const TcFwdParams p)
+tc_fwd_kernel(const __grid_constant__ TcFwdParams p)
 {
     extern __shared__ unsigned char smem_raw[];
     TcFwdSmem &sm = *reinterpret_cast<TcFwdSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
@@ -61,6 +95,7 @@ tc_fwd_kernel(const TcFwdParams p)
     const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
     const int M = p.M;
     if (tid < kTStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
+    if (tid < 2) { mbar_init(smem_u32(&sm.yload[tid]), 1); fence_proxy_async(); }   // completed by TMA loads (async proxy)
     pdl_wait();
     for (int i = tid; i < p.K; i += kTcThreads) { sm.sa[i] = p.a ? p.a[i] : 1.f; sm.sb[i] = p.a ? p.b[i] : 0.f; }
     __syncthreads();
@@ -153,11 +188,23 @@ tc_fwd_kernel(const TcFwdParams p)
         wa[ks][3] = __float_as_uint(ok ? to_tf32(p.W[(size_t)(oc + 8) * p.ldw + k + 4]) : 0.f);
     }
     const float bias0 = p.bias ? p.bias[oc] : 0.f, bias1 = p.bias ? p.bias[oc + 8] : 0.f;
-    const int ldy = p.ldy;
+    // staging: this warpgroup's channels 64 c .. 64 c + 63 are columns ocl = oc - 64 c of its half; thread 0 of the warpgroup moves it
+    const int wg = (warp - 4) >> 2, ocl = oc - 64 * wg;
+    const bool leader = (tid & 127) == 0;
+    unsigned char *ys = sm.ys[wg];
+    const uint32_t ys_u = smem_u32(ys), yload = smem_u32(&sm.yload[wg]);
     double dsum[2] = {0.0, 0.0}, dsq[2] = {0.0, 0.0};
     for (int j = 0; j < ntl; ++j) {
         const int tile = blockIdx.x + j * gstep, st = j % kTStages;
         const uint32_t xs_u = x0s + (uint32_t)st * kTStageBytes;
+        if (leader) {
+            bulk_wait_read<0>();                       // the stores of tile j - 1 have read the staging half
+            if (p.accumulate) {                        // the existing Y lands in the half while the MMAs run
+                mbar_arrive_expect_tx(yload, 2 * kTChunk);
+#pragma unroll
+                for (int c = 0; c < 2; ++c) tma_load_2d(ys_u + c * kTChunk, &p.ymap, yload, 64 * wg + 32 * c, tile * kTPx);
+            }
+        }
         mbar_wait(smem_u32(&sm.full[st]), (j / kTStages) & 1);
 
         float acc[8][4];
@@ -167,24 +214,26 @@ tc_fwd_kernel(const TcFwdParams p)
 #pragma unroll
         for (int ks = 0; ks < 16; ++ks) wgmma_tf32_n64(acc, wa[ks], wgmma_desc(kstep_addr(xs_u, ks, kTChunk)));
         wgmma_commit();
+        warpgroup_bar(2 + wg);                         // the staging half is free (under the MMAs)
         wgmma_wait<0>();
         wgmma_fence_operand(acc);
         mbar_arrive(smem_u32(&sm.empty[st]));
+        if (p.accumulate) mbar_wait(yload, j & 1);
 
         // ---- epilogue: acc[nt] = {Y^T(oc, px), Y^T(oc, px + 1), Y^T(oc + 8, px), Y^T(oc + 8, px + 1)}, px = 8 nt + 2 t4
         float cs[2] = {0.f, 0.f}, cq[2] = {0.f, 0.f};
-        const int rows = M - tile * kTPx;              // valid pixels of this tile
-        float *yt = p.Y + (size_t)tile * kTPx * ldy;
+        const int rows = M - tile * kTPx;              // valid pixels of this tile; the stores clip the rest
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 const int px = 8 * nt + 2 * t4 + e;
+                float *y0 = reinterpret_cast<float *>(ys + kmajor_off(px, ocl, kTChunk));
+                float *y1 = reinterpret_cast<float *>(ys + kmajor_off(px, ocl + 8, kTChunk));
+                float v0 = acc[nt][e] + bias0, v1 = acc[nt][2 + e] + bias1;
+                if (p.accumulate) { v0 += *y0; v1 += *y1; }
+                *y0 = v0; *y1 = v1;
                 if (px < rows) {
-                    float *yp = yt + (size_t)px * ldy + oc;
-                    float v0 = acc[nt][e] + bias0, v1 = acc[nt][2 + e] + bias1;
-                    if (p.accumulate) { v0 += yp[0]; v1 += yp[8]; }
-                    yp[0] = v0; yp[8] = v1;
                     cs[0] += v0; cq[0] = fmaf(v0, v0, cq[0]);
                     cs[1] += v1; cq[1] = fmaf(v1, v1, cq[1]);
                 }
@@ -192,7 +241,15 @@ tc_fwd_kernel(const TcFwdParams p)
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) { dsum[h] += (double)cs[h]; dsq[h] += (double)cq[h]; }
+        fence_proxy_async();                           // the staged values are read by the TMA stores (async proxy)
+        warpgroup_bar(2 + wg);
+        if (leader) {
+#pragma unroll
+            for (int c = 0; c < 2; ++c) tma_store_2d(&p.ymap, ys_u + c * kTChunk, 64 * wg + 32 * c, tile * kTPx);
+            bulk_commit();
+        }
     }
+    if (leader) bulk_wait<0>();                        // nothing in flight when the CTA exits
     if (p.sum) {                                       // the four lanes of a channel meet by shuffles: 2 atomics per channel per CTA
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -214,7 +271,8 @@ int launch_tc_fwd(const float *X, int ldx, int K, const float *a, const float *b
 {
     GA_REQUIRE(K % 8 == 0 && K >= 8 && K <= 128, "tensor-core layer: K=%d must be a multiple of 8 in [8,128]", K);
     GA_REQUIRE(ldx % 4 == 0 && ldw % 4 == 0 && ldy % 4 == 0, "tensor-core layer: leading dimensions must be multiples of 4");
-    TcFwdParams p{X, ldx, K, a, b, W, ldw, bias, Y, ldy, accumulate, sum, sumsq, M};
+    TcFwdParams p{{}, X, ldx, K, a, b, W, ldw, bias, accumulate, sum, sumsq, M};
+    if (int rc = make_tmap(&p.ymap, Y, 128, M, ldy, kTPx)) return rc;
     static PerDeviceOnce attr_t_set;
     if (attr_t_set.first()) {
         GA_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcFwdSmem) + 1024));
@@ -255,7 +313,9 @@ extern "C" int ga_tc_linear_forward(int32_t M, int32_t K, const float *X, int32_
 // register behind a load in flight), two 32-pixel tiles ahead over four 48 KB stages, converts them (G in place; X, after a
 // producer-only barrier, from the landed Y_{l-1} pieces of any producer thread, written transposed over the raw Y_l) and hands each
 // stage over through mbarriers; the consumers run the data-gradient MMAs, then the weight-gradient MMAs, whose completion they only wait for after the
-// epilogue.
+// epilogue.  The epilogue stages dZ_{l-1} (or the raw dX) in the warpgroup's own 8 KB half of a staging tile laid out like the G image
+// (the TMA SWIZZLE_128B box), and one thread moves it with TMA tensor stores, or tensor reduce-adds for the accumulating mode; a
+// mode that finishes on top of the existing values TMA-loads them into the half under the MMAs.
 // =====================================================================================================================
 namespace ga {
 namespace {
@@ -269,13 +329,13 @@ static_assert(kXtTile == kGkTile, "X is written over the raw Y_l");
 static_assert(kLook <= kBStages - 2, "lookahead must leave the stages being converted and read alone");
 
 struct TcBwdParams {
+    CUtensorMap omap;                                  // dZprev [M][kin] (leading dimension ldo) in boxes of 32 channels x 32 pixels
     const float *dZ, *Y; int ldg;                      // layer l: [M][ldg], 128 output channels from the pointer
     const float *ga, *m1, *m2, *mu, *rstd;             // BatchNorm backward of layer l (ga == nullptr: G = dZ)
     const float *Yprev; int ldp;                       // layer l-1 pre-BN output, 128 channels
     const float *pa, *pb, *pmu, *prstd;                // BatchNorm (folded) of layer l-1
     const float *W; int ldw;                           // [128 out][128 in]
     float *dW; int lddw;                               // += (atomics)
-    float *dZprev; int ldo;
     int mode;                                          // 0 final, 1 store raw dX, 2 accumulate raw dX, 3 final on (existing + dX)
     double *s1, *s2;
     int M;
@@ -287,13 +347,16 @@ struct alignas(1024) TcBwdSmem {
     unsigned char gk[kBStages][kGkTile];               // G   rows = pixel, K = output channel (K-major); dZ lands here
     unsigned char yx[kBStages][kXtTile];               // raw Y_l (gk's layout) for the G conversion, then X: rows = input channel, K = pixel
     unsigned char xm[kBStages][kXtTile];               // raw Y_{l-1}, pixel-major: rows = pixel, 32-byte pieces XOR px % 4
+    unsigned char os[2][2 * kGkChunk];                 // dZ_{l-1} staging of consumer warpgroup c: its 2 chunks of 32 channels, gk's layout
     float gA[128], gB[128], gC[128];                   // dY = gA dZ + gB Y + gC  (BatchNorm backward folded to two FMAs)
     float pa[128], pb[128], pbeta[128], pinvg[128];    // layer l-1: z log2e = y pa + pb ; xhat = (z - pbeta) * pinvg
     uint64_t full[kBStages], empty[kBStages];          // producer -> consumers (128 arrivals), consumers -> producer (256 arrivals)
+    uint64_t oload[2];                                 // mode 3: the existing values of the tile have landed in os[c] (TMA load)
 };
+static_assert(sizeof(TcBwdSmem) + 1024 <= kMaxSmemPerBlock, "backward shared memory");
 
 __global__ void __launch_bounds__(kTcThreads, 1)
-tc_bwd_kernel(const TcBwdParams p)
+tc_bwd_kernel(const __grid_constant__ TcBwdParams p)
 {
     extern __shared__ unsigned char smem_raw[];
     TcBwdSmem &sm = *reinterpret_cast<TcBwdSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
@@ -303,6 +366,7 @@ tc_bwd_kernel(const TcBwdParams p)
     const int gstep = gridDim.x;
     const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
     if (tid < kBStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
+    if (tid < 2) { mbar_init(smem_u32(&sm.oload[tid]), 1); fence_proxy_async(); }   // completed by TMA loads (async proxy)
     pdl_wait();
     for (int i = tid; i < 128; i += kTcThreads) {
         if (p.ga) {   // ga (dZ - m1 - (Y - mu) rstd m2)
@@ -445,7 +509,14 @@ tc_bwd_kernel(const TcBwdParams p)
     }
     // ---- per-thread constants of the epilogue: input channels ic + 8 h
     const bool final_mode = p.mode == 0 || p.mode == 3;
-    const bool add_existing = p.mode >= 2;
+    // staging: this warpgroup's input channels 64 c .. 64 c + 63 are columns icl = ic - 64 c of its half; its chunks at or past kin are
+    // never moved.  Thread 0 of the warpgroup moves the half.
+    const int wg = (warp - 4) >> 2, icl = ic - 64 * wg;
+    const int nchunks = max(0, min(2, (p.kin - 64 * wg + 31) / 32));
+    const bool load_existing = p.mode == 3 && nchunks > 0;   // mode 2 adds in L2 (TMA reduce-add): the SM reads nothing
+    const bool leader = (tid & 127) == 0;
+    unsigned char *os = sm.os[wg];
+    const uint32_t os_u = smem_u32(os), oload = smem_u32(&sm.oload[wg]);
     float cinvg[2], cbg[2], cl2g[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -453,7 +524,6 @@ tc_bwd_kernel(const TcBwdParams p)
         const int c = ic + 8 * h;
         cinvg[h] = sm.pinvg[c]; cbg[h] = sm.pbeta[c] * cinvg[h]; cl2g[h] = 0.69314718056f * cinvg[h];
     }
-    const int ldo = p.ldo;
     float dw[16][4];
 #pragma unroll
     for (int nt = 0; nt < 16; ++nt) dw[nt][0] = dw[nt][1] = dw[nt][2] = dw[nt][3] = 0.f;
@@ -463,6 +533,13 @@ tc_bwd_kernel(const TcBwdParams p)
         const int tile = blockIdx.x + jt * gstep, st = jt % kBStages;
         const int m0 = tile * kPx;
         const uint32_t gks = gk0 + (uint32_t)st * kGkTile, xts = yx0 + (uint32_t)st * kXtTile;
+        if (leader && nchunks > 0) {
+            bulk_wait_read<0>();                       // the stores of tile jt - 1 have read the staging half
+            if (load_existing) {                       // the existing values land in the half while the MMAs run
+                mbar_arrive_expect_tx(oload, nchunks * kGkChunk);
+                for (int c = 0; c < nchunks; ++c) tma_load_2d(os_u + c * kGkChunk, &p.omap, oload, 64 * wg + 32 * c, m0);
+            }
+        }
         mbar_wait(smem_u32(&sm.full[st]), (jt / kBStages) & 1);
 
         // dX^T[in, px] = sum_out W^T[in, out] G[px, out]: 16 k-steps of 8 output channels, N = 32 pixels
@@ -484,13 +561,14 @@ tc_bwd_kernel(const TcBwdParams p)
 #pragma unroll
         for (int ks = 0; ks < kPx / 8; ++ks) wgmma_tf32_n128(dw, a[ks], wgmma_desc(kstep_addr(xts, ks, 0)));
         wgmma_commit();
+        warpgroup_bar(2 + wg);                         // the staging half is free (under the MMAs)
         wgmma_wait<1>();                               // the data gradient; the weight-gradient MMAs run on under the epilogue
         wgmma_fence_operand(dx);
+        if (load_existing) mbar_wait(oload, jt & 1);
 
-        // ---- epilogue: dx[nt] = {dX^T(ic, px), dX^T(ic, px + 1), dX^T(ic + 8, px), dX^T(ic + 8, px + 1)}, px = 8 nt + 2 t4
-        const int rows = M - m0;
+        // ---- epilogue: dx[nt] = {dX^T(ic, px), dX^T(ic, px + 1), dX^T(ic + 8, px), dX^T(ic + 8, px + 1)}, px = 8 nt + 2 t4;
+        // pixels >= M and channels >= kin are staged too and clipped by the stores
         float t1[2] = {0.f, 0.f}, t2[2] = {0.f, 0.f};
-        float *ot = p.dZprev + (size_t)m0 * ldo;
 #pragma unroll
         for (int nt = 0; nt < 4; ++nt) {
 #pragma unroll
@@ -500,9 +578,8 @@ tc_bwd_kernel(const TcBwdParams p)
                 for (int h = 0; h < 2; ++h) {
                     const int c = ic + 8 * h;
                     float v = dx[nt][2 * h + e];
-                    float *op = ot + (size_t)px * ldo + c;
-                    const bool store = px < rows && c < p.kin;
-                    if (add_existing && store) v += *op;
+                    float *op = reinterpret_cast<float *>(os + kmajor_off(px, icl + 8 * h, kGkChunk));
+                    if (load_existing) v += *op;                                    // zeros past M / kin
                     if (final_mode) {
                         // the conversion stored x + half a TF32 ulp (bit pattern + 0x1000, nothing truncated): undo it -> exact fp32 x
                         const float x = __uint_as_float(lds32(xts + kmajor_off(c, px, 0)) - 0x1000u);
@@ -514,12 +591,21 @@ tc_bwd_kernel(const TcBwdParams p)
                         t1[h] += v;
                         t2[h] = fmaf(v, fmaf(ls, cl2g[h], fmaf(x, cinvg[h], -cbg[h])), t2[h]);
                     }
-                    if (store) *op = v;
+                    *op = v;
                 }
             }
         }
 #pragma unroll
         for (int h = 0; h < 2; ++h) { d1[h] += (double)t1[h]; d2[h] += (double)t2[h]; }
+        fence_proxy_async();                           // the staged values are read by the TMA stores (async proxy)
+        warpgroup_bar(2 + wg);
+        if (leader) {
+            for (int c = 0; c < nchunks; ++c) {
+                if (p.mode == 2) tma_reduce_add_2d(&p.omap, os_u + c * kGkChunk, 64 * wg + 32 * c, m0);
+                else tma_store_2d(&p.omap, os_u + c * kGkChunk, 64 * wg + 32 * c, m0);
+            }
+            bulk_commit();
+        }
         wgmma_wait<0>();
         wgmma_fence_operand(a);
         wgmma_fence_operand(dw);
@@ -545,6 +631,7 @@ tc_bwd_kernel(const TcBwdParams p)
             red_add_v2(p.dW + (size_t)(ic + 8) * p.lddw + in, dw[nt][2], dw[nt][3]);
         }
     }
+    if (leader) bulk_wait<0>();                        // nothing in flight when the CTA exits
 }
 
 }  // namespace
@@ -560,7 +647,8 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
     if (attr_set.first()) {
         GA_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcBwdSmem) + 1024));
     }
-    TcBwdParams p{dZ, Y, ldg, ga, m1, m2, mu, rstd, Yprev, ldp, pa, pb, pmu, prstd, W, ldw, dW, lddw, dZprev, ldo, mode, s1, s2, M, kin, x_raw};
+    TcBwdParams p{{}, dZ, Y, ldg, ga, m1, m2, mu, rstd, Yprev, ldp, pa, pb, pmu, prstd, W, ldw, dW, lddw, mode, s1, s2, M, kin, x_raw};
+    if (int rc = make_tmap(&p.omap, dZprev, kin, M, ldo, kPx)) return rc;
     const int tiles = cdiv(M, kPx), sms = num_sms();
     const int grid = tiles < sms ? tiles : sms;
     {

@@ -3,7 +3,9 @@
 //   * wgmma.mma_async (TF32 in, fp32 accumulate, one warpgroup per m64 slab), used by the decoder-MLP layers (mlp_tc.cu): A in
 //     registers, B read by the tensor cores through a shared-memory matrix descriptor.  TF32 wgmma reads shared-memory operands
 //     K-major only, so every image a descriptor points at is K-major (the backward layer writes its X tile transposed for that);
-//     the mbarrier / setmaxnreg wrappers serve the warp-specialised pipeline around it.
+//     the mbarrier / setmaxnreg wrappers serve the warp-specialised pipeline around it, and the TMA wrappers (tensor store,
+//     reduce-add and load of a 128-byte-swizzled box, bulk-group waits) move the layers' output tiles, which are staged in the
+//     same K-major layout.
 //   * mma.sync m16n8k8 with fragments from ld.shared, kept only by the convolutions (conv_tc.cu): their weight gradient reads the
 //     pixel-major images as they lie, which TF32 wgmma cannot.
 #pragma once
@@ -168,8 +170,40 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
         "DONE_%=:\n"
         "}\n" ::"r"(bar), "r"(parity) : "memory");
 }
-// generic-proxy shared-memory writes (st.shared) made visible to the async proxy (wgmma operand reads)
+// arms the barrier's current phase for `bytes` of asynchronous copies (one arrival)
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes)
+{
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// generic-proxy shared-memory writes (st.shared) made visible to the async proxy (wgmma operand reads, TMA stores)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---- TMA (bulk tensor copies) ------------------------------------------------------------------------------------------
+// `tmap` is the address of a CUtensorMap kernel parameter (__grid_constant__) of a 2-D fp32 matrix with 128-byte-swizzled boxes of
+// 32 columns x `rows` rows; coordinates are {column, row}.  In shared memory such a box is one chunk of the K-major image above:
+// element (row r, column k) at sw128_offset(r, k / 4) + (k % 4) * 4, the box starting on a 1024-byte boundary.  Rows and columns
+// outside the matrix are not written by a store and read as zeros by a load.
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const void *tmap, uint32_t bar, int col, int row)
+{
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+                 ::"r"(dst), "l"(tmap), "r"(bar), "r"(col), "r"(row) : "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const void *tmap, uint32_t src, int col, int row)
+{
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src), "r"(col), "r"(row)
+                 : "memory");
+}
+// global += box, added in L2 (f32: round to nearest even, subnormal inputs and results flushed to sign-preserving zero)
+__device__ __forceinline__ void tma_reduce_add_2d(const void *tmap, uint32_t src, int col, int row)
+{
+    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(src), "r"(col),
+                 "r"(row) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still READ their shared-memory source (the buffer may be rewritten)
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are incomplete (their global writes not yet performed)
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 // barrier of the 128 threads of one warpgroup (id 0 is __syncthreads)
 __device__ __forceinline__ void warpgroup_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
