@@ -81,6 +81,9 @@ _SIGNATURES = {
                                             ctypes.c_int32, ctypes.c_int32, c_vp, c_vp, c_vp]),
     "ga_tc_linear_backward": (ctypes.c_int, [ctypes.c_int32, c_vp, c_vp, ctypes.c_int32, c_vp, c_vp, ctypes.c_int32, c_vp, c_vp, ctypes.c_int32, c_vp,
                                              ctypes.c_int32, c_vp, ctypes.c_int32, ctypes.c_int32, c_vp, c_vp, c_vp]),
+    "ga_tc_linear_backward_ex": (ctypes.c_int, [ctypes.c_int32, c_vp, c_vp, ctypes.c_int32, c_vp, c_vp, ctypes.c_int32, c_vp, c_vp, ctypes.c_int32,
+                                                c_vp, ctypes.c_int32, c_vp, ctypes.c_int32, ctypes.c_int32, c_vp, c_vp, ctypes.c_int32, ctypes.c_int32,
+                                                c_vp]),
     "ga_raster_views": (ctypes.c_int, [ctypes.c_int32] * 4 + [ctypes.c_int64, c_vp, c_vp, c_vp, ctypes.POINTER(GaRasterViews)]),
     "ga_rasterb_geom_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
     "ga_rasterb_img_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 3),

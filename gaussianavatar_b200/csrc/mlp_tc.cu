@@ -641,6 +641,8 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
                   float *dW, int lddw, float *dZprev, int ldo, int mode, double *s1, double *s2, int M, int kin, int x_raw, cudaStream_t st)
 {
     GA_REQUIRE(kin % 4 == 0 && kin >= 4 && kin <= 128 && (!x_raw || mode == 1 || mode == 2), "tensor-core backward: bad kin / mode");
+    // the final modes take s1 / s2 over all 128 channels, and mode 3 adds staging chunks that were only loaded below kin
+    GA_REQUIRE(kin == 128 || mode == 1 || mode == 2, "tensor-core backward: mode %d needs kin = 128 (kin = %d)", mode, kin);
     GA_REQUIRE(ldg % 4 == 0 && ldp % 4 == 0 && ldw % 4 == 0 && ldo % 4 == 0, "tensor-core backward: leading dimensions must be multiples of 4");
     GA_REQUIRE(lddw % 4 == 0 && (reinterpret_cast<uintptr_t>(dW) & 15) == 0, "tensor-core backward: dW must be 16-byte aligned with lddw a multiple of 4");
     static PerDeviceOnce attr_set;
@@ -661,14 +663,24 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
 
 }  // namespace ga
 
-// Unit-test / building-block entry for the fused backward layer (see tc_bwd_kernel).
-extern "C" int ga_tc_linear_backward(int32_t M, const float *dZ, const float *Y, int32_t ldg, const float *bwd_coef /*[5][128] ga,m1,m2,mu,rstd or NULL*/,
-                                     const float *Yprev, int32_t ldp, const float *prev_coef /*[4][128] a,b,mu,rstd*/, const float *W, int32_t ldw,
-                                     float *dW, int32_t lddw, float *dZprev, int32_t ldo, int32_t mode, double *s1, double *s2, void *stream)
+// Unit-test / building-block entry for the fused backward layer (see tc_bwd_kernel), with every input width the decoder uses.
+extern "C" int ga_tc_linear_backward_ex(int32_t M, const float *dZ, const float *Y, int32_t ldg, const float *bwd_coef /*[5][128] ga,m1,m2,mu,rstd or NULL*/,
+                                        const float *Yprev, int32_t ldp, const float *prev_coef /*[4][128] a,b,mu,rstd; NULL if x_raw*/, const float *W,
+                                        int32_t ldw, float *dW, int32_t lddw, float *dZprev, int32_t ldo, int32_t mode, double *s1, double *s2,
+                                        int32_t kin, int32_t x_raw, void *stream)
 {
-    GA_REQUIRE(M > 0 && dZ && Yprev && prev_coef && W && dW && dZprev, "bad arguments");
-    const float *bc = bwd_coef;
+    GA_REQUIRE(M > 0 && dZ && Yprev && (prev_coef || x_raw) && W && dW && dZprev, "bad arguments");
+    const float *bc = bwd_coef, *pc = prev_coef;
     return ga::launch_tc_bwd(dZ, Y, ldg, bc, bc ? bc + 128 : nullptr, bc ? bc + 256 : nullptr, bc ? bc + 384 : nullptr, bc ? bc + 512 : nullptr, Yprev,
-                             ldp, prev_coef, prev_coef + 128, prev_coef + 256, prev_coef + 384, W, ldw, dW, lddw, dZprev, ldo, mode, s1, s2, M,
-                             128, 0, static_cast<cudaStream_t>(stream));
+                             ldp, pc, pc ? pc + 128 : nullptr, pc ? pc + 256 : nullptr, pc ? pc + 384 : nullptr, W, ldw, dW, lddw, dZprev, ldo, mode,
+                             s1, s2, M, kin, x_raw, static_cast<cudaStream_t>(stream));
+}
+
+// The 128-input-channel, BatchNorm + Softplus input form of the above (the hidden layers).
+extern "C" int ga_tc_linear_backward(int32_t M, const float *dZ, const float *Y, int32_t ldg, const float *bwd_coef, const float *Yprev, int32_t ldp,
+                                     const float *prev_coef, const float *W, int32_t ldw, float *dW, int32_t lddw, float *dZprev, int32_t ldo,
+                                     int32_t mode, double *s1, double *s2, void *stream)
+{
+    GA_REQUIRE(prev_coef, "bad arguments");
+    return ga_tc_linear_backward_ex(M, dZ, Y, ldg, bwd_coef, Yprev, ldp, prev_coef, W, ldw, dW, lddw, dZprev, ldo, mode, s1, s2, 128, 0, stream);
 }

@@ -242,6 +242,12 @@ int ga_adam_step_dev(int64_t n, float *param, const float *grad, float *exp_avg,
 int ga_tc_linear_backward(int32_t M, const float *dZ, const float *Y, int32_t ldg, const float *bwd_coef, const float *Yprev, int32_t ldp,
                           const float *prev_coef, const float *W, int32_t ldw, float *dW, int32_t lddw, float *dZprev, int32_t ldo,
                           int32_t mode, double *s1, double *s2, void *stream);
+/* The same with the input width and form as arguments (ga_tc_linear_backward is kin = 128, x_raw = 0): only the first kin input
+ * channels exist (kin % 4 == 0, kin <= 128; modes 0 and 3 need kin == 128): W and dW columns, Y_{l-1} and dZprev channels.
+ * x_raw != 0 (modes 1, 2 only): x = Y_{l-1} as is (the network input), and prev_coef may be NULL. */
+int ga_tc_linear_backward_ex(int32_t M, const float *dZ, const float *Y, int32_t ldg, const float *bwd_coef, const float *Yprev, int32_t ldp,
+                             const float *prev_coef, const float *W, int32_t ldw, float *dW, int32_t lddw, float *dZprev, int32_t ldo,
+                             int32_t mode, double *s1, double *s2, int32_t kin, int32_t x_raw, void *stream);
 
 /* One 5x5, 64->64 channel, padding-2 convolution of the geometry net (model/modules.py:122-137; network.py:26,57) on the
  * tensor cores (building block of ga_decoder_forward/backward, exposed for unit tests).  Feature maps are NHWC [Hf*Hf][64],
