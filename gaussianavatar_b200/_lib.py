@@ -22,6 +22,11 @@ class GaRasterSettings(ctypes.Structure):
                 ("tanfovx", ctypes.c_float), ("tanfovy", ctypes.c_float), ("scale_modifier", ctypes.c_float)]
 
 
+class GaRasterColorCov(ctypes.Structure):
+    _fields_ = [("shs", c_vp), ("sh_degree", ctypes.c_int32), ("sh_coeffs", ctypes.c_int32), ("campos", c_vp),
+                ("cov3D_precomp", c_vp), ("rgb", c_vp), ("clamped", c_vp)]
+
+
 class GaRasterBatchDesc(ctypes.Structure):
     _fields_ = [("B", ctypes.c_int32), ("P", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32),
                 ("capacity", ctypes.c_int64), ("rot_stride", ctypes.c_int64), ("opac_stride", ctypes.c_int64),
@@ -63,6 +68,10 @@ _SIGNATURES = {
     "ga_raster_forward_preprocess": (ctypes.c_int, [ctypes.POINTER(GaRasterSettings)] + [c_vp] * 9 + [ctypes.POINTER(ctypes.c_int64), c_vp]),
     "ga_raster_forward_render": (ctypes.c_int, [ctypes.POINTER(GaRasterSettings), c_vp, c_vp, c_vp, c_vp, ctypes.c_size_t, ctypes.c_int64, c_vp, c_vp, c_vp]),
     "ga_raster_backward": (ctypes.c_int, [ctypes.POINTER(GaRasterSettings)] + [c_vp] * 11 + [ctypes.c_int64] + [c_vp] * 9),
+    "ga_raster_forward_preprocess_ex": (ctypes.c_int, [ctypes.POINTER(GaRasterSettings), ctypes.POINTER(GaRasterColorCov)] + [c_vp] * 9
+                                        + [ctypes.POINTER(ctypes.c_int64), c_vp]),
+    "ga_raster_backward_ex": (ctypes.c_int, [ctypes.POINTER(GaRasterSettings), ctypes.POINTER(GaRasterColorCov)] + [c_vp] * 11
+                              + [ctypes.c_int64] + [c_vp] * 11),
     "ga_smpl_forward": (ctypes.c_int, [ctypes.c_int32] + [c_vp] * 7),
     "ga_smpl_backward": (ctypes.c_int, [ctypes.c_int32] + [c_vp] * 8),
     "ga_lbs_forward": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_int64] + [c_vp] * 9),

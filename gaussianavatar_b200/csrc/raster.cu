@@ -180,12 +180,146 @@ struct CamSrc {
     float tanx, tany;
 };
 
-// Per-Gaussian part of K1; returns the tile rect (zero area if the Gaussian is culled).
+// Colour and covariance sources of the per-frame API beyond precomputed colours + scale / rotation (GaRasterColorCov): spherical-
+// harmonic colours evaluated in K1 (kSH) and precomputed 3D covariances (kCov).  The batched path passes it zeroed.
+struct ColorCov {
+    const float *shs;        // [P, M, 3] coefficient-major RGB triples
+    int D, M;                // active degree 0..3, coefficients per Gaussian
+    bool vec4;               // every row starts 16-byte aligned (M % 4 == 0, aligned base): whole-sector float4 accesses
+    const float *campos;     // [3]
+    const float *cov3D;      // [P, 6] (xx, xy, xz, yy, yz, zz)
+    float *rgb;              // [P, 3] evaluated colour (K1 writes, K4 packs it)
+    uint8_t *clamped;        // [P] bit c: channel c was clamped at 0
+    const float *d_rgb;      // [P, 3] dL/drgb accumulated by K7 (backward)
+    float *d_sh;             // [P, M, 3]
+    float *d_cov3D;          // [P, 6]
+};
+
+constexpr float kShC0 = 0.28209479177387814f, kShC1 = 0.4886025119029199f;
+constexpr float kShC2_0 = 1.0925484305920792f, kShC2_1 = -1.0925484305920792f, kShC2_2 = 0.31539156525252005f,
+                kShC2_3 = -1.0925484305920792f, kShC2_4 = 0.5462742152960396f;
+constexpr float kShC3_0 = -0.5900435899266435f, kShC3_1 = 2.890611442640554f, kShC3_2 = -0.4570457994644658f,
+                kShC3_3 = 0.3731763325901154f, kShC3_4 = -0.4570457994644658f, kShC3_5 = 1.445305721320277f,
+                kShC3_6 = -0.5900435899266435f;
+
+// The 16 real SH basis functions up to degree 3 at the unit direction (x, y, z).
+__device__ __forceinline__ void sh_basis(float x, float y, float z, float b[16])
+{
+    const float xx = x * x, yy = y * y, zz = z * z;
+    b[0] = kShC0;
+    b[1] = -kShC1 * y; b[2] = kShC1 * z; b[3] = -kShC1 * x;
+    b[4] = kShC2_0 * x * y; b[5] = kShC2_1 * y * z; b[6] = kShC2_2 * (2.f * zz - xx - yy); b[7] = kShC2_3 * x * z;
+    b[8] = kShC2_4 * (xx - yy);
+    b[9] = kShC3_0 * y * (3.f * xx - yy); b[10] = kShC3_1 * x * y * z; b[11] = kShC3_2 * y * (4.f * zz - xx - yy);
+    b[12] = kShC3_3 * z * (2.f * zz - 3.f * xx - 3.f * yy); b[13] = kShC3_4 * x * (4.f * zz - xx - yy);
+    b[14] = kShC3_5 * z * (xx - yy); b[15] = kShC3_6 * x * (xx - 3.f * yy);
+}
+
+// Visits the first n (<= 48) floats of one Gaussian's SH row as f(e, value), e compile-time after unrolling.  With vec4 the row is
+// read in float4s, so a warp's loads use whole 32-byte sectors although its lanes' rows lie 12*M bytes apart.
+template <class F>
+__device__ __forceinline__ void sh_row_load(const float *__restrict__ row, int n, bool vec4, F f)
+{
+    if (vec4) {
+#pragma unroll
+        for (int q = 0; q < 12; ++q)
+            if (4 * q < n) {
+                const float4 v = __ldg(reinterpret_cast<const float4 *>(row) + q);
+                f(4 * q, v.x); f(4 * q + 1, v.y); f(4 * q + 2, v.z); f(4 * q + 3, v.w);
+            }
+    } else {
+#pragma unroll
+        for (int e = 0; e < 48; ++e)
+            if (e < n) f(e, __ldg(row + e));
+    }
+}
+
+// Writes a whole SH row of nrow = 3*M floats: f(e) for e < 48 (compile-time after unrolling), 0 beyond.
+template <class F>
+__device__ __forceinline__ void sh_row_store(float *__restrict__ row, int nrow, bool vec4, F f)
+{
+    if (vec4) {
+        float4 *r4 = reinterpret_cast<float4 *>(row);
+#pragma unroll
+        for (int q = 0; q < 12; ++q)
+            if (4 * q < nrow) r4[q] = make_float4(f(4 * q), f(4 * q + 1), f(4 * q + 2), f(4 * q + 3));
+        for (int q = 12; 4 * q < nrow; ++q) r4[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+#pragma unroll
+        for (int e = 0; e < 48; ++e)
+            if (e < nrow) row[e] = f(e);
+        for (int e = 48; e < nrow; ++e) row[e] = 0.f;
+    }
+}
+
+// K1's SH colour of Gaussian i: rgb = max(sum_k basis_k(dir) sh_k + 0.5, 0), dir = (mean - campos) / |mean - campos|.  Culled
+// Gaussians (live = false) get rgb 0 and no clamp bits; ordinary fp32, no integer decision depends on it.
+__device__ __forceinline__ void sh_color_fwd(const ColorCov &cc, size_t i, float px, float py, float pz, bool live)
+{
+    float r[3] = {0.f, 0.f, 0.f};
+    uint32_t cl = 0;
+    if (live) {
+        const float vx = px - __ldg(cc.campos), vy = py - __ldg(cc.campos + 1), vz = pz - __ldg(cc.campos + 2);
+        const float inv = 1.f / sqrtf(vx * vx + vy * vy + vz * vz);
+        float b[16];
+        sh_basis(vx * inv, vy * inv, vz * inv, b);
+        const int n = 3 * (cc.D + 1) * (cc.D + 1);
+        sh_row_load(cc.shs + i * 3 * cc.M, n, cc.vec4, [&](int e, float v) { if (e < n) r[e % 3] += b[e / 3] * v; });
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) {
+            r[ch] += 0.5f;
+            if (r[ch] < 0.f) { cl |= 1u << ch; r[ch] = 0.f; }
+        }
+    }
+    cc.rgb[3 * i] = r[0]; cc.rgb[3 * i + 1] = r[1]; cc.rgb[3 * i + 2] = r[2];
+    cc.clamped[i] = (uint8_t)cl;
+}
+
+// Backward of sh_color_fwd for a visible Gaussian: writes the whole d_sh row (basis_k * dL/drgb, 0 on clamped channels and for
+// k >= (D+1)^2) and adds the direction term, pushed through the normalisation, to dmean.
+__device__ __forceinline__ void sh_color_bwd(const ColorCov &cc, size_t i, float px, float py, float pz, float dmean[3])
+{
+    const uint32_t cl = cc.clamped[i];
+    float g[3];
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) g[ch] = (cl >> ch) & 1u ? 0.f : cc.d_rgb[3 * i + ch];
+    const float vx = px - __ldg(cc.campos), vy = py - __ldg(cc.campos + 1), vz = pz - __ldg(cc.campos + 2);
+    const float inv = 1.f / sqrtf(vx * vx + vy * vy + vz * vz);
+    const float x = vx * inv, y = vy * inv, z = vz * inv;
+    float b[16];
+    sh_basis(x, y, z, b);
+    const int n = 3 * (cc.D + 1) * (cc.D + 1);
+    float s[16];                     // s_k = sh_k . dL/drgb
+#pragma unroll
+    for (int k = 0; k < 16; ++k) s[k] = 0.f;
+    sh_row_load(cc.shs + i * 3 * cc.M, n, cc.vec4, [&](int e, float v) { if (e < n) s[e / 3] += v * g[e % 3]; });
+    sh_row_store(cc.d_sh + i * 3 * cc.M, 3 * cc.M, cc.vec4, [&](int e) { return e < n ? b[e / 3] * g[e % 3] : 0.f; });
+    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+    const float ddx = -kShC1 * s[3] + kShC2_0 * y * s[4] - 2.f * kShC2_2 * x * s[6] + kShC2_3 * z * s[7] + 2.f * kShC2_4 * x * s[8] +
+                      6.f * kShC3_0 * xy * s[9] + kShC3_1 * yz * s[10] - 2.f * kShC3_2 * xy * s[11] - 6.f * kShC3_3 * xz * s[12] +
+                      kShC3_4 * (4.f * zz - 3.f * xx - yy) * s[13] + 2.f * kShC3_5 * xz * s[14] + 3.f * kShC3_6 * (xx - yy) * s[15];
+    const float ddy = -kShC1 * s[1] + kShC2_0 * x * s[4] + kShC2_1 * z * s[5] - 2.f * kShC2_2 * y * s[6] - 2.f * kShC2_4 * y * s[8] +
+                      3.f * kShC3_0 * (xx - yy) * s[9] + kShC3_1 * xz * s[10] + kShC3_2 * (4.f * zz - xx - 3.f * yy) * s[11] -
+                      6.f * kShC3_3 * yz * s[12] - 2.f * kShC3_4 * xy * s[13] - 2.f * kShC3_5 * yz * s[14] - 6.f * kShC3_6 * xy * s[15];
+    const float ddz = kShC1 * s[2] + kShC2_1 * y * s[5] + 4.f * kShC2_2 * z * s[6] + kShC2_3 * x * s[7] + kShC3_1 * xy * s[10] +
+                      8.f * kShC3_2 * yz * s[11] + kShC3_3 * (6.f * zz - 3.f * xx - 3.f * yy) * s[12] + 8.f * kShC3_4 * xz * s[13] +
+                      kShC3_5 * (xx - yy) * s[14];
+    // d dir / d mean = (I - dir dir^T) / |v|
+    const float dot = x * ddx + y * ddy + z * ddz;
+    dmean[0] += (ddx - x * dot) * inv;
+    dmean[1] += (ddy - y * dot) * inv;
+    dmean[2] += (ddz - z * dot) * inv;
+}
+
+// Per-Gaussian part of K1; returns the tile rect (zero area if the Gaussian is culled).  kCov: Sigma is read from cov_pre (this
+// Gaussian's six values) instead of being built from scales / rotations / mod; everything after Sigma is the same op sequence.
+template <bool kCov>
 __device__ __forceinline__ ushort4
 preprocess_one(int il, size_t i, int H, int W, int gx, int gy, const float *view, const float *proj, float tanfovx, float tanfovy,
                float mod, const float *__restrict__ means3D, const float *__restrict__ scales, const float *__restrict__ rq,
-               float opacity, float *__restrict__ depth, float2 *__restrict__ xy, float4 *__restrict__ conic_o,
-               float *__restrict__ cov3d, uint32_t *__restrict__ tiles, ushort4 *__restrict__ rect, int32_t *__restrict__ radii)
+               const float *__restrict__ cov_pre, float opacity, float *__restrict__ depth, float2 *__restrict__ xy,
+               float4 *__restrict__ conic_o, float *__restrict__ cov3d, uint32_t *__restrict__ tiles, ushort4 *__restrict__ rect,
+               int32_t *__restrict__ radii)
 {
     const ushort4 none = make_ushort4(0, 0, 0, 0);
     radii[i] = 0;
@@ -205,25 +339,30 @@ preprocess_one(int il, size_t i, int H, int W, int gx, int gy, const float *view
     const float p_w = div_(1.f, add_(hw, 0.0000001f));
     const float ndc_x = mul_(hx, p_w), ndc_y = mul_(hy, p_w);
 
-    const float sv[3] = {mul_(mod, scales[3 * (size_t)i]), mul_(mod, scales[3 * (size_t)i + 1]), mul_(mod, scales[3 * (size_t)i + 2])};
-    float Rm[3][3];
-    quat_to_rot(rq[0], rq[1], rq[2], rq[3], Rm);
-    float Mm[3][3];
+    float S00, S01, S02, S11, S12, S22;
+    if constexpr (kCov) {
+        S00 = cov_pre[0]; S01 = cov_pre[1]; S02 = cov_pre[2]; S11 = cov_pre[3]; S12 = cov_pre[4]; S22 = cov_pre[5];
+    } else {
+        const float sv[3] = {mul_(mod, scales[3 * (size_t)i]), mul_(mod, scales[3 * (size_t)i + 1]), mul_(mod, scales[3 * (size_t)i + 2])};
+        float Rm[3][3];
+        quat_to_rot(rq[0], rq[1], rq[2], rq[3], Rm);
+        float Mm[3][3];
 #pragma unroll
-    for (int a = 0; a < 3; ++a)
+        for (int a = 0; a < 3; ++a)
 #pragma unroll
-        for (int k = 0; k < 3; ++k) Mm[a][k] = mul_(sv[a], Rm[k][a]);
-    float Sg[3][3];
+            for (int k = 0; k < 3; ++k) Mm[a][k] = mul_(sv[a], Rm[k][a]);
+        float Sg[3][3];
 #pragma unroll
-    for (int j = 0; j < 3; ++j)
+        for (int j = 0; j < 3; ++j)
 #pragma unroll
-        for (int k = j; k < 3; ++k) {
-            float t = mul_(Mm[0][j], Mm[0][k]);
-            t = fma_(Mm[1][j], Mm[1][k], t);
-            t = fma_(Mm[2][j], Mm[2][k], t);
-            Sg[j][k] = t;
-        }
-    const float S00 = Sg[0][0], S01 = Sg[0][1], S02 = Sg[0][2], S11 = Sg[1][1], S12 = Sg[1][2], S22 = Sg[2][2];
+            for (int k = j; k < 3; ++k) {
+                float t = mul_(Mm[0][j], Mm[0][k]);
+                t = fma_(Mm[1][j], Mm[1][k], t);
+                t = fma_(Mm[2][j], Mm[2][k], t);
+                Sg[j][k] = t;
+            }
+        S00 = Sg[0][0]; S01 = Sg[0][1]; S02 = Sg[0][2]; S11 = Sg[1][1]; S12 = Sg[1][2]; S22 = Sg[2][2];
+    }
 
     const float focal_x = div_((float)W, mul_(2.f, tanfovx)), focal_y = div_((float)H, mul_(2.f, tanfovy));
     const float limx = mul_(1.3f, tanfovx), limy = mul_(1.3f, tanfovy);
@@ -336,14 +475,15 @@ __device__ __forceinline__ int tile_slot_find(const uint32_t *s_key, uint32_t ti
 // The CTA's 256 Gaussians first count into a shared-memory tile table and then add only its occupied slots to the global counters — a
 // few hundred thousand atomics on a few hundred hot addresses (which serialise in L2 and used to set this kernel's duration)
 // become one per (CTA, touched tile).
-template <bool kSmemHist>
+// kSH / kCov (per-frame API only, B = 1): SH colours into cc.rgb / cc.clamped, Sigma from cc.cov3D.
+template <bool kSmemHist, bool kSH = false, bool kCov = false>
 __global__ void __launch_bounds__(256)
 preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod, const float *__restrict__ means3D,
                       const float *__restrict__ scales, const float *__restrict__ rots, long long rot_stride,
                       const float *__restrict__ opac, long long opac_stride, float *__restrict__ depth,
                       float2 *__restrict__ xy, float4 *__restrict__ conic_o, float *__restrict__ cov3d,
                       uint32_t *__restrict__ tiles, ushort4 *__restrict__ rect, int32_t *__restrict__ radii,
-                      uint32_t *__restrict__ tile_count)
+                      uint32_t *__restrict__ tile_count, ColorCov cc)
 {
     pdl_wait();
     const int b = blockIdx.y;
@@ -355,10 +495,13 @@ preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod
     const float tanfovy = cam.tan ? cam.tan[(size_t)b * cam.stride + 1] : cam.tany;
     const int il = blockIdx.x * blockDim.x + threadIdx.x;
     ushort4 rc = make_ushort4(0, 0, 0, 0);
-    if (il < P)
-        rc = preprocess_one(il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, means3D, scales,
-                            rots + (size_t)b * rot_stride + 4 * (size_t)il, opac[(size_t)b * opac_stride + il], depth, xy, conic_o, cov3d,
-                            tiles, rect, radii);
+    if (il < P) {
+        rc = preprocess_one<kCov>(il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, means3D, scales,
+                                  rots + (size_t)b * rot_stride + 4 * (size_t)il, cc.cov3D + 6 * (size_t)il,
+                                  opac[(size_t)b * opac_stride + il], depth, xy, conic_o, cov3d, tiles, rect, radii);
+        if constexpr (kSH)
+            sh_color_fwd(cc, (size_t)il, means3D[3 * (size_t)il], means3D[3 * (size_t)il + 1], means3D[3 * (size_t)il + 2], rc.z > rc.x);
+    }
     uint32_t *tc = tile_count + (size_t)b * gx * gy;
     if (kSmemHist) {
         __shared__ uint32_t s_key[kTileSlots], s_cnt[kTileSlots];
@@ -1027,13 +1170,16 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
 }
 
 // Fused K8 (conic -> cov2D -> cov3D / mean) + K9 (mean2D -> mean3D, cov3D -> scale / rotation): one thread per Gaussian.
+// kSH: also the SH colour backward (d_sh, direction term of d_means3D); kCov: dL/dSigma goes to cc.d_cov3D and the scale /
+// rotation chain is skipped (per-frame API only, B = 1).
+template <bool kSH = false, bool kCov = false>
 __global__ void __launch_bounds__(256)
 preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *__restrict__ means3D,
                       const float *__restrict__ scales, const float *__restrict__ rots, long long rot_stride,
                       const int32_t *__restrict__ radii, const float *__restrict__ cov3d,
                       const float2 *__restrict__ d_mean2D, const float4 *__restrict__ d_conic_op,
                       float *__restrict__ d_means3D, float *__restrict__ d_scales, float *__restrict__ d_rots,
-                      float *__restrict__ d_opac, float *__restrict__ d_means2D_out)
+                      float *__restrict__ d_opac, float *__restrict__ d_means2D_out, ColorCov cc)
 {
     pdl_wait();
     const int fb = blockIdx.y;
@@ -1054,8 +1200,14 @@ preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *_
     if (d_means2D_out) { d_means2D_out[i3] = g2.x; d_means2D_out[i3 + 1] = g2.y; d_means2D_out[i3 + 2] = 0.f; }
     if (radii[i] <= 0) {
         d_means3D[i3] = d_means3D[i3 + 1] = d_means3D[i3 + 2] = 0.f;
-        d_scales[i3] = d_scales[i3 + 1] = d_scales[i3 + 2] = 0.f;
-        if (d_rots) { d_rots[4 * (size_t)i] = d_rots[4 * (size_t)i + 1] = d_rots[4 * (size_t)i + 2] = d_rots[4 * (size_t)i + 3] = 0.f; }
+        if constexpr (kSH) sh_row_store(cc.d_sh + i * 3 * cc.M, 3 * cc.M, cc.vec4, [](int) { return 0.f; });
+        if constexpr (kCov) {
+#pragma unroll
+            for (int k = 0; k < 6; ++k) cc.d_cov3D[6 * i + k] = 0.f;
+        } else {
+            d_scales[i3] = d_scales[i3 + 1] = d_scales[i3 + 2] = 0.f;
+            if (d_rots) { d_rots[4 * (size_t)i] = d_rots[4 * (size_t)i + 1] = d_rots[4 * (size_t)i + 2] = d_rots[4 * (size_t)i + 3] = 0.f; }
+        }
         return;
     }
     const float px = means3D[i3], py = means3D[i3 + 1], pz = means3D[i3 + 2];
@@ -1122,7 +1274,13 @@ preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *_
 #pragma unroll
     for (int k = 0; k < 3; ++k)
         dmean[k] += (proj[4 * k + 0] * m_w - proj[4 * k + 3] * mul1) * g2.x + (proj[4 * k + 1] * m_w - proj[4 * k + 3] * mul2) * g2.y;
+    if constexpr (kSH) sh_color_bwd(cc, i, px, py, pz, dmean);
     d_means3D[i3] = dmean[0]; d_means3D[i3 + 1] = dmean[1]; d_means3D[i3 + 2] = dmean[2];
+    if constexpr (kCov) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) cc.d_cov3D[6 * i + k] = dc[k];
+        return;
+    }
 
     const float sv[3] = {mod * scales[i3], mod * scales[i3 + 1], mod * scales[i3 + 2]};
     const float qr = rq[0], qx = rq[1], qy = rq[2], qz = rq[3];
@@ -1179,17 +1337,18 @@ struct FwdArgs {
     float mod;
 };
 
-// K1 + K2 for all frames.
-int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, long long capacity, const GeomViews &g, const ImgViews &iv,
-                      int32_t *radii, cudaStream_t stream)
+// K1 + K2 for all frames.  cc selects the K1 variant (all zero: precomputed colours, Sigma from scales / rotations).
+int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const ColorCov &cc, long long capacity, const GeomViews &g,
+                      const ImgViews &iv, int32_t *radii, cudaStream_t stream)
 {
     const size_t BT = (size_t)d.B * d.T;
     GA_CHECK_CUDA(cudaMemsetAsync(iv.count, 0, sizeof(uint32_t) * BT, stream));
     if (d.P > 0) {
         ProfScope _ps("preprocess_fwd_kernel", stream);
-        launch_k(preprocess_fwd_kernel<true>, dim3(cdiv(d.P, 256), d.B), 256, 0, stream, d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D, a.scales,
-                                                                                  a.rotations, a.rot_stride, a.opacities, a.opac_stride, g.depth,
-                                                                                  g.xy, g.conic_o, g.cov3d, g.tiles, g.rect, radii, iv.count);
+        auto *k1 = cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true, true> : preprocess_fwd_kernel<true, true, false>)
+                          : (cc.cov3D ? preprocess_fwd_kernel<true, false, true> : preprocess_fwd_kernel<true>);
+        launch_k(k1, dim3(cdiv(d.P, 256), d.B), 256, 0, stream, d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D, a.scales, a.rotations,
+                 a.rot_stride, a.opacities, a.opac_stride, g.depth, g.xy, g.conic_o, g.cov3d, g.tiles, g.rect, radii, iv.count, cc);
         GA_CHECK_LAUNCH("preprocess_fwd_kernel");
     }
     {
@@ -1251,8 +1410,9 @@ size_t bwd_scratch_bytes(size_t BP)
     return align_up(n * sizeof(float2)) + align_up(n * sizeof(float4));
 }
 
-int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, const int32_t *radii, const GeomViews &g, const ImgViews &iv,
-                    const BinViews &bv, void *scratch, cudaStream_t stream)
+// K7 + fused K8/K9.  cc selects the K8/K9 variant as in launch_preprocess; with SH, K7's d_colors is dL/drgb (cc.d_rgb).
+int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, ColorCov cc, const int32_t *radii, const GeomViews &g,
+                    const ImgViews &iv, const BinViews &bv, void *scratch, cudaStream_t stream)
 {
     const size_t BP = (size_t)d.B * d.P;
     Carver sc(scratch);
@@ -1275,9 +1435,11 @@ int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, const in
     GA_CHECK_LAUNCH("render_bwd_kernel");
     {
         ProfScope _ps("preprocess_bwd_kernel", stream);
-        launch_k(preprocess_bwd_kernel, dim3(cdiv(d.P, 256), d.B), 256, 0, stream, d.P, d.H, d.W, cam, a.mod, a.means3D, a.scales, a.rotations,
-                                                                            a.rot_stride, radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D,
-                                                                            a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D);
+        cc.d_rgb = a.d_colors;
+        auto *k89 = cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<true, false>)
+                           : (cc.cov3D ? preprocess_bwd_kernel<false, true> : preprocess_bwd_kernel<>);
+        launch_k(k89, dim3(cdiv(d.P, 256), d.B), 256, 0, stream, d.P, d.H, d.W, cam, a.mod, a.means3D, a.scales, a.rotations, a.rot_stride,
+                 radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D, a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D, cc);
     }
     GA_CHECK_LAUNCH("preprocess_bwd_kernel");
     return GA_OK;
@@ -1296,27 +1458,61 @@ extern "C" size_t ga_raster_img_bytes(int32_t H, int32_t W) { return carve_img(n
 extern "C" size_t ga_raster_binning_bytes(int64_t R, int32_t H, int32_t W) { return carve_bin(nullptr, R, make_dims(1, 0, H, W)).total; }
 extern "C" size_t ga_raster_bwd_scratch_bytes(int32_t P) { return bwd_scratch_bytes((size_t)(P > 0 ? P : 0)); }
 
-extern "C" int ga_raster_forward_preprocess(const GaRasterSettings *s, const float *means3D, const float *scales,
-                                            const float *rotations, const float *opacities, const float *viewmatrix,
-                                            const float *projmatrix, void *geom, void *img, int32_t *radii,
-                                            int64_t *num_rendered_host, void *stream_)
+// Validates a GaRasterColorCov (NULL: neither mode) and turns it into the kernels' ColorCov.
+static int color_cov_of(const GaRasterColorCov *in, ColorCov &out)
+{
+    out = ColorCov{};
+    if (!in) return GA_OK;
+    if (in->shs) {
+        GA_REQUIRE(in->sh_degree >= 0 && in->sh_degree <= 3, "sh_degree %d outside 0..3", (int)in->sh_degree);
+        GA_REQUIRE(in->sh_coeffs >= (in->sh_degree + 1) * (in->sh_degree + 1), "sh_coeffs %d < (sh_degree + 1)^2 = %d", (int)in->sh_coeffs,
+                   (int)((in->sh_degree + 1) * (in->sh_degree + 1)));
+        GA_REQUIRE(in->campos && in->rgb && in->clamped, "shs given without campos / rgb / clamped");
+        out.shs = in->shs;
+        out.D = in->sh_degree;
+        out.M = in->sh_coeffs;
+        out.vec4 = in->sh_coeffs % 4 == 0 && reinterpret_cast<uintptr_t>(in->shs) % 16 == 0;
+        out.campos = in->campos;
+        out.rgb = in->rgb;
+        out.clamped = in->clamped;
+    }
+    out.cov3D = in->cov3D_precomp;
+    return GA_OK;
+}
+
+extern "C" int ga_raster_forward_preprocess_ex(const GaRasterSettings *s, const GaRasterColorCov *cc_in, const float *means3D,
+                                               const float *scales, const float *rotations, const float *opacities,
+                                               const float *viewmatrix, const float *projmatrix, void *geom, void *img, int32_t *radii,
+                                               int64_t *num_rendered_host, void *stream_)
 {
     if (int rc = check_settings(s)) return rc;
     GA_REQUIRE(num_rendered_host && img, "NULL pointer argument");
     *num_rendered_host = 0;
-    GA_REQUIRE(s->P == 0 || (means3D && scales && rotations && opacities && viewmatrix && projmatrix && geom && radii), "NULL pointer argument");
+    ColorCov cc;
+    if (int rc = color_cov_of(cc_in, cc)) return rc;
+    GA_REQUIRE(s->P == 0 || (means3D && (cc.cov3D || (scales && rotations)) && opacities && viewmatrix && projmatrix && geom && radii),
+               "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const Dims d = make_dims(1, s->P, s->H, s->W);
     GeomViews g = carve_geom(geom, (size_t)s->P);
     ImgViews iv = carve_img(img, d);
     const CamSrc cam{viewmatrix, projmatrix, nullptr, 0, s->tanfovx, s->tanfovy};
     const FwdArgs a{means3D, nullptr, scales, rotations, opacities, nullptr, 0, 0, s->scale_modifier};
-    if (int rc = launch_preprocess(d, cam, a, kNoCapacity, g, iv, radii, stream)) return rc;
+    if (int rc = launch_preprocess(d, cam, a, cc, kNoCapacity, g, iv, radii, stream)) return rc;
     int32_t total = 0;
     GA_CHECK_CUDA(cudaMemcpyAsync(&total, iv.status, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
     GA_CHECK_CUDA(cudaStreamSynchronize(stream));
     *num_rendered_host = (int64_t)total;
     return GA_OK;
+}
+
+extern "C" int ga_raster_forward_preprocess(const GaRasterSettings *s, const float *means3D, const float *scales,
+                                            const float *rotations, const float *opacities, const float *viewmatrix,
+                                            const float *projmatrix, void *geom, void *img, int32_t *radii,
+                                            int64_t *num_rendered_host, void *stream_)
+{
+    return ga_raster_forward_preprocess_ex(s, nullptr, means3D, scales, rotations, opacities, viewmatrix, projmatrix, geom, img, radii,
+                                           num_rendered_host, stream_);
 }
 
 extern "C" int ga_raster_forward_render(const GaRasterSettings *s, const float *colors, const float *bg, void *geom, void *binning,
@@ -1337,24 +1533,43 @@ extern "C" int ga_raster_forward_render(const GaRasterSettings *s, const float *
     return launch_binning_and_render(d, a, R, carve_geom(geom, (size_t)s->P), carve_img(img, d), bv, out_color, stream);
 }
 
+extern "C" int ga_raster_backward_ex(const GaRasterSettings *s, const GaRasterColorCov *cc_in, const float *means3D,
+                                     const float *colors, const float *scales, const float *rotations, const float *bg,
+                                     const float *viewmatrix, const float *projmatrix, const int32_t *radii, const void *geom,
+                                     const void *binning, const void *img, int64_t R, const float *dL_dout, void *scratch,
+                                     float *d_means3D, float *d_colors, float *d_scales, float *d_rotations, float *d_opacities,
+                                     float *d_means2D, float *d_sh, float *d_cov3D, void *stream_)
+{
+    if (int rc = check_settings(s)) return rc;
+    ColorCov cc;
+    if (int rc = color_cov_of(cc_in, cc)) return rc;
+    if (s->P == 0) return GA_OK;
+    GA_REQUIRE(means3D && (colors || cc.shs) && (cc.cov3D || (scales && rotations && d_scales)) && bg && viewmatrix && projmatrix &&
+                   radii && geom && img && binning && dL_dout && scratch && d_means3D && d_colors,
+               "NULL pointer argument");
+    GA_REQUIRE(!cc.shs || d_sh, "shs given without d_sh");
+    GA_REQUIRE(!cc.cov3D || d_cov3D, "cov3D_precomp given without d_cov3D");
+    cc.vec4 = cc.vec4 && reinterpret_cast<uintptr_t>(d_sh) % 16 == 0;
+    cc.d_sh = d_sh;
+    cc.d_cov3D = d_cov3D;
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const Dims d = make_dims(1, s->P, s->H, s->W);
+    const CamSrc cam{viewmatrix, projmatrix, nullptr, 0, s->tanfovx, s->tanfovy};
+    const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, 0, s->scale_modifier, d_means3D, d_colors, d_scales, d_rotations,
+                    d_opacities, d_means2D};
+    return launch_backward(d, cam, a, cc, radii, carve_geom(const_cast<void *>(geom), (size_t)s->P),
+                           carve_img(const_cast<void *>(img), d), carve_bin(const_cast<void *>(binning), R, d), scratch, stream);
+}
+
 extern "C" int ga_raster_backward(const GaRasterSettings *s, const float *means3D, const float *colors, const float *scales,
                                   const float *rotations, const float *bg, const float *viewmatrix, const float *projmatrix,
                                   const int32_t *radii, const void *geom, const void *binning, const void *img, int64_t R,
                                   const float *dL_dout, void *scratch, float *d_means3D, float *d_colors, float *d_scales,
                                   float *d_rotations, float *d_opacities, float *d_means2D, void *stream_)
 {
-    if (int rc = check_settings(s)) return rc;
-    if (s->P == 0) return GA_OK;
-    GA_REQUIRE(means3D && colors && scales && rotations && bg && viewmatrix && projmatrix && radii && geom && img && binning &&
-                   dL_dout && scratch && d_means3D && d_colors && d_scales,
-               "NULL pointer argument");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const Dims d = make_dims(1, s->P, s->H, s->W);
-    const CamSrc cam{viewmatrix, projmatrix, nullptr, 0, s->tanfovx, s->tanfovy};
-    const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, 0, s->scale_modifier, d_means3D, d_colors, d_scales, d_rotations,
-                    d_opacities, d_means2D};
-    return launch_backward(d, cam, a, radii, carve_geom(const_cast<void *>(geom), (size_t)s->P), carve_img(const_cast<void *>(img), d),
-                           carve_bin(const_cast<void *>(binning), R, d), scratch, stream);
+    return ga_raster_backward_ex(s, nullptr, means3D, colors, scales, rotations, bg, viewmatrix, projmatrix, radii, geom, binning, img, R,
+                                 dL_dout, scratch, d_means3D, d_colors, d_scales, d_rotations, d_opacities, d_means2D, nullptr, nullptr,
+                                 stream_);
 }
 
 // ---- batched API: every frame of a step in one set of launches, no host read-back ------------------------------------------
@@ -1418,7 +1633,7 @@ extern "C" int ga_rasterb_forward(const GaRasterBatchDesc *bd, const float *cams
     BinViews bv = carve_bin(binning, bd->capacity, d);
     const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
     const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
-    if (int rc = launch_preprocess(d, cam, a, bd->capacity, g, iv, radii, stream)) return rc;
+    if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
     return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream);
 }
 
@@ -1438,7 +1653,7 @@ extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cam
     const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
     const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, bd->rot_stride, bd->scale_modifier, d_means3D, d_colors, d_scales,
                     d_rotations, d_opacities, d_means2D};
-    return launch_backward(d, cam, a, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P), carve_img(const_cast<void *>(img), d),
+    return launch_backward(d, cam, a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P), carve_img(const_cast<void *>(img), d),
                            carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream);
 }
 

@@ -6,9 +6,11 @@ colors_precomp=, opacities=, scales=, rotations=, cov3D_precomp=) -> (color[3,H,
 input order.  Validation behaviour follows [UPSTREAM] (SURVEY.md §8b): exactly one of shs / colors_precomp and exactly
 one of (scales+rotations) / cov3D_precomp, else ``Exception``.
 
-Only the path GaussianAvatar exercises is implemented on the device: precomputed colours, scales + rotations.
-SH evaluation and cov3D_precomp raise NotImplementedError (never used by the reference: shs=None at
-model/avatar_model.py:350, cov3D_precomp=None at gaussian_renderer/__init__.py:37).
+All four input combinations run on the device: colours precomputed or evaluated from spherical harmonics (``shs`` [P, M, 3]
+with ``raster_settings.sh_degree`` D in 0..3, (D+1)^2 <= M, seen from ``raster_settings.campos``), and 3D covariances built from
+``scales`` + ``rotations`` (times ``scale_modifier``) or given as ``cov3D_precomp`` [P, 6] = (xx, xy, xz, yy, yz, zz).
+GaussianAvatar itself passes precomputed colours with scales + rotations (shs=None at model/avatar_model.py:350,
+cov3D_precomp=None at gaussian_renderer/__init__.py:37); the batched training path supports only that combination.
 """
 from __future__ import annotations
 
@@ -101,8 +103,10 @@ def _views(B, P, H, W, capacity, geom, binning, img, radii):
 
 
 class RasterContext:
-    """Buffers one forward leaves behind for its backward (upstream's geomBuffer / binningBuffer / imgBuffer)."""
-    __slots__ = ("settings", "geom", "binning", "img", "num_rendered", "radii")
+    """Buffers one forward leaves behind for its backward (upstream's geomBuffer / binningBuffer / imgBuffer).  With shs or
+    cov3D_precomp, `cc` is the GaRasterColorCov of the forward and `keep` holds the tensors it points to (rgb [P,3] is the
+    evaluated SH colour, clamped [P] uint8 its per-channel clamp bits)."""
+    __slots__ = ("settings", "geom", "binning", "img", "num_rendered", "radii", "cc", "keep", "rgb", "clamped")
 
     def views(self) -> dict:
         """Typed tensor copies of the internal per-stage state (parity tests)."""
@@ -110,56 +114,117 @@ class RasterContext:
         return _views(1, s.P, s.H, s.W, self.num_rendered, self.geom, self.binning, self.img, self.radii)[0]
 
 
-def rasterize_forward(means3D, colors, opacities, scales, rotations, rs: GaussianRasterizationSettings):
-    """K1..K6 on the current CUDA stream.  Returns (color [3,H,W], radii [P] int32, RasterContext)."""
+def _on_device(dev, **tensors):
+    for name, t in tensors.items():
+        if t is not None and t.device != dev:
+            raise RuntimeError(f"gaussianavatar_b200 rasterizer: {name} is on {t.device}, means3D on {dev} (no CPU fallback)")
+
+
+def _color_cov(P, dev, rs, shs, cov3D_precomp):
+    """Checks shs / cov3D_precomp and returns (GaRasterColorCov or None, tensors it points to, rgb, clamped)."""
+    if shs is None and cov3D_precomp is None:
+        return None, (), None, None
+    _on_device(dev, shs=shs, cov3D_precomp=cov3D_precomp)
+    cc = _lib.GaRasterColorCov()
+    keep, rgb, clamped = [], None, None
+    if shs is not None:
+        D = int(rs.sh_degree)
+        if shs.dim() != 3 or shs.shape[0] != P or shs.shape[2] != 3:
+            raise ValueError(f"shs must have shape [P={P}, M, 3], got {tuple(shs.shape)}")
+        M = int(shs.shape[1])
+        if not 0 <= D <= 3:
+            raise ValueError(f"sh_degree must be in 0..3, got {D}")
+        if (D + 1) ** 2 > M:
+            raise ValueError(f"sh_degree {D} needs (D+1)^2 = {(D + 1) ** 2} coefficients, shs has {M}")
+        if rs.campos is None or torch.as_tensor(rs.campos).numel() != 3:
+            raise ValueError("shs needs raster_settings.campos (3 values)")
+        shs = _c(shs)
+        campos = _c(torch.as_tensor(rs.campos)).reshape(3).to(dev)
+        rgb = torch.empty(P, 3, dtype=torch.float32, device=dev)
+        clamped = torch.empty(P, dtype=torch.uint8, device=dev)
+        cc.shs, cc.sh_degree, cc.sh_coeffs, cc.campos = ptr(shs), D, M, ptr(campos)
+        cc.rgb, cc.clamped = ptr(rgb), ptr(clamped)
+        keep += [shs, campos]
+    if cov3D_precomp is not None:
+        if tuple(cov3D_precomp.shape) != (P, 6):
+            raise ValueError(f"cov3D_precomp must have shape [P={P}, 6], got {tuple(cov3D_precomp.shape)}")
+        cov3D_precomp = _c(cov3D_precomp)
+        cc.cov3D_precomp = ptr(cov3D_precomp)
+        keep.append(cov3D_precomp)
+    return cc, tuple(keep), rgb, clamped
+
+
+def rasterize_forward(means3D, colors, opacities, scales, rotations, rs: GaussianRasterizationSettings, *, shs=None,
+                      cov3D_precomp=None):
+    """K1..K6 on the current CUDA stream.  Returns (color [3,H,W], radii [P] int32, RasterContext).
+    shs [P,M,3] (colors None; degree and camera position from rs) and cov3D_precomp [P,6] (scales, rotations None) select
+    the other input modes of upstream's API; every check runs before anything is launched."""
     if not means3D.is_cuda:
         raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
     L = _lib.lib()
     dev = means3D.device
     P, H, W = int(means3D.shape[0]), int(rs.image_height), int(rs.image_width)
     s = GaRasterSettings(P, H, W, float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier))
-    means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
+    cc, keep, rgb, clamped = _color_cov(P, dev, rs, shs, cov3D_precomp)
+    opt = lambda t: None if t is None else _c(t)
+    means3D, colors, scales, rotations = _c(means3D), opt(colors), opt(scales), opt(rotations)
+    _on_device(dev, colors=colors, scales=scales, rotations=rotations, opacities=opacities)
     opacities = _c(opacities).reshape(-1)
     bg, view, proj = _c(rs.bg).to(dev), _c(rs.viewmatrix).to(dev), _c(rs.projmatrix).to(dev)
 
     ctx = RasterContext()
     ctx.settings = s
+    ctx.cc, ctx.keep, ctx.rgb, ctx.clamped = cc, keep, rgb, clamped
     ctx.geom = torch.empty(L.ga_raster_geom_bytes(P), dtype=torch.uint8, device=dev)
     ctx.img = torch.empty(L.ga_raster_img_bytes(H, W), dtype=torch.uint8, device=dev)
     ctx.radii = torch.empty(P, dtype=torch.int32, device=dev)
     n = ctypes.c_int64(0)
     st = _stream()
-    _lib.check(L.ga_raster_forward_preprocess(ctypes.byref(s), ptr(means3D), ptr(scales), ptr(rotations), ptr(opacities),
-                                              ptr(view), ptr(proj), ptr(ctx.geom), ptr(ctx.img), ptr(ctx.radii), ctypes.byref(n), st),
-               "ga_raster_forward_preprocess")
+    _lib.check(L.ga_raster_forward_preprocess_ex(ctypes.byref(s), None if cc is None else ctypes.byref(cc), ptr(means3D), ptr(scales),
+                                                 ptr(rotations), ptr(opacities), ptr(view), ptr(proj), ptr(ctx.geom), ptr(ctx.img),
+                                                 ptr(ctx.radii), ctypes.byref(n), st), "ga_raster_forward_preprocess_ex")
     ctx.num_rendered = int(n.value)
     nb = L.ga_raster_binning_bytes(ctx.num_rendered, H, W)
     ctx.binning = torch.empty(nb, dtype=torch.uint8, device=dev)
     color = torch.empty(3, H, W, dtype=torch.float32, device=dev)
-    _lib.check(L.ga_raster_forward_render(ctypes.byref(s), ptr(colors), ptr(bg), ptr(ctx.geom), ptr(ctx.binning), nb,
-                                          ctx.num_rendered, ptr(ctx.img), ptr(color), st), "ga_raster_forward_render")
+    _lib.check(L.ga_raster_forward_render(ctypes.byref(s), ptr(colors if rgb is None else rgb), ptr(bg), ptr(ctx.geom), ptr(ctx.binning),
+                                          nb, ctx.num_rendered, ptr(ctx.img), ptr(color), st), "ga_raster_forward_render")
     return color, ctx.radii, ctx
 
 
 def rasterize_backward(ctx: RasterContext, means3D, colors, scales, rotations, rs, grad_color, want_opacity=True,
-                       want_rotations=True, want_means2D=True):
+                       want_rotations=True, want_means2D=True, *, return_sh_cov3D=False):
+    """Gradients of the forward that filled ctx: (d_means3D, d_means2D, d_colors, d_opacities, d_scales, d_rotations), and with
+    return_sh_cov3D=True also (d_sh, d_cov3D).  Gradients of inputs the forward did not take are None: with shs, d_colors (the
+    colour is evaluated); with cov3D_precomp, d_scales and d_rotations."""
+    if ctx.cc is not None and not return_sh_cov3D:
+        raise ValueError("this forward took shs / cov3D_precomp: call rasterize_backward(..., return_sh_cov3D=True)")
     L = _lib.lib()
     dev = means3D.device
     s = ctx.settings
     P = s.P
+    sh = ctx.rgb is not None
+    cov = ctx.cc is not None and bool(ctx.cc.cov3D_precomp)
+    opt = lambda t: None if t is None else _c(t)
+    colors, scales, rotations = opt(colors), opt(scales), opt(rotations)
     grad_color = _c(grad_color)
     bg, view, proj = _c(rs.bg).to(dev), _c(rs.viewmatrix).to(dev), _c(rs.projmatrix).to(dev)
     scratch = torch.empty(L.ga_raster_bwd_scratch_bytes(P), dtype=torch.uint8, device=dev)
     d_means3D = torch.empty(P, 3, dtype=torch.float32, device=dev)
     d_colors = torch.empty(P, 3, dtype=torch.float32, device=dev)
-    d_scales = torch.empty(P, 3, dtype=torch.float32, device=dev)
-    d_rot = torch.empty(P, 4, dtype=torch.float32, device=dev) if want_rotations else None
+    d_scales = torch.empty(P, 3, dtype=torch.float32, device=dev) if not cov else None
+    d_rot = torch.empty(P, 4, dtype=torch.float32, device=dev) if want_rotations and not cov else None
     d_opac = torch.empty(P, 1, dtype=torch.float32, device=dev) if want_opacity else None
     d_m2d = torch.empty(P, 3, dtype=torch.float32, device=dev) if want_means2D else None
-    _lib.check(L.ga_raster_backward(ctypes.byref(s), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(bg),
-                                    ptr(view), ptr(proj), ptr(ctx.radii), ptr(ctx.geom), ptr(ctx.binning), ptr(ctx.img),
-                                    ctx.num_rendered, ptr(grad_color), ptr(scratch), ptr(d_means3D), ptr(d_colors),
-                                    ptr(d_scales), ptr(d_rot), ptr(d_opac), ptr(d_m2d), _stream()), "ga_raster_backward")
+    d_sh = torch.empty(ctx.keep[0].shape, dtype=torch.float32, device=dev) if sh else None
+    d_cov3D = torch.empty(P, 6, dtype=torch.float32, device=dev) if cov else None
+    _lib.check(L.ga_raster_backward_ex(ctypes.byref(s), None if ctx.cc is None else ctypes.byref(ctx.cc), ptr(means3D), ptr(colors),
+                                       ptr(scales), ptr(rotations), ptr(bg), ptr(view), ptr(proj), ptr(ctx.radii), ptr(ctx.geom),
+                                       ptr(ctx.binning), ptr(ctx.img), ctx.num_rendered, ptr(grad_color), ptr(scratch), ptr(d_means3D),
+                                       ptr(d_colors), ptr(d_scales), ptr(d_rot), ptr(d_opac), ptr(d_m2d), ptr(d_sh), ptr(d_cov3D),
+                                       _stream()), "ga_raster_backward_ex")
+    if return_sh_cov3D:
+        return d_means3D, d_m2d, None if sh else d_colors, d_opac, d_scales, d_rot, d_sh, d_cov3D
     return d_means3D, d_m2d, d_colors, d_opac, d_scales, d_rot
 
 
@@ -295,13 +360,14 @@ def rasterize_batch(means3D, colors, scales, rotations, opacities, cams, bg, pla
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):
-        if sh.numel() != 0:
-            raise NotImplementedError("SH colour evaluation is not on GaussianAvatar's path (shs=None, "
-                                      "model/avatar_model.py:350); pass colors_precomp")
-        if cov3Ds_precomp.numel() != 0:
-            raise NotImplementedError("cov3D_precomp is not on GaussianAvatar's path (gaussian_renderer/__init__.py:37)")
-        means3D_c, colors_c, scales_c, rot_c = _c(means3D), _c(colors_precomp), _c(scales), _c(rotations)
-        color, radii, rctx = rasterize_forward(means3D_c, colors_c, opacities, scales_c, rot_c, raster_settings)
+        given = lambda t: t is not None and t.numel() != 0
+        sh = sh if given(sh) else None
+        cov3Ds_precomp = cov3Ds_precomp if given(cov3Ds_precomp) else None
+        colors_c = None if sh is not None else _c(colors_precomp)
+        scales_c, rot_c = (None, None) if cov3Ds_precomp is not None else (_c(scales), _c(rotations))
+        means3D_c = _c(means3D)
+        color, radii, rctx = rasterize_forward(means3D_c, colors_c, opacities, scales_c, rot_c, raster_settings, shs=sh,
+                                               cov3D_precomp=cov3Ds_precomp)
         ctx.rctx = rctx
         ctx.raster_settings = raster_settings
         ctx.save_for_backward(means3D_c, colors_c, scales_c, rot_c)
@@ -312,10 +378,11 @@ class _RasterizeGaussians(torch.autograd.Function):
     def backward(ctx, grad_color, _grad_radii):
         means3D, colors, scales, rotations = ctx.saved_tensors
         need = ctx.needs_input_grad
-        d_means3D, d_m2d, d_colors, d_opac, d_scales, d_rot = rasterize_backward(
+        d_means3D, d_m2d, d_colors, d_opac, d_scales, d_rot, d_sh, d_cov3D = rasterize_backward(
             ctx.rctx, means3D, colors, scales, rotations, ctx.raster_settings, grad_color,
-            want_opacity=need[4], want_rotations=need[6], want_means2D=need[1])
-        return (d_means3D, d_m2d, None, d_colors, d_opac, d_scales, d_rot, None, None)
+            want_opacity=need[4], want_rotations=need[6], want_means2D=need[1], return_sh_cov3D=True)
+        keep = lambda g, k: g if need[k] else None
+        return (d_means3D, d_m2d, keep(d_sh, 2), d_colors, d_opac, d_scales, d_rot, keep(d_cov3D, 7), None)
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):

@@ -83,6 +83,36 @@ int ga_raster_backward(const GaRasterSettings *s, const float *means3D, const fl
                        int64_t num_rendered, const float *dL_dout, void *scratch, float *d_means3D, float *d_colors,
                        float *d_scales, float *d_rotations, float *d_opacities, float *d_means2D, void *stream);
 
+/* The other colour and covariance inputs of upstream's API (per-frame path only).
+ * SH colours: rgb = max(sum_k basis_k(dir) shs[k] + 0.5, 0) per channel, dir = (mean - campos) / |mean - campos|, evaluated in
+ * stage 1 for the Gaussians that survive the culls into `rgb` (then passed as `colors` to ga_raster_forward_render), with the
+ * clamped channels recorded in `clamped` for the backward.  Precomputed covariances replace scales / rotations / scale_modifier. */
+typedef struct GaRasterColorCov {
+    const float *shs;            /* [P, sh_coeffs, 3] or NULL: colours are precomputed                     */
+    int32_t sh_degree, sh_coeffs;/* active degree 0..3; coefficients per Gaussian >= (sh_degree + 1)^2    */
+    const float *campos;         /* [3] device; required with shs                                          */
+    const float *cov3D_precomp;  /* [P, 6] (xx, xy, xz, yy, yz, zz) or NULL: Sigma from scales / rotations */
+    float *rgb;                  /* [P, 3] written by the forward, read by the backward (with shs)         */
+    uint8_t *clamped;            /* [P] bit c = channel c clamped (with shs)                               */
+} GaRasterColorCov;
+/* ga_raster_forward_preprocess with a colour / covariance descriptor (cc NULL: identical to it).  scales / rotations may be NULL
+ * with cov3D_precomp. */
+int ga_raster_forward_preprocess_ex(const GaRasterSettings *s, const GaRasterColorCov *cc, const float *means3D,
+                                    const float *scales, const float *rotations, const float *opacities,
+                                    const float *viewmatrix, const float *projmatrix, void *geom, void *img, int32_t *radii,
+                                    int64_t *num_rendered_host, void *stream);
+/* ga_raster_backward with the same descriptor as the forward (cc NULL: identical to it).  With shs: colors may be NULL, d_colors
+ * receives dL/drgb before the clamp mask, and d_sh [P, sh_coeffs, 3] is overwritten (0 for k >= (sh_degree + 1)^2, clamped
+ * channels and culled Gaussians); the direction term is included in d_means3D.  With cov3D_precomp: d_cov3D [P, 6] receives
+ * dL/dSigma (an off-diagonal entry stands for both symmetric entries); scales, rotations, d_scales, d_rotations may be NULL and are
+ * not written. */
+int ga_raster_backward_ex(const GaRasterSettings *s, const GaRasterColorCov *cc, const float *means3D, const float *colors,
+                          const float *scales, const float *rotations, const float *bg, const float *viewmatrix,
+                          const float *projmatrix, const int32_t *radii, const void *geom, const void *binning, const void *img,
+                          int64_t num_rendered, const float *dL_dout, void *scratch, float *d_means3D, float *d_colors,
+                          float *d_scales, float *d_rotations, float *d_opacities, float *d_means2D, float *d_sh, float *d_cov3D,
+                          void *stream);
+
 /* Batched API: the B <= 8 frames a training step renders (model/avatar_model.py:332-365 loops them) in ONE set of launches
  * and WITHOUT any host read-back, so a whole step can be captured in a CUDA graph.  All frames share H, W and P.
  * Arrays are [B,P,*] (rotations / opacities: [P,*] shared by every frame when the stride is 0); out_color [B,3,H,W];
