@@ -76,6 +76,10 @@ _SIGNATURES = {
     "ga_smpl_backward": (ctypes.c_int, [ctypes.c_int32] + [c_vp] * 8),
     "ga_lbs_forward": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_int64] + [c_vp] * 9),
     "ga_lbs_backward": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, ctypes.c_float, ctypes.c_int64] + [c_vp] * 11),
+    "ga_smplx_forward": (ctypes.c_int, [ctypes.c_int32] + [c_vp] * 8),
+    "ga_smplx_backward": (ctypes.c_int, [ctypes.c_int32] + [c_vp] * 9),
+    "ga_lbs_forward_ex": (ctypes.c_int, [ctypes.c_int32] * 4 + [ctypes.c_float, ctypes.c_int64] + [c_vp] * 9),
+    "ga_lbs_backward_ex": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float, ctypes.c_int64] + [c_vp] * 11),
     "ga_decoder_layout": (ctypes.c_int, [ctypes.POINTER(GaDecoderDesc), ctypes.POINTER(GaDecoderLayout)]),
     "ga_decoder_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(GaDecoderDesc)]),
     "ga_decoder_forward": (ctypes.c_int, [ctypes.POINTER(GaDecoderDesc)] + [c_vp] * 7),

@@ -1,6 +1,7 @@
 """`AvatarModel` with the reference's public surface (/root/reference model/avatar_model.py:19-649) over the fused
-sm_90a kernels: SMPL pose -> cano2live (one kernel), feature net (once per step), fused LBS + attribute assembly,
-tile rasterizer per frame.
+sm_90a kernels: SMPL / SMPL-X pose -> cano2live (one kernel), feature net (once per step), fused LBS + attribute assembly,
+tile rasterizer per frame.  `smpl_type='smplx'` (55 joints) takes the hand / face pose of every frame from the batch's
+`rest_pose` [B,99], as the reference does (model/avatar_model.py:279-289).
 
 Same methods / attributes as the reference: train_stage1, render_free_stage1, training_setup, zero_grad, step, save,
 load, stage_load, getTrainDataloader ..., `.net .pose .transl .geo_feature .model_path`.  Stage 2 (pose encoder U-Net,
@@ -23,7 +24,7 @@ import torch.nn as nn
 
 from .config import ModelParams, NetworkParams, OptimizationParams
 from .network import POP_no_unet
-from .ops import LbsAssemble, SmplCano2Live
+from .ops import LbsAssemble, SmplCano2Live, SmplxCano2Live
 from .renderer import render_batch
 
 
@@ -54,8 +55,8 @@ class AvatarModel:
             raise RuntimeError("AvatarModel runs on CUDA only (no CPU fallback)")
         self.batch_size = model_parms.batch_size if train else 1      # avatar_model.py:31-34
         assert model_parms.smpl_type in ["smplx", "smpl"]
-        if model_parms.smpl_type != "smpl":
-            raise NotImplementedError("only smpl_type='smpl' (24 joints, the reference default) is built")
+        self.smplx = model_parms.smpl_type == "smplx"
+        self.num_joints = 55 if self.smplx else 24
         if model_parms.train_stage not in (0, 1, 2):
             raise ValueError(f"train_stage {model_parms.train_stage} is not one of 1, 2")
 
@@ -75,17 +76,28 @@ class AvatarModel:
         rots = torch.zeros((N, 4), device=dev)
         rots[:, 0] = 1
         self.fix_rotation = rots
-        self._query_lbs = _assets["query_lbs"].to(dev).float().contiguous()            # [N,24], ONE copy for all frames
-        self.query_lbs = self._query_lbs[None].expand(self.batch_size, -1, -1)          # view only (reference materialises B copies, :86-87)
+        J = self.num_joints
+        lbs = _assets["query_lbs"].to(dev).float()
+        if tuple(lbs.shape) != (N, J):
+            raise ValueError(f"query_lbs {tuple(lbs.shape)}: expected [{N},{J}] for smpl_type={model_parms.smpl_type!r}")
+        if self.smplx:      # 220-byte rows -> 224: whole float4s for the LBS kernel's TMA copy and row reads (zero last column)
+            lbs = torch.nn.functional.pad(lbs, (0, 1))
+        self._query_lbs = lbs.contiguous()                                              # [N,24] / [N,56], ONE copy for all frames
+        self.query_lbs = self._query_lbs[None, :, :J].expand(self.batch_size, -1, -1)  # view only (reference materialises B copies, :86-87)
         cano = _assets["cano_joint_mats"].to(dev).float()
-        self._inv_cano = torch.linalg.inv(cano).contiguous()                            # [24,4,4]  avatar_model.py:89
+        if tuple(cano.shape) != (J, 4, 4) or tuple(_assets["rest_joints"].shape) != (J, 3):
+            raise ValueError(f"cano_joint_mats {tuple(cano.shape)} / rest_joints {tuple(_assets['rest_joints'].shape)}: expected [{J},4,4] / [{J},3]")
+        self._inv_cano = torch.linalg.inv(cano).contiguous()                            # [J,4,4]  avatar_model.py:89
         self.inv_mats = self._inv_cano[None].expand(self.batch_size, -1, -1, -1)
         self._rest_joints = _assets["rest_joints"].to(dev).float().contiguous()        # J(beta): constant per subject
         self.betas = _assets["betas"].to(dev).float()[None].expand(self.batch_size, -1) if "betas" in _assets else None
 
         self.train_dataset = _FrameSet(_frames) if isinstance(_frames, list) else _frames
         num_training_frames = _pose_data.shape[0]
-        self.pose = torch.nn.Embedding(num_training_frames, 72, _weight=_pose_data.clone().float(), sparse=True).to(dev)
+        pose_dim = 66 if self.smplx else 72          # SMPL-X: global + 21 body joints are trained, the rest comes with the frame
+        if _pose_data.shape[1] != pose_dim:
+            raise ValueError(f"pose data {tuple(_pose_data.shape)}: expected [F,{pose_dim}] for smpl_type={model_parms.smpl_type!r}")
+        self.pose = torch.nn.Embedding(num_training_frames, pose_dim, _weight=_pose_data.clone().float(), sparse=True).to(dev)
         self.transl = torch.nn.Embedding(num_training_frames, 3, _weight=_transl_data.clone().float(), sparse=True).to(dev)
         self.optimizer_pose = torch.optim.SparseAdam(list(self.pose.parameters()) + list(self.transl.parameters()), 5.0e-3)
         bg_color = [1, 1, 1] if model_parms.white_background else [0, 0, 0]
@@ -99,11 +111,13 @@ class AvatarModel:
     # ------------------------------------------------------------------------------------------------------------------
     @classmethod
     def from_assets(cls, assets, frames, pose_data, transl_data, batch_size=2, train=True, opt_parms=None, device="cuda"):
-        """assets: gaussianavatar_b200.synthetic.SyntheticAvatarAssets (or a dict with the same fields)."""
+        """assets: gaussianavatar_b200.synthetic.SyntheticAvatarAssets (or a dict with the same fields).  55 rest joints make an
+        SMPL-X model (its frames then carry `rest_pose`)."""
         if not isinstance(assets, dict):
             assets = dict(valid_idx=assets.valid_idx, query_points=assets.query_points, query_lbs=assets.query_lbs,
                           cano_joint_mats=assets.cano_joint_mats, rest_joints=assets.rest_joints, betas=assets.body.betas[0], S=assets.S)
-        mp = ModelParams(batch_size=batch_size, query_posmap_size=int(assets["S"]))
+        smpl_type = "smplx" if assets["rest_joints"].shape[0] == 55 else "smpl"
+        mp = ModelParams(batch_size=batch_size, query_posmap_size=int(assets["S"]), smpl_type=smpl_type)
         return cls(mp, NetworkParams(), opt_parms or OptimizationParams(), train=train, _assets=assets, _frames=frames,
                    _pose_data=pose_data, _transl_data=transl_data, device=device)
 
@@ -116,6 +130,8 @@ class AvatarModel:
         split = "train" if train else "test"
         dataset = MonoDataset_train(mp)
         S = int(mp.query_posmap_size)
+        if mp.smpl_type == "smplx":
+            return self._load_reference_assets_smplx(mp, split, dataset, S)
         mask = np.load(join(mp.project_path, "assets", "uv_masks", f"uv_mask{S}_with_faceid_smpl.npy")).reshape(S, S)
         valid = torch.from_numpy(mask != -1).reshape(-1)
         qmap = torch.from_numpy(np.load(join(mp.source_path, split, f"query_posemap_{S}_cano_smpl.npz"))[f"posmap{S}"]).reshape(-1, 3)
@@ -136,6 +152,23 @@ class AvatarModel:
         assets = dict(valid_idx=valid, query_points=qmap[valid].float(), query_lbs=lbs[valid].float(), cano_joint_mats=cano, rest_joints=rest,
                       betas=beta, S=S)
         return assets, dataset, pose, transl
+
+    def _load_reference_assets_smplx(self, mp, split, dataset, S):
+        """The SMPL-X branch of the folder contract (model/avatar_model.py:45-53): `uv_mask{S}_with_faceid_smplx.npy`,
+        `query_posemap_{S}_cano_smplx.npz`, `lbs_map_smplx_{S}.npy` [S*S,55], `smplx_cano_joint_mat.pth` [55,4,4], and the rest joints
+        from `SMPLX_{GENDER}.npz` under smplx_model_path (the shape directions past the 10 betas are expression: the reference passes
+        none, so they drop out)."""
+        from .synthetic import SMPLX_PARENTS
+        mask = np.load(join(mp.project_path, "assets", "uv_masks", f"uv_mask{S}_with_faceid_smplx.npy")).reshape(S, S)
+        valid = torch.from_numpy(mask != -1).reshape(-1)
+        qmap = torch.from_numpy(np.load(join(mp.source_path, split, f"query_posemap_{S}_cano_smplx.npz"))[f"posmap{S}"]).reshape(-1, 3)
+        lbs = torch.from_numpy(np.load(join(mp.project_path, "assets", f"lbs_map_smplx_{S}.npy"))).reshape(S * S, 55)
+        cano = torch.as_tensor(torch.load(join(mp.source_path, split, "smplx_cano_joint_mat.pth"), weights_only=False)).reshape(55, 4, 4).float()
+        beta = torch.as_tensor(dataset.smpl_data["beta"][0]).float()
+        rest = smplx_rest_joints(join(mp.smplx_model_path, f"SMPLX_{mp.smpl_gender.upper()}.npz"), beta, SMPLX_PARENTS)
+        assets = dict(valid_idx=valid, query_points=qmap[valid].float(), query_lbs=lbs[valid].float(), cano_joint_mats=cano, rest_joints=rest,
+                      betas=beta, S=S)
+        return assets, dataset, dataset.pose_data.float(), dataset.transl_data.float()
 
     # ------------------------------------------------------------------------------------------------------------------
     def net_set(self, mode):
@@ -273,15 +306,28 @@ class AvatarModel:
             self.optimizer_pose.step()
 
     # ------------------------------------------------------------------------------------------------------------------
-    def _posed_gaussians(self, idx, iteration, ramp=True):
-        """SMPL -> cano2live -> net (once) -> fused LBS/assembly.  Returns means3D, scales, colors [B,N,3] and dec_out."""
+    def _cano2live(self, pose_batch, transl_batch, rest_pose=None):
+        """[B,J,12] for the body model: SMPL from pose [B,72]; SMPL-X from pose [B,66] and the frames' rest_pose [B,99]."""
+        if not self.smplx:
+            return SmplCano2Live.apply(pose_batch, transl_batch, self._rest_joints, self._inv_cano)
+        B = pose_batch.shape[0]
+        if rest_pose is None:
+            raise ValueError("smpl_type='smplx': the batch has no 'rest_pose' (jaw, eyes and hands, [B,99])")
+        rest_pose = torch.as_tensor(rest_pose)
+        if rest_pose.dim() != 2 or tuple(rest_pose.shape) != (B, 99):
+            raise ValueError(f"smpl_type='smplx': rest_pose {tuple(rest_pose.shape)}, expected [{B},99] (jaw, eyes, 2 x 15 finger joints)")
+        rest_pose = rest_pose.to(device=self.device, dtype=torch.float32)
+        return SmplxCano2Live.apply(pose_batch, rest_pose, transl_batch, self._rest_joints, self._inv_cano)
+
+    def _posed_gaussians(self, idx, iteration, ramp=True, rest_pose=None):
+        """SMPL / SMPL-X -> cano2live -> net (once) -> fused LBS/assembly.  Returns means3D, scales, colors [B,N,3] and dec_out."""
         if getattr(self, "_detach_pose", False):      # pose optimisation inactive (epoch <= pose_op_start_iter): its gradients are never read
             pose_batch, transl_batch = self.pose.weight.detach()[idx], self.transl.weight.detach()[idx]
         else:
             pose_batch = self.pose(idx)
             transl_batch = self.transl(idx)
         B = pose_batch.shape[0]
-        cano2live = SmplCano2Live.apply(pose_batch, transl_batch, self._rest_joints, self._inv_cano)     # [B,24,12]
+        cano2live = self._cano2live(pose_batch, transl_batch, rest_pose)                                  # [B,J,12]
         S = int(self.model_parms.query_posmap_size)
         dec = self.net.forward_packed(self.geo_feature, S, B)                                             # [S*S, 8]
         scale_mul = 1e-3 * iteration if (ramp and iteration < 1000) else 1.0                              # avatar_model.py:316-319
@@ -396,7 +442,7 @@ class AvatarModel:
     def train_stage1(self, batch_data, iteration):
         """model/avatar_model.py:272-367: returns (images [B,3,H,W], full_pred [B,N,3], offset_loss, geo_loss, scale_loss)."""
         idx = batch_data["pose_idx"]
-        means, scales, colors, dec = self._posed_gaussians(idx, iteration)
+        means, scales, colors, dec = self._posed_gaussians(idx, iteration, rest_pose=batch_data.get("rest_pose"))
         # regularisers exactly as the reference forms them (avatar_model.py:328-330): mean over ALL S*S pixels of
         # (0.02 res)^2 (identical for every frame of the batch), mean of the repeated scales, mean of geo_feature^2
         offset_loss = torch.mean((dec[:, :3] * 0.02) ** 2)
@@ -412,7 +458,7 @@ class AvatarModel:
         them); no scale ramp in this stage."""
         inp = batch_data["inp_pos_map"].to(self.device).float()
         idx = batch_data["pose_idx"]
-        cano2live = SmplCano2Live.apply(self.pose(idx), self.transl(idx), self._rest_joints, self._inv_cano)
+        cano2live = self._cano2live(self.pose(idx), self.transl(idx), batch_data.get("rest_pose"))
         S = int(self.model_parms.query_posmap_size)
         pose_featmap = self.pose_encoder(inp)                                                         # [B,64,h,h]
         dec = self.net.forward_packed_frames(self.geo_feature, pose_featmap, S)                      # [B*S*S, 8]
@@ -443,7 +489,7 @@ class AvatarModel:
             idx = batch_data["pose_idx"]
             pose_batch, transl_batch = self.pose(idx), self.transl(idx)
         B = pose_batch.shape[0]
-        cano2live = SmplCano2Live.apply(pose_batch, transl_batch, self._rest_joints, self._inv_cano)
+        cano2live = self._cano2live(pose_batch, transl_batch, batch_data.get("rest_pose"))
         cached = getattr(self, "_dec_cache", None)
         if self.cache_decoder and not torch.is_grad_enabled() and cached is not None:
             dec = cached
@@ -462,3 +508,19 @@ class AvatarModel:
         """model/avatar_model.py:557-649: the stage-2 forward without the losses."""
         means, scales, colors, _, _ = self._stage2_gaussians(batch_data)
         return self._render_frames(batch_data, means, scales, colors)
+
+
+def smplx_rest_joints(npz_path, beta, parents) -> torch.Tensor:
+    """Rest joints J = J_regressor (v_template + shapedirs[:, :, :10] beta) [55,3] of an SMPLX_{GENDER}.npz.  The file's
+    kintree_table must be the SMPL-X tree the joint-transform kernel is built for."""
+    sm = np.load(npz_path, allow_pickle=True)
+    kt = np.asarray(sm["kintree_table"]).astype(np.int64)[0].copy()
+    kt[0] = -1
+    if kt.shape != (len(parents),) or not np.array_equal(kt, np.asarray(parents)):
+        raise ValueError(f"{npz_path}: kintree_table[0] is not the 55-joint SMPL-X tree this library is built for")
+    beta = torch.as_tensor(beta).double().reshape(-1)
+    v_t = torch.as_tensor(np.asarray(sm["v_template"])).double()
+    sd = torch.as_tensor(np.asarray(sm["shapedirs"])[:, :, :beta.numel()]).double()
+    Jr = sm["J_regressor"]
+    Jr = torch.as_tensor(np.asarray(Jr.todense() if hasattr(Jr, "todense") else Jr)).double()
+    return (Jr @ (v_t + torch.einsum("l,mkl->mk", beta, sd))).float()

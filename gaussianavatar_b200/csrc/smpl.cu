@@ -1,16 +1,52 @@
-// SMPL joint transforms -> canonical-to-live matrices, forward + backward, one warp per pose.
+// SMPL / SMPL-X joint transforms -> canonical-to-live matrices, forward + backward, one CTA per pose.
 //
 // Replaces `smpl_model.forward(...).A` followed by `torch.matmul(live_smpl.A, self.inv_mats)`
 // (/root/reference model/avatar_model.py:291-296), i.e. submodules/smplx/lbs.py:152-252 reduced to what feeds A:
 // Rodrigues with the shifted norm (:299-333), the 23-step kinematic chain (:349-405, a Python loop of ~150 tiny kernel
 // launches in the reference), `A = G - pad(G J)` (:402-403), `A[:, :, :3, 3] += transl` (body_models.py:380-383).
 // The rest joints J depend only on the (fixed) betas and are precomputed once on the host side.
+//
+// Both kernels are templates over the body model:
+//   SMPL    24 joints, all trainable (pose [B,72]); one warp per pose.
+//   SMPL-X  55 joints (global, 21 body, jaw, left / right eye, 15 + 15 finger joints), the first 22 trainable (pose [B,66]), the
+//           other 33 read from rest_pose [B,99] (jaw, eyes, hands: data, never differentiated); a 64-thread CTA per pose.
+//           The chain is 54 dependent 3x4 products walked in index order, a few microseconds with no bandwidth at stake.
 #include "common.cuh"
 
 namespace ga {
 namespace {
 
 __constant__ int c_parents[24] = {-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21};
+// SMPL-X kintree_table[0] (the asset loader checks the model file against this table)
+__constant__ int c_parents_x[55] = {-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 15, 15, 15, 20, 25,
+                                    26, 20, 28, 29, 20, 31, 32, 20, 34, 35, 20, 37, 38, 21, 40, 41, 21, 43, 44, 21, 46, 47, 21, 49, 50,
+                                    21, 52, 53};
+
+// kJ joints, the first kTrain of them from `pose` [B, 3 kTrain], the rest from `rest` [B, 3 (kJ - kTrain)]; kThreads per CTA
+template <int kJ> struct Body;
+template <> struct Body<24> { static constexpr int kTrain = 24, kThreads = 32; };
+template <> struct Body<55> { static constexpr int kTrain = 22, kThreads = 64; };
+
+template <int kJ> __device__ __forceinline__ int parent_of(int j) { return kJ == 24 ? c_parents[j] : c_parents_x[j]; }
+
+template <int kThreads> __device__ __forceinline__ void cta_sync()
+{
+    if constexpr (kThreads == 32) __syncwarp();
+    else __syncthreads();
+}
+
+// axis-angle of joint j of pose b
+template <int kJ> __device__ __forceinline__ void load_axis_angle(const float *__restrict__ pose, const float *__restrict__ rest, int b, int j, float r[3])
+{
+    constexpr int kT = Body<kJ>::kTrain;
+    if (kT == kJ || j < kT) {
+        r[0] = pose[(size_t)b * (kT * 3) + j * 3]; r[1] = pose[(size_t)b * (kT * 3) + j * 3 + 1]; r[2] = pose[(size_t)b * (kT * 3) + j * 3 + 2];
+    } else {
+        const int k = j - kT;
+        r[0] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3]; r[1] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3 + 1];
+        r[2] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3 + 2];
+    }
+}
 
 // 3x4 affine helpers (row-major, implicit last row 0 0 0 1)
 __device__ __forceinline__ void aff_mul(const float *A, const float *B, float *C)  // C = A * B
@@ -44,22 +80,25 @@ __device__ __forceinline__ void rodrigues(const float r[3], float R[9], float *t
     *theta_out = theta;
 }
 
-// One block (32 threads) per pose.  Lane j < 24 owns joint j for the per-joint steps; the chain itself is walked
+// One block (kThreads) per pose.  Thread j < kJ owns joint j for the per-joint steps; the chain itself is walked
 // in index order through shared memory (children always have a larger index than their parent).
-__global__ void __launch_bounds__(32)
+template <int kJ>
+__global__ void __launch_bounds__(Body<kJ>::kThreads)
 smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__ transl, const float *__restrict__ J,
-                const float *__restrict__ inv_cano /*[24,4,4]*/, float *__restrict__ C /*[B,24,12]*/,
-                float *__restrict__ G_out /*[B,24,12] saved for backward*/)
+                const float *__restrict__ inv_cano /*[kJ,4,4]*/, float *__restrict__ C /*[B,kJ,12]*/,
+                float *__restrict__ G_out /*[B,kJ,12] saved for backward*/, const float *__restrict__ rest /*[B,99] (SMPL-X)*/)
 {
+    constexpr int kThreads = Body<kJ>::kThreads;
     pdl_wait();
-    __shared__ float sL[24][12], sG[24][12];
+    __shared__ float sL[kJ][12], sG[kJ][12];
     const int b = blockIdx.x, j = threadIdx.x;
     if (b >= B) return;
-    if (j < 24) {
-        float r[3] = {pose[(size_t)b * 72 + j * 3], pose[(size_t)b * 72 + j * 3 + 1], pose[(size_t)b * 72 + j * 3 + 2]};
+    if (j < kJ) {
+        float r[3];
+        load_axis_angle<kJ>(pose, rest, b, j, r);
         float R[9], th;
         rodrigues(r, R, &th);
-        const int p = c_parents[j];
+        const int p = parent_of<kJ>(j);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             sL[j][k * 4 + 0] = R[k * 3 + 0]; sL[j][k * 4 + 1] = R[k * 3 + 1]; sL[j][k * 4 + 2] = R[k * 3 + 2];
@@ -70,13 +109,13 @@ smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
             for (int k = 0; k < 12; ++k) sG[0][k] = sL[0][k];
         }
     }
-    __syncwarp();
-    // 23 dependent 3x4 products: lane 0 walks the chain (latency ~ a few microseconds, B poses run in parallel CTAs)
-    for (int i = 1; i < 24; ++i) {
-        if (j == 0) aff_mul(sG[c_parents[i]], sL[i], sG[i]);
-        __syncwarp();
+    cta_sync<kThreads>();
+    // kJ - 1 dependent 3x4 products: thread 0 walks the chain (latency ~ a few microseconds, B poses run in parallel CTAs)
+    for (int i = 1; i < kJ; ++i) {
+        if (j == 0) aff_mul(sG[parent_of<kJ>(i)], sL[i], sG[i]);
+        cta_sync<kThreads>();
     }
-    if (j < 24) {
+    if (j < kJ) {
         float A[12];
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
@@ -86,7 +125,7 @@ smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
         }
         // cano2live = A * inv(A_cano)  (both affine)
         const float *Ic = inv_cano + j * 16;
-        float *Cj = C + ((size_t)b * 24 + j) * 12;
+        float *Cj = C + ((size_t)b * kJ + j) * 12;
 #pragma unroll
         for (int r = 0; r < 3; ++r)
 #pragma unroll
@@ -94,37 +133,40 @@ smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
                 float t = A[r * 4 + 0] * Ic[0 * 4 + c] + A[r * 4 + 1] * Ic[1 * 4 + c] + A[r * 4 + 2] * Ic[2 * 4 + c] + A[r * 4 + 3] * Ic[3 * 4 + c];
                 Cj[r * 4 + c] = t;
             }
-        float *Gj = G_out + ((size_t)b * 24 + j) * 12;
+        float *Gj = G_out + ((size_t)b * kJ + j) * 12;
 #pragma unroll
         for (int k = 0; k < 12; ++k) Gj[k] = sG[j][k];
     }
 }
 
-__global__ void __launch_bounds__(32)
+// d_pose [B, 3 kTrain] only: the rest_pose joints of SMPL-X are data.
+template <int kJ>
+__global__ void __launch_bounds__(Body<kJ>::kThreads)
 smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__ J, const float *__restrict__ inv_cano,
-                const float *__restrict__ G_saved, const float *__restrict__ dC /*[B,24,12]*/,
-                float *__restrict__ d_pose /*[B,72]*/, float *__restrict__ d_transl /*[B,3]*/)
+                const float *__restrict__ G_saved, const float *__restrict__ dC /*[B,kJ,12]*/,
+                float *__restrict__ d_pose /*[B,3 kTrain]*/, float *__restrict__ d_transl /*[B,3]*/, const float *__restrict__ rest)
 {
+    constexpr int kThreads = Body<kJ>::kThreads, kT = Body<kJ>::kTrain;
     pdl_wait();
-    __shared__ float sL[24][12], sG[24][12], sdG[24][12], sdL[24][9];
+    __shared__ float sL[kJ][12], sG[kJ][12], sdG[kJ][12], sdL[kJ][9];
     const int b = blockIdx.x, j = threadIdx.x;
     if (b >= B) return;
     float r[3] = {0.f, 0.f, 0.f}, R[9], theta = 1.f;
-    if (j < 24) {
-        r[0] = pose[(size_t)b * 72 + j * 3]; r[1] = pose[(size_t)b * 72 + j * 3 + 1]; r[2] = pose[(size_t)b * 72 + j * 3 + 2];
+    if (j < kJ) {
+        load_axis_angle<kJ>(pose, rest, b, j, r);
         rodrigues(r, R, &theta);
-        const int p = c_parents[j];
+        const int p = parent_of<kJ>(j);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             sL[j][k * 4 + 0] = R[k * 3 + 0]; sL[j][k * 4 + 1] = R[k * 3 + 1]; sL[j][k * 4 + 2] = R[k * 3 + 2];
             sL[j][k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
         }
-        const float *Gj = G_saved + ((size_t)b * 24 + j) * 12;
+        const float *Gj = G_saved + ((size_t)b * kJ + j) * 12;
 #pragma unroll
         for (int k = 0; k < 12; ++k) sG[j][k] = Gj[k];
         // dA[:3,:4] = dC[:3,:4] * inv_cano^T   (C = A * Ic, rows of A are 4-vectors)
         const float *Ic = inv_cano + j * 16;
-        const float *dCj = dC + ((size_t)b * 24 + j) * 12;
+        const float *dCj = dC + ((size_t)b * kJ + j) * 12;
         float dA[12];
 #pragma unroll
         for (int rr = 0; rr < 3; ++rr)
@@ -140,18 +182,18 @@ smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
             sdG[j][rr * 4 + 3] = dA[rr * 4 + 3];
         }
     }
-    __syncwarp();
+    cta_sync<kThreads>();
     // d transl = sum_j dA_t
     if (j == 0) {
         float t0 = 0.f, t1 = 0.f, t2 = 0.f;
-        for (int k = 0; k < 24; ++k) { t0 += sdG[k][3]; t1 += sdG[k][7]; t2 += sdG[k][11]; }
+        for (int k = 0; k < kJ; ++k) { t0 += sdG[k][3]; t1 += sdG[k][7]; t2 += sdG[k][11]; }
         d_transl[(size_t)b * 3 + 0] = t0; d_transl[(size_t)b * 3 + 1] = t1; d_transl[(size_t)b * 3 + 2] = t2;
     }
-    __syncwarp();
+    cta_sync<kThreads>();
     // reverse chain: G_i = G_p * L_i
     if (j == 0) {
-        for (int i = 23; i >= 1; --i) {
-            const int p = c_parents[i];
+        for (int i = kJ - 1; i >= 1; --i) {
+            const int p = parent_of<kJ>(i);
             const float *Gp = sG[p], *Li = sL[i], *dGi = sdG[i];
             // dL_R = Gp_R^T dGi_R ; (dL_t not needed: J is constant)
 #pragma unroll
@@ -173,8 +215,8 @@ smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
 #pragma unroll
             for (int c = 0; c < 3; ++c) sdL[0][a * 3 + c] = sdG[0][a * 4 + c];
     }
-    __syncwarp();
-    if (j < 24) {
+    cta_sync<kThreads>();
+    if (j < kT) {
         // Rodrigues backward.  R = I + s K + (1-c) K^2, K = skew(d), d = r/theta, theta = |r + 1e-8|
         const float *dR = sdL[j];
         const float dx = r[0] / theta, dy = r[1] / theta, dz = r[2] / theta;
@@ -206,9 +248,9 @@ smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
         dtheta += -(dd[0] * r[0] + dd[1] * r[1] + dd[2] * r[2]) / (theta * theta);
         const float nx = r[0] + 1e-8f, ny = r[1] + 1e-8f, nz = r[2] + 1e-8f;
         dr[0] += dtheta * nx / theta; dr[1] += dtheta * ny / theta; dr[2] += dtheta * nz / theta;
-        d_pose[(size_t)b * 72 + j * 3 + 0] = dr[0];
-        d_pose[(size_t)b * 72 + j * 3 + 1] = dr[1];
-        d_pose[(size_t)b * 72 + j * 3 + 2] = dr[2];
+        d_pose[(size_t)b * (kT * 3) + j * 3 + 0] = dr[0];
+        d_pose[(size_t)b * (kT * 3) + j * 3 + 1] = dr[1];
+        d_pose[(size_t)b * (kT * 3) + j * 3 + 2] = dr[2];
     }
 }
 
@@ -223,7 +265,7 @@ extern "C" int ga_smpl_forward(int32_t B, const float *pose, const float *transl
     GA_REQUIRE(B >= 0, "bad batch %d", B);
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && transl && rest_joints && inv_cano && cano2live && saved_G, "NULL pointer argument");
-    { ProfScope _ps("smpl_fwd_kernel", static_cast<cudaStream_t>(stream_)); launch_k(smpl_fwd_kernel, B, 32, 0, static_cast<cudaStream_t>(stream_), B, pose, transl, rest_joints, inv_cano, cano2live, saved_G); }
+    { ProfScope _ps("smpl_fwd_kernel", static_cast<cudaStream_t>(stream_)); launch_k(smpl_fwd_kernel<24>, B, 32, 0, static_cast<cudaStream_t>(stream_), B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, nullptr); }
     GA_CHECK_LAUNCH("smpl_fwd_kernel");
     return GA_OK;
 }
@@ -234,7 +276,31 @@ extern "C" int ga_smpl_backward(int32_t B, const float *pose, const float *rest_
     GA_REQUIRE(B >= 0, "bad batch %d", B);
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && rest_joints && inv_cano && saved_G && d_cano2live && d_pose && d_transl, "NULL pointer argument");
-    { ProfScope _ps("smpl_bwd_kernel", static_cast<cudaStream_t>(stream_)); launch_k(smpl_bwd_kernel, B, 32, 0, static_cast<cudaStream_t>(stream_), B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl); }
+    { ProfScope _ps("smpl_bwd_kernel", static_cast<cudaStream_t>(stream_)); launch_k(smpl_bwd_kernel<24>, B, 32, 0, static_cast<cudaStream_t>(stream_), B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, nullptr); }
     GA_CHECK_LAUNCH("smpl_bwd_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_smplx_forward(int32_t B, const float *pose, const float *rest_pose, const float *transl, const float *rest_joints,
+                                const float *inv_cano, float *cano2live, float *saved_G, void *stream_)
+{
+    GA_REQUIRE(B >= 0, "bad batch %d", B);
+    if (B == 0) return GA_OK;
+    GA_REQUIRE(pose && rest_pose && transl && rest_joints && inv_cano && cano2live && saved_G, "NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    { ProfScope _ps("smplx_fwd_kernel", stream); launch_k(smpl_fwd_kernel<55>, B, Body<55>::kThreads, 0, stream, B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, rest_pose); }
+    GA_CHECK_LAUNCH("smplx_fwd_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_smplx_backward(int32_t B, const float *pose, const float *rest_pose, const float *rest_joints, const float *inv_cano,
+                                 const float *saved_G, const float *d_cano2live, float *d_pose, float *d_transl, void *stream_)
+{
+    GA_REQUIRE(B >= 0, "bad batch %d", B);
+    if (B == 0) return GA_OK;
+    GA_REQUIRE(pose && rest_pose && rest_joints && inv_cano && saved_G && d_cano2live && d_pose && d_transl, "NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    { ProfScope _ps("smplx_bwd_kernel", stream); launch_k(smpl_bwd_kernel<55>, B, Body<55>::kThreads, 0, stream, B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, rest_pose); }
+    GA_CHECK_LAUNCH("smplx_bwd_kernel");
     return GA_OK;
 }

@@ -54,8 +54,40 @@ class SmplCano2Live(torch.autograd.Function):
         return d_pose, d_transl, None, None
 
 
+class SmplxCano2Live(torch.autograd.Function):
+    """SMPL-X: pose [B,66] (global + 21 body joints), rest_pose [B,99] (jaw, eyes, 2 x 15 finger joints), transl [B,3]
+    -> cano2live [B,55,12].  Gradients flow to pose and transl only: rest_pose is data (model/avatar_model.py:279-296)."""
+
+    @staticmethod
+    def forward(ctx, pose, rest_pose, transl, rest_joints, inv_cano):
+        _need_cuda(pose, "SmplxCano2Live")
+        pose, rest_pose, transl = _f32c(pose), _f32c(rest_pose), _f32c(transl)
+        B = pose.shape[0]
+        if tuple(pose.shape) != (B, 66) or tuple(rest_pose.shape) != (B, 99) or tuple(transl.shape) != (B, 3):
+            raise ValueError(f"SmplxCano2Live: pose {tuple(pose.shape)}, rest_pose {tuple(rest_pose.shape)}, transl {tuple(transl.shape)}; "
+                             f"expected [B,66], [B,99], [B,3]")
+        C = torch.empty(B, 55, 12, device=pose.device, dtype=torch.float32)
+        G = torch.empty(B, 55, 12, device=pose.device, dtype=torch.float32)
+        _lib.check(_lib.lib().ga_smplx_forward(B, ptr(pose), ptr(rest_pose), ptr(transl), ptr(rest_joints), ptr(inv_cano), ptr(C), ptr(G),
+                                               _stream()), "ga_smplx_forward")
+        ctx.save_for_backward(pose, rest_pose, rest_joints, inv_cano, G)
+        return C
+
+    @staticmethod
+    def backward(ctx, dC):
+        pose, rest_pose, rest_joints, inv_cano, G = ctx.saved_tensors
+        B = pose.shape[0]
+        dC = _f32c(dC)
+        d_pose = torch.empty_like(pose)
+        d_transl = torch.empty(B, 3, device=pose.device, dtype=torch.float32)
+        _lib.check(_lib.lib().ga_smplx_backward(B, ptr(pose), ptr(rest_pose), ptr(rest_joints), ptr(inv_cano), ptr(G), ptr(dC),
+                                                ptr(d_pose), ptr(d_transl), _stream()), "ga_smplx_backward")
+        return d_pose, None, d_transl, None, None
+
+
 class LbsAssemble(torch.autograd.Function):
-    """dec_out [S*S,8] (stage 1: one output for all frames) or [B*S*S,8] (stage 2: per frame), cano2live [B,24,12]
+    """dec_out [S*S,8] (stage 1: one output for all frames) or [B*S*S,8] (stage 2: per frame), cano2live [B,J,12] (J = 24 for SMPL,
+    55 for SMPL-X), query_lbs [N,ld] (ld = 24, or 56 for SMPL-X: the 55 weights and a zero column)
     -> means3D, scales, colors [B,N,3] (model/avatar_model.py:308-326 / :407-420)."""
 
     @staticmethod
@@ -63,6 +95,7 @@ class LbsAssemble(torch.autograd.Function):
         _need_cuda(dec_out, "LbsAssemble")
         dec_out, cano2live = _f32c(dec_out), _f32c(cano2live)
         N, B = int(query_points.shape[0]), int(cano2live.shape[0])
+        J, ld = int(cano2live.shape[1]), int(query_lbs.shape[1])
         stride = (dec_out.shape[0] // B) * 8 if per_frame else 0
         if per_frame and dec_out.shape[0] % B:
             raise RuntimeError("per-frame decoder output must have B * S*S rows")
@@ -70,8 +103,9 @@ class LbsAssemble(torch.autograd.Function):
         means = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
         scales = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
         colors = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
-        _lib.check(_lib.lib().ga_lbs_forward(N, B, float(scale_mul), stride, ptr(dec_out), ptr(valid_index), ptr(query_points), ptr(query_lbs),
-                                             ptr(cano2live), ptr(means), ptr(scales), ptr(colors), _stream()), "ga_lbs_forward")
+        _lib.check(_lib.lib().ga_lbs_forward_ex(N, B, J, ld, float(scale_mul), stride, ptr(dec_out), ptr(valid_index), ptr(query_points),
+                                                ptr(query_lbs), ptr(cano2live), ptr(means), ptr(scales), ptr(colors), _stream()),
+                   "ga_lbs_forward_ex")
         ctx.save_for_backward(dec_out, cano2live, valid_index, query_points, query_lbs)
         ctx.scale_mul, ctx.stride = float(scale_mul), stride
         return means, scales, colors
@@ -94,9 +128,10 @@ class LbsAssemble(torch.autograd.Function):
         d_means, d_scales, d_colors = z(d_means), z(d_scales), z(d_colors)
         d_dec = torch.empty_like(dec_out)
         dC = torch.empty_like(cano2live)
-        _lib.check(_lib.lib().ga_lbs_backward(N, B, int(dec_out.shape[0]), ctx.scale_mul, ctx.stride, ptr(dec_out), ptr(valid_index),
-                                              ptr(query_points), ptr(query_lbs), ptr(cano2live), ptr(d_means), ptr(d_scales),
-                                              ptr(d_colors), ptr(d_dec), ptr(dC), _stream()), "ga_lbs_backward")
+        J, ld = int(cano2live.shape[1]), int(query_lbs.shape[1])
+        _lib.check(_lib.lib().ga_lbs_backward_ex(N, B, J, ld, int(dec_out.shape[0]), ctx.scale_mul, ctx.stride, ptr(dec_out), ptr(valid_index),
+                                                 ptr(query_points), ptr(query_lbs), ptr(cano2live), ptr(d_means), ptr(d_scales),
+                                                 ptr(d_colors), ptr(d_dec), ptr(dC), _stream()), "ga_lbs_backward_ex")
         return d_dec, dC, None, None, None, None, None
 
 

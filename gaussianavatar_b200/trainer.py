@@ -38,7 +38,7 @@ def allreduce_gradients(grads, group=None):
 
 class _StepGraph:
     """One captured forward + loss + backward of a stage-1 step and its static input / output tensors."""
-    __slots__ = ("graph", "idx", "gt", "cams", "loss", "g_flat", "g_geo", "capacity", "plan", "states", "launches")
+    __slots__ = ("graph", "idx", "rest", "gt", "cams", "loss", "g_flat", "g_geo", "capacity", "plan", "states", "launches")
 
 
 class Stage1Trainer:
@@ -239,6 +239,11 @@ class Stage1Trainer:
         sb = dict(batch)
         sb.update(pose_idx=G.idx, original_image=G.gt, _cams=G.cams, height=m._scalar_list(batch["height"], B),
                   width=m._scalar_list(batch["width"], B))
+        # SMPL-X: the frames' hand / face pose is a step input like pose_idx; a replay must read this step's, not the captured one's
+        G.rest = None
+        if getattr(m, "smplx", False) and batch.get("rest_pose") is not None:
+            G.rest = torch.as_tensor(batch["rest_pose"]).to(device=dev, dtype=torch.float32).contiguous().clone()
+            sb["rest_pose"] = G.rest
         m._detach_pose = True
         run_backup = m.net.bn_running.clone()
         states = [(st, st.num_batches_tracked) for st in m.net._states.values()]
@@ -286,6 +291,11 @@ class Stage1Trainer:
         if G is None:
             G = self._capture(batch, iteration, epoch, key)
         G.idx.copy_(batch["pose_idx"], non_blocking=True)
+        if G.rest is not None:
+            rest = torch.as_tensor(batch["rest_pose"])
+            if tuple(rest.shape) != tuple(G.rest.shape):
+                raise ValueError(f"rest_pose {tuple(rest.shape)}: expected {tuple(G.rest.shape)}")
+            G.rest.copy_(rest, non_blocking=True)
         G.gt.copy_(batch["original_image"], non_blocking=True)
         G.cams.copy_(m._batch_cameras(batch, B, m.device))
         G.plan.bump_serial()

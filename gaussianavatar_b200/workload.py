@@ -27,15 +27,21 @@ def load_poses(num: int = 32):
 
 
 class Stage1Workload:
+    """body="smplx": the same workload on the synthetic 55-joint body; the body pose is the shipped poses' first 66 values and every
+    frame carries a synthetic hand / face pose (`rest_pose` [99]) in its batch."""
     def __init__(self, config: int = 3, frames_per_gpu: int = 2, device="cuda:0", seed: int = 0, N=None, S=None, side=None,
-                 inp_posmap_size: int = 128, num_frames: int = 32):
+                 inp_posmap_size: int = 128, num_frames: int = 32, body: str = "smpl"):
         cN, cS, cside = syn.CONFIGS[config]
         self.N, self.S, self.side = N or cN, S or cS, side or cside
         self.B = frames_per_gpu
         self.device = torch.device(device)
-        assets = syn.make_avatar_assets(self.N, self.S, seed=seed)
+        assets = syn.make_avatar_assets(self.N, self.S, seed=seed, body=body)
         pose, transl, self.pose_source = load_poses(num_frames)
         self.num_frames = pose.shape[0]
+        self.rest_dev = None
+        if body == "smplx":
+            pose = pose[:, :66].contiguous()
+            self.rest_dev = syn.synthetic_smplx_poses(self.num_frames, seed=seed)[1].to(self.device)
         cam = make_camera(scaled_intrinsics(TEST_POSE_K, self.side), TEST_POSE_EXTRINSIC, self.side, self.side)
         self.cam = cam
         frames = [dict(pose_idx=i) for i in range(self.num_frames)]
@@ -73,6 +79,8 @@ class Stage1Workload:
             while idx.numel() < self.B:
                 idx = torch.cat([idx, idx[-1:]])
             batch = dict(pose_idx=idx, **self.camera_fields(self.B))
+            if self.rest_dev is not None:
+                batch["rest_pose"] = self.rest_dev[idx]
             imgs.append(m.render_free_stage1(batch, 59400)[: min(self.B, self.num_frames - f0)].clone())
         m.geo_feature.data.copy_(geo_backup)
         m.net.bn_running.copy_(run_backup)
@@ -98,7 +106,10 @@ class Stage1Workload:
         idx = cache[key]
         B = len(ids)
         img = self.gt_dev[ids[0]:ids[0] + B] if all(ids[j] == ids[0] + j for j in range(B)) else self.gt_dev[idx]     # a view when contiguous
-        return dict(pose_idx=idx, original_image=img, **self.camera_fields(B))
+        out = dict(pose_idx=idx, original_image=img, **self.camera_fields(B))
+        if self.rest_dev is not None:
+            out["rest_pose"] = self.rest_dev[idx]
+        return out
 
     def host_batch(self, ids):
         """The same batch as HOST tensors (pinned), as a DataLoader would hand it over (train.py:63-66)."""

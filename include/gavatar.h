@@ -174,6 +174,14 @@ int ga_smpl_forward(int32_t B, const float *pose, const float *transl, const flo
                     float *cano2live, float *saved_G, void *stream);
 int ga_smpl_backward(int32_t B, const float *pose, const float *rest_joints, const float *inv_cano, const float *saved_G,
                      const float *d_cano2live, float *d_pose, float *d_transl, void *stream);
+/* SMPL-X (55 joints: global, 21 body, jaw, left / right eye, 15 left-hand, 15 right-hand).  pose [B,66] holds the 22 trainable
+ * joints, rest_pose [B,99] the other 33 (model/avatar_model.py:279-289; flat_hand_mean=True, no PCA, no expression).
+ * rest_joints [55,3], inv_cano [55,4,4] -> cano2live [B,55,12]; saved_G [B,55,12].  The backward writes d_pose [B,66] and
+ * d_transl [B,3]; rest_pose gets no gradient. */
+int ga_smplx_forward(int32_t B, const float *pose, const float *rest_pose, const float *transl, const float *rest_joints,
+                     const float *inv_cano, float *cano2live, float *saved_G, void *stream);
+int ga_smplx_backward(int32_t B, const float *pose, const float *rest_pose, const float *rest_joints, const float *inv_cano,
+                      const float *saved_G, const float *d_cano2live, float *d_pose, float *d_transl, void *stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Fused Gaussian LBS + attribute assembly (model/avatar_model.py:308-326).  dec_out [S*S,8] pixel-major packed decoder
@@ -192,6 +200,16 @@ int ga_lbs_backward(int32_t N, int32_t B, int32_t num_pixels, float scale_mul, i
                     const int32_t *valid_index, const float *query_points, const float *query_lbs, const float *cano2live,
                     const float *d_means3D, const float *d_scales3, const float *d_colors, float *d_dec_out,
                     float *d_cano2live, void *stream);
+/* The same for either body model: num_joints 24 (SMPL) or 55 (SMPL-X); query_lbs is [N, lbs_ld] with lbs_ld a multiple of 4 and
+ * >= num_joints (the columns past num_joints are ignored); cano2live / d_cano2live are [B, num_joints, 12].  Built layouts:
+ * (24, 24) and (55, 56); ga_lbs_forward / ga_lbs_backward are the (24, 24) case. */
+int ga_lbs_forward_ex(int32_t N, int32_t B, int32_t num_joints, int32_t lbs_ld, float scale_mul, int64_t dec_frame_stride,
+                      const float *dec_out, const int32_t *valid_index, const float *query_points, const float *query_lbs,
+                      const float *cano2live, float *means3D, float *scales3, float *colors, void *stream);
+int ga_lbs_backward_ex(int32_t N, int32_t B, int32_t num_joints, int32_t lbs_ld, int32_t num_pixels, float scale_mul,
+                       int64_t dec_frame_stride, const float *dec_out, const int32_t *valid_index, const float *query_points,
+                       const float *query_lbs, const float *cano2live, const float *d_means3D, const float *d_scales3,
+                       const float *d_colors, float *d_dec_out, float *d_cano2live, void *stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Stage-1 feature net (model/network.py:39-83; model/modules.py:114-137,508-582,745-754): geometry convs -> bilinear
