@@ -54,6 +54,11 @@ class GaDecoderViews(ctypes.Structure):
     _fields_ = [(n, c_vp) for n in ("conv3_nhwc", "feat", "y1", "y5", "bn_mean", "bn_rstd", "d_feat")]
 
 
+class GaLpipsViews(ctypes.Structure):
+    _fields_ = [("relu", c_vp * 5), ("pool", c_vp * 2), ("pool_arg", c_vp * 2), ("partials", c_vp), ("in_scale", c_vp),
+                ("dz", c_vp * 5), ("dnext", c_vp * 4), ("dpool", c_vp * 2)]
+
+
 # name -> (restype, argtypes); every symbol include/gavatar.h declares must be listed here (tests check both ways)
 _SIGNATURES = {
     "ga_version": (ctypes.c_int, []),
@@ -108,6 +113,11 @@ _SIGNATURES = {
     "ga_rasterb_backward": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc)] + [c_vp] * 19),
     "ga_tc_conv5x5": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, c_vp, c_vp, c_vp, ctypes.c_int32, c_vp]),
     "ga_round_tf32": (ctypes.c_int, [c_vp, c_vp, ctypes.c_int64, c_vp]),
+    "ga_lpips_weights_floats": (ctypes.c_size_t, []),
+    "ga_lpips_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 3),
+    "ga_lpips_forward": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp] * 3 + [ctypes.c_float] * 2 + [c_vp] * 3),
+    "ga_lpips_backward": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp] * 5),
+    "ga_lpips_views": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp, ctypes.POINTER(GaLpipsViews)]),
 }
 
 _lib = None

@@ -1,4 +1,4 @@
-"""Stage-1 training step — the loop body of the reference's train.py:66-97 (before LPIPS starts at epoch 30) — over the
+"""Stage-1 training step — the loop body of the reference's train.py:66-97 (LPIPS from epoch 31 on when an `LPIPS` is given) — over the
 fused kernels, with optional frame-level data parallelism (one process per GPU; the only collective is one all-reduce of
 the shared feature-net / geo_feature gradients, SURVEY.md §8e).
 
@@ -12,6 +12,7 @@ import torch
 import torch.distributed as dist
 
 from .losses import image_loss
+from .lpips import LPIPS
 from .optim import FusedAdam
 
 
@@ -45,8 +46,8 @@ class Stage1Trainer:
     """The loop body of train.py:66-97 for either training stage (the name dates from when only stage 1 existed; `AvatarTrainer` is an alias)."""
     def __init__(self, model, fused_adam: bool = True, process_group=None, use_graph=None, perceptual_loss=None):
         self.model = model
-        # train.py:26,89-91: after `lpips_start_iter` epochs the reference adds lambda_lpips * LPIPS((image-0.5)*2, (gt-0.5)*2).  LPIPS is
-        # an external pretrained network (out of scope, SURVEY.md §2 #6): pass any callable(image, gt) -> scalar here to get the term
+        # train.py:26,89-91: after `lpips_start_iter` epochs the reference adds lambda_lpips * LPIPS((image-0.5)*2, (gt-0.5)*2).  Pass an
+        # `lpips.LPIPS` (the library's kernels; the step stays graphable) or any callable(image, gt) -> scalar (run eagerly) to get the term
         self.perceptual_loss = perceptual_loss
         self._warned_lpips = False
         # whole-step CUDA graph (forward + loss + backward in ONE launch; all-reduce and Adam follow eagerly): on unless GA_STEP_GRAPH=0
@@ -90,7 +91,11 @@ class Stage1Trainer:
         if epoch > o.lpips_start_iter:                   # train.py:89-91
             if self.perceptual_loss is not None:
                 gt = batch["original_image"]
-                loss = loss + o.lambda_lpips * torch.mean(self.perceptual_loss((image - 0.5) * 2, (gt - 0.5) * 2))
+                if isinstance(self.perceptual_loss, LPIPS):      # (x - 0.5) * 2 folded into the kernels' input affine
+                    lp = self.perceptual_loss(image, gt, normalize=True)
+                else:
+                    lp = self.perceptual_loss((image - 0.5) * 2, (gt - 0.5) * 2)
+                loss = loss + o.lambda_lpips * torch.mean(lp)
             elif not self._warned_lpips:
                 import warnings
                 warnings.warn(f"epoch {epoch} > lpips_start_iter {o.lpips_start_iter}: the reference adds lambda_lpips * LPIPS from here on "
@@ -224,7 +229,7 @@ class Stage1Trainer:
         img = batch.get("original_image")
         return (self.use_graph and isinstance(m.optimizer, FusedAdam) and getattr(m.model_parms, "train_stage", 1) != 2
                 and iteration >= 1000 and epoch <= self.opt.pose_op_start_iter
-                and not (self.perceptual_loss is not None and epoch > self.opt.lpips_start_iter)
+                and not (self.perceptual_loss is not None and not isinstance(self.perceptual_loss, LPIPS) and epoch > self.opt.lpips_start_iter)
                 and torch.is_tensor(img) and img.is_cuda and img.shape[0] <= 8 and os.environ.get("GA_RASTER_BATCHED", "1") != "0"
                 and m._uniform_frames(batch, img.shape[0]))
 
@@ -284,7 +289,8 @@ class Stage1Trainer:
         m, o = self.model, self.opt
         B = batch["original_image"].shape[0]
         wdecay_rgl = adjust_loss_weights(o.lambda_rgl, epoch, mode="decay", start=self.epoch_start, every=20)
-        key = (B, tuple(batch["original_image"].shape[-2:]), float(wdecay_rgl))
+        lpips_active = self.perceptual_loss is not None and epoch > o.lpips_start_iter
+        key = (B, tuple(batch["original_image"].shape[-2:]), float(wdecay_rgl), lpips_active)
         G = self._graphs.get(key)
         if G is not None and G.capacity != G.plan.capacity:      # the rasterizer's buffers were re-allocated: the graph points at freed memory
             G = None

@@ -21,6 +21,7 @@
  *                                                                                    model/network.py:39-83, model/modules.py:114-137,508-582
  *   ga_loss_*            l1_loss_w + ssim                                            utils/loss_utils.py:7-53
  *   ga_adam_*            torch.optim.Adam step on net + geo_feature                  model/avatar_model.py:148-155,264-267
+ *   ga_lpips_*           lpips.LPIPS(net='alex')((image-0.5)*2, (gt_image-0.5)*2)     train.py:26,89-91
  */
 #ifndef GAVATAR_H_
 #define GAVATAR_H_
@@ -305,6 +306,39 @@ int ga_tc_linear_backward_ex(int32_t M, const float *dZ, const float *Y, int32_t
 int ga_tc_conv5x5(int32_t mode, int32_t Hf, const float *in, const float *w, float *out, int32_t round_out, void *stream);
 /* out[i] = in[i] rounded to TF32 (nearest, ties away; low 13 mantissa bits cleared).  n % 4 == 0; in-place allowed. */
 int ga_round_tf32(const float *in, float *out, int64_t n, void *stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * LPIPS perceptual distance, lpips.LPIPS(net='alex', version='0.1') in eval mode (train.py:89-91), forward and the gradient
+ * with respect to in0.  Images planar fp32 [B,3,H,W], H, W >= 31; the network sees in * in_scale + in_shift (lpips's range
+ * [-1,1]: 1, 0; images in [0,1]: 2, -1) through its scaling layer.  out[B] (device) = the distance per image pair.
+ * Convolutions run TF32 with fp32 accumulation; nothing uses atomics, so both calls are bit-reproducible.
+ *
+ * weights: ga_lpips_weights_floats() device floats, 16-byte aligned, in this order (each block contiguous, row-major):
+ *   for l = 1..5:  W_l  [C_out][tap][C_in]  (tap = ky * k + kx; conv1: [64][384] with index tap * 3 + c, zero from 363 on)
+ *                  b_l  [C_out]
+ *   for l = 2..5:  Wd_l [C_in][tap'][C_out] with tap' = (k-1-ky) * k + (k-1-kx)   (data gradient: flipped, transposed)
+ *   for l = 1..5:  lin_l [C_out]   (the lin layers' 1x1 weights)
+ *   with (C_in, C_out, k) = (3, 64, 11), (64, 192, 5), (192, 384, 3), (384, 256, 3), (256, 256, 3).
+ * workspace: ga_lpips_workspace_bytes(B, H, W) bytes, 256-byte aligned; a forward leaves in it what its backward reads.
+ * g[B] (device): dL/d out.  d_in0 [B,3,H,W] is overwritten.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct GaLpipsViews {
+    float *relu[5];          /* relu_k maps NHWC [2B][H_k][W_k][C_k]: images 0..B-1 from in0, B..2B-1 from in1 */
+    float *pool[2];          /* max-pool outputs NHWC [2B][..][..][C] (before conv2, conv3) */
+    uint8_t *pool_arg[2];    /* window index 0..8 each pool output took */
+    float *partials;         /* [5][B][128] per-CTA distance sums */
+    float *in_scale;         /* in_scale of the last forward */
+    float *dz[5];            /* backward: gradient at conv_k's output (before ReLU), NHWC [B][H_k][W_k][C_k] */
+    float *dnext[4];         /* gradient reaching relu_k from slice k+1 (conv_{k+1} data gradient, un-pooled for k < 2) */
+    float *dpool[2];         /* data gradients of conv2, conv3 at the pool outputs */
+} GaLpipsViews;
+size_t ga_lpips_weights_floats(void);
+size_t ga_lpips_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int ga_lpips_forward(int32_t B, int32_t H, int32_t W, const float *weights, const float *in0, const float *in1, float in_scale,
+                     float in_shift, void *workspace, float *out, void *stream);
+int ga_lpips_backward(int32_t B, int32_t H, int32_t W, const float *weights, void *workspace, const float *g, float *d_in0, void *stream);
+/* The workspace regions above (for tests and inspection). */
+int ga_lpips_views(int32_t B, int32_t H, int32_t W, void *workspace, GaLpipsViews *out);
 
 #ifdef __cplusplus
 }
