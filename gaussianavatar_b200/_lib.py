@@ -85,7 +85,10 @@ _SIGNATURES = {
     "ga_smplx_backward": (ctypes.c_int, [ctypes.c_int32] + [c_vp] * 9),
     "ga_lbs_forward_ex": (ctypes.c_int, [ctypes.c_int32] * 4 + [ctypes.c_float, ctypes.c_int64] + [c_vp] * 9),
     "ga_lbs_backward_ex": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float, ctypes.c_int64] + [c_vp] * 11),
-    "ga_decoder_layout": (ctypes.c_int, [ctypes.POINTER(GaDecoderDesc), ctypes.POINTER(GaDecoderLayout)]),
+    "ga_smpl_vertices": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 8),
+    "ga_posmap_layout": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 4),
+    "ga_posmap_fill": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp] * 6),
+    "ga_decoder_layout":(ctypes.c_int, [ctypes.POINTER(GaDecoderDesc), ctypes.POINTER(GaDecoderLayout)]),
     "ga_decoder_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(GaDecoderDesc)]),
     "ga_decoder_forward": (ctypes.c_int, [ctypes.POINTER(GaDecoderDesc)] + [c_vp] * 7),
     "ga_decoder_backward": (ctypes.c_int, [ctypes.POINTER(GaDecoderDesc)] + [c_vp] * 8),

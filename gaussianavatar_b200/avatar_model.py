@@ -59,6 +59,9 @@ class AvatarModel:
         self.num_joints = 55 if self.smplx else 24
         if model_parms.train_stage not in (0, 1, 2):
             raise ValueError(f"train_stage {model_parms.train_stage} is not one of 1, 2")
+        self.posmap_from_pose = model_parms.train_stage == 2 and bool(getattr(model_parms, "inp_posmap_from_pose", False))
+        if self.posmap_from_pose and self.smplx:
+            raise NotImplementedError("inp_posmap_from_pose: device position maps are built for the SMPL mesh only (smpl_type='smpl')")
 
         if _assets is None:
             _assets, _frames, _pose_data, _transl_data = self._load_reference_assets(model_parms, train)
@@ -107,18 +110,28 @@ class AvatarModel:
         self.cache_decoder = not train     # inference models evaluate the frame-invariant stage-1 net once (see render_free_stage1)
         self._dec_cache = None
         self.net_set(model_parms.train_stage)
+        self.pose_mapper = None
+        if self.posmap_from_pose:         # stage-2 input maps from the pose, on the device (posmap.py)
+            from .posmap import PoseMapper
+            if "smpl_mesh" not in _assets or "uv_template" not in _assets:
+                raise ValueError("inp_posmap_from_pose: the assets carry no 'smpl_mesh' / 'uv_template' (the SMPL mesh model and its UV template)")
+            self.pose_mapper = PoseMapper(_assets["smpl_mesh"], _assets["betas"], _assets["uv_template"], int(model_parms.inp_posmap_size),
+                                          device=dev)
 
     # ------------------------------------------------------------------------------------------------------------------
     @classmethod
-    def from_assets(cls, assets, frames, pose_data, transl_data, batch_size=2, train=True, opt_parms=None, device="cuda"):
+    def from_assets(cls, assets, frames, pose_data, transl_data, batch_size=2, train=True, opt_parms=None, device="cuda", net_parms=None,
+                    **model_fields):
         """assets: gaussianavatar_b200.synthetic.SyntheticAvatarAssets (or a dict with the same fields).  55 rest joints make an
-        SMPL-X model (its frames then carry `rest_pose`)."""
+        SMPL-X model (its frames then carry `rest_pose`).  model_fields override ModelParams fields (e.g. train_stage=2,
+        inp_posmap_size, inp_posmap_from_pose=True; the last needs the dict keys `smpl_mesh`, the SMPL_{GENDER}.pkl fields, and
+        `uv_template`, a path or what posmap.load_uv_template_obj returns)."""
         if not isinstance(assets, dict):
             assets = dict(valid_idx=assets.valid_idx, query_points=assets.query_points, query_lbs=assets.query_lbs,
                           cano_joint_mats=assets.cano_joint_mats, rest_joints=assets.rest_joints, betas=assets.body.betas[0], S=assets.S)
         smpl_type = "smplx" if assets["rest_joints"].shape[0] == 55 else "smpl"
-        mp = ModelParams(batch_size=batch_size, query_posmap_size=int(assets["S"]), smpl_type=smpl_type)
-        return cls(mp, NetworkParams(), opt_parms or OptimizationParams(), train=train, _assets=assets, _frames=frames,
+        mp = ModelParams(batch_size=batch_size, query_posmap_size=int(assets["S"]), smpl_type=smpl_type, **model_fields)
+        return cls(mp, net_parms or NetworkParams(), opt_parms or OptimizationParams(), train=train, _assets=assets, _frames=frames,
                    _pose_data=pose_data, _transl_data=transl_data, device=device)
 
     def _load_reference_assets(self, mp, train):
@@ -151,6 +164,16 @@ class AvatarModel:
         transl = dataset.transl_data.float()
         assets = dict(valid_idx=valid, query_points=qmap[valid].float(), query_lbs=lbs[valid].float(), cano_joint_mats=cano, rest_joints=rest,
                       betas=beta, S=S)
+        if mp.train_stage == 2 and getattr(mp, "inp_posmap_from_pose", False):
+            # the mesh comes from the same SMPL_{GENDER}.pkl as the rest joints; the UV template from where the reference's scripts read it
+            from .posmap import SMPL_MESH_FIELDS
+            missing = [k for k in SMPL_MESH_FIELDS if k not in sm]
+            if missing:
+                raise ValueError(f"{f.name}: no {', '.join(missing)}; inp_posmap_from_pose needs the full SMPL mesh model")
+            template = join(mp.project_path, "assets", "template_mesh_smpl_uv.obj")
+            if not os.path.exists(template):
+                raise FileNotFoundError(f"inp_posmap_from_pose: UV template {template} not found")
+            assets.update(smpl_mesh=sm, uv_template=template)
         return assets, dataset, pose, transl
 
     def _load_reference_assets_smplx(self, mp, split, dataset, S):
@@ -456,7 +479,8 @@ class AvatarModel:
         """Stage 2 (model/avatar_model.py:369-420 / :557-612): the pose encoder turns each frame's posed-body position map into a
         feature map that is ADDED to the geometry features, so the decoder runs per frame (B*S*S rows, BatchNorm statistics over all of
         them); no scale ramp in this stage."""
-        inp = batch_data["inp_pos_map"].to(self.device).float()
+        inp = batch_data.get("inp_pos_map")
+        inp = self._pose_map(batch_data) if inp is None else inp.to(self.device).float()
         idx = batch_data["pose_idx"]
         cano2live = self._cano2live(self.pose(idx), self.transl(idx), batch_data.get("rest_pose"))
         S = int(self.model_parms.query_posmap_size)
@@ -464,6 +488,19 @@ class AvatarModel:
         dec = self.net.forward_packed_frames(self.geo_feature, pose_featmap, S)                      # [B*S*S, 8]
         means, scales, colors = LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, 1.0, True)
         return means, scales, colors, dec, pose_featmap
+
+    def _pose_map(self, batch_data):
+        """Input position maps [B,3,s,s] of a batch that carries none: from its `pose_data` / `transl_data` when it has them (test,
+        novel pose), else from the model's pose / transl rows at `pose_idx` (in stage 2 those are smpl_parms_pred.pth, never stepped)."""
+        if self.pose_mapper is None:
+            raise KeyError("inp_pos_map: the batch has no stage-2 input position map (set ModelParams.inp_posmap_from_pose to build it "
+                           "from the pose)")
+        if "pose_data" in batch_data:
+            pose, transl = batch_data["pose_data"], batch_data["transl_data"]
+        else:
+            idx = torch.as_tensor(batch_data["pose_idx"], device=self.device).long()
+            pose, transl = self.pose.weight.detach()[idx], self.transl.weight.detach()[idx]
+        return self.pose_mapper(pose, transl)
 
     def train_stage2(self, batch_data, iteration):
         """model/avatar_model.py:369-463: returns (images [B,3,H,W], full_pred [B,N,3], pose_loss, offset_loss)."""

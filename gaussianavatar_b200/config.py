@@ -29,6 +29,9 @@ class ModelParams:
     batch_size: int = 2
     query_posmap_size: int = 512
     inp_posmap_size: int = 128
+    # stage 2: build each frame's input position map on the device from its SMPL pose instead of reading inp_map/*.npz
+    # (not a reference option; read with getattr(..., False) so the reference's own namespaces keep working)
+    inp_posmap_from_pose: bool = False
 
 
 @dataclass

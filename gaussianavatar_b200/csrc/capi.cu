@@ -95,6 +95,6 @@ extern "C" int ga_profile_report(char *buf, size_t cap)
     return GA_OK;
 }
 
-extern "C" int ga_version(void) { return 102; }
+extern "C" int ga_version(void) { return 103; }
 extern "C" const char *ga_last_error(void) { return ga::g_err; }
 extern "C" long long ga_launch_count(void) { return ga::g_launches.load(std::memory_order_relaxed); }

@@ -12,6 +12,7 @@
 //           other 33 read from rest_pose [B,99] (jaw, eyes, hands: data, never differentiated); a 64-thread CTA per pose.
 //           The chain is 54 dependent 3x4 products walked in index order, a few microseconds with no bandwidth at stake.
 #include "common.cuh"
+#include "smpl_math.cuh"
 
 namespace ga {
 namespace {
@@ -46,38 +47,6 @@ template <int kJ> __device__ __forceinline__ void load_axis_angle(const float *_
         r[0] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3]; r[1] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3 + 1];
         r[2] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3 + 2];
     }
-}
-
-// 3x4 affine helpers (row-major, implicit last row 0 0 0 1)
-__device__ __forceinline__ void aff_mul(const float *A, const float *B, float *C)  // C = A * B
-{
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            float t = A[r * 4 + 0] * B[0 * 4 + c] + A[r * 4 + 1] * B[1 * 4 + c] + A[r * 4 + 2] * B[2 * 4 + c];
-            if (c == 3) t += A[r * 4 + 3];
-            C[r * 4 + c] = t;
-        }
-    }
-}
-
-__device__ __forceinline__ void rodrigues(const float r[3], float R[9], float *theta_out)
-{
-    const float nx = r[0] + 1e-8f, ny = r[1] + 1e-8f, nz = r[2] + 1e-8f;
-    const float theta = sqrtf(nx * nx + ny * ny + nz * nz);
-    const float dx = r[0] / theta, dy = r[1] / theta, dz = r[2] / theta;
-    float s, c;
-    sincosf(theta, &s, &c);
-    const float K[9] = {0.f, -dz, dy, dz, 0.f, -dx, -dy, dx, 0.f};
-    float K2[9];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) K2[i * 3 + j] = K[i * 3] * K[j] + K[i * 3 + 1] * K[3 + j] + K[i * 3 + 2] * K[6 + j];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) R[i] = ((i % 4 == 0) ? 1.f : 0.f) + s * K[i] + (1.f - c) * K2[i];
-    *theta_out = theta;
 }
 
 // One block (kThreads) per pose.  Thread j < kJ owns joint j for the per-joint steps; the chain itself is walked

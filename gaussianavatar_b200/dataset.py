@@ -111,6 +111,11 @@ class _MonoFolder(Dataset):
     def __len__(self):
         return self.data_length
 
+    def _reads_inp_map(self):
+        """Stage 2 reads inp_map/ unless the model builds the maps from the pose (ModelParams.inp_posmap_from_pose)."""
+        p = self.dataset_parms
+        return p.train_stage == 2 and not getattr(p, "inp_posmap_from_pose", False)
+
     def _inp_posmap(self, pose_idx):
         S = self.dataset_parms.inp_posmap_size
         d = np.load(join(self.data_folder, "inp_map", "inp_posemap_%s_%s.npz" % (str(S), str(pose_idx).zfill(8))))
@@ -142,7 +147,7 @@ class MonoDataset_train(_MonoFolder):
     def __getitem__(self, index, ignore_list=None):
         pose_idx, name = self.name_list[index]
         item, width, height = self._image_item(name)
-        if self.dataset_parms.train_stage == 2:
+        if self._reads_inp_map():
             item["inp_pos_map"] = self._inp_posmap(pose_idx)
         K, E = self._camera(name)
         item.update(camera_item(K, E, height, width, self.znear, self.zfar))
@@ -177,7 +182,7 @@ class MonoDataset_novel_pose(_MonoFolder):
 
     def __getitem__(self, index, ignore_list=None):
         item = {}
-        if self.dataset_parms.train_stage == 2:
+        if self._reads_inp_map():
             item["inp_pos_map"] = self._inp_posmap(index)
         item.update(camera_item(self.intrinsic, self.extr_npy, 1024, 1024, self.znear, self.zfar))         # size hard-coded at :492
         item.update(pose_idx=index, pose_data=self.pose_data[index], transl_data=self.transl_data[index])
@@ -243,7 +248,7 @@ class MonoDataset_novel_view(_MonoFolder):
         width, height = Image.open(join(self.data_folder, "images", name + "." + self.image_fix)).size
         E = rotate_camera_by_frame_idx(self.extr_npy, index, trans=self.Th, period=self.data_length, **self.ROT_CAM_PARAMS[self.src_type])
         item = {}
-        if self.dataset_parms.train_stage == 2:
+        if self._reads_inp_map():
             item["inp_pos_map"] = self._inp_posmap(pose_idx)
         item.update(camera_item(self.intrinsic, E, height, width, self.znear, self.zfar))
         item.update(pose_idx=pose_idx, pose_data=self.pose_data[pose_idx], transl_data=self.transl_data[pose_idx])

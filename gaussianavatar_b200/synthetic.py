@@ -271,6 +271,67 @@ def synthetic_poses(n: int, seed: int = 0) -> tuple[torch.Tensor, torch.Tensor]:
     return pose.float(), transl.float()
 
 
+UV_GRID = (53, 130)      # rows x columns of the synthetic UV template's vertex grid: 53 * 130 = 6890 vertices
+
+
+def make_uv_template(seed: int = 0, jitter: float = 0.2):
+    """A UV template for the 6890 synthetic vertices, in the form `posmap.load_uv_template_obj` returns: (verts, faces, uvs,
+    faces_uv).  Vertex r * 130 + c sits at row r, column c of a grid; each grid cell gives two triangles (the diagonal alternates),
+    row-major, 13416 faces.  The atlas has two islands side by side: columns 0..64 in u 0.02..0.48 and columns 64..129 in u
+    0.52..0.98, so column 64 has two texture coordinates (a seam) and the vt indices differ from the v indices.  Interior texture
+    coordinates are jittered by up to `jitter` of a cell."""
+    R, C = UV_GRID
+    g = np.random.default_rng(4000 + seed)
+    islands = [(np.arange(0, 65), 0.02, 0.48), (np.arange(64, C), 0.52, 0.98)]
+    uvs, vt_of = [], []
+    for cols, u0, u1 in islands:
+        n = cols.size
+        u = np.linspace(u0, u1, n)[None, :].repeat(R, 0)
+        v = np.linspace(0.02, 0.98, R)[:, None].repeat(n, 1)
+        du, dv = (u1 - u0) / (n - 1), 0.96 / (R - 1)
+        inner = np.zeros((R, n), bool)
+        inner[1:-1, 1:-1] = True
+        u = u + inner * g.uniform(-jitter, jitter, (R, n)) * du
+        v = v + inner * g.uniform(-jitter, jitter, (R, n)) * dv
+        base = sum(len(x) for x in uvs)
+        vt_of.append({int(c): base + np.arange(R) * n + k for k, c in enumerate(cols)})
+        uvs.append(np.stack([u, v], -1).reshape(-1, 2))
+    uvs = np.concatenate(uvs)
+    faces, faces_uv = [], []
+    for r in range(R - 1):
+        for c in range(C - 1):
+            isl = vt_of[0] if c < 64 else vt_of[1]
+            a, b, cc, d = (r, c), (r, c + 1), (r + 1, c + 1), (r + 1, c)
+            tris = [(a, b, cc), (a, cc, d)] if (r + c) % 2 == 0 else [(a, b, d), (b, cc, d)]
+            for t in tris:
+                faces.append([i * C + j for i, j in t])
+                faces_uv.append([int(isl[j][i]) for i, j in t])
+    faces, faces_uv = np.asarray(faces, np.int64), np.asarray(faces_uv, np.int64)
+    p = uvs[faces_uv]
+    area = (p[:, 1, 0] - p[:, 0, 0]) * (p[:, 2, 1] - p[:, 0, 1]) - (p[:, 1, 1] - p[:, 0, 1]) * (p[:, 2, 0] - p[:, 0, 0])
+    assert (area > 0).all(), "jitter folded a triangle"
+    verts = make_body(seed).v_template.double().numpy()
+    return verts, faces, uvs, faces_uv
+
+
+def write_uv_template_obj(path: str, template) -> None:
+    """Write (verts, faces, uvs, faces_uv) as an OBJ with `v`, `vt` and `f v/vt` lines (the layout of template_mesh_smpl_uv.obj)."""
+    verts, faces, uvs, faces_uv = template
+    with open(path, "w") as fh:
+        fh.writelines(f"v {x:.6f} {y:.6f} {z:.6f}\n" for x, y, z in verts)
+        fh.writelines(f"vt {u!r} {v!r}\n" for u, v in uvs.tolist())
+        fh.writelines(f"f {a + 1}/{ta + 1} {b + 1}/{tb + 1} {c + 1}/{tc + 1}\n" for (a, b, c), (ta, tb, tc) in zip(faces.tolist(), faces_uv.tolist()))
+
+
+def smpl_mesh_model(body: SyntheticBody, template) -> dict:
+    """The fields of SMPL_{GENDER}.pkl the position maps need, for a synthetic body: v_template, shapedirs, posedirs [V,3,207],
+    weights, f (the template's faces), J_regressor, kintree_table."""
+    V = body.v_template.shape[0]
+    return dict(v_template=body.v_template.numpy(), shapedirs=body.shapedirs.numpy(), J_regressor=body.J_regressor.numpy(),
+                posedirs=body.posedirs.T.reshape(V, 3, 207).contiguous().numpy(), weights=body.lbs_weights.numpy(),
+                f=np.asarray(template[1], np.uint32), kintree_table=np.stack([np.array(SMPL_PARENTS), np.arange(24)]))
+
+
 def synthetic_smplx_poses(n: int, seed: int = 0) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Smooth random SMPL-X poses: pose [n,66] (global + body), rest_pose [n,99] (jaw, eyes, fingers curled up to ~0.5 rad), transl."""
     g = torch.Generator().manual_seed(3500 + seed)

@@ -185,6 +185,27 @@ int ga_smplx_backward(int32_t B, const float *pose, const float *rest_pose, cons
                       const float *saved_G, const float *d_cano2live, float *d_pose, float *d_transl, void *stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
+ * Stage-2 input position maps (scripts/gen_pose_map_our_smpl.py: smplx forward, then PosRender in UV space).
+ *
+ * ga_smpl_vertices: posed SMPL mesh vertices of B <= 8 frames (submodules/smplx/lbs.py:lbs vertices + body_models.py:380-382):
+ *   verts[b] = sum_j w_vj A_j(b) [v_shaped + posedirs^T (R_j(b) - I)_{j=1..23}; 1] + transl[b].  pose [B,72], transl [B,3],
+ *   rest_joints [24,3], v_shaped [V,3] = v_template + shapedirs beta (constant per subject), posedirs [207, 3V] (the layout the
+ *   reference's smplx.SMPL keeps), weights [V,24] -> verts [B,V,3].  posedirs is read once per call for all B frames.
+ * ga_posmap_layout: which face covers each texel of an S x S map (1 <= S <= 512) and with which barycentric weights, from the UV
+ *   corners of every face uv_corners [F,3,2] (uv[faces_uv]).  face_id [S,S] int32 (-1: no face; the reference's
+ *   uv_mask{S}_with_faceid_smpl.npy format), bary [S,S,3].  Output row r, column c samples u = (c+0.5)/S, v = 1-(r+0.5)/S.
+ *   Coverage is exact integer arithmetic on coordinates snapped to 1/256 texel, lowest face index wins; the rules are in
+ *   csrc/posmap.cu and DESIGN.md.  Run once per (template, S).
+ * ga_posmap_fill: out [B,3,S,S] = sum_i bary_i verts[b, faces[face_id, i]] (0 where face_id is -1); faces [F,3] int32 must index
+ *   vertices below V and face_id must come from ga_posmap_layout over the same F faces.  Every element of `out` is written.
+ * ---------------------------------------------------------------------------------------------------------------- */
+int ga_smpl_vertices(int32_t B, int32_t V, const float *pose, const float *transl, const float *rest_joints, const float *v_shaped,
+                     const float *posedirs, const float *weights, float *verts, void *stream);
+int ga_posmap_layout(int32_t F, int32_t S, const float *uv_corners, int32_t *face_id, float *bary, void *stream);
+int ga_posmap_fill(int32_t B, int32_t S, int32_t V, const float *verts, const int32_t *faces, const int32_t *face_id,
+                   const float *bary, float *out, void *stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
  * Fused Gaussian LBS + attribute assembly (model/avatar_model.py:308-326).  dec_out [S*S,8] pixel-major packed decoder
  * output (res.xyz, scale, rgb, pad); valid_index [N] int32 = flat UV index of the n-th valid pixel; query_points [N,3];
  * query_lbs [N,24]; cano2live [B,24,12]; scale_mul = 1e-3*iteration if iteration<1000 else 1 (avatar_model.py:316-319).
