@@ -430,8 +430,7 @@ class AvatarModel:
         return len(set(h)) == 1 and len(set(w)) == 1
 
     def _render_frames(self, batch_data, means, scales, colors):
-        if (means.is_cuda and means.shape[0] <= 8 and os.environ.get("GA_RASTER_BATCHED", "1") != "0"
-                and self._uniform_frames(batch_data, means.shape[0])):
+        if means.is_cuda and means.shape[0] <= 8 and self._uniform_frames(batch_data, means.shape[0]):
             return self._render_batched(batch_data, means, scales, colors)
         return self._render_frames_one_by_one(batch_data, means, scales, colors)
 
@@ -439,9 +438,9 @@ class AvatarModel:
         """The reference rasterizes the frames of a batch one after the other (avatar_model.py:332-365).  Frames are independent, and
         the compositing kernels end in a long tail of a few crowded tiles, so consecutive frames go to two alternating side
         streams: frame b+1's preprocess / sort (and, in the backward, its replay) fill the SMs frame b's tail leaves idle.
-        autograd runs each frame's backward on the stream of its forward.  GA_FRAME_STREAMS=0 keeps everything on one stream."""
+        autograd runs each frame's backward on the stream of its forward."""
         B = means.shape[0]
-        if B < 2 or not means.is_cuda or os.environ.get("GA_FRAME_STREAMS", "1") == "0":
+        if B < 2 or not means.is_cuda:
             return torch.stack([self._render_one(batch_data, means, scales, colors, b) for b in range(B)], dim=0)
         main = torch.cuda.current_stream()
         if getattr(self, "_frame_streams", None) is None:

@@ -1,6 +1,5 @@
 // Process-wide plumbing of the C ABI: error string, version, launch counter.
 #include <atomic>
-#include <cstdlib>
 #include <cstdarg>
 #include <map>
 #include <string>
@@ -24,12 +23,6 @@ void set_error(const char *fmt, ...)
 }
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
-
-bool pdl_enabled()
-{
-    static const bool on = [] { const char *e = getenv("GA_PDL"); return e && e[0] == '1'; }();
-    return on;
-}
 
 int num_sms()
 {

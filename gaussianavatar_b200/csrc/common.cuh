@@ -84,27 +84,6 @@ struct PerDeviceOnce {
 constexpr int kNumSMs = 132;  // H100 SXM (compile-time grid constants of the heads / split-K kernels)
 int num_sms();                // multiProcessorCount of the current device, queried once per device
 
-// ---- programmatic dependent launch -------------------------------------------------------------------------------------------
-// Every kernel of this library is launched with the programmatic-stream-serialization attribute and begins with pdl_wait():
-// the grid may be scheduled (and run anything placed BEFORE the wait: barrier / tensor-memory setup) while its predecessor in the
-// stream is still draining, and reads or writes global memory only after the predecessor has completed and flushed.  A step is
-// ~120 dependent launches.  It is OFF unless GA_PDL=1 (the waits are then the only cost: one instruction per kernel).
-#ifdef __CUDACC__
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-#endif
-bool pdl_enabled();
-template <typename... KArgs, typename... Args>
-inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args &&...args)
-{
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);      // errors surface through cudaGetLastError in GA_CHECK_LAUNCH
-}
-
 // 16-byte vector reduction to global memory (sm_90+): one L2 atomic for four consecutive floats (16-byte aligned address)
 __device__ __forceinline__ void red_add_v4(float *addr, float a, float b, float c, float d)
 {

@@ -47,7 +47,6 @@ template <int MODE>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_tc_kernel(const ConvParams p)
 {
-    pdl_wait();
     extern __shared__ unsigned char smem_raw[];
     ConvSmem &sm = *reinterpret_cast<ConvSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -187,7 +186,6 @@ conv_tc_kernel(const ConvParams p)
 
 __global__ void __launch_bounds__(256) round_tf32_kernel(const float *__restrict__ in, float *__restrict__ out, size_t n4)
 {
-    pdl_wait();
     const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
     if (i >= n4) return;
     float4 v = reinterpret_cast<const float4 *>(in)[i];
@@ -204,7 +202,7 @@ int launch_mode(const ConvParams &p, int grid, const char *name, cudaStream_t st
     }
     {
         ProfScope _ps(name, st);
-        launch_k(conv_tc_kernel<MODE>, grid, kConvThreads, sizeof(ConvSmem) + 1024, st, p);
+        conv_tc_kernel<MODE><<<grid, kConvThreads, sizeof(ConvSmem) + 1024, st>>>(p);
     }
     GA_CHECK_LAUNCH(name);
     return GA_OK;
@@ -219,7 +217,7 @@ int launch_round_tf32(const float *in, float *out, size_t n, cudaStream_t st)
     if (n == 0) return GA_OK;
     {
         ProfScope _ps("round_tf32_kernel", st);
-        launch_k(round_tf32_kernel, (unsigned)cdiv((long long)(n / 4), 256), 256, 0, st, in, out, n / 4);
+        round_tf32_kernel<<<(unsigned)cdiv((long long)(n / 4), 256), 256, 0, st>>>(in, out, n / 4);
     }
     GA_CHECK_LAUNCH("round_tf32_kernel");
     return GA_OK;

@@ -25,16 +25,9 @@ int launch_conv_tc(int mode, const float *in, const float *w, float *out, int Hf
 int launch_round_tf32(const float *in, float *out, size_t n, cudaStream_t st);
 namespace {
 
-#ifndef GA_HEADS_MINB
-#define GA_HEADS_MINB 2
-#endif
-#ifndef GA_HEADS_UNROLL
-#define GA_HEADS_UNROLL 4
-#endif
-#ifndef GA_HEADS_CTAS_PER_SM
-#define GA_HEADS_CTAS_PER_SM GA_HEADS_MINB
-#endif
-constexpr int kHeadsGrid = GA_HEADS_CTAS_PER_SM * kNumSMs;   // grid-stride CTAs of the heads kernels (= resident CTAs per SM at <= 80 registers)
+constexpr int kHeadsMinBlocks = 2;    // __launch_bounds__ min blocks per SM of the heads kernels
+constexpr int kHeadsUnroll = 4;       // pixels per grid-stride trip of heads_bwd_kernel
+constexpr int kHeadsGrid = kHeadsMinBlocks * kNumSMs;   // grid-stride CTAs of the heads kernels: all resident at once (<= 80 registers)
 constexpr int kCg = 64;        // c_geom
 constexpr int kH = 128;        // hsize
 constexpr int kFeatLd = 72;    // 64 sampled + 2 uv + 6 zero pad (multiple of 8)
@@ -114,7 +107,6 @@ Workspace carve_ws(void *buf, int S, int Hf, int frames)
 // [C, P] <-> [P, C] with C = 64 (tile transpose through shared memory)
 __global__ void __launch_bounds__(256) chw_to_hwc_kernel(const float *__restrict__ in, float *__restrict__ out, int P)
 {
-    pdl_wait();
     __shared__ float t[64][65];
     const int p0 = blockIdx.x * 64;
     for (int i = threadIdx.x; i < 64 * 64; i += 256) {
@@ -129,7 +121,6 @@ __global__ void __launch_bounds__(256) chw_to_hwc_kernel(const float *__restrict
 }
 __global__ void __launch_bounds__(256) hwc_to_chw_kernel(const float *__restrict__ in, float *__restrict__ out, int P)
 {
-    pdl_wait();
     __shared__ float t[64][65];
     const int p0 = blockIdx.x * 64;
     for (int i = threadIdx.x; i < 64 * 64; i += 256) {
@@ -146,7 +137,6 @@ __global__ void __launch_bounds__(256) hwc_to_chw_kernel(const float *__restrict
 // out[p][c] = in_chw[c][p] + base[p][c]: the per-frame decoder input map of stage 2, pose_featmap + geom_featmap (model/network.py:58)
 __global__ void __launch_bounds__(256) chw_to_hwc_add_kernel(const float *__restrict__ in, const float *__restrict__ base, float *__restrict__ out, int P)
 {
-    pdl_wait();
     __shared__ float t[64][65];
     const int p0 = blockIdx.x * 64;
     in += (size_t)blockIdx.y * 64 * P; out += (size_t)blockIdx.y * 64 * P;
@@ -163,7 +153,6 @@ __global__ void __launch_bounds__(256) chw_to_hwc_add_kernel(const float *__rest
 // out[i] = sum_f in[f][i]
 __global__ void __launch_bounds__(256) sum_frames_kernel(const float4 *__restrict__ in, float4 *__restrict__ out, size_t n4, int frames)
 {
-    pdl_wait();
     const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
     if (i >= n4) return;
     float4 a = in[i];
@@ -193,7 +182,6 @@ __device__ __forceinline__ Taps make_taps(int i, int j, int S, int Hf)
 __global__ void __launch_bounds__(256)
 sample_feat_fwd_kernel(int S, int Hf, int frames, size_t frame_stride, const float *__restrict__ F, float *__restrict__ feat)
 {
-    pdl_wait();
     const size_t gid = (size_t)blockIdx.x * 256 + threadIdx.x;
     const size_t m = gid >> 4;
     const int q = (int)(gid & 15);
@@ -229,7 +217,6 @@ sample_feat_fwd_kernel(int S, int Hf, int frames, size_t frame_stride, const flo
 __global__ void __launch_bounds__(256)
 sample_feat_bwd_kernel(int S, int Hf, int frames, size_t frame_stride, const float *__restrict__ d_feat, float *__restrict__ dF)
 {
-    pdl_wait();
     const size_t gid = (size_t)blockIdx.x * 256 + threadIdx.x;
     const size_t m = gid >> 4;
     const int q = (int)(gid & 15);
@@ -261,7 +248,6 @@ __global__ void bn_finalize_fwd_kernel(int C, double count, double count_running
                                        float *__restrict__ mean, float *__restrict__ rstd, float *__restrict__ a,
                                        float *__restrict__ b, float *__restrict__ run_mean, float *__restrict__ run_var)
 {
-    pdl_wait();
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
     const double mu = sum[c] / count;
@@ -282,7 +268,6 @@ __global__ void bn_finalize_bwd_kernel(int C, double count, const double *__rest
                                        float *__restrict__ ga, float *__restrict__ m1, float *__restrict__ m2,
                                        float *__restrict__ d_gamma, float *__restrict__ d_beta)
 {
-    pdl_wait();
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
     ga[c] = gamma[c] * rstd[c];
@@ -327,11 +312,10 @@ __device__ __forceinline__ float heads_reduce8(float (&v)[8], int lane)
 // modules.py:566-580) fused with the last BN + Softplus.  One warp per pixel, lane = 4 channels of each head (every
 // coefficient is a thread constant; a pixel's 1.5 KB is three 512-byte warp loads), 7 dot products reduced with 9 shuffles.
 template <bool FAST>
-__global__ void __launch_bounds__(256, GA_HEADS_MINB)
+__global__ void __launch_bounds__(256, kHeadsMinBlocks)
 heads_fwd_kernel(size_t M, const float *__restrict__ Y7 /*[M,384]*/, const float *__restrict__ a7, const float *__restrict__ b7,
                  const float *__restrict__ W8 /*[8,128]*/, const float *__restrict__ b8, float *__restrict__ dec /*[M,8]*/)
 {
-    pdl_wait();
     const int lane = threadIdx.x & 31, c = lane * 4;
     float4 A[3], B[3], Wv[7];
 #pragma unroll
@@ -378,13 +362,12 @@ heads_fwd_kernel(size_t M, const float *__restrict__ Y7 /*[M,384]*/, const float
 // 1: scale (row 3), 2: colour (rows 4-6).  Writes dZ7[:, head*128 ...], accumulates s1/s2 (double), dW8 rows, db8.
 // One warp per pixel, lane = 4 channels: the running sums for dW8 / BatchNorm statistics are 4 x (NOUT + 2) registers.
 template <int HEAD, bool FAST>
-__global__ void __launch_bounds__(256, GA_HEADS_MINB)
+__global__ void __launch_bounds__(256, kHeadsMinBlocks)
 heads_bwd_kernel(size_t M, const float *__restrict__ Y7, const float *__restrict__ a7, const float *__restrict__ b7,
                  const float *__restrict__ mu7, const float *__restrict__ rstd7, const float *__restrict__ W8,
                  const float *__restrict__ dec, const float *__restrict__ d_dec, float *__restrict__ dZ7,
                  double *__restrict__ s1, double *__restrict__ s2, float *__restrict__ dW8, float *__restrict__ db8)
 {
-    pdl_wait();
     constexpr int NOUT = (HEAD == 1) ? 1 : 3;
     constexpr int ROW0 = (HEAD == 0) ? 0 : (HEAD == 1 ? 3 : 4);
     __shared__ float sacc[NOUT + 2][kH];
@@ -410,7 +393,7 @@ heads_bwd_kernel(size_t M, const float *__restrict__ Y7, const float *__restrict
     for (int e = 0; e < 4; ++e) a1[e] = a2[e] = 0.f;
 
     const size_t nwarps = (size_t)gridDim.x * 8;
-    constexpr int U = GA_HEADS_UNROLL;                                    // pixels per trip: U 512-byte warp loads in flight
+    constexpr int U = kHeadsUnroll;                                       // pixels per trip: U 512-byte warp loads in flight
     for (size_t mb = (size_t)blockIdx.x * 8 + (threadIdx.x >> 5); mb < M; mb += U * nwarps) {
         float4 yv[U]; float dpv[U][NOUT];
 #pragma unroll
@@ -549,7 +532,7 @@ int launch_gemm(const char *name, const AL &A, const BL &B, const EP &E, int Mg,
     dim3 grid(cdiv(Mg, BM), cdiv(Ng, BN), splits);
     {
         ProfScope _ps(name, st);
-        launch_k(gemm_kernel<BM, BN, AL, BL, EP>, grid, kGemmThreads, 0, st, A, B, E, Kg, kps);
+        gemm_kernel<BM, BN, AL, BL, EP><<<grid, kGemmThreads, 0, st>>>(A, B, E, Kg, kps);
     }
     GA_CHECK_LAUNCH(name);
     return GA_OK;
@@ -613,7 +596,7 @@ extern "C" int ga_decoder_forward(const GaDecoderDesc *d, const float *params, c
 
     {
         ProfScope _ps("chw_to_hwc_kernel", st);
-        launch_k(chw_to_hwc_kernel, cdiv(P, 64), 256, 0, st, geo_nchw, w.F[0], P);
+        chw_to_hwc_kernel<<<cdiv(P, 64), 256, 0, st>>>(geo_nchw, w.F[0], P);
     }
     GA_CHECK_LAUNCH("chw_to_hwc_kernel");
     if (d->flags & GA_DECODER_TENSOR_CORES) {
@@ -637,13 +620,13 @@ extern "C" int ga_decoder_forward(const GaDecoderDesc *d, const float *params, c
     if (pose_feat_nchw) {          // stage 2: pix_feature = pose_featmap + geom_featmap (model/network.py:58), one map per frame
         ProfScope _ps("chw_to_hwc_add_kernel", st);
         float *Fp = frames > 1 ? w.Fp : w.F[3];
-        launch_k(chw_to_hwc_add_kernel, dim3(cdiv(P, 64), frames), 256, 0, st, pose_feat_nchw, w.F[3], Fp, P);
+        chw_to_hwc_add_kernel<<<dim3(cdiv(P, 64), frames), 256, 0, st>>>(pose_feat_nchw, w.F[3], Fp, P);
         Fsrc = Fp; fstride = frames > 1 ? (size_t)P * kCg : 0;
     }
     if (pose_feat_nchw) GA_CHECK_LAUNCH("chw_to_hwc_add_kernel");
     {
         ProfScope _ps("sample_feat_fwd_kernel", st);
-        launch_k(sample_feat_fwd_kernel, cdiv((long long)M * 16, 256), 256, 0, st, S, Hf, frames, fstride, Fsrc, w.feat);
+        sample_feat_fwd_kernel<<<cdiv((long long)M * 16, 256), 256, 0, st>>>(S, Hf, frames, fstride, Fsrc, w.feat);
     }
     GA_CHECK_LAUNCH("sample_feat_fwd_kernel");
     GA_CHECK_CUDA(cudaMemsetAsync(w.stat, 0, sizeof(double) * 2 * kBnCh, st));
@@ -653,7 +636,7 @@ extern "C" int ga_decoder_forward(const GaDecoderDesc *d, const float *params, c
         const int o = kBnOff[l];
         {
             ProfScope _ps("bn_finalize_fwd_kernel", st);
-            launch_k(bn_finalize_fwd_kernel, cdiv(C, 128), 128, 0, st, C, (double)M, (double)S * S * d->batch, d->bn_eps, d->bn_momentum, sum + o, sumsq + o,
+            bn_finalize_fwd_kernel<<<cdiv(C, 128), 128, 0, st>>>(C, (double)M, (double)S * S * d->batch, d->bn_eps, d->bn_momentum, sum + o, sumsq + o,
                                                                  params + L.gamma[l] , params + L.beta[l], cf.mean + o, cf.rstd + o, cf.a + o, cf.b + o,
                                                                  bn_running ? bn_running + o : nullptr, bn_running ? bn_running + kBnCh + o : nullptr);
         }
@@ -724,9 +707,9 @@ extern "C" int ga_decoder_forward(const GaDecoderDesc *d, const float *params, c
     {
         ProfScope _ps("heads_fwd_kernel", st);
         if (d->flags & GA_DECODER_TENSOR_CORES)
-            launch_k(heads_fwd_kernel<true>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + kBnOff[6], cf.b + kBnOff[6], params + L.w8, params + L.b8, dec_out);
+            heads_fwd_kernel<true><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + kBnOff[6], cf.b + kBnOff[6], params + L.w8, params + L.b8, dec_out);
         else
-            launch_k(heads_fwd_kernel<false>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + kBnOff[6], cf.b + kBnOff[6], params + L.w8, params + L.b8, dec_out);
+            heads_fwd_kernel<false><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + kBnOff[6], cf.b + kBnOff[6], params + L.w8, params + L.b8, dec_out);
     }
     GA_CHECK_LAUNCH("heads_fwd_kernel");
     return GA_OK;
@@ -755,7 +738,7 @@ extern "C" int ga_decoder_backward(const GaDecoderDesc *d, const float *params, 
         const int o = kBnOff[l];
         {
             ProfScope _ps("bn_finalize_bwd_kernel", st);
-            launch_k(bn_finalize_bwd_kernel, cdiv(C, 128), 128, 0, st, C, (double)M, s1 + o, s2 + o, params + L.gamma[l], cf.rstd + o, cf.ga + o, cf.m1 + o,
+            bn_finalize_bwd_kernel<<<cdiv(C, 128), 128, 0, st>>>(C, (double)M, s1 + o, s2 + o, params + L.gamma[l], cf.rstd + o, cf.ga + o, cf.m1 + o,
                                                                  cf.m2 + o, d_params + L.gamma[l], d_params + L.beta[l]);
         }
         GA_CHECK_LAUNCH("bn_finalize_bwd_kernel");
@@ -769,30 +752,30 @@ extern "C" int ga_decoder_backward(const GaDecoderDesc *d, const float *params, 
         {
             ProfScope _ps("heads_bwd_kernel<0>", st);
             if (d->flags & GA_DECODER_TENSOR_CORES)
-                launch_k(heads_bwd_kernel<0, true>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
+                heads_bwd_kernel<0, true><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
                                                                    dec_out, d_dec_out, w.dZ7, s1 + o7, s2 + o7, d_params + L.w8, d_params + L.b8);
             else
-                launch_k(heads_bwd_kernel<0, false>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
+                heads_bwd_kernel<0, false><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
                                                                     dec_out, d_dec_out, w.dZ7, s1 + o7, s2 + o7, d_params + L.w8, d_params + L.b8);
         }
         GA_CHECK_LAUNCH("heads_bwd_kernel<0>");
         {
             ProfScope _ps("heads_bwd_kernel<1>", st);
             if (d->flags & GA_DECODER_TENSOR_CORES)
-                launch_k(heads_bwd_kernel<1, true>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
+                heads_bwd_kernel<1, true><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
                                                                    dec_out, d_dec_out, w.dZ7, s1 + o7, s2 + o7, d_params + L.w8, d_params + L.b8);
             else
-                launch_k(heads_bwd_kernel<1, false>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
+                heads_bwd_kernel<1, false><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
                                                                     dec_out, d_dec_out, w.dZ7, s1 + o7, s2 + o7, d_params + L.w8, d_params + L.b8);
         }
         GA_CHECK_LAUNCH("heads_bwd_kernel<1>");
         {
             ProfScope _ps("heads_bwd_kernel<2>", st);
             if (d->flags & GA_DECODER_TENSOR_CORES)
-                launch_k(heads_bwd_kernel<2, true>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
+                heads_bwd_kernel<2, true><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
                                                                    dec_out, d_dec_out, w.dZ7, s1 + o7, s2 + o7, d_params + L.w8, d_params + L.b8);
             else
-                launch_k(heads_bwd_kernel<2, false>, kHeadsGrid, 256, 0, st, (size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
+                heads_bwd_kernel<2, false><<<kHeadsGrid, 256, 0, st>>>((size_t)M, w.Y7, cf.a + o7, cf.b + o7, cf.mean + o7, cf.rstd + o7, params + L.w8,
                                                                     dec_out, d_dec_out, w.dZ7, s1 + o7, s2 + o7, d_params + L.w8, d_params + L.b8);
         }
         GA_CHECK_LAUNCH("heads_bwd_kernel<2>");
@@ -912,19 +895,19 @@ extern "C" int ga_decoder_backward(const GaDecoderDesc *d, const float *params, 
     GA_CHECK_CUDA(cudaMemsetAsync(dsink, 0, sizeof(float) * (size_t)frames * P * kCg, st));
     {
         ProfScope _ps("sample_feat_bwd_kernel", st);
-        launch_k(sample_feat_bwd_kernel, cdiv((long long)M * 16, 256), 256, 0, st, S, Hf, frames, frames > 1 ? (size_t)P * kCg : 0, w.d_feat, dsink);
+        sample_feat_bwd_kernel<<<cdiv((long long)M * 16, 256), 256, 0, st>>>(S, Hf, frames, frames > 1 ? (size_t)P * kCg : 0, w.d_feat, dsink);
     }
     GA_CHECK_LAUNCH("sample_feat_bwd_kernel");
     if (d_pose_feat_nchw) {        // d pose_featmap[f] = d pix[f] (NCHW); d geom_featmap = sum over the frames
         for (int f = 0; f < frames; ++f) {
             ProfScope _ps("hwc_to_chw_kernel", st);
-            launch_k(hwc_to_chw_kernel, cdiv(P, 64), 256, 0, st, dsink + (size_t)f * P * kCg, d_pose_feat_nchw + (size_t)f * P * kCg, P);
+            hwc_to_chw_kernel<<<cdiv(P, 64), 256, 0, st>>>(dsink + (size_t)f * P * kCg, d_pose_feat_nchw + (size_t)f * P * kCg, P);
             GA_CHECK_LAUNCH("hwc_to_chw_kernel");
         }
     }
     if (frames > 1) {
         ProfScope _ps("sum_frames_kernel", st);
-        launch_k(sum_frames_kernel, cdiv((long long)P * kCg / 4, 256), 256, 0, st, reinterpret_cast<const float4 *>(w.dFp), reinterpret_cast<float4 *>(w.dF[0]),
+        sum_frames_kernel<<<cdiv((long long)P * kCg / 4, 256), 256, 0, st>>>(reinterpret_cast<const float4 *>(w.dFp), reinterpret_cast<float4 *>(w.dF[0]),
                                                                             (size_t)P * kCg / 4, frames);
     }
     if (frames > 1) GA_CHECK_LAUNCH("sum_frames_kernel");
@@ -956,7 +939,7 @@ extern "C" int ga_decoder_backward(const GaDecoderDesc *d, const float *params, 
     }
     {
         ProfScope _ps("hwc_to_chw_kernel", st);
-        launch_k(hwc_to_chw_kernel, cdiv(P, 64), 256, 0, st, dcur, d_geo_nchw, P);
+        hwc_to_chw_kernel<<<cdiv(P, 64), 256, 0, st>>>(dcur, d_geo_nchw, P);
     }
     GA_CHECK_LAUNCH("hwc_to_chw_kernel");
     return GA_OK;

@@ -267,7 +267,6 @@ template <int BM, int BN, class ALoad, class BLoad, class Epi>
 __global__ void __launch_bounds__(kGemmThreads)
 gemm_kernel(const ALoad A, const BLoad B, const Epi epi, int Kg, int k_per_split)
 {
-    pdl_wait();
     using TT = ThreadTile<BM, BN>;
     constexpr int TM = TT::TM, TN = TT::TN;
     __shared__ __align__(16) float As[kBK * (BM + kPad)];

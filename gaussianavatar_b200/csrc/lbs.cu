@@ -80,7 +80,6 @@ lbs_kernel(int N, int B, float scale_mul, long long dec_stride /*floats between 
     static_assert(kLd % 4 == 0 && kLd >= kJ, "weight rows are whole float4s");
     constexpr bool kRegW = kJ <= 24;           // weights of this thread's Gaussian kept in registers across the frames
     constexpr int kOut = (kJ * 12 + kTileN - 1) / kTileN;   // dC outputs per thread per frame
-    pdl_wait();
     extern __shared__ __align__(128) unsigned char smem_raw[];
     LbsSmem<kJ, kLd> &sm = *reinterpret_cast<LbsSmem<kJ, kLd> *>(smem_raw);
     const int tid = threadIdx.x;
@@ -261,7 +260,7 @@ int lbs_forward(int N, int B, float scale_mul, int64_t dec_frame_stride, const f
         GA_CHECK_CUDA(cudaFuncSetAttribute(lbs_kernel<false, kJ, kLd>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LbsSmem<kJ, kLd>)));
         GA_CHECK_CUDA(cudaFuncSetAttribute(lbs_kernel<true, kJ, kLd>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LbsSmem<kJ, kLd>)));
     }
-    { ProfScope _ps(name, stream); launch_k(lbs_kernel<false, kJ, kLd>, launch_cfg<kJ, kLd>(N), kTileN, sizeof(LbsSmem<kJ, kLd>), stream,
+    { ProfScope _ps(name, stream); lbs_kernel<false, kJ, kLd><<<launch_cfg<kJ, kLd>(N), kTileN, sizeof(LbsSmem<kJ, kLd>), stream>>>(
         N, B, scale_mul, (long long)dec_frame_stride, dec_out, valid_index, query_points, query_lbs, cano2live, means3D, scales3, colors, nullptr, nullptr,
         nullptr, nullptr, nullptr); }
     GA_CHECK_LAUNCH(name);
@@ -277,7 +276,7 @@ int lbs_backward(int N, int B, float scale_mul, int64_t dec_frame_stride, const 
     if (attr_set.first()) {
         GA_CHECK_CUDA(cudaFuncSetAttribute(lbs_kernel<true, kJ, kLd>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(LbsSmem<kJ, kLd>)));
     }
-    { ProfScope _ps(name, stream); launch_k(lbs_kernel<true, kJ, kLd>, launch_cfg<kJ, kLd>(N), kTileN, sizeof(LbsSmem<kJ, kLd>), stream, N, B, scale_mul,
+    { ProfScope _ps(name, stream); lbs_kernel<true, kJ, kLd><<<launch_cfg<kJ, kLd>(N), kTileN, sizeof(LbsSmem<kJ, kLd>), stream>>>(N, B, scale_mul,
         (long long)dec_frame_stride, dec_out, valid_index, query_points, query_lbs, cano2live, nullptr, nullptr, nullptr,
         d_means3D, d_scales3, d_colors, d_dec_out, d_cano2live); }
     GA_CHECK_LAUNCH(name);

@@ -32,7 +32,6 @@ __global__ void __launch_bounds__(kTX * kTY)
 ssim_l1_fwd_kernel(int H, int W, const float *__restrict__ img, const float *__restrict__ gt, float *__restrict__ dm_dmu1,
                    float *__restrict__ dm_ds1, float *__restrict__ dm_ds12, double *__restrict__ acc /*[2]: ssim sum, l1 sum*/)
 {
-    pdl_wait();
     __shared__ float sA[kSY][kSX + 1], sB[kSY][kSX + 1];
     __shared__ float sH[5][kSY][kTX + 1];
     __shared__ float sred[2][kTX * kTY / 32];
@@ -124,7 +123,6 @@ ssim_l1_bwd_kernel(int H, int W, const float *__restrict__ img, const float *__r
                    const float *__restrict__ dm_ds1, const float *__restrict__ dm_ds12, const float *__restrict__ coef /*[2]*/,
                    float *__restrict__ d_img)
 {
-    pdl_wait();
     __shared__ float sM[3][kSY][kSX + 1];
     __shared__ float sH[3][kSY][kTX + 1];
     const int tx = threadIdx.x, ty = threadIdx.y, tid = ty * kTX + tx;
@@ -182,7 +180,6 @@ ssim_l1_bwd_kernel(int H, int W, const float *__restrict__ img, const float *__r
 // out[0] = w_l1 * l1_mean + w_ssim * (1 - ssim_mean); out[1] = ssim_mean; out[2] = l1_mean
 __global__ void loss_finalize_kernel(const double *__restrict__ acc, double inv_n, float w_l1, float w_ssim, float *__restrict__ out)
 {
-    pdl_wait();
     const double s = acc[0] * inv_n, l = acc[1] * inv_n;
     out[0] = (float)(w_l1 * l + w_ssim * (1.0 - s));
     out[1] = (float)s;
@@ -192,7 +189,6 @@ __global__ void loss_finalize_kernel(const double *__restrict__ acc, double inv_
 // coef[0] = g * w_l1 / n ; coef[1] = -g * w_ssim / n   (d(1 - ssim)/d ssim = -1)
 __global__ void loss_coef_kernel(const float *__restrict__ g, float w_l1, float w_ssim, float inv_n, float *__restrict__ coef)
 {
-    pdl_wait();
     const float gv = g ? g[0] : 1.f;
     coef[0] = gv * w_l1 * inv_n;
     coef[1] = -gv * w_ssim * inv_n;
@@ -236,9 +232,9 @@ extern "C" int ga_loss_forward(int32_t B, int32_t H, int32_t W, const float *ima
     double *acc = c.take<double>(2);
     GA_CHECK_CUDA(cudaMemsetAsync(acc, 0, 2 * sizeof(double), st));
     dim3 grid(cdiv(W, kTX), cdiv(H, kTY), B * 3), block(kTX, kTY);
-    { ProfScope _ps("ssim_l1_fwd_kernel", st); launch_k(ssim_l1_fwd_kernel, grid, block, 0, st, H, W, image, gt, maps, maps + n, maps + 2 * n, acc); }
+    { ProfScope _ps("ssim_l1_fwd_kernel", st); ssim_l1_fwd_kernel<<<grid, block, 0, st>>>(H, W, image, gt, maps, maps + n, maps + 2 * n, acc); }
     GA_CHECK_LAUNCH("ssim_l1_fwd_kernel");
-    { ProfScope _ps("loss_finalize_kernel", st); launch_k(loss_finalize_kernel, 1, 1, 0, st, acc, 1.0 / (double)n, w_l1, w_ssim, out3); }
+    { ProfScope _ps("loss_finalize_kernel", st); loss_finalize_kernel<<<1, 1, 0, st>>>(acc, 1.0 / (double)n, w_l1, w_ssim, out3); }
     GA_CHECK_LAUNCH("loss_finalize_kernel");
     return GA_OK;
 }
@@ -255,10 +251,10 @@ extern "C" int ga_loss_backward(int32_t B, int32_t H, int32_t W, const float *im
     float *maps = c.take<float>(3 * n);
     (void)c.take<double>(2);
     float *coef = c.take<float>(4);
-    { ProfScope _ps("loss_coef_kernel", st); launch_k(loss_coef_kernel, 1, 1, 0, st, grad_out, w_l1, w_ssim, (float)(1.0 / (double)n), coef); }
+    { ProfScope _ps("loss_coef_kernel", st); loss_coef_kernel<<<1, 1, 0, st>>>(grad_out, w_l1, w_ssim, (float)(1.0 / (double)n), coef); }
     GA_CHECK_LAUNCH("loss_coef_kernel");
     dim3 grid(cdiv(W, kTX), cdiv(H, kTY), B * 3), block(kTX, kTY);
-    { ProfScope _ps("ssim_l1_bwd_kernel", st); launch_k(ssim_l1_bwd_kernel, grid, block, 0, st, H, W, image, gt, maps, maps + n, maps + 2 * n, coef, d_image); }
+    { ProfScope _ps("ssim_l1_bwd_kernel", st); ssim_l1_bwd_kernel<<<grid, block, 0, st>>>(H, W, image, gt, maps, maps + n, maps + 2 * n, coef, d_image); }
     GA_CHECK_LAUNCH("ssim_l1_bwd_kernel");
     return GA_OK;
 }
@@ -277,7 +273,6 @@ adam_kernel(size_t n, float *__restrict__ p, const float *__restrict__ g, float 
             float beta1, float beta2, float eps, float bc1, float bc2_sqrt, float grad_scale, const float *__restrict__ hyper,
             const int32_t *__restrict__ skip)
 {
-    pdl_wait();
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     if (skip && *skip != 0) return;
@@ -299,7 +294,7 @@ extern "C" int ga_adam_step(int64_t n, float *param, const float *grad, float *e
     if (n == 0) return GA_OK;
     GA_REQUIRE(param && grad && exp_avg && exp_avg_sq, "NULL pointer argument");
     const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);
-    { ProfScope _ps("adam_kernel", static_cast<cudaStream_t>(stream_)); launch_k(adam_kernel, cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream_), (size_t)n, param, grad, exp_avg, exp_avg_sq, lr, beta1, beta2, eps,
+    { ProfScope _ps("adam_kernel", static_cast<cudaStream_t>(stream_)); adam_kernel<<<cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream_)>>>((size_t)n, param, grad, exp_avg, exp_avg_sq, lr, beta1, beta2, eps,
                                                                              (float)bc1, (float)sqrt(bc2), grad_scale, nullptr, skip_flag); }
     GA_CHECK_LAUNCH("adam_kernel");
     return GA_OK;
@@ -311,7 +306,7 @@ extern "C" int ga_adam_step_dev(int64_t n, float *param, const float *grad, floa
     GA_REQUIRE(n >= 0, "bad adam args n=%lld", (long long)n);
     if (n == 0) return GA_OK;
     GA_REQUIRE(param && grad && exp_avg && exp_avg_sq && hyper7, "NULL pointer argument");
-    { ProfScope _ps("adam_kernel", static_cast<cudaStream_t>(stream_)); launch_k(adam_kernel, cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream_), (size_t)n, param, grad, exp_avg, exp_avg_sq, 0.f, 0.f, 0.f, 0.f,
+    { ProfScope _ps("adam_kernel", static_cast<cudaStream_t>(stream_)); adam_kernel<<<cdiv(n, 256), 256, 0, static_cast<cudaStream_t>(stream_)>>>((size_t)n, param, grad, exp_avg, exp_avg_sq, 0.f, 0.f, 0.f, 0.f,
                                                                              1.f, 1.f, 1.f, hyper7, skip_flag); }
     GA_CHECK_LAUNCH("adam_kernel");
     return GA_OK;

@@ -111,7 +111,6 @@ __global__ void __launch_bounds__(kThreads, 1) lpips_conv_kernel(const __grid_co
     const int nchunks = p.K / 32;
     if (tid < kStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
     fence_proxy_async();
-    pdl_wait();
     __syncthreads();
 
     if (warp < 4) {
@@ -242,7 +241,6 @@ __global__ void __launch_bounds__(kThreads, 1) lpips_conv_kernel(const __grid_co
 __global__ void lpips_pool_kernel(const float *__restrict__ in, float *__restrict__ out, uint8_t *__restrict__ arg, int imgs, int Hi, int Wi,
                                   int C, int Ho, int Wo)
 {
-    pdl_wait();
     const long long total = (long long)imgs * Ho * Wo * C;
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
         const int c = (int)(e % C);
@@ -266,7 +264,6 @@ __global__ void lpips_pool_kernel(const float *__restrict__ in, float *__restric
 __global__ void lpips_unpool_kernel(const float *__restrict__ gout, const uint8_t *__restrict__ arg, float *__restrict__ gin, int imgs, int Hi,
                                     int Wi, int C, int Ho, int Wo)
 {
-    pdl_wait();
     const long long total = (long long)imgs * Hi * Wi * C;
     for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
         const int c = (int)(e % C);
@@ -288,7 +285,6 @@ template <int J>
 __global__ void __launch_bounds__(32 * kDistWarps) lpips_dist_kernel(const float *__restrict__ f, const float *__restrict__ lin, int B, int HW,
                                                                   float *__restrict__ part)
 {
-    pdl_wait();
     __shared__ float red[kDistWarps];
     constexpr int C = 32 * J;
     const int b = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -334,7 +330,6 @@ struct SumParams {
 // out[b] = sum_k (sum of layer k's partials, in CTA order) / HW_k; also records the input scale for the backward
 __global__ void lpips_sum_kernel(const __grid_constant__ SumParams p)
 {
-    pdl_wait();
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b == 0) *p.in_scale_ws = p.in_scale;
     if (b >= p.B) return;
@@ -355,7 +350,6 @@ __global__ void __launch_bounds__(32 * kDistWarps) lpips_dnorm_kernel(const floa
                                                                    const float *__restrict__ g, const float *__restrict__ gnext, int B, int HW,
                                                                    float *__restrict__ dz)
 {
-    pdl_wait();
     constexpr int C = 32 * J;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long q = (long long)blockIdx.x * kDistWarps + warp;
@@ -398,7 +392,6 @@ __global__ void __launch_bounds__(kImgThreads) lpips_img_grad_kernel(const float
                                                                   const float *__restrict__ in_scale, int H, int W, int H1, int W1,
                                                                   float *__restrict__ d_in)
 {
-    pdl_wait();
     __shared__ float ws[9][64][3];
     const int ph = blockIdx.y, ry = ph >> 2, rx = ph & 3, b = blockIdx.z;
     const int qy = (ry + 2) & 3, qx = (rx + 2) & 3;           // first tap of the phase: (y + 2 - ky) % 4 == 0
@@ -510,7 +503,7 @@ template <int BN> int launch_conv(const ConvParams &p, const char *name, cudaStr
     const dim3 grid(cdiv(p.P, kBM), p.N / BN);
     {
         ProfScope _ps(name, st);
-        launch_k(lpips_conv_kernel<BN>, grid, kThreads, smem, st, p);
+        lpips_conv_kernel<BN><<<grid, kThreads, smem, st>>>(p);
     }
     GA_CHECK_LAUNCH(name);
     return GA_OK;
@@ -538,7 +531,7 @@ int simple_launch(const char *name, void (*k)(KArgs...), dim3 grid, dim3 block, 
 {
     {
         ProfScope _ps(name, st);
-        launch_k(k, grid, block, 0, st, std::forward<Args>(args)...);
+        k<<<grid, block, 0, st>>>(std::forward<Args>(args)...);
     }
     GA_CHECK_LAUNCH(name);
     return GA_OK;

@@ -96,7 +96,6 @@ tc_fwd_kernel(const __grid_constant__ TcFwdParams p)
     const int M = p.M;
     if (tid < kTStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
     if (tid < 2) { mbar_init(smem_u32(&sm.yload[tid]), 1); fence_proxy_async(); }   // completed by TMA loads (async proxy)
-    pdl_wait();
     for (int i = tid; i < p.K; i += kTcThreads) { sm.sa[i] = p.a ? p.a[i] : 1.f; sm.sb[i] = p.a ? p.b[i] : 0.f; }
     __syncthreads();
     const uint32_t x0s = smem_u32(sm.x[0]);
@@ -281,7 +280,7 @@ int launch_tc_fwd(const float *X, int ldx, int K, const float *a, const float *b
     const int grid = tiles < sms ? tiles : sms;
     {
         ProfScope _ps("mlp_tc_fwd", st);
-        launch_k(tc_fwd_kernel, grid, kTcThreads, sizeof(TcFwdSmem) + 1024, st, p);
+        tc_fwd_kernel<<<grid, kTcThreads, sizeof(TcFwdSmem) + 1024, st>>>(p);
     }
     GA_CHECK_LAUNCH("tc_fwd_kernel");
     return GA_OK;
@@ -367,7 +366,6 @@ tc_bwd_kernel(const __grid_constant__ TcBwdParams p)
     const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
     if (tid < kBStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
     if (tid < 2) { mbar_init(smem_u32(&sm.oload[tid]), 1); fence_proxy_async(); }   // completed by TMA loads (async proxy)
-    pdl_wait();
     for (int i = tid; i < 128; i += kTcThreads) {
         if (p.ga) {   // ga (dZ - m1 - (Y - mu) rstd m2)
             const float ga = p.ga[i], k = p.rstd[i] * p.m2[i];
@@ -655,7 +653,7 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
     const int grid = tiles < sms ? tiles : sms;
     {
         ProfScope _ps("mlp_tc_bwd", st);
-        launch_k(tc_bwd_kernel, grid, kTcThreads, sizeof(TcBwdSmem) + 1024, st, p);
+        tc_bwd_kernel<<<grid, kTcThreads, sizeof(TcBwdSmem) + 1024, st>>>(p);
     }
     GA_CHECK_LAUNCH("tc_bwd_kernel");
     return GA_OK;

@@ -47,7 +47,6 @@ smpl_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,72]*/, co
     __shared__ float sL[kMaxB][kJoints][12], sA[kMaxB][kJoints][12];
     __shared__ float sFeat[kMaxB][kPoseFeat];
     __shared__ float sPart[kRowGroups][kMaxB][kCols];
-    pdl_wait();
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     if (warp < B && lane < kJoints) {
         const int b = warp, j = lane;
@@ -166,7 +165,6 @@ __device__ __forceinline__ bool edge_owns(long long e, long long dx, long long d
 __global__ void __launch_bounds__(128)
 posmap_raster_kernel(int F, int S, const float *__restrict__ uv, int *__restrict__ face_id)
 {
-    pdl_wait();
     const int f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= F) return;
     Snapped s = snap_face(uv, f, S);
@@ -201,7 +199,6 @@ posmap_raster_kernel(int F, int S, const float *__restrict__ uv, int *__restrict
 __global__ void __launch_bounds__(256)
 posmap_resolve_kernel(int F, int S, const float *__restrict__ uv, int *__restrict__ face_id, float *__restrict__ bary)
 {
-    pdl_wait();
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= S * S) return;
     const int f = face_id[t];
@@ -227,7 +224,6 @@ __global__ void __launch_bounds__(256)
 posmap_fill_kernel(int S, int V, const float *__restrict__ verts, const int *__restrict__ faces, const int *__restrict__ face_id,
                    const float *__restrict__ bary, float *__restrict__ out)
 {
-    pdl_wait();
     const int t = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
     const int n = S * S;
     if (t >= n) return;
@@ -260,7 +256,7 @@ extern "C" int ga_smpl_vertices(int32_t B, int32_t V, const float *pose, const f
     GA_REQUIRE(pose && transl && rest_joints && v_shaped && posedirs && weights && verts, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     { ProfScope _ps("smpl_vertices_kernel", stream);
-      launch_k(smpl_vertices_kernel, cdiv(V, kVertsPerCta), kVertThreads, 0, stream, B, V, pose, transl, rest_joints, v_shaped, posedirs,
+      smpl_vertices_kernel<<<cdiv(V, kVertsPerCta), kVertThreads, 0, stream>>>(B, V, pose, transl, rest_joints, v_shaped, posedirs,
                weights, verts); }
     GA_CHECK_LAUNCH("smpl_vertices_kernel");
     return GA_OK;
@@ -274,10 +270,10 @@ extern "C" int ga_posmap_layout(int32_t F, int32_t S, const float *uv_corners, i
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     GA_CHECK_CUDA(cudaMemsetAsync(face_id, 0x7f, sizeof(int32_t) * S * S, stream));      // kNoFace > any face index
     if (F > 0) {
-        { ProfScope _ps("posmap_raster_kernel", stream); launch_k(posmap_raster_kernel, cdiv(F, 128), 128, 0, stream, F, S, uv_corners, face_id); }
+        { ProfScope _ps("posmap_raster_kernel", stream); posmap_raster_kernel<<<cdiv(F, 128), 128, 0, stream>>>(F, S, uv_corners, face_id); }
         GA_CHECK_LAUNCH("posmap_raster_kernel");
     }
-    { ProfScope _ps("posmap_resolve_kernel", stream); launch_k(posmap_resolve_kernel, cdiv(S * S, 256), 256, 0, stream, F, S, uv_corners, face_id, bary); }
+    { ProfScope _ps("posmap_resolve_kernel", stream); posmap_resolve_kernel<<<cdiv(S * S, 256), 256, 0, stream>>>(F, S, uv_corners, face_id, bary); }
     GA_CHECK_LAUNCH("posmap_resolve_kernel");
     return GA_OK;
 }
@@ -291,7 +287,7 @@ extern "C" int ga_posmap_fill(int32_t B, int32_t S, int32_t V, const float *vert
     GA_REQUIRE(verts && faces && face_id && bary && out, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     { ProfScope _ps("posmap_fill_kernel", stream);
-      launch_k(posmap_fill_kernel, dim3(cdiv(S * S, 256), B), 256, 0, stream, S, V, verts, faces, face_id, bary, out); }
+      posmap_fill_kernel<<<dim3(cdiv(S * S, 256), B), 256, 0, stream>>>(S, V, verts, faces, face_id, bary, out); }
     GA_CHECK_LAUNCH("posmap_fill_kernel");
     return GA_OK;
 }

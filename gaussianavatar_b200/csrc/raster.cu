@@ -472,11 +472,11 @@ __device__ __forceinline__ int tile_slot_find(const uint32_t *s_key, uint32_t ti
 
 // K1: one thread per Gaussian (blockIdx.y = frame).  Besides the per-Gaussian state it counts, per tile, the instances the
 // tile will receive (tile_count[frame][tile]): the binning that follows is a bucket sort by tile, not a global sort.
-// The CTA's 256 Gaussians first count into a shared-memory tile table and then add only its occupied slots to the global counters — a
-// few hundred thousand atomics on a few hundred hot addresses (which serialise in L2 and used to set this kernel's duration)
-// become one per (CTA, touched tile).
+// The CTA's 256 Gaussians first count into the shared-memory tile table and then add only its occupied slots to the global counters:
+// one global atomic per (CTA, touched tile) instead of one per instance, which would put a few hundred thousand atomics on a few
+// hundred hot addresses that serialise in L2.
 // kSH / kCov (per-frame API only, B = 1): SH colours into cc.rgb / cc.clamped, Sigma from cc.cov3D.
-template <bool kSmemHist, bool kSH = false, bool kCov = false>
+template <bool kSH = false, bool kCov = false>
 __global__ void __launch_bounds__(256)
 preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod, const float *__restrict__ means3D,
                       const float *__restrict__ scales, const float *__restrict__ rots, long long rot_stride,
@@ -485,7 +485,6 @@ preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod
                       uint32_t *__restrict__ tiles, ushort4 *__restrict__ rect, int32_t *__restrict__ radii,
                       uint32_t *__restrict__ tile_count, ColorCov cc)
 {
-    pdl_wait();
     const int b = blockIdx.y;
     __shared__ float view[16], proj[16];
     if (threadIdx.x < 16) view[threadIdx.x] = cam.view[(size_t)b * cam.stride + threadIdx.x];
@@ -503,22 +502,18 @@ preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod
             sh_color_fwd(cc, (size_t)il, means3D[3 * (size_t)il], means3D[3 * (size_t)il + 1], means3D[3 * (size_t)il + 2], rc.z > rc.x);
     }
     uint32_t *tc = tile_count + (size_t)b * gx * gy;
-    if (kSmemHist) {
-        __shared__ uint32_t s_key[kTileSlots], s_cnt[kTileSlots];
-        for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) { s_key[t] = kEmptySlot; s_cnt[t] = 0u; }
-        __syncthreads();
-        for_each_tile_balanced(rc, gx, 0ull, [&](uint32_t tile, uint64_t) {
-            const int slot = tile_slot_insert(s_key, tile);
-            if (slot >= 0) atomicAdd(&s_cnt[slot], 1u);
-            else atomicAdd(&tc[tile], 1u);
-        });
-        __syncthreads();
-        for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) {
-            const uint32_t c = s_cnt[t];
-            if (c) atomicAdd(&tc[s_key[t]], c);
-        }
-    } else {
-        for_each_tile_balanced(rc, gx, 0ull, [&](uint32_t tile, uint64_t) { atomicAdd(&tc[tile], 1u); });
+    __shared__ uint32_t s_key[kTileSlots], s_cnt[kTileSlots];
+    for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) { s_key[t] = kEmptySlot; s_cnt[t] = 0u; }
+    __syncthreads();
+    for_each_tile_balanced(rc, gx, 0ull, [&](uint32_t tile, uint64_t) {
+        const int slot = tile_slot_insert(s_key, tile);
+        if (slot >= 0) atomicAdd(&s_cnt[slot], 1u);
+        else atomicAdd(&tc[tile], 1u);
+    });
+    __syncthreads();
+    for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) {
+        const uint32_t c = s_cnt[t];
+        if (c) atomicAdd(&tc[s_key[t]], c);
     }
 }
 
@@ -533,7 +528,6 @@ tile_scan_kernel(int n, int T, long long capacity, const uint32_t *__restrict__ 
                  uint32_t *__restrict__ cursor, uint32_t *__restrict__ seg_start, uint32_t *__restrict__ order,
                  int32_t *__restrict__ status)
 {
-    pdl_wait();
     using Scan = cub::BlockScan<unsigned long long, 1024>;
     __shared__ typename Scan::TempStorage tmp;
     __shared__ unsigned long long carry_c, carry_s;
@@ -594,15 +588,13 @@ tile_scan_kernel(int n, int T, long long capacity, const uint32_t *__restrict__ 
 }
 
 // K3: one thread per Gaussian drops (depth bits << 32 | index) into the bucket of every tile its rect touches (large rects are
-// spread over the warp, see for_each_tile_balanced).  kSmemHist: as in K1 the CTA counts into shared memory first, reserves ONE
+// spread over the warp, see for_each_tile_balanced).  As in K1 the CTA counts into the shared-memory tile table first, reserves ONE
 // contiguous run per touched tile with a single global atomic, and hands out the places inside the run with shared-memory atomics.
-template <bool kSmemHist>
 __global__ void __launch_bounds__(256)
 bucket_scatter_kernel(int P, int gx, int T, long long capacity, const float *__restrict__ depth,
                       const uint32_t *__restrict__ tiles, const ushort4 *__restrict__ rect, uint32_t *__restrict__ cursor,
                       uint64_t *__restrict__ bucket)
 {
-    pdl_wait();
     const int b = blockIdx.y;
     const int il = blockIdx.x * blockDim.x + threadIdx.x;
     ushort4 rc = make_ushort4(0, 0, 0, 0);
@@ -615,31 +607,24 @@ bucket_scatter_kernel(int P, int gx, int T, long long capacity, const float *__r
         }
     }
     uint32_t *cur = cursor + (size_t)b * T;
-    if (kSmemHist) {
-        __shared__ uint32_t s_key[kTileSlots], s_cnt[kTileSlots];   // counts, then the next place inside the CTA's run of each tile
-        for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) { s_key[t] = kEmptySlot; s_cnt[t] = 0u; }
-        __syncthreads();
-        for_each_tile_balanced(rc, gx, 0ull, [&](uint32_t tile, uint64_t) {
-            const int slot = tile_slot_insert(s_key, tile);
-            if (slot >= 0) atomicAdd(&s_cnt[slot], 1u);
-        });
-        __syncthreads();
-        for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) {
-            const uint32_t c = s_cnt[t];
-            if (c) s_cnt[t] = atomicAdd(&cur[s_key[t]], c);
-        }
-        __syncthreads();
-        for_each_tile_balanced(rc, gx, key, [&](uint32_t tile, uint64_t k) {
-            const int slot = tile_slot_find(s_key, tile);
-            const uint32_t pos = slot >= 0 ? atomicAdd(&s_cnt[slot], 1u) : atomicAdd(&cur[tile], 1u);
-            if ((long long)pos < capacity) bucket[pos] = k;
-        });
-    } else {
-        for_each_tile_balanced(rc, gx, key, [&](uint32_t tile, uint64_t k) {
-            const uint32_t pos = atomicAdd(&cur[tile], 1u);
-            if ((long long)pos < capacity) bucket[pos] = k;
-        });
+    __shared__ uint32_t s_key[kTileSlots], s_cnt[kTileSlots];   // counts, then the next place inside the CTA's run of each tile
+    for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) { s_key[t] = kEmptySlot; s_cnt[t] = 0u; }
+    __syncthreads();
+    for_each_tile_balanced(rc, gx, 0ull, [&](uint32_t tile, uint64_t) {
+        const int slot = tile_slot_insert(s_key, tile);
+        if (slot >= 0) atomicAdd(&s_cnt[slot], 1u);
+    });
+    __syncthreads();
+    for (int t = threadIdx.x; t < kTileSlots; t += blockDim.x) {
+        const uint32_t c = s_cnt[t];
+        if (c) s_cnt[t] = atomicAdd(&cur[s_key[t]], c);
     }
+    __syncthreads();
+    for_each_tile_balanced(rc, gx, key, [&](uint32_t tile, uint64_t k) {
+        const int slot = tile_slot_find(s_key, tile);
+        const uint32_t pos = slot >= 0 ? atomicAdd(&s_cnt[slot], 1u) : atomicAdd(&cur[tile], 1u);
+        if ((long long)pos < capacity) bucket[pos] = k;
+    });
 }
 
 // Squared distance from a Gaussian's centre beyond which it is certain that the compositing loop skips it
@@ -696,7 +681,6 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
                  float4 *__restrict__ recB, float4 *__restrict__ recC, uint32_t *__restrict__ seg_tile,
                  uint32_t *__restrict__ tile_maxc)
 {
-    pdl_wait();
     extern __shared__ uint64_t s_keys[];
     using BinScan = cub::BlockScan<uint32_t, kThreads>;
     constexpr int kBins = 2 * kThreads;              // at most two depth bins per thread
@@ -863,19 +847,11 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
 // exp(x) for the compositing kernels, x in [-5.6, 0] (anything smaller ends below the 1/255 alpha cut-off): one FMUL + MUFU.EX2 instead
 // of the ~10-instruction library expf.  Relative error <= ~6e-7 (0.5 ulp of x*log2(e) plus ex2.approx's 2 ulp), three orders of
 // magnitude inside the 1e-4 image bar; forward and backward use the same function, so the replay stays consistent.
-// GA_EXACT_EXP=1 builds the library expf instead (measurement aid).
-#ifndef GA_EXACT_EXP
-#define GA_EXACT_EXP 0
-#endif
 __device__ __forceinline__ float comp_exp(float x)
 {
-#if GA_EXACT_EXP
-    return expf(x);
-#else
     float r;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x * 1.4426950408889634f));
     return r;
-#endif
 }
 
 // One compositing step of pixel (pxf, pyf) against a staged record: SURVEY.md §8 a-8 K6 (power > 0 skip, alpha = min(0.99, o e^p),
@@ -922,7 +898,6 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
                   uint32_t *__restrict__ n_contrib, float4 *__restrict__ final_state, uint32_t *__restrict__ tile_maxc,
                   float *__restrict__ out)
 {
-    pdl_wait();
     __shared__ float4 s_a[kBlock / 32][32], s_b[kBlock / 32][32], s_c[kBlock / 32][32];
 
     const int blk = (int)order[blockIdx.x];           // longest tile lists first
@@ -1040,7 +1015,6 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
                   const uint32_t *__restrict__ n_contrib, const float *__restrict__ dL_dout,
                   float2 *__restrict__ d_mean2D, float4 *__restrict__ d_conic_op, float *__restrict__ d_colors)
 {
-    pdl_wait();
     __shared__ float4 s_a[kSeg], s_b[kSeg], s_c[kSeg];
     __shared__ float s_acc[9][kSeg + 1];      // + 1: the 8 lanes that own a Gaussian's 8 sums hit 8 different banks
 
@@ -1181,7 +1155,6 @@ preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *_
                       float *__restrict__ d_means3D, float *__restrict__ d_scales, float *__restrict__ d_rots,
                       float *__restrict__ d_opac, float *__restrict__ d_means2D_out, ColorCov cc)
 {
-    pdl_wait();
     const int fb = blockIdx.y;
     __shared__ float view[16], proj[16];
     if (threadIdx.x < 16) view[threadIdx.x] = cam.view[(size_t)fb * cam.stride + threadIdx.x];
@@ -1345,15 +1318,15 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
     GA_CHECK_CUDA(cudaMemsetAsync(iv.count, 0, sizeof(uint32_t) * BT, stream));
     if (d.P > 0) {
         ProfScope _ps("preprocess_fwd_kernel", stream);
-        auto *k1 = cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true, true> : preprocess_fwd_kernel<true, true, false>)
-                          : (cc.cov3D ? preprocess_fwd_kernel<true, false, true> : preprocess_fwd_kernel<true>);
-        launch_k(k1, dim3(cdiv(d.P, 256), d.B), 256, 0, stream, d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D, a.scales, a.rotations,
+        auto *k1 = cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true> : preprocess_fwd_kernel<true, false>)
+                          : (cc.cov3D ? preprocess_fwd_kernel<false, true> : preprocess_fwd_kernel<>);
+        k1<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D, a.scales, a.rotations,
                  a.rot_stride, a.opacities, a.opac_stride, g.depth, g.xy, g.conic_o, g.cov3d, g.tiles, g.rect, radii, iv.count, cc);
         GA_CHECK_LAUNCH("preprocess_fwd_kernel");
     }
     {
         ProfScope _ps("tile_scan_kernel", stream);
-        launch_k(tile_scan_kernel, 1, 1024, 0, stream, (int)BT, d.T, capacity, iv.count, iv.ranges, iv.cursor, iv.seg_start, iv.order, iv.status);
+        tile_scan_kernel<<<1, 1024, 0, stream>>>((int)BT, d.T, capacity, iv.count, iv.ranges, iv.cursor, iv.seg_start, iv.order, iv.status);
     }
     GA_CHECK_LAUNCH("tile_scan_kernel");
     return GA_OK;
@@ -1372,25 +1345,25 @@ int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacit
     if (d.P > 0) {
         {
             ProfScope _ps("bucket_scatter_kernel", stream);
-            launch_k(bucket_scatter_kernel<true>, dim3(cdiv(d.P, 256), d.B), 256, 0, stream, d.P, d.gx, d.T, capacity, g.depth, g.tiles, g.rect, iv.cursor,
-                                                                                      bv.bucket);
+            bucket_scatter_kernel<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(d.P, d.gx, d.T, capacity, g.depth, g.tiles, g.rect, iv.cursor,
+                                                                                bv.bucket);
         }
         GA_CHECK_LAUNCH("bucket_scatter_kernel");
     }
     {
         ProfScope _ps("tile_sort_kernel", stream);
-        launch_k(tile_sort_kernel<kSortThreads, kSortMax, true>, min(BT, 3 * num_sms()), kSortThreads, kSortMax * sizeof(uint64_t), stream,
+        tile_sort_kernel<kSortThreads, kSortMax, true><<<min(BT, 3 * num_sms()), kSortThreads, kSortMax * sizeof(uint64_t), stream>>>(
                  d.P, d.T, BT, iv.status, iv.order, iv.ranges, iv.seg_start, bv.bucket, g.xy, g.conic_o, a.colors, bv.point_list, bv.recA, bv.recB,
                  bv.recC, bv.seg_tile, iv.tile_maxc);
         count_launch();
-        launch_k(tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false>, min(BT, 12 * num_sms()), kSortSmallThreads,
-                 kSortSmallMax * sizeof(uint64_t), stream, d.P, d.T, BT, iv.status, iv.order, iv.ranges, iv.seg_start, bv.bucket, g.xy, g.conic_o,
-                 a.colors, bv.point_list, bv.recA, bv.recB, bv.recC, bv.seg_tile, iv.tile_maxc);
+        tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false><<<min(BT, 12 * num_sms()), kSortSmallThreads, kSortSmallMax * sizeof(uint64_t), stream>>>(
+                 d.P, d.T, BT, iv.status, iv.order, iv.ranges, iv.seg_start, bv.bucket, g.xy, g.conic_o, a.colors, bv.point_list, bv.recA, bv.recB,
+                 bv.recC, bv.seg_tile, iv.tile_maxc);
     }
     GA_CHECK_LAUNCH("tile_sort_kernel");
     {
         ProfScope _ps("render_fwd_kernel", stream);
-        launch_k(render_fwd_kernel, BT, kBlock, 0, stream, d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC, a.bg, bv.ckpt,
+        render_fwd_kernel<<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC, a.bg, bv.ckpt,
                                                     iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color);
     }
     GA_CHECK_LAUNCH("render_fwd_kernel");
@@ -1424,11 +1397,11 @@ int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, ColorCov
         ProfScope _ps("render_bwd_kernel", stream);
         const int grid = (int)bv.max_segments;
         if (a.d_opacities)
-            launch_k(render_bwd_kernel<true>, grid, kBlock, 0, stream, d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges,
+            render_bwd_kernel<true><<<grid, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges,
                                                                  iv.tile_maxc, bv.recA, bv.recB, bv.recC, bv.ckpt, a.bg, iv.final_state,
                                                                  iv.n_contrib, a.dL_dout, d_mean2D, d_conic_op, a.d_colors);
         else
-            launch_k(render_bwd_kernel<false>, grid, kBlock, 0, stream, d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges,
+            render_bwd_kernel<false><<<grid, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges,
                                                                   iv.tile_maxc, bv.recA, bv.recB, bv.recC, bv.ckpt, a.bg, iv.final_state,
                                                                   iv.n_contrib, a.dL_dout, d_mean2D, d_conic_op, a.d_colors);
     }
@@ -1438,7 +1411,7 @@ int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, ColorCov
         cc.d_rgb = a.d_colors;
         auto *k89 = cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<true, false>)
                            : (cc.cov3D ? preprocess_bwd_kernel<false, true> : preprocess_bwd_kernel<>);
-        launch_k(k89, dim3(cdiv(d.P, 256), d.B), 256, 0, stream, d.P, d.H, d.W, cam, a.mod, a.means3D, a.scales, a.rotations, a.rot_stride,
+        k89<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(d.P, d.H, d.W, cam, a.mod, a.means3D, a.scales, a.rotations, a.rot_stride,
                  radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D, a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D, cc);
     }
     GA_CHECK_LAUNCH("preprocess_bwd_kernel");
@@ -1598,7 +1571,6 @@ namespace ga {
 namespace {
 __global__ void stamp_serial_kernel(int32_t *status, const int32_t *serial)
 {
-    pdl_wait();
     status[kStatusInts - 1] = *serial;
 }
 }  // namespace
@@ -1613,7 +1585,7 @@ extern "C" int ga_rasterb_status_to_host(int32_t B, int32_t H, int32_t W, void *
     GA_REQUIRE(img && serial_dev && host16, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     int32_t *status = carve_img(img, make_dims(B, 0, H, W)).status;
-    launch_k(stamp_serial_kernel, 1, 1, 0, stream, status, serial_dev);
+    stamp_serial_kernel<<<1, 1, 0, stream>>>(status, serial_dev);
     GA_CHECK_LAUNCH("stamp_serial_kernel");
     GA_CHECK_CUDA(cudaMemcpyAsync(host16, status, sizeof(int32_t) * kStatusInts, cudaMemcpyDeviceToHost, stream));
     return GA_OK;

@@ -58,7 +58,6 @@ smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
                 float *__restrict__ G_out /*[B,kJ,12] saved for backward*/, const float *__restrict__ rest /*[B,99] (SMPL-X)*/)
 {
     constexpr int kThreads = Body<kJ>::kThreads;
-    pdl_wait();
     __shared__ float sL[kJ][12], sG[kJ][12];
     const int b = blockIdx.x, j = threadIdx.x;
     if (b >= B) return;
@@ -116,7 +115,6 @@ smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
                 float *__restrict__ d_pose /*[B,3 kTrain]*/, float *__restrict__ d_transl /*[B,3]*/, const float *__restrict__ rest)
 {
     constexpr int kThreads = Body<kJ>::kThreads, kT = Body<kJ>::kTrain;
-    pdl_wait();
     __shared__ float sL[kJ][12], sG[kJ][12], sdG[kJ][12], sdL[kJ][9];
     const int b = blockIdx.x, j = threadIdx.x;
     if (b >= B) return;
@@ -234,7 +232,7 @@ extern "C" int ga_smpl_forward(int32_t B, const float *pose, const float *transl
     GA_REQUIRE(B >= 0, "bad batch %d", B);
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && transl && rest_joints && inv_cano && cano2live && saved_G, "NULL pointer argument");
-    { ProfScope _ps("smpl_fwd_kernel", static_cast<cudaStream_t>(stream_)); launch_k(smpl_fwd_kernel<24>, B, 32, 0, static_cast<cudaStream_t>(stream_), B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, nullptr); }
+    { ProfScope _ps("smpl_fwd_kernel", static_cast<cudaStream_t>(stream_)); smpl_fwd_kernel<24><<<B, 32, 0, static_cast<cudaStream_t>(stream_)>>>(B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, nullptr); }
     GA_CHECK_LAUNCH("smpl_fwd_kernel");
     return GA_OK;
 }
@@ -245,7 +243,7 @@ extern "C" int ga_smpl_backward(int32_t B, const float *pose, const float *rest_
     GA_REQUIRE(B >= 0, "bad batch %d", B);
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && rest_joints && inv_cano && saved_G && d_cano2live && d_pose && d_transl, "NULL pointer argument");
-    { ProfScope _ps("smpl_bwd_kernel", static_cast<cudaStream_t>(stream_)); launch_k(smpl_bwd_kernel<24>, B, 32, 0, static_cast<cudaStream_t>(stream_), B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, nullptr); }
+    { ProfScope _ps("smpl_bwd_kernel", static_cast<cudaStream_t>(stream_)); smpl_bwd_kernel<24><<<B, 32, 0, static_cast<cudaStream_t>(stream_)>>>(B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, nullptr); }
     GA_CHECK_LAUNCH("smpl_bwd_kernel");
     return GA_OK;
 }
@@ -257,7 +255,7 @@ extern "C" int ga_smplx_forward(int32_t B, const float *pose, const float *rest_
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && rest_pose && transl && rest_joints && inv_cano && cano2live && saved_G, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    { ProfScope _ps("smplx_fwd_kernel", stream); launch_k(smpl_fwd_kernel<55>, B, Body<55>::kThreads, 0, stream, B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, rest_pose); }
+    { ProfScope _ps("smplx_fwd_kernel", stream); smpl_fwd_kernel<55><<<B, Body<55>::kThreads, 0, stream>>>(B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, rest_pose); }
     GA_CHECK_LAUNCH("smplx_fwd_kernel");
     return GA_OK;
 }
@@ -269,7 +267,7 @@ extern "C" int ga_smplx_backward(int32_t B, const float *pose, const float *rest
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && rest_pose && rest_joints && inv_cano && saved_G && d_cano2live && d_pose && d_transl, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    { ProfScope _ps("smplx_bwd_kernel", stream); launch_k(smpl_bwd_kernel<55>, B, Body<55>::kThreads, 0, stream, B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, rest_pose); }
+    { ProfScope _ps("smplx_bwd_kernel", stream); smpl_bwd_kernel<55><<<B, Body<55>::kThreads, 0, stream>>>(B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, rest_pose); }
     GA_CHECK_LAUNCH("smplx_bwd_kernel");
     return GA_OK;
 }

@@ -230,8 +230,7 @@ class Stage1Trainer:
         return (self.use_graph and isinstance(m.optimizer, FusedAdam) and getattr(m.model_parms, "train_stage", 1) != 2
                 and iteration >= 1000 and epoch <= self.opt.pose_op_start_iter
                 and not (self.perceptual_loss is not None and not isinstance(self.perceptual_loss, LPIPS) and epoch > self.opt.lpips_start_iter)
-                and torch.is_tensor(img) and img.is_cuda and img.shape[0] <= 8 and os.environ.get("GA_RASTER_BATCHED", "1") != "0"
-                and m._uniform_frames(batch, img.shape[0]))
+                and torch.is_tensor(img) and img.is_cuda and img.shape[0] <= 8 and m._uniform_frames(batch, img.shape[0]))
 
     def _capture(self, batch, iteration, epoch, key):
         m = self.model
