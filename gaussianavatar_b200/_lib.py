@@ -86,6 +86,8 @@ _SIGNATURES = {
     "ga_lbs_forward_ex": (ctypes.c_int, [ctypes.c_int32] * 4 + [ctypes.c_float, ctypes.c_int64] + [c_vp] * 9),
     "ga_lbs_backward_ex": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float, ctypes.c_int64] + [c_vp] * 11),
     "ga_smpl_vertices": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 8),
+    "ga_smplx_vertices": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 9),
+    "ga_posmap_weights": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 6),
     "ga_posmap_layout": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 4),
     "ga_posmap_fill": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp] * 6),
     "ga_decoder_layout":(ctypes.c_int, [ctypes.POINTER(GaDecoderDesc), ctypes.POINTER(GaDecoderLayout)]),

@@ -133,6 +133,141 @@ smpl_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,72]*/, co
     }
 }
 
+// ---- SMPL-X (55 joints: global, 21 body, jaw, eyes, 2 x 15 finger joints; kintree_table[0] of SMPLX_*.npz)
+constexpr int kJointsX = 55;
+constexpr int kTrainX = 22;                      // joints taken from pose [B,66]; the other 33 from rest_pose [B,99]
+constexpr int kPoseFeatX = 9 * (kJointsX - 1);   // 486 pose blend-shape coefficients
+
+__constant__ int c_parents_vx[kJointsX] = {-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 15, 15, 15, 20,
+                                           25, 26, 20, 28, 29, 20, 31, 32, 20, 34, 35, 20, 37, 38, 21, 40, 41, 21, 43, 44, 21, 46, 47,
+                                           21, 49, 50, 21, 52, 53};
+
+// 56.4 KB, above the 48 KB of static shared memory: dynamic, with the opt-in.  The local transforms are dead once A is formed, so
+// the row-group partial sums reuse their space.
+struct SmplxVertSmem {
+    float A[kMaxB][kJointsX][12];
+    float feat[kMaxB][kPoseFeatX];
+    union {
+        float L[kMaxB][kJointsX][12];
+        float part[kRowGroups][kMaxB][kCols];
+    } u;
+};
+
+// The SMPL-X counterpart of smpl_vertices_kernel, same three phases.  55 joints do not fit one lane each in a warp per frame, so
+// the B x 55 (frame, joint) pairs are spread over the whole CTA; each pair still forms its own product of ancestors, so a frame's
+// result does not depend on the batch it is in.
+__global__ void __launch_bounds__(kVertThreads)
+smplx_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,66]*/, const float *__restrict__ rest_pose /*[B,99]*/,
+                      const float *__restrict__ transl /*[B,3]*/, const float *__restrict__ J /*[55,3]*/,
+                      const float *__restrict__ v_shaped /*[V,3]*/, const float *__restrict__ posedirs /*[486,3V]*/,
+                      const float *__restrict__ weights /*[V,55]*/, float *__restrict__ verts /*[B,V,3]*/)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    SmplxVertSmem &sm = *reinterpret_cast<SmplxVertSmem *>(smem_raw);
+    const int tid = threadIdx.x;
+    for (int i = tid; i < B * kJointsX; i += kVertThreads) {
+        const int b = i / kJointsX, j = i % kJointsX;
+        const float *src = (j < kTrainX) ? pose + (size_t)b * (3 * kTrainX) + j * 3
+                                         : rest_pose + (size_t)b * (3 * (kJointsX - kTrainX)) + (j - kTrainX) * 3;
+        const float r[3] = {src[0], src[1], src[2]};
+        float R[9], th;
+        rodrigues(r, R, &th);
+        const int p = c_parents_vx[j];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            sm.u.L[b][j][k * 4 + 0] = R[k * 3 + 0]; sm.u.L[b][j][k * 4 + 1] = R[k * 3 + 1]; sm.u.L[b][j][k * 4 + 2] = R[k * 3 + 2];
+            sm.u.L[b][j][k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
+        }
+        if (j > 0) {
+#pragma unroll
+            for (int k = 0; k < 9; ++k) sm.feat[b][(j - 1) * 9 + k] = R[k] - ((k % 4 == 0) ? 1.f : 0.f);
+        }
+    }
+    __syncthreads();
+    for (int i = tid; i < B * kJointsX; i += kVertThreads) {
+        const int b = i / kJointsX, j = i % kJointsX;
+        float G[12], T[12];
+#pragma unroll
+        for (int k = 0; k < 12; ++k) G[k] = sm.u.L[b][j][k];
+        for (int p = c_parents_vx[j]; p >= 0; p = c_parents_vx[p]) {
+            aff_mul(sm.u.L[b][p], G, T);
+#pragma unroll
+            for (int k = 0; k < 12; ++k) G[k] = T[k];
+        }
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            sm.A[b][j][r * 4 + 0] = G[r * 4 + 0]; sm.A[b][j][r * 4 + 1] = G[r * 4 + 1]; sm.A[b][j][r * 4 + 2] = G[r * 4 + 2];
+            sm.A[b][j][r * 4 + 3] = G[r * 4 + 3] - (G[r * 4 + 0] * J[j * 3] + G[r * 4 + 1] * J[j * 3 + 1] + G[r * 4 + 2] * J[j * 3 + 2]);
+        }
+    }
+    __syncthreads();        // L is dead from here on: part may overwrite it
+
+    const int col = tid % kCols, rg = tid / kCols;
+    const long long ncol = 3LL * V;
+    const long long k = (long long)blockIdx.x * kCols + col;
+    float acc[kMaxB];
+#pragma unroll
+    for (int b = 0; b < kMaxB; ++b) acc[b] = 0.f;
+    if (k < ncol) {
+#pragma unroll 4
+        for (int r = rg; r < kPoseFeatX; r += kRowGroups) {
+            const float pd = __ldg(posedirs + (long long)r * ncol + k);
+#pragma unroll
+            for (int b = 0; b < kMaxB; ++b)
+                if (b < B) acc[b] = fmaf(sm.feat[b][r], pd, acc[b]);
+        }
+    }
+#pragma unroll
+    for (int b = 0; b < kMaxB; ++b)
+        if (b < B) sm.u.part[rg][b][col] = acc[b];
+    __syncthreads();
+
+    for (int i = tid; i < kVertsPerCta * B; i += kVertThreads) {
+        const int vl = i % kVertsPerCta, b = i / kVertsPerCta;
+        const int v = blockIdx.x * kVertsPerCta + vl;
+        if (v >= V) continue;
+        float x[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            float off = 0.f;
+#pragma unroll
+            for (int g = 0; g < kRowGroups; ++g) off += sm.u.part[g][b][vl * 3 + c];
+            x[c] = v_shaped[(size_t)v * 3 + c] + off;
+        }
+        float T[12];
+#pragma unroll
+        for (int q = 0; q < 12; ++q) T[q] = 0.f;
+        const float *w = weights + (size_t)v * kJointsX;
+        for (int j = 0; j < kJointsX; ++j) {
+            const float wj = w[j];
+#pragma unroll
+            for (int q = 0; q < 12; ++q) T[q] = fmaf(wj, sm.A[b][j][q], T[q]);
+        }
+        float *o = verts + ((size_t)b * V + v) * 3;
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+            o[r] = T[r * 4 + 0] * x[0] + T[r * 4 + 1] * x[1] + T[r * 4 + 2] * x[2] + T[r * 4 + 3] + transl[b * 3 + r];
+    }
+}
+
+// out[t, j] = sum_i bary[t, i] W[faces[face_id[t], i], j] (fp32, i in order), 0 where face_id is -1: the texel skinning weights of
+// the reference's gen_lbs_weight_from_ori (utils/general_utils.py:245-259).  One thread per output element, so the stores coalesce.
+__global__ void __launch_bounds__(256)
+posmap_weights_kernel(int n, int J, const float *__restrict__ W, const int *__restrict__ faces, const int *__restrict__ face_id,
+                      const float *__restrict__ bary, float *__restrict__ out)
+{
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const int t = e / J, j = e - t * J;
+    const int f = face_id[t];
+    float o = 0.f;
+    if (f >= 0) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) o = fmaf(bary[(size_t)t * 3 + i], W[(size_t)faces[(size_t)f * 3 + i] * J + j], o);
+    }
+    out[e] = o;
+}
+
 struct Snapped { long long x[3], y[3]; bool ok; };
 
 __device__ __forceinline__ Snapped snap_face(const float *__restrict__ uv, int f, int S)
@@ -259,6 +394,38 @@ extern "C" int ga_smpl_vertices(int32_t B, int32_t V, const float *pose, const f
       smpl_vertices_kernel<<<cdiv(V, kVertsPerCta), kVertThreads, 0, stream>>>(B, V, pose, transl, rest_joints, v_shaped, posedirs,
                weights, verts); }
     GA_CHECK_LAUNCH("smpl_vertices_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_smplx_vertices(int32_t B, int32_t V, const float *pose, const float *rest_pose, const float *transl, const float *rest_joints,
+                                 const float *v_shaped, const float *posedirs, const float *weights, float *verts, void *stream_)
+{
+    GA_REQUIRE(B >= 0 && B <= kMaxB, "ga_smplx_vertices: batch %d outside [0, %d]", B, kMaxB);
+    GA_REQUIRE(V > 0 && V <= (1 << 24), "ga_smplx_vertices: bad vertex count %d", V);
+    if (B == 0) return GA_OK;
+    GA_REQUIRE(pose && rest_pose && transl && rest_joints && v_shaped && posedirs && weights && verts, "NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    static PerDeviceOnce attr_set;
+    if (attr_set.first())
+        GA_CHECK_CUDA(cudaFuncSetAttribute(smplx_vertices_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmplxVertSmem)));
+    { ProfScope _ps("smplx_vertices_kernel", stream);
+      smplx_vertices_kernel<<<cdiv(V, kVertsPerCta), kVertThreads, sizeof(SmplxVertSmem), stream>>>(B, V, pose, rest_pose, transl, rest_joints,
+               v_shaped, posedirs, weights, verts); }
+    GA_CHECK_LAUNCH("smplx_vertices_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_posmap_weights(int32_t S, int32_t J, const float *weights, const int32_t *faces, const int32_t *face_id, const float *bary,
+                                 float *out, void *stream_)
+{
+    GA_REQUIRE(S >= 1 && S <= kMaxS, "ga_posmap_weights: map size %d outside [1, %d]", S, kMaxS);
+    GA_REQUIRE(J == kJoints || J == kJointsX, "ga_posmap_weights: joint count %d is neither %d (SMPL) nor %d (SMPL-X)", J, kJoints, kJointsX);
+    GA_REQUIRE(weights && faces && face_id && bary && out, "NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const int n = S * S * J;
+    { ProfScope _ps("posmap_weights_kernel", stream);
+      posmap_weights_kernel<<<cdiv(n, 256), 256, 0, stream>>>(n, J, weights, faces, face_id, bary, out); }
+    GA_CHECK_LAUNCH("posmap_weights_kernel");
     return GA_OK;
 }
 

@@ -207,18 +207,23 @@ def make_smplx_body(seed: int = 0) -> SyntheticBody:
                          W.float(), betas.float())
 
 
-def write_smplx_model_npz(path: str, body: SyntheticBody, seed: int = 0) -> None:
+def write_smplx_model_npz(path: str, body: SyntheticBody, seed: int = 0, posedirs=None, faces=None) -> None:
     """SMPLX_{GENDER}.npz in the layout the reference's `smplx.SMPLX(..., use_pca=False, flat_hand_mean=True)` loads: faces,
-    template, shape / pose directions (pose directions zero), dense J_regressor, kintree_table, skinning weights, hand PCA
-    placeholders and the landmark embedding."""
+    template, shape / pose directions, dense J_regressor, kintree_table, skinning weights, hand PCA placeholders and the landmark
+    embedding.  By default the pose directions are zero and the faces random; posedirs [486, 3V] (smplx_posedirs) and faces [F,3]
+    (a template's, make_smplx_uv_template) make a model whose mesh can be posed and drawn into position maps."""
     rng = np.random.default_rng(seed)
     V, nj = body.v_template.shape[0], len(SMPLX_PARENTS)
     kt = np.zeros((2, nj), np.int64)
     kt[0] = SMPLX_PARENTS
     kt[0, 0] = 4294967295          # uint32 -1, as the released model files store it
     kt[1] = np.arange(nj)
-    np.savez_compressed(path, f=rng.integers(0, V, (20908, 3)).astype(np.int64), v_template=body.v_template.double().numpy(),
-                        shapedirs=body.shapedirs.double().numpy(), posedirs=np.zeros((V, 3, 486), np.float32),
+    f = rng.integers(0, V, (20908, 3)).astype(np.int64)
+    if faces is not None:
+        f = np.asarray(faces, np.int64)
+    pd = np.zeros((V, 3, 486), np.float32) if posedirs is None else _posedirs_per_vertex(posedirs, V, 486)
+    np.savez_compressed(path, f=f, v_template=body.v_template.double().numpy(),
+                        shapedirs=body.shapedirs.double().numpy(), posedirs=pd,
                         J_regressor=body.J_regressor.double().numpy(), kintree_table=kt, weights=body.lbs_weights.double().numpy(),
                         hands_componentsl=np.eye(45), hands_componentsr=np.eye(45), hands_meanl=rng.normal(size=45) * 0.1,
                         hands_meanr=rng.normal(size=45) * 0.1, lmk_faces_idx=np.arange(51, dtype=np.int64),
@@ -280,9 +285,21 @@ def make_uv_template(seed: int = 0, jitter: float = 0.2):
     row-major, 13416 faces.  The atlas has two islands side by side: columns 0..64 in u 0.02..0.48 and columns 64..129 in u
     0.52..0.98, so column 64 has two texture coordinates (a seam) and the vt indices differ from the v indices.  Interior texture
     coordinates are jittered by up to `jitter` of a cell."""
-    R, C = UV_GRID
-    g = np.random.default_rng(4000 + seed)
-    islands = [(np.arange(0, 65), 0.02, 0.48), (np.arange(64, C), 0.52, 0.98)]
+    return _grid_uv_template(UV_GRID, 64, np.random.default_rng(4000 + seed), jitter, make_body(seed).v_template.double().numpy())
+
+
+UV_GRID_X = (50, 209)    # the SMPL-X template's grid: 10450 of the 10475 vertices (the last 25 belong to no face)
+
+
+def make_smplx_uv_template(seed: int = 0, jitter: float = 0.2):
+    """The SMPL-X counterpart of make_uv_template: a 50 x 209 grid over the first 10450 synthetic SMPL-X vertices (the other 25
+    belong to no face), 20384 faces, two islands with the seam at column 104."""
+    return _grid_uv_template(UV_GRID_X, 104, np.random.default_rng(4500 + seed), jitter, make_smplx_body(seed).v_template.double().numpy())
+
+
+def _grid_uv_template(grid, seam, g, jitter, verts):
+    R, C = grid
+    islands = [(np.arange(0, seam + 1), 0.02, 0.48), (np.arange(seam, C), 0.52, 0.98)]
     uvs, vt_of = [], []
     for cols, u0, u1 in islands:
         n = cols.size
@@ -300,7 +317,7 @@ def make_uv_template(seed: int = 0, jitter: float = 0.2):
     faces, faces_uv = [], []
     for r in range(R - 1):
         for c in range(C - 1):
-            isl = vt_of[0] if c < 64 else vt_of[1]
+            isl = vt_of[0] if c < seam else vt_of[1]
             a, b, cc, d = (r, c), (r, c + 1), (r + 1, c + 1), (r + 1, c)
             tris = [(a, b, cc), (a, cc, d)] if (r + c) % 2 == 0 else [(a, b, d), (b, cc, d)]
             for t in tris:
@@ -310,7 +327,6 @@ def make_uv_template(seed: int = 0, jitter: float = 0.2):
     p = uvs[faces_uv]
     area = (p[:, 1, 0] - p[:, 0, 0]) * (p[:, 2, 1] - p[:, 0, 1]) - (p[:, 1, 1] - p[:, 0, 1]) * (p[:, 2, 0] - p[:, 0, 0])
     assert (area > 0).all(), "jitter folded a triangle"
-    verts = make_body(seed).v_template.double().numpy()
     return verts, faces, uvs, faces_uv
 
 
@@ -330,6 +346,26 @@ def smpl_mesh_model(body: SyntheticBody, template) -> dict:
     return dict(v_template=body.v_template.numpy(), shapedirs=body.shapedirs.numpy(), J_regressor=body.J_regressor.numpy(),
                 posedirs=body.posedirs.T.reshape(V, 3, 207).contiguous().numpy(), weights=body.lbs_weights.numpy(),
                 f=np.asarray(template[1], np.uint32), kintree_table=np.stack([np.array(SMPL_PARENTS), np.arange(24)]))
+
+
+def smplx_posedirs(seed: int = 0) -> torch.Tensor:
+    """Non-zero SMPL-X pose blend shapes [486, 3 * 10475] (the layout smplx.SMPLX keeps), of the scale of make_body's."""
+    g = torch.Generator().manual_seed(5500 + seed)
+    return (torch.randn(486, SMPLX_NUM_VERTS * 3, generator=g, dtype=torch.float64) * 0.001).float()
+
+
+def _posedirs_per_vertex(posedirs, V, n) -> np.ndarray:
+    """[n, 3V] -> [V,3,n], the layout of the model files."""
+    return torch.as_tensor(posedirs).T.reshape(V, 3, n).contiguous().numpy()
+
+
+def smplx_mesh_model(body: SyntheticBody, template, posedirs) -> dict:
+    """The fields of SMPLX_{GENDER}.npz the position maps need, for a synthetic SMPL-X body: v_template, shapedirs, posedirs
+    [V,3,486], weights [V,55], f (the template's faces), J_regressor, kintree_table."""
+    V = body.v_template.shape[0]
+    return dict(v_template=body.v_template.numpy(), shapedirs=body.shapedirs.numpy(), J_regressor=body.J_regressor.numpy(),
+                posedirs=_posedirs_per_vertex(posedirs, V, 486), weights=body.lbs_weights.numpy(),
+                f=np.asarray(template[1], np.int64), kintree_table=np.stack([np.array(SMPLX_PARENTS), np.arange(55)]))
 
 
 def synthetic_smplx_poses(n: int, seed: int = 0) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor]:

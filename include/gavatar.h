@@ -202,6 +202,17 @@ int ga_smplx_backward(int32_t B, const float *pose, const float *rest_pose, cons
  * ---------------------------------------------------------------------------------------------------------------- */
 int ga_smpl_vertices(int32_t B, int32_t V, const float *pose, const float *transl, const float *rest_joints, const float *v_shaped,
                      const float *posedirs, const float *weights, float *verts, void *stream);
+/* ga_smplx_vertices: the SMPL-X counterpart of ga_smpl_vertices (smplx.SMPLX(use_pca=False, flat_hand_mean=True) vertices +
+ *   transl, body_models.py:1273-1275): pose [B,66] (global + 21 body joints), rest_pose [B,99] (jaw, left / right eye, 15 + 15
+ *   finger joints), transl [B,3], rest_joints [55,3], v_shaped [V,3], posedirs [486, 3V], weights [V,55] -> verts [B,V,3], B <= 8.
+ *   posedirs is read once per call for all B frames, and a frame's result does not depend on the batch it is in.
+ * ga_posmap_weights: the texel skinning-weight map out [S,S,J] = sum_i bary_i weights[faces[face_id, i], :] (0 where face_id is
+ *   -1), J = 24 or 55; weights [V,J], faces [F,3] int32 indexing vertices below V, face_id / bary from ga_posmap_layout over the
+ *   same F faces (utils/general_utils.py:245-259, the lbs_map_{body}_{S}.npy format).  Every element of `out` is written. */
+int ga_smplx_vertices(int32_t B, int32_t V, const float *pose, const float *rest_pose, const float *transl, const float *rest_joints,
+                      const float *v_shaped, const float *posedirs, const float *weights, float *verts, void *stream);
+int ga_posmap_weights(int32_t S, int32_t J, const float *weights, const int32_t *faces, const int32_t *face_id, const float *bary,
+                      float *out, void *stream);
 int ga_posmap_layout(int32_t F, int32_t S, const float *uv_corners, int32_t *face_id, float *bary, void *stream);
 int ga_posmap_fill(int32_t B, int32_t S, int32_t V, const float *verts, const int32_t *faces, const int32_t *face_id,
                    const float *bary, float *out, void *stream);

@@ -2,11 +2,14 @@
 
     python tools/pose_maps.py FOLDER --smpl_model SMPL_NEUTRAL.pkl --uv_template template_mesh_smpl_uv.obj --size 128
     python tools/pose_maps.py FOLDER ... --check [--uv_mask uv_mask128_with_faceid_smpl.npy]
+    python tools/pose_maps.py FOLDER --body smplx --smpl_model SMPLX_NEUTRAL.npz --uv_template template_mesh_smplx_uv.obj --size 128
 
 Reads the SMPL parameters of FOLDER (smpl_parms_pred.pth if it exists, which is what the stage-2 datasets read, else
 smpl_parms.pth; or --params), builds every frame's map with gaussianavatar_b200.posmap.PoseMapper and writes
 FOLDER/inp_map/inp_posemap_{S}_{idx:08d}.npz with the key posmap{S}, [S,S,3] float32: the files the reference's
-scripts/gen_pose_map_our_smpl.py renders with OpenGL.
+scripts/gen_pose_map_our_smpl.py renders with OpenGL.  With --body smplx the model is an SMPLX_{GENDER}.npz and each frame's
+body_pose [165] splits into the pose [:66] and the jaw, eye and hand pose [66:] (scene/dataset_mono.py:141-146), posed by
+gaussianavatar_b200.posmap.SmplxPoseMapper.
 
 --check writes nothing: it compares the maps with the files already in FOLDER/inp_map (and the face ids with --uv_mask, the
 reference's uv_mask{S}_with_faceid_smpl.npy) and prints one JSON line with the largest absolute map difference and the number of
@@ -22,7 +25,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from gaussianavatar_b200.posmap import PoseMapper  # noqa: E402
+from gaussianavatar_b200.posmap import PoseMapper, SmplxPoseMapper, load_body_model  # noqa: E402
 
 CHUNK = 64      # frames per device call
 
@@ -30,7 +33,8 @@ CHUNK = 64      # frames per device call
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("folder")
-    ap.add_argument("--smpl_model", required=True, help="SMPL_{GENDER}.pkl")
+    ap.add_argument("--body", choices=("smpl", "smplx"), default="smpl")
+    ap.add_argument("--smpl_model", required=True, help="SMPL_{GENDER}.pkl (--body smplx: SMPLX_{GENDER}.npz)")
     ap.add_argument("--uv_template", required=True, help="template_mesh_smpl_uv.obj")
     ap.add_argument("--size", type=int, default=128)
     ap.add_argument("--params", default=None, help="SMPL parameter file in FOLDER (default: smpl_parms_pred.pth, else smpl_parms.pth)")
@@ -43,15 +47,23 @@ def main(argv=None):
     pose = torch.as_tensor(smpl_data["body_pose"]).float()
     transl = torch.as_tensor(smpl_data["trans"]).float()
     beta = torch.as_tensor(smpl_data["beta"]).float().reshape(-1, 10)[0]
-    with open(a.smpl_model, "rb") as fh:
-        sm = pickle.load(fh, encoding="latin1")
-    mapper = PoseMapper(sm, beta, a.uv_template, S)
+    if a.body == "smplx":
+        mapper = SmplxPoseMapper(load_body_model(a.smpl_model), beta, a.uv_template, S)
+        pose, rest_pose = pose[:, :66], pose[:, 66:]
+    else:
+        with open(a.smpl_model, "rb") as fh:
+            sm = pickle.load(fh, encoding="latin1")
+        mapper = PoseMapper(sm, beta, a.uv_template, S)
     out_dir = os.path.join(a.folder, "inp_map")
     if not a.check:
         os.makedirs(out_dir, exist_ok=True)
     max_err, n_missing = 0.0, 0
     for s in range(0, pose.shape[0], CHUNK):
-        maps = mapper(pose[s:s + CHUNK], transl[s:s + CHUNK]).permute(0, 2, 3, 1).cpu().numpy()      # [b,S,S,3]
+        if a.body == "smplx":
+            maps = mapper(pose[s:s + CHUNK], rest_pose[s:s + CHUNK], transl[s:s + CHUNK])
+        else:
+            maps = mapper(pose[s:s + CHUNK], transl[s:s + CHUNK])
+        maps = maps.permute(0, 2, 3, 1).cpu().numpy()      # [b,S,S,3]
         for i, m in enumerate(maps):
             fn = os.path.join(out_dir, "inp_posemap_%s_%s.npz" % (S, str(s + i).zfill(8)))
             if a.check:
