@@ -125,6 +125,8 @@ _SIGNATURES = {
     "ga_lpips_views": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp, ctypes.POINTER(GaLpipsViews)]),
     "ga_metrics_partials_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 4),
     "ga_metrics_ssim_sse": (ctypes.c_int, [ctypes.c_int32] * 4 + [c_vp, c_vp, ctypes.c_float] + [c_vp] * 4),
+    "ga_mesh_render_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 5),
+    "ga_mesh_render": (ctypes.c_int, [ctypes.c_int32] * 5 + [c_vp] * 5 + [ctypes.c_float] * 3 + [c_vp] * 6),
 }
 
 _lib = None

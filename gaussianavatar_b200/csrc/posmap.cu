@@ -18,6 +18,7 @@
 //     functions exact);
 //   - barycentric weights from the snapped coordinates: w_i = E_i / area in fp64, rounded to fp32.
 #include "common.cuh"
+#include "fixed_raster.cuh"
 #include "smpl_math.cuh"
 
 namespace ga {
@@ -279,21 +280,10 @@ __device__ __forceinline__ Snapped snap_face(const float *__restrict__ uv, int f
     for (int i = 0; i < 3; ++i) {
         const float u = uv[(size_t)f * 6 + i * 2], v = uv[(size_t)f * 6 + i * 2 + 1];
         if (!(fabsf(u) <= 4096.f) || !(fabsf(v) <= 4096.f)) s.ok = false;     // also false for NaN
-        s.x[i] = s.ok ? __double2ll_rn((double)u * scale) : 0;
-        s.y[i] = s.ok ? __double2ll_rn((double)v * scale) : 0;
+        s.x[i] = s.ok ? snap_fixed((double)u * scale) : 0;
+        s.y[i] = s.ok ? snap_fixed((double)v * scale) : 0;
     }
     return s;
-}
-
-// edge function of (a -> b) at p: > 0 when p is to the left (y up)
-__device__ __forceinline__ long long edge_fn(long long ax, long long ay, long long bx, long long by, long long px, long long py)
-{
-    return (bx - ax) * (py - ay) - (by - ay) * (px - ax);
-}
-
-__device__ __forceinline__ bool edge_owns(long long e, long long dx, long long dy)
-{
-    return e > 0 || (e == 0 && (dy < 0 || (dy == 0 && dx < 0)));
 }
 
 // One thread per face: walk the texel centres of its bounding box and keep the lowest covering face index per texel.

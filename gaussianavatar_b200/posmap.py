@@ -5,7 +5,8 @@ one OBJ per frame, then an OpenGL render of each mesh in UV space.  Because that
 texel (and with which barycentric weights) does not depend on the pose: `PoseMapper` computes that layout once on the device
 (`ga_posmap_layout`), and a frame costs the posed vertices (`ga_smpl_vertices`) and a gather (`ga_posmap_fill`).  The coverage
 rules are the library's own statement of what the GL rasterizer does (csrc/posmap.cu; DESIGN.md, PARITY UNPINNED).
-`SmplxPoseMapper` does the same for SMPL-X (`ga_smplx_vertices`).
+`SmplxPoseMapper` does the same for SMPL-X (`ga_smplx_vertices`).  Their vertex-posing half, which needs no UV template, is
+`BodyPoser` / `SmplxBodyPoser`; the mesh overlay (`mesh_render`) uses it too.
 
 `canonical_assets` builds, from the same pieces, the per-subject and per-size files the reference makes with OpenGL
 (scripts/gen_pose_map_cano_smpl.py) or ships pre-rendered: the canonical query map and joint matrices, the UV face-id mask, the
@@ -69,29 +70,24 @@ def _dense(x):
     return np.asarray(x.todense() if hasattr(x, "todense") else x)
 
 
-class PoseMapper:
-    """Posed-body position maps [B,3,S,S] from SMPL poses, channel-first as the pose encoder takes them.
+class BodyPoser:
+    """Posed SMPL vertices [B,V,3] on the device, from the body model alone (no UV template): the vertex-posing half of `PoseMapper`,
+    which the position maps and the mesh overlay (`mesh_render`) share.
 
     smpl: the SMPL model as stored in SMPL_{GENDER}.pkl (any mapping with v_template [V,3], shapedirs [V,3,>=10], posedirs
-    [V,3,207], weights [V,24], f [F,3], J_regressor [24,V] dense or sparse); betas [10]; uv_template: a path to the UV template OBJ
-    or what `load_uv_template_obj` returns; S: map size (1..512).  Face i of the map is the mesh face f[i] drawn at the UV corners
-    of template face i, so the template must have exactly F faces.  Everything runs on the current CUDA stream under no_grad."""
+    [V,3,207], weights [V,24], f [F,3], J_regressor [24,V] dense or sparse); betas [10].  Everything runs on the current CUDA
+    stream under no_grad."""
 
     BODY, JOINTS, POSE_FEATURES, POSE_WIDTH = "SMPL", 24, 207, 72
 
-    def __init__(self, smpl, betas, uv_template, S: int, device="cuda"):
+    def __init__(self, smpl, betas, device="cuda"):
         missing = [k for k in SMPL_MESH_FIELDS if k not in smpl]
         if missing:
             raise ValueError(f"the {self.BODY} model has no {', '.join(missing)}: device position maps need the full mesh model")
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError(f"{type(self).__name__} runs on CUDA only (no CPU fallback)")
-        self.S = int(S)
-        if not 1 <= self.S <= 512:
-            raise ValueError(f"map size {S} outside 1..512")
-        if isinstance(uv_template, (str, os.PathLike)):
-            uv_template = load_uv_template_obj(uv_template)
-        _, _, uvs, faces_uv = uv_template
+        self._check_model(smpl)
         v_t = np.asarray(smpl["v_template"], np.float64)
         V = v_t.shape[0]
         nj, nf, body = self.JOINTS, self.POSE_FEATURES, self.BODY
@@ -106,9 +102,6 @@ class PoseMapper:
                              f"expected [{V},3,{nf}], [{V},{nj}], [{nj},{V}], [F,3]")
         if faces.size and (faces.min() < 0 or faces.max() >= V):
             raise ValueError(f"{body} model: a face indexes a vertex outside 0..{V - 1}")
-        if faces_uv.shape[0] != faces.shape[0]:
-            raise ValueError(f"the UV template has {faces_uv.shape[0]} faces, the {body} mesh {faces.shape[0]}: face i of one must be face i of "
-                             "the other")
         v_shaped = v_t + np.einsum("l,mkl->mk", beta, sd)
         dev = self.device
         self.V, self.F = V, faces.shape[0]
@@ -117,11 +110,9 @@ class PoseMapper:
         self.posedirs = torch.from_numpy(posedirs.reshape(V * 3, nf).T.copy()).to(dev)                  # [207 / 486, 3V] as smplx keeps it
         self.weights = torch.from_numpy(weights).to(dev).contiguous()                                   # [V,J]
         self.faces = torch.from_numpy(faces.astype(np.int32)).to(dev).contiguous()                      # [F,3]
-        corners = torch.from_numpy(np.asarray(uvs, np.float32)[faces_uv]).to(dev).contiguous()        # [F,3,2]
-        self.face_id = torch.empty(self.S, self.S, dtype=torch.int32, device=dev)
-        self.bary = torch.empty(self.S, self.S, 3, dtype=torch.float32, device=dev)
-        _lib.check(_lib.lib().ga_posmap_layout(self.F, self.S, ptr(corners), ptr(self.face_id), ptr(self.bary), self._stream()),
-                   "ga_posmap_layout")
+
+    def _check_model(self, model):
+        pass
 
     @staticmethod
     def _stream() -> int:
@@ -146,6 +137,71 @@ class PoseMapper:
             _lib.check(L.ga_smpl_vertices(e - s, self.V, ptr(pose[s:e]), ptr(transl[s:e]), ptr(self.rest_joints), ptr(self.v_shaped),
                                           ptr(self.posedirs), ptr(self.weights), ptr(out[s:e]), self._stream()), "ga_smpl_vertices")
         return out
+
+
+class SmplxBodyPoser(BodyPoser):
+    """The SMPL-X counterpart of `BodyPoser`: the model as stored in SMPLX_{GENDER}.npz (v_template, shapedirs [V,3,>=10] of which
+    the first len(betas) columns are used, posedirs [V,3,486], weights [V,55], f, J_regressor [55,V], kintree_table, which must be
+    the 55-joint tree of `synthetic.SMPLX_PARENTS`).  Poses are the reference's smplx.SMPLX(use_pca=False, flat_hand_mean=True)
+    split: pose [B,66] (global + 21 body joints) and rest_pose [B,99] (jaw, left / right eye, 15 + 15 finger joints)."""
+
+    BODY, JOINTS, POSE_FEATURES, POSE_WIDTH = "SMPL-X", 55, 486, 66
+
+    def _check_model(self, smplx):
+        from .synthetic import SMPLX_PARENTS
+        if "kintree_table" not in smplx:
+            raise ValueError("the SMPL-X model has no kintree_table")
+        kt = np.asarray(smplx["kintree_table"]).astype(np.int64)[0].copy()
+        kt[0] = -1
+        if kt.shape != (len(SMPLX_PARENTS),) or not np.array_equal(kt, np.asarray(SMPLX_PARENTS)):
+            raise ValueError("SMPL-X model: kintree_table[0] is not the 55-joint SMPL-X tree this library is built for")
+
+    def _inputs(self, pose, rest_pose, transl):
+        pose, transl = super()._inputs(pose, transl)
+        rest_pose = torch.as_tensor(rest_pose).to(device=self.device, dtype=torch.float32).reshape(-1, 99).contiguous()
+        if rest_pose.shape[0] != pose.shape[0]:
+            raise ValueError(f"pose {tuple(pose.shape)} and rest_pose {tuple(rest_pose.shape)} have different frame counts")
+        return pose, rest_pose, transl
+
+    @torch.no_grad()
+    def vertices(self, pose, rest_pose, transl) -> torch.Tensor:
+        """Posed SMPL-X vertices [B,V,3] for pose [B,66], rest_pose [B,99] and transl [B,3] (`SMPLX.forward(...).vertices`)."""
+        pose, rest_pose, transl = self._inputs(pose, rest_pose, transl)
+        B = pose.shape[0]
+        out = torch.empty(B, self.V, 3, dtype=torch.float32, device=self.device)
+        L = _lib.lib()
+        for s in range(0, B, MAX_FRAMES_PER_CALL):
+            e = min(B, s + MAX_FRAMES_PER_CALL)
+            _lib.check(L.ga_smplx_vertices(e - s, self.V, ptr(pose[s:e]), ptr(rest_pose[s:e]), ptr(transl[s:e]), ptr(self.rest_joints),
+                                           ptr(self.v_shaped), ptr(self.posedirs), ptr(self.weights), ptr(out[s:e]), self._stream()),
+                       "ga_smplx_vertices")
+        return out
+
+
+class PoseMapper(BodyPoser):
+    """Posed-body position maps [B,3,S,S] from SMPL poses, channel-first as the pose encoder takes them.
+
+    smpl, betas: as `BodyPoser` takes them; uv_template: a path to the UV template OBJ or what `load_uv_template_obj` returns; S: map
+    size (1..512).  Face i of the map is the mesh face f[i] drawn at the UV corners of template face i, so the template must have
+    exactly F faces.  Everything runs on the current CUDA stream under no_grad."""
+
+    def __init__(self, smpl, betas, uv_template, S: int, device="cuda"):
+        BodyPoser.__init__(self, smpl, betas, device)
+        self.S = int(S)
+        if not 1 <= self.S <= 512:
+            raise ValueError(f"map size {S} outside 1..512")
+        if isinstance(uv_template, (str, os.PathLike)):
+            uv_template = load_uv_template_obj(uv_template)
+        _, _, uvs, faces_uv = uv_template
+        if faces_uv.shape[0] != self.F:
+            raise ValueError(f"the UV template has {faces_uv.shape[0]} faces, the {self.BODY} mesh {self.F}: face i of one must be face i of "
+                             "the other")
+        dev = self.device
+        corners = torch.from_numpy(np.asarray(uvs, np.float32)[faces_uv]).to(dev).contiguous()        # [F,3,2]
+        self.face_id = torch.empty(self.S, self.S, dtype=torch.int32, device=dev)
+        self.bary = torch.empty(self.S, self.S, 3, dtype=torch.float32, device=dev)
+        _lib.check(_lib.lib().ga_posmap_layout(self.F, self.S, ptr(corners), ptr(self.face_id), ptr(self.bary), self._stream()),
+                   "ga_posmap_layout")
 
     @torch.no_grad()
     def fill(self, verts: torch.Tensor) -> torch.Tensor:
@@ -173,44 +229,11 @@ class PoseMapper:
         return out
 
 
-class SmplxPoseMapper(PoseMapper):
-    """The SMPL-X counterpart of `PoseMapper`: the model as stored in SMPLX_{GENDER}.npz (v_template, shapedirs [V,3,>=10] of which
-    the first len(betas) columns are used, posedirs [V,3,486], weights [V,55], f, J_regressor [55,V], kintree_table, which must be
-    the 55-joint tree of `synthetic.SMPLX_PARENTS`).  Poses are the reference's smplx.SMPLX(use_pca=False, flat_hand_mean=True)
-    split: pose [B,66] (global + 21 body joints) and rest_pose [B,99] (jaw, left / right eye, 15 + 15 finger joints)."""
-
-    BODY, JOINTS, POSE_FEATURES, POSE_WIDTH = "SMPL-X", 55, 486, 66
+class SmplxPoseMapper(SmplxBodyPoser, PoseMapper):
+    """The SMPL-X counterpart of `PoseMapper`: the model and poses as `SmplxBodyPoser` takes them."""
 
     def __init__(self, smplx, betas, uv_template, S: int, device="cuda"):
-        from .synthetic import SMPLX_PARENTS
-        if "kintree_table" not in smplx:
-            raise ValueError("the SMPL-X model has no kintree_table")
-        kt = np.asarray(smplx["kintree_table"]).astype(np.int64)[0].copy()
-        kt[0] = -1
-        if kt.shape != (len(SMPLX_PARENTS),) or not np.array_equal(kt, np.asarray(SMPLX_PARENTS)):
-            raise ValueError("SMPL-X model: kintree_table[0] is not the 55-joint SMPL-X tree this library is built for")
-        super().__init__(smplx, betas, uv_template, S, device)
-
-    def _inputs(self, pose, rest_pose, transl):
-        pose, transl = super()._inputs(pose, transl)
-        rest_pose = torch.as_tensor(rest_pose).to(device=self.device, dtype=torch.float32).reshape(-1, 99).contiguous()
-        if rest_pose.shape[0] != pose.shape[0]:
-            raise ValueError(f"pose {tuple(pose.shape)} and rest_pose {tuple(rest_pose.shape)} have different frame counts")
-        return pose, rest_pose, transl
-
-    @torch.no_grad()
-    def vertices(self, pose, rest_pose, transl) -> torch.Tensor:
-        """Posed SMPL-X vertices [B,V,3] for pose [B,66], rest_pose [B,99] and transl [B,3] (`SMPLX.forward(...).vertices`)."""
-        pose, rest_pose, transl = self._inputs(pose, rest_pose, transl)
-        B = pose.shape[0]
-        out = torch.empty(B, self.V, 3, dtype=torch.float32, device=self.device)
-        L = _lib.lib()
-        for s in range(0, B, MAX_FRAMES_PER_CALL):
-            e = min(B, s + MAX_FRAMES_PER_CALL)
-            _lib.check(L.ga_smplx_vertices(e - s, self.V, ptr(pose[s:e]), ptr(rest_pose[s:e]), ptr(transl[s:e]), ptr(self.rest_joints),
-                                           ptr(self.v_shaped), ptr(self.posedirs), ptr(self.weights), ptr(out[s:e]), self._stream()),
-                       "ga_smplx_vertices")
-        return out
+        PoseMapper.__init__(self, smplx, betas, uv_template, S, device)
 
     def __call__(self, pose, rest_pose, transl) -> torch.Tensor:
         """pose [B,66], rest_pose [B,99], transl [B,3] -> position maps [B,3,S,S]."""

@@ -388,6 +388,26 @@ size_t ga_metrics_partials_bytes(int32_t B, int32_t C, int32_t H, int32_t W);
 int ga_metrics_ssim_sse(int32_t B, int32_t C, int32_t H, int32_t W, const float *pred, const float *target, float data_range,
                         void *partials, double *ssim_sum, double *sse, void *stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Screen-space mesh render (the posed-body overlay): B <= 8 frames of verts [B,V,3] (fp32), faces [F,3] (int32, each in
+ * [0, V)), cams [B,40] (the ga_rasterb_* camera block: transposed view 0..15, transposed full projection 16..31).
+ * adj_offsets [V+1] / adj_faces [3F]: vertex -> face CSR, faces of vertex v at adj_faces[adj_offsets[v] .. adj_offsets[v+1]),
+ * each face once per corner it has there, in ascending face order (the normal is the normalised sum of their cross products).
+ * Coverage: pixel centres, the Gaussian preprocess's projection and pixel convention, window coordinates snapped to 1/256
+ * pixel, exact int64 edge functions with posmap.cu's tie rule; nearest face wins (perspective-correct depth, fp64, rounded
+ * to fp32 once), lower face index at equal depth; no culling; a face with a corner at view depth <= 0.01 or beyond 2^20
+ * pixels is not drawn.  Shading: glTF metallic-roughness BRDF (metallic 0.2, roughness 0.6, base colour base_*), one
+ * headlight of intensity 3 along the camera's optical axis, no ambient, clamped to [0,1].
+ * Outputs (every element written): face_id [B,H,W] (-1: nothing drawn), depth [B,H,W] (view-space z, 0: nothing drawn),
+ * rgb [B,3,H,W] (background [B,3,H,W] where nothing is drawn, 0 if background is NULL).
+ * workspace: ga_mesh_render_workspace_bytes(B, V, F, H, W) bytes, 256-byte aligned.  No floating-point atomics and no host
+ * read-back: the outputs are bit-reproducible and a frame's do not depend on the batch it is drawn in.  H, W in [1, 16384].
+ * ---------------------------------------------------------------------------------------------------------------- */
+size_t ga_mesh_render_workspace_bytes(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W);
+int ga_mesh_render(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, const float *verts, const int32_t *faces,
+                   const int32_t *adj_offsets, const int32_t *adj_faces, const float *cams, float base_r, float base_g, float base_b,
+                   const float *background, void *workspace, int32_t *face_id, float *depth, float *rgb, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
