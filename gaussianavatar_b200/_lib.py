@@ -127,6 +127,8 @@ _SIGNATURES = {
     "ga_metrics_ssim_sse": (ctypes.c_int, [ctypes.c_int32] * 4 + [c_vp, c_vp, ctypes.c_float] + [c_vp] * 4),
     "ga_mesh_render_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 5),
     "ga_mesh_render": (ctypes.c_int, [ctypes.c_int32] * 5 + [c_vp] * 5 + [ctypes.c_float] * 3 + [c_vp] * 6),
+    "ga_motion_sample": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 2 + [ctypes.c_int32] + [c_vp] * 5),
+    "ga_frame_pack": (ctypes.c_int, [ctypes.c_int32] * 4 + [c_vp] * 5),
 }
 
 _lib = None

@@ -474,14 +474,17 @@ class AvatarModel:
         images = self._render_frames(batch_data, means, scales, colors)
         return images, means, offset_loss, geo_loss, scale_loss
 
-    def _stage2_gaussians(self, batch_data):
+    def _stage2_gaussians(self, batch_data, pose=None, transl=None):
         """Stage 2 (model/avatar_model.py:369-420 / :557-612): the pose encoder turns each frame's posed-body position map into a
         feature map that is ADDED to the geometry features, so the decoder runs per frame (B*S*S rows, BatchNorm statistics over all of
-        them); no scale ramp in this stage."""
+        them); no scale ramp in this stage.  The skeleton is posed with the model's pose / transl rows at `pose_idx`, as the reference
+        does, unless `pose` [B,72|66] and `transl` [B,3] are given (the animation player's sampled poses)."""
         inp = batch_data.get("inp_pos_map")
         inp = self._pose_map(batch_data) if inp is None else inp.to(self.device).float()
-        idx = batch_data["pose_idx"]
-        cano2live = self._cano2live(self.pose(idx), self.transl(idx), batch_data.get("rest_pose"))
+        if pose is None:
+            idx = batch_data["pose_idx"]
+            pose, transl = self.pose(idx), self.transl(idx)
+        cano2live = self._cano2live(pose, transl, batch_data.get("rest_pose"))
         S = int(self.model_parms.query_posmap_size)
         pose_featmap = self.pose_encoder(inp)                                                         # [B,64,h,h]
         dec = self.net.forward_packed_frames(self.geo_feature, pose_featmap, S)                      # [B*S*S, 8]

@@ -310,9 +310,13 @@ class RasterBatchPlan:
         self.pending = False
         if int(self.status_host[1]) == 0:
             return True
-        self.capacity = int(1.5 * int(self.status_host[0])) + 1024
-        self._alloc_binning()
+        self.grow(int(self.status_host[0]))
         return False
+
+    def grow(self, needed: int):
+        """Re-allocate the binning buffer for a forward that needed `needed` instances (status word 0), with headroom."""
+        self.capacity = int(1.5 * int(needed)) + 1024
+        self._alloc_binning()
 
     def views(self):
         return _views(self.B, self.P, self.H, self.W, self.capacity, self.geom, self.binning, self.img, self.radii)

@@ -408,6 +408,27 @@ int ga_mesh_render(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, const 
                    const int32_t *adj_offsets, const int32_t *adj_faces, const float *cams, float base_r, float base_g, float base_b,
                    const float *background, void *workspace, int32_t *face_id, float *depth, float *rgb, void *stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Animation player.
+ * ga_motion_sample: a clip of T keys of J-joint axis-angle poses key_pose [T,J*3] (J = 24 for SMPL, 55 for SMPL-X's 165-wide
+ * layout) and translations key_trans [T,3] (fp32, device), sampled at n fractional key indices times [n] (device double).
+ * tau = clamp(times[k], 0, T-1) (NaN -> 0), i = floor(tau), f = tau - i.  Per joint, keys i and i+1 become unit quaternions,
+ * the second negated when their dot product is negative, then slerp at f (normalised lerp above a dot of 1 - 1e-12); back to
+ * axis-angle with w >= 0, so the angle is in [0, pi].  align [12] (device double): a row-major rotation R_a and an offset c;
+ * the root becomes R_a R_root and the translation R_a lerp(t_i, t_i+1, f) + c.  All maths in fp64, rounded to fp32 once;
+ * every element of pose_out [n,J*3] and trans_out [n,3] is written.  T >= 1, n >= 1.
+ * ga_frame_pack: rendered frames image [B,3,H,W] (fp32, the batched rasterizer's C + T bg) -> interleaved bytes out
+ * [B,H,W,channels].  q(x) = (uint8) clamp(fp32(fp32(x 255) + 0.5), 0, 255), NaN -> 0 (torchvision's save_image).
+ * channels 3: q(image); final_T and bg may be NULL.  channels 4 (straight alpha; out 4-byte aligned): a = 1 - T with T =
+ * final_T [B,H,W] (the rasterizer's image buffer, ga_raster_views), A = q(a); A = 0 gives (0,0,0,0), otherwise the colour
+ * bytes are q((x - T bg_c) / a) and the fourth byte A.  Explicit fp32 roundings in that order (no contraction).
+ * B in [1, 8]; H, W in [1, 16384].  No host read-back; both run on `stream` and are capturable in a CUDA graph.
+ * ---------------------------------------------------------------------------------------------------------------- */
+int ga_motion_sample(int32_t T, int32_t J, const float *key_pose, const float *key_trans, int32_t n, const double *times,
+                     const double *align, float *pose_out, float *trans_out, void *stream);
+int ga_frame_pack(int32_t B, int32_t H, int32_t W, int32_t channels, const float *image, const float *final_T, const float *bg,
+                  uint8_t *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
