@@ -90,6 +90,12 @@ _SIGNATURES = {
     "ga_posmap_weights": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 6),
     "ga_posmap_layout": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 4),
     "ga_posmap_fill": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp] * 6),
+    "ga_smpl_vertices_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "ga_smplx_vertices_backward_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "ga_smpl_vertices_backward": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 7 + [ctypes.c_size_t] + [c_vp] * 3),
+    "ga_smplx_vertices_backward": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 8 + [ctypes.c_size_t] + [c_vp] * 3),
+    "ga_posmap_vertex_csr": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 5),
+    "ga_posmap_fill_backward": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp] * 6),
     "ga_decoder_layout":(ctypes.c_int, [ctypes.POINTER(GaDecoderDesc), ctypes.POINTER(GaDecoderLayout)]),
     "ga_decoder_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(GaDecoderDesc)]),
     "ga_decoder_forward": (ctypes.c_int, [ctypes.POINTER(GaDecoderDesc)] + [c_vp] * 7),

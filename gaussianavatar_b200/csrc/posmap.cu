@@ -367,6 +367,462 @@ posmap_fill_kernel(int S, int V, const float *__restrict__ verts, const int *__r
     ob[t] = o[0]; ob[n + t] = o[1]; ob[2 * n + t] = o[2];
 }
 
+// ---- backward of vertex posing (ga_smpl_vertices_backward / ga_smplx_vertices_backward)
+//
+// With g_v = d_verts[b,v], x_v = v_shaped_v + posedirs^T feat (the blend-shaped vertex) and T_v = sum_j w_vj A_j:
+//   d_transl = sum_v g_v,   d_A_j = sum_v w_vj g_v [x_v; 1]^T,   d_feat[r] = sum_{v,c} posedirs[r, 3v+c] (T_v[:, :3]^T g_v)_c.
+// Pass 1 (one CTA per 32 vertices, as the forward) streams posedirs once for all B frames: it needs T_v^T g_v (from A) before the
+// stream and x_v (from the stream) after it.  Each CTA writes its per-frame sums [d_A | d_feat | d_transl] to its own workspace slot.
+// Pass 2 (one CTA per frame) adds the slots in CTA order, then runs the joint chain and the Rodrigues map backwards.  No atomics:
+// the results are bit-reproducible, and a frame's sums never mix with another frame's, so they do not depend on the batch.
+constexpr int kBwdThreads = 256;
+constexpr int kBwdWarps = kBwdThreads / 32;
+
+template <int kJ> struct BodyDims;
+template <> struct BodyDims<kJoints> {
+    static constexpr int kFeat = kPoseFeat, kTrained = kJoints;
+    static __device__ __forceinline__ int parent(int j) { return c_parents_v[j]; }
+};
+template <> struct BodyDims<kJointsX> {
+    static constexpr int kFeat = kPoseFeatX, kTrained = kTrainX;
+    static __device__ __forceinline__ int parent(int j) { return c_parents_vx[j]; }
+};
+
+// per-frame sums of one CTA: d_A [J,12], d_feat [kFeat], d_transl [3]
+template <int kJ> constexpr int bwd_sums() { return kJ * 12 + BodyDims<kJ>::kFeat + 3; }
+
+template <int kJ> struct VertBwdSmem {
+    float A[kMaxB][kJ][12];
+    float feat[kMaxB][BodyDims<kJ>::kFeat];
+    float g[kMaxB][kCols];           // d_verts of the CTA's 32 vertices
+    float dx[kMaxB][kCols];          // T_v[:, :3]^T g_v
+    float x[kMaxB][kCols];           // blend-shaped vertices
+    union {
+        float L[kMaxB][kJ][12];
+        float part[kBwdWarps][kMaxB][kCols];
+        float gx[kMaxB][kVertsPerCta][12];     // g_v [x_v; 1]^T
+    } u;
+};
+
+template <int kJ> struct VertFinishSmem {
+    float sums[bwd_sums<kJ>()];
+    float L[kJ][12], G[kJ][12], dG[kJ][12], dR[kJ][9];
+};
+
+// axis-angle of joint j of frame b: SMPL takes all 24 from pose [B,72]; SMPL-X the first 22 from pose [B,66], the rest from rest_pose
+template <int kJ>
+__device__ __forceinline__ void joint_axis_angle(const float *__restrict__ pose, const float *__restrict__ rest_pose, int b, int j, float r[3])
+{
+    constexpr int kT = BodyDims<kJ>::kTrained;
+    const float *src = (j < kT) ? pose + (size_t)b * (3 * kT) + j * 3 : rest_pose + (size_t)b * (3 * (kJ - kT)) + (j - kT) * 3;
+    r[0] = src[0]; r[1] = src[1]; r[2] = src[2];
+}
+
+// local transform of joint j (rotation | offset to its parent) from its rotation R
+template <int kJ>
+__device__ __forceinline__ void local_transform(const float R[9], const float *__restrict__ J, int j, float *L)
+{
+    const int p = BodyDims<kJ>::parent(j);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        L[k * 4 + 0] = R[k * 3 + 0]; L[k * 4 + 1] = R[k * 3 + 1]; L[k * 4 + 2] = R[k * 3 + 2];
+        L[k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
+    }
+}
+
+// global transform of joint j: the product of its ancestors' local transforms, root first (the forwards' order)
+template <int kJ>
+__device__ __forceinline__ void chain_product(const float (*L)[12], int j, float G[12])
+{
+    float T[12];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) G[k] = L[j][k];
+    for (int p = BodyDims<kJ>::parent(j); p >= 0; p = BodyDims<kJ>::parent(p)) {
+        aff_mul(L[p], G, T);
+#pragma unroll
+        for (int k = 0; k < 12; ++k) G[k] = T[k];
+    }
+}
+
+template <int kJ>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+vertices_bwd_kernel(int B, int V, const float *__restrict__ pose, const float *__restrict__ rest_pose, const float *__restrict__ J,
+                    const float *__restrict__ v_shaped, const float *__restrict__ posedirs, const float *__restrict__ weights,
+                    const float *__restrict__ d_verts, float *__restrict__ sums /*[ctas][B][bwd_sums]*/)
+{
+    constexpr int kF = BodyDims<kJ>::kFeat, kN = bwd_sums<kJ>();
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    VertBwdSmem<kJ> &sm = *reinterpret_cast<VertBwdSmem<kJ> *>(smem_raw);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const long long ncol = 3LL * V, k0 = (long long)blockIdx.x * kCols;
+    float *out = sums + (size_t)blockIdx.x * B * kN;
+
+    for (int i = tid; i < B * kCols; i += kBwdThreads) {
+        const int b = i / kCols, col = i % kCols;
+        sm.g[b][col] = (k0 + col < ncol) ? d_verts[(size_t)b * ncol + k0 + col] : 0.f;
+    }
+    for (int i = tid; i < B * kJ; i += kBwdThreads) {
+        const int b = i / kJ, j = i % kJ;
+        float r[3], R[9], th;
+        joint_axis_angle<kJ>(pose, rest_pose, b, j, r);
+        rodrigues(r, R, &th);
+        local_transform<kJ>(R, J, j, sm.u.L[b][j]);
+        if (j > 0) {
+#pragma unroll
+            for (int k = 0; k < 9; ++k) sm.feat[b][(j - 1) * 9 + k] = R[k] - ((k % 4 == 0) ? 1.f : 0.f);
+        }
+    }
+    __syncthreads();
+    for (int i = tid; i < B * kJ; i += kBwdThreads) {
+        const int b = i / kJ, j = i % kJ;
+        float G[12];
+        chain_product<kJ>(sm.u.L[b], j, G);
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            sm.A[b][j][r * 4 + 0] = G[r * 4 + 0]; sm.A[b][j][r * 4 + 1] = G[r * 4 + 1]; sm.A[b][j][r * 4 + 2] = G[r * 4 + 2];
+            sm.A[b][j][r * 4 + 3] = G[r * 4 + 3] - (G[r * 4 + 0] * J[j * 3] + G[r * 4 + 1] * J[j * 3 + 1] + G[r * 4 + 2] * J[j * 3 + 2]);
+        }
+    }
+    __syncthreads();        // L is dead from here on
+
+    // dx_v = T_v[:, :3]^T g_v
+    for (int i = tid; i < B * kVertsPerCta; i += kBwdThreads) {
+        const int b = i / kVertsPerCta, vl = i % kVertsPerCta;
+        const int v = blockIdx.x * kVertsPerCta + vl;
+        float d[3] = {0.f, 0.f, 0.f};
+        if (v < V) {
+            float T[12];
+#pragma unroll
+            for (int q = 0; q < 12; ++q) T[q] = 0.f;
+            const float *w = weights + (size_t)v * kJ;
+            for (int j = 0; j < kJ; ++j) {
+                const float wj = w[j];
+#pragma unroll
+                for (int q = 0; q < 12; ++q) T[q] = fmaf(wj, sm.A[b][j][q], T[q]);
+            }
+            const float *g = sm.g[b] + vl * 3;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) d[c] = T[c] * g[0] + T[4 + c] * g[1] + T[8 + c] * g[2];
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) sm.dx[b][vl * 3 + c] = d[c];
+    }
+    __syncthreads();
+
+    // posedirs, once for all frames: warp w takes rows w, w + 8, ...; lane takes columns lane, lane + 32, lane + 64.  Per row, the
+    // warp sums pd dx over its 96 columns (d_feat) and every lane accumulates feat pd into its columns (the forward's offsets).
+    float dxr[kMaxB][3], off[kMaxB][3];
+#pragma unroll
+    for (int b = 0; b < kMaxB; ++b)
+#pragma unroll
+        for (int m = 0; m < 3; ++m) { dxr[b][m] = (b < B) ? sm.dx[b][lane + 32 * m] : 0.f; off[b][m] = 0.f; }
+    for (int r = warp; r < kF; r += kBwdWarps) {
+        float pd[3];
+#pragma unroll
+        for (int m = 0; m < 3; ++m) {
+            const long long k = k0 + lane + 32 * m;
+            pd[m] = (k < ncol) ? __ldg(posedirs + (long long)r * ncol + k) : 0.f;
+        }
+#pragma unroll
+        for (int b = 0; b < kMaxB; ++b) {
+            if (b < B) {
+                const float f = sm.feat[b][r];
+                float s = pd[0] * dxr[b][0] + pd[1] * dxr[b][1] + pd[2] * dxr[b][2];
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+                if (lane == b) out[(size_t)b * kN + kJ * 12 + r] = s;
+#pragma unroll
+                for (int m = 0; m < 3; ++m) off[b][m] = fmaf(f, pd[m], off[b][m]);
+            }
+        }
+    }
+#pragma unroll
+    for (int b = 0; b < kMaxB; ++b)
+        if (b < B)
+#pragma unroll
+            for (int m = 0; m < 3; ++m) sm.u.part[warp][b][lane + 32 * m] = off[b][m];
+    __syncthreads();
+    for (int i = tid; i < B * kCols; i += kBwdThreads) {
+        const int b = i / kCols, col = i % kCols;
+        float o = 0.f;
+#pragma unroll
+        for (int w = 0; w < kBwdWarps; ++w) o += sm.u.part[w][b][col];
+        sm.x[b][col] = (k0 + col < ncol) ? v_shaped[k0 + col] + o : 0.f;
+    }
+    __syncthreads();        // part is dead from here on
+    for (int i = tid; i < B * kVertsPerCta; i += kBwdThreads) {
+        const int b = i / kVertsPerCta, vl = i % kVertsPerCta;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            const float g = sm.g[b][vl * 3 + r];
+            sm.u.gx[b][vl][r * 4 + 0] = g * sm.x[b][vl * 3 + 0];
+            sm.u.gx[b][vl][r * 4 + 1] = g * sm.x[b][vl * 3 + 1];
+            sm.u.gx[b][vl][r * 4 + 2] = g * sm.x[b][vl * 3 + 2];
+            sm.u.gx[b][vl][r * 4 + 3] = g;
+        }
+    }
+    __syncthreads();
+    const int vbase = blockIdx.x * kVertsPerCta, nv = min(kVertsPerCta, V - vbase);
+    for (int i = tid; i < B * kJ * 12; i += kBwdThreads) {
+        const int b = i / (kJ * 12), jq = i % (kJ * 12), j = jq / 12, q = jq % 12;
+        float s = 0.f;
+        for (int vl = 0; vl < nv; ++vl) s = fmaf(weights[(size_t)(vbase + vl) * kJ + j], sm.u.gx[b][vl][q], s);
+        out[(size_t)b * kN + jq] = s;
+    }
+    for (int i = tid; i < B * 3; i += kBwdThreads) {
+        const int b = i / 3, c = i % 3;
+        float s = 0.f;
+        for (int vl = 0; vl < nv; ++vl) s += sm.g[b][vl * 3 + c];
+        out[(size_t)b * kN + kJ * 12 + kF + c] = s;
+    }
+}
+
+// Backward of rodrigues(): R = I + s K + (1 - c) K^2 with K the cross matrix of d = r / theta, theta = |r + 1e-8|.
+__device__ __forceinline__ void rodrigues_bwd(const float r[3], const float gR[9], float gr[3])
+{
+    const float n[3] = {r[0] + 1e-8f, r[1] + 1e-8f, r[2] + 1e-8f};
+    const float theta = sqrtf(n[0] * n[0] + n[1] * n[1] + n[2] * n[2]);
+    const float dx = r[0] / theta, dy = r[1] / theta, dz = r[2] / theta;
+    float s, c;
+    sincosf(theta, &s, &c);
+    const float K[9] = {0.f, -dz, dy, dz, 0.f, -dx, -dy, dx, 0.f};
+    float K2[9], gK[9];
+    float gs = 0.f, g1c = 0.f;
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) K2[i * 3 + j] = K[i * 3] * K[j] + K[i * 3 + 1] * K[3 + j] + K[i * 3 + 2] * K[6 + j];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) { gs = fmaf(gR[i], K[i], gs); g1c = fmaf(gR[i], K2[i], g1c); }
+    // d(K^2) = dK K + K dK: gK = s gR + (1 - c) (gR K^T + K^T gR)
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            float t = 0.f;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) t += gR[i * 3 + k] * K[j * 3 + k] + K[k * 3 + i] * gR[k * 3 + j];
+            gK[i * 3 + j] = s * gR[i * 3 + j] + (1.f - c) * t;
+        }
+    const float gd[3] = {gK[7] - gK[5], gK[2] - gK[6], gK[3] - gK[1]};
+    float gth = gs * c + g1c * s - (gd[0] * r[0] + gd[1] * r[1] + gd[2] * r[2]) / (theta * theta);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) gr[k] = gd[k] / theta + gth * n[k] / theta;
+}
+
+// One CTA per frame: add the CTAs' sums in order, then d_A -> d_G -> (joint chain, leaves first) d_L -> d_R (+ d_feat) -> d_pose.
+template <int kJ>
+__global__ void __launch_bounds__(kBwdThreads)
+vertices_bwd_finish_kernel(int B, int ctas, const float *__restrict__ pose, const float *__restrict__ rest_pose,
+                           const float *__restrict__ J, const float *__restrict__ sums, float *__restrict__ d_pose, float *__restrict__ d_transl)
+{
+    constexpr int kF = BodyDims<kJ>::kFeat, kN = bwd_sums<kJ>(), kT = BodyDims<kJ>::kTrained;
+    __shared__ VertFinishSmem<kJ> sm;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+    for (int e = tid; e < kN; e += kBwdThreads) {
+        float s = 0.f;
+        for (int c = 0; c < ctas; ++c) s += sums[((size_t)c * B + b) * kN + e];
+        sm.sums[e] = s;
+    }
+    for (int j = tid; j < kJ; j += kBwdThreads) {
+        float r[3], R[9], th;
+        joint_axis_angle<kJ>(pose, rest_pose, b, j, r);
+        rodrigues(r, R, &th);
+        local_transform<kJ>(R, J, j, sm.L[j]);
+    }
+    __syncthreads();
+    for (int i = tid; i < kJ * 12; i += kBwdThreads) {
+        const int j = i / 12, q = i % 12, rr = q / 4, c = q % 4;
+        if (q == 0) chain_product<kJ>(sm.L, j, sm.G[j]);
+        // A[:, 3] = G[:, 3] - G[:, :3] J_j
+        const float *dA = sm.sums + j * 12;
+        sm.dG[j][q] = (c == 3) ? dA[rr * 4 + 3] : dA[rr * 4 + c] - dA[rr * 4 + 3] * J[j * 3 + c];
+    }
+    __syncthreads();
+    if (tid < 32) {
+        // G_j = G_p L_j, leaves first (every parent index is below its child's); lane q owns element q of d_G_p, lane < 9 of d_L_j
+        for (int j = kJ - 1; j >= 0; --j) {
+            const int p = BodyDims<kJ>::parent(j);
+            const float *dG = sm.dG[j];
+            if (lane < 9) {
+                const int rr = lane / 3, k = lane % 3;
+                sm.dR[j][lane] = (p < 0) ? dG[rr * 4 + k]
+                                         : sm.G[p][rr] * dG[k] + sm.G[p][4 + rr] * dG[4 + k] + sm.G[p][8 + rr] * dG[8 + k];
+            }
+            if (p >= 0 && lane < 12) {
+                const int rr = lane / 4, c = lane % 4;
+                const float *L = sm.L[j];
+                const float u = (c == 3) ? dG[rr * 4 + 3]
+                                         : dG[rr * 4] * L[c * 4] + dG[rr * 4 + 1] * L[c * 4 + 1] + dG[rr * 4 + 2] * L[c * 4 + 2] +
+                                               dG[rr * 4 + 3] * L[c * 4 + 3];
+                sm.dG[p][lane] += u;
+            }
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    for (int j = tid; j < kT; j += kBwdThreads) {
+        float r[3], gR[9], gr[3];
+        joint_axis_angle<kJ>(pose, rest_pose, b, j, r);
+#pragma unroll
+        for (int k = 0; k < 9; ++k) gR[k] = sm.dR[j][k] + ((j > 0) ? sm.sums[kJ * 12 + (j - 1) * 9 + k] : 0.f);
+        rodrigues_bwd(r, gR, gr);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) d_pose[(size_t)b * 3 * kT + j * 3 + k] = gr[k];
+    }
+    if (tid < 3) d_transl[b * 3 + tid] = sm.sums[kJ * 12 + kF + tid];
+}
+
+// ---- backward of the fill through a vertex -> (texel, corner) CSR
+//
+// entries hold 3 t + i for texel t whose covering face has the vertex as corner i, in ascending order per vertex.  Built once per
+// layout: count (integer atomics), inclusive scan, scatter (a cursor that counts down from each vertex's end to its start), then a
+// per-vertex sort, so the order does not depend on the scatter's.
+__global__ void __launch_bounds__(256)
+posmap_csr_count_kernel(int n, const int *__restrict__ faces, const int *__restrict__ face_id, int *__restrict__ offsets)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const int f = face_id[t];
+    if (f < 0) return;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) atomicAdd(offsets + faces[(size_t)f * 3 + i], 1);
+}
+
+// one CTA: offsets[v] = count[0] + ... + count[v] (inclusive), offsets[V] = the total
+__global__ void __launch_bounds__(1024)
+posmap_csr_scan_kernel(int V, int *__restrict__ offsets)
+{
+    __shared__ int warp_sums[32];
+    __shared__ int carry;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) carry = 0;
+    __syncthreads();
+    for (int base = 0; base < V; base += 1024) {
+        const int i = base + tid;
+        int x = (i < V) ? offsets[i] : 0;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, x, o);
+            if (lane >= o) x += y;
+        }
+        if (lane == 31) warp_sums[warp] = x;
+        __syncthreads();
+        if (warp == 0) {
+            int w = warp_sums[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, w, o);
+                if (lane >= o) w += y;
+            }
+            warp_sums[lane] = w;
+        }
+        __syncthreads();
+        const int c = carry;
+        x += c + (warp > 0 ? warp_sums[warp - 1] : 0);
+        if (i < V) offsets[i] = x;
+        __syncthreads();
+        if (tid == 1023) carry = x;
+        __syncthreads();
+    }
+    if (tid == 0) offsets[V] = carry;
+}
+
+__global__ void __launch_bounds__(256)
+posmap_csr_scatter_kernel(int n, const int *__restrict__ faces, const int *__restrict__ face_id, int *__restrict__ offsets,
+                          int *__restrict__ entries)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const int f = face_id[t];
+    if (f < 0) return;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) entries[atomicSub(offsets + faces[(size_t)f * 3 + i], 1) - 1] = 3 * t + i;
+}
+
+// one thread per vertex: heapsort of its entries (any length, no extra memory)
+__global__ void __launch_bounds__(256)
+posmap_csr_sort_kernel(int V, const int *__restrict__ offsets, int *__restrict__ entries)
+{
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= V) return;
+    int *a = entries + offsets[v];
+    const int n = offsets[v + 1] - offsets[v];
+    auto sift = [a](int root, int end) {
+        while (2 * root + 1 < end) {
+            int c = 2 * root + 1;
+            if (c + 1 < end && a[c + 1] > a[c]) ++c;
+            if (a[root] >= a[c]) return;
+            const int t = a[root]; a[root] = a[c]; a[c] = t;
+            root = c;
+        }
+    };
+    for (int i = n / 2 - 1; i >= 0; --i) sift(i, n);
+    for (int end = n - 1; end > 0; --end) {
+        const int t = a[0]; a[0] = a[end]; a[end] = t;
+        sift(0, end);
+    }
+}
+
+// d_verts[b, v, :] = sum over v's entries (t, i) of bary[t, i] d_out[b, :, t].  One warp per (vertex, frame): lanes stride over the
+// entries, then a fixed butterfly; every element of d_verts is written (0 for a vertex no texel uses).
+constexpr int kFillBwdWarps = 8;
+
+__global__ void __launch_bounds__(kFillBwdWarps * 32)
+posmap_fill_bwd_kernel(int S, int V, const int *__restrict__ offsets, const int *__restrict__ entries, const float *__restrict__ bary,
+                       const float *__restrict__ d_out, float *__restrict__ d_verts)
+{
+    const int v = blockIdx.x * kFillBwdWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31, b = blockIdx.y;
+    if (v >= V) return;
+    const int n = S * S;
+    const float *g = d_out + (size_t)b * 3 * n;
+    float a[3] = {0.f, 0.f, 0.f};
+    for (int e = offsets[v] + lane; e < offsets[v + 1]; e += 32) {
+        const int ti = entries[e], t = ti / 3;
+        const float w = bary[ti];
+        a[0] = fmaf(w, g[t], a[0]); a[1] = fmaf(w, g[n + t], a[1]); a[2] = fmaf(w, g[2 * n + t], a[2]);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) a[c] += __shfl_xor_sync(0xffffffffu, a[c], o);
+    }
+    if (lane < 3) d_verts[((size_t)b * V + v) * 3 + lane] = a[lane];
+}
+
+template <int kJ> size_t vertices_bwd_workspace(int B, int V)
+{
+    if (B < 1 || B > kMaxB || V < 1 || V > (1 << 24)) return 0;
+    return (size_t)cdiv(V, kVertsPerCta) * B * bwd_sums<kJ>() * sizeof(float);
+}
+
+template <int kJ>
+int vertices_backward(const char *name, int B, int V, const float *pose, const float *rest_pose, const float *rest_joints, const float *v_shaped,
+                      const float *posedirs, const float *weights, const float *d_verts, void *workspace, size_t workspace_bytes,
+                      float *d_pose, float *d_transl, cudaStream_t stream)
+{
+    GA_REQUIRE(B >= 1 && B <= kMaxB, "%s: batch %d outside [1, %d]", name, B, kMaxB);
+    GA_REQUIRE(V > 0 && V <= (1 << 24), "%s: bad vertex count %d", name, V);
+    GA_REQUIRE(pose && (kJ == kJoints || rest_pose) && rest_joints && v_shaped && posedirs && weights && d_verts && workspace && d_pose && d_transl,
+               "%s: NULL pointer argument", name);
+    const size_t need = vertices_bwd_workspace<kJ>(B, V);
+    GA_REQUIRE(workspace_bytes >= need, "%s: workspace of %zu bytes, %zu needed", name, workspace_bytes, need);
+    GA_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 3) == 0, "%s: workspace must be 4-byte aligned", name);
+    static PerDeviceOnce attr_set;
+    if (attr_set.first())
+        GA_CHECK_CUDA(cudaFuncSetAttribute(vertices_bwd_kernel<kJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VertBwdSmem<kJ>)));
+    const int ctas = cdiv(V, kVertsPerCta);
+    float *sums = static_cast<float *>(workspace);
+    { ProfScope _ps(kJ == kJoints ? "smpl_vertices_bwd_kernel" : "smplx_vertices_bwd_kernel", stream);
+      vertices_bwd_kernel<kJ><<<ctas, kBwdThreads, sizeof(VertBwdSmem<kJ>), stream>>>(B, V, pose, rest_pose, rest_joints, v_shaped,
+                                                                                      posedirs, weights, d_verts, sums); }
+    GA_CHECK_LAUNCH("vertices_bwd_kernel");
+    { ProfScope _ps(kJ == kJoints ? "smpl_vertices_bwd_finish_kernel" : "smplx_vertices_bwd_finish_kernel", stream);
+      vertices_bwd_finish_kernel<kJ><<<B, kBwdThreads, 0, stream>>>(B, ctas, pose, rest_pose, rest_joints, sums, d_pose, d_transl); }
+    GA_CHECK_LAUNCH("vertices_bwd_finish_kernel");
+    return GA_OK;
+}
+
 }  // namespace
 }  // namespace ga
 
@@ -446,5 +902,61 @@ extern "C" int ga_posmap_fill(int32_t B, int32_t S, int32_t V, const float *vert
     { ProfScope _ps("posmap_fill_kernel", stream);
       posmap_fill_kernel<<<dim3(cdiv(S * S, 256), B), 256, 0, stream>>>(S, V, verts, faces, face_id, bary, out); }
     GA_CHECK_LAUNCH("posmap_fill_kernel");
+    return GA_OK;
+}
+
+extern "C" size_t ga_smpl_vertices_backward_workspace_bytes(int32_t B, int32_t V) { return vertices_bwd_workspace<kJoints>(B, V); }
+extern "C" size_t ga_smplx_vertices_backward_workspace_bytes(int32_t B, int32_t V) { return vertices_bwd_workspace<kJointsX>(B, V); }
+
+extern "C" int ga_smpl_vertices_backward(int32_t B, int32_t V, const float *pose, const float *rest_joints, const float *v_shaped,
+                                         const float *posedirs, const float *weights, const float *d_verts, void *workspace,
+                                         size_t workspace_bytes, float *d_pose, float *d_transl, void *stream_)
+{
+    return vertices_backward<kJoints>("ga_smpl_vertices_backward", B, V, pose, nullptr, rest_joints, v_shaped, posedirs, weights, d_verts,
+                                      workspace, workspace_bytes, d_pose, d_transl, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ga_smplx_vertices_backward(int32_t B, int32_t V, const float *pose, const float *rest_pose, const float *rest_joints,
+                                          const float *v_shaped, const float *posedirs, const float *weights, const float *d_verts,
+                                          void *workspace, size_t workspace_bytes, float *d_pose, float *d_transl, void *stream_)
+{
+    return vertices_backward<kJointsX>("ga_smplx_vertices_backward", B, V, pose, rest_pose, rest_joints, v_shaped, posedirs, weights,
+                                       d_verts, workspace, workspace_bytes, d_pose, d_transl, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ga_posmap_vertex_csr(int32_t S, int32_t V, const int32_t *faces, const int32_t *face_id, int32_t *offsets, int32_t *entries,
+                                    void *stream_)
+{
+    GA_REQUIRE(S >= 1 && S <= kMaxS, "ga_posmap_vertex_csr: map size %d outside [1, %d]", S, kMaxS);
+    GA_REQUIRE(V > 0 && V <= (1 << 24), "ga_posmap_vertex_csr: bad vertex count %d", V);
+    GA_REQUIRE(faces && face_id && offsets && entries, "ga_posmap_vertex_csr: NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const int n = S * S;
+    GA_CHECK_CUDA(cudaMemsetAsync(offsets, 0, sizeof(int32_t) * ((size_t)V + 1), stream));
+    { ProfScope _ps("posmap_csr_count_kernel", stream);
+      posmap_csr_count_kernel<<<cdiv(n, 256), 256, 0, stream>>>(n, faces, face_id, offsets); }
+    GA_CHECK_LAUNCH("posmap_csr_count_kernel");
+    { ProfScope _ps("posmap_csr_scan_kernel", stream); posmap_csr_scan_kernel<<<1, 1024, 0, stream>>>(V, offsets); }
+    GA_CHECK_LAUNCH("posmap_csr_scan_kernel");
+    { ProfScope _ps("posmap_csr_scatter_kernel", stream);
+      posmap_csr_scatter_kernel<<<cdiv(n, 256), 256, 0, stream>>>(n, faces, face_id, offsets, entries); }
+    GA_CHECK_LAUNCH("posmap_csr_scatter_kernel");
+    { ProfScope _ps("posmap_csr_sort_kernel", stream); posmap_csr_sort_kernel<<<cdiv(V, 256), 256, 0, stream>>>(V, offsets, entries); }
+    GA_CHECK_LAUNCH("posmap_csr_sort_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_posmap_fill_backward(int32_t B, int32_t S, int32_t V, const int32_t *csr_offsets, const int32_t *csr_entries,
+                                       const float *bary, const float *d_out, float *d_verts, void *stream_)
+{
+    GA_REQUIRE(B >= 1 && B <= kMaxB, "ga_posmap_fill_backward: batch %d outside [1, %d]", B, kMaxB);
+    GA_REQUIRE(S >= 1 && S <= kMaxS, "ga_posmap_fill_backward: map size %d outside [1, %d]", S, kMaxS);
+    GA_REQUIRE(V > 0 && V <= (1 << 24), "ga_posmap_fill_backward: bad vertex count %d", V);
+    GA_REQUIRE(csr_offsets && csr_entries && bary && d_out && d_verts, "ga_posmap_fill_backward: NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    { ProfScope _ps("posmap_fill_bwd_kernel", stream);
+      posmap_fill_bwd_kernel<<<dim3(cdiv(V, kFillBwdWarps), B), kFillBwdWarps * 32, 0, stream>>>(S, V, csr_offsets, csr_entries, bary, d_out,
+                                                                                                  d_verts); }
+    GA_CHECK_LAUNCH("posmap_fill_bwd_kernel");
     return GA_OK;
 }

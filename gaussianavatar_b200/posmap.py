@@ -5,8 +5,9 @@ one OBJ per frame, then an OpenGL render of each mesh in UV space.  Because that
 texel (and with which barycentric weights) does not depend on the pose: `PoseMapper` computes that layout once on the device
 (`ga_posmap_layout`), and a frame costs the posed vertices (`ga_smpl_vertices`) and a gather (`ga_posmap_fill`).  The coverage
 rules are the library's own statement of what the GL rasterizer does (csrc/posmap.cu; DESIGN.md, PARITY UNPINNED).
-`SmplxPoseMapper` does the same for SMPL-X (`ga_smplx_vertices`).  Their vertex-posing half, which needs no UV template, is
-`BodyPoser` / `SmplxBodyPoser`; the mesh overlay (`mesh_render`) uses it too.
+`SmplxPoseMapper` does the same for SMPL-X (`ga_smplx_vertices`).  Both are differentiable with respect to pose and transl
+(test-time pose fitting, `posefit.py`).  Their vertex-posing half, which needs no UV template, is `BodyPoser` / `SmplxBodyPoser`;
+the mesh overlay (`mesh_render`) uses it too.
 
 `canonical_assets` builds, from the same pieces, the per-subject and per-size files the reference makes with OpenGL
 (scripts/gen_pose_map_cano_smpl.py) or ships pre-rendered: the canonical query map and joint matrices, the UV face-id mask, the
@@ -183,7 +184,8 @@ class PoseMapper(BodyPoser):
 
     smpl, betas: as `BodyPoser` takes them; uv_template: a path to the UV template OBJ or what `load_uv_template_obj` returns; S: map
     size (1..512).  Face i of the map is the mesh face f[i] drawn at the UV corners of template face i, so the template must have
-    exactly F faces.  Everything runs on the current CUDA stream under no_grad."""
+    exactly F faces.  Everything runs on the current CUDA stream; calling the mapper with grad on and a pose or transl that requires
+    grad makes the maps differentiable with respect to both (`ga_posmap_fill_backward`, then the vertex-posing backward)."""
 
     def __init__(self, smpl, betas, uv_template, S: int, device="cuda"):
         BodyPoser.__init__(self, smpl, betas, device)
@@ -216,8 +218,33 @@ class PoseMapper(BodyPoser):
         return out
 
     def __call__(self, pose, transl) -> torch.Tensor:
-        """pose [B,72], transl [B,3] -> position maps [B,3,S,S]."""
+        """pose [B,72], transl [B,3] -> position maps [B,3,S,S], differentiable with respect to pose and transl when grad is on."""
+        if _wants_grad(pose, transl):
+            return _PoseMap.apply(self, pose, None, transl)
         return self.fill(self.vertices(pose, transl))
+
+    def vertex_csr(self):
+        """(offsets [V+1], entries [3 S^2]) int32: each vertex's (texel, corner) pairs, entry 3 t + i, ascending per vertex
+        (`ga_posmap_vertex_csr`); what the fill's backward runs over.  Built on first use, once per mapper."""
+        if getattr(self, "_csr", None) is None:
+            offsets = torch.empty(self.V + 1, dtype=torch.int32, device=self.device)
+            entries = torch.empty(3 * self.S * self.S, dtype=torch.int32, device=self.device)
+            _lib.check(_lib.lib().ga_posmap_vertex_csr(self.S, self.V, ptr(self.faces), ptr(self.face_id), ptr(offsets), ptr(entries),
+                                                       self._stream()), "ga_posmap_vertex_csr")
+            self._csr = (offsets, entries)
+        return self._csr
+
+    def fill_backward(self, d_maps: torch.Tensor) -> torch.Tensor:
+        """d_verts [B,V,3] of position-map gradients d_maps [B,3,S,S] (`ga_posmap_fill_backward`)."""
+        d_maps = d_maps.to(device=self.device, dtype=torch.float32).contiguous()
+        B = d_maps.shape[0]
+        offsets, entries = self.vertex_csr()
+        out = torch.empty(B, self.V, 3, dtype=torch.float32, device=self.device)
+        for s in range(0, B, MAX_FRAMES_PER_CALL):
+            e = min(B, s + MAX_FRAMES_PER_CALL)
+            _lib.check(_lib.lib().ga_posmap_fill_backward(e - s, self.S, self.V, ptr(offsets), ptr(entries), ptr(self.bary), ptr(d_maps[s:e]),
+                                                          ptr(out[s:e]), self._stream()), "ga_posmap_fill_backward")
+        return out
 
     @torch.no_grad()
     def weight_map(self) -> torch.Tensor:
@@ -236,8 +263,61 @@ class SmplxPoseMapper(SmplxBodyPoser, PoseMapper):
         PoseMapper.__init__(self, smplx, betas, uv_template, S, device)
 
     def __call__(self, pose, rest_pose, transl) -> torch.Tensor:
-        """pose [B,66], rest_pose [B,99], transl [B,3] -> position maps [B,3,S,S]."""
+        """pose [B,66], rest_pose [B,99], transl [B,3] -> position maps [B,3,S,S], differentiable with respect to pose and transl
+        (not rest_pose) when grad is on."""
+        if _wants_grad(pose, transl):
+            return _PoseMap.apply(self, pose, rest_pose, transl)
         return self.fill(self.vertices(pose, rest_pose, transl))
+
+
+def _wants_grad(*ts) -> bool:
+    return torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in ts)
+
+
+def vertices_backward(poser, pose, rest_pose, d_verts):
+    """(d_pose [B,72|66], d_transl [B,3]) of vertex gradients d_verts [B,V,3] at pose (and SMPL-X rest_pose), through
+    `ga_smpl_vertices_backward` / `ga_smplx_vertices_backward`."""
+    smplx = isinstance(poser, SmplxBodyPoser)
+    d_verts = d_verts.to(device=poser.device, dtype=torch.float32).contiguous()
+    B = pose.shape[0]
+    d_pose = torch.empty(B, poser.POSE_WIDTH, dtype=torch.float32, device=poser.device)
+    d_transl = torch.empty(B, 3, dtype=torch.float32, device=poser.device)
+    L = _lib.lib()
+    ws_fn = L.ga_smplx_vertices_backward_workspace_bytes if smplx else L.ga_smpl_vertices_backward_workspace_bytes
+    ws = torch.empty(ws_fn(min(B, MAX_FRAMES_PER_CALL), poser.V), dtype=torch.uint8, device=poser.device)
+    for s in range(0, B, MAX_FRAMES_PER_CALL):
+        e = min(B, s + MAX_FRAMES_PER_CALL)
+        common = (ptr(poser.rest_joints), ptr(poser.v_shaped), ptr(poser.posedirs), ptr(poser.weights), ptr(d_verts[s:e]), ptr(ws), ws.numel(),
+                  ptr(d_pose[s:e]), ptr(d_transl[s:e]), poser._stream())
+        if smplx:
+            _lib.check(L.ga_smplx_vertices_backward(e - s, poser.V, ptr(pose[s:e]), ptr(rest_pose[s:e]), *common), "ga_smplx_vertices_backward")
+        else:
+            _lib.check(L.ga_smpl_vertices_backward(e - s, poser.V, ptr(pose[s:e]), *common), "ga_smpl_vertices_backward")
+    return d_pose, d_transl
+
+
+class _PoseMap(torch.autograd.Function):
+    """(pose, [rest_pose,] transl) -> position maps [B,3,S,S] of a `PoseMapper` / `SmplxPoseMapper`: the forward kernels as the mapper
+    launches them, and backward through `ga_posmap_fill_backward` then the vertex-posing backward.  rest_pose is data."""
+
+    @staticmethod
+    def forward(ctx, mapper, pose, rest_pose, transl):
+        if rest_pose is None:
+            pose, transl = mapper._inputs(pose, transl)
+            verts = mapper.vertices(pose, transl)
+        else:
+            pose, rest_pose, transl = mapper._inputs(pose, rest_pose, transl)
+            verts = mapper.vertices(pose, rest_pose, transl)
+        ctx.mapper = mapper
+        ctx.save_for_backward(pose, rest_pose)
+        return mapper.fill(verts)
+
+    @staticmethod
+    def backward(ctx, d_maps):
+        pose, rest_pose = ctx.saved_tensors
+        mapper = ctx.mapper
+        d_pose, d_transl = vertices_backward(mapper, pose, rest_pose, mapper.fill_backward(d_maps))
+        return None, d_pose, None, d_transl
 
 
 def load_body_model(path):

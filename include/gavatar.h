@@ -217,6 +217,32 @@ int ga_posmap_layout(int32_t F, int32_t S, const float *uv_corners, int32_t *fac
 int ga_posmap_fill(int32_t B, int32_t S, int32_t V, const float *verts, const int32_t *faces, const int32_t *face_id,
                    const float *bary, float *out, void *stream);
 
+/* Gradients of the position maps with respect to pose and transl (test-time pose fitting through a stage-2 avatar).
+ *
+ * ga_smpl_vertices_backward / ga_smplx_vertices_backward: the adjoints of ga_smpl_vertices / ga_smplx_vertices.  From the forward's
+ *   inputs (transl does not enter the gradient) and d_verts [B,V,3] they write d_pose [B,72] (SMPL) or [B,66] (SMPL-X) and d_transl
+ *   [B,3], through both the pose blend shapes (posedirs, R_j - I) and the skinning transforms A_j (the joint chain).  SMPL-X's
+ *   rest_pose [B,99] is data and has no gradient.  1 <= B <= 8; posedirs is read once per call for all frames.  workspace:
+ *   ga_*_vertices_backward_workspace_bytes(B, V) bytes, 4-byte aligned, scratch of the call (per-CTA partial sums, added in a fixed
+ *   order by a second kernel).  No floating-point atomics: the results are bit-reproducible and a frame's do not depend on the batch.
+ * ga_posmap_vertex_csr: for the layout face_id [S,S] of faces [F,3] (indices below V), the vertex -> (texel, corner) lists the fill
+ *   backward runs over: offsets [V+1] and entries [3 S^2] (int32; the first offsets[V] are used), entry 3 t + i for texel t whose
+ *   covering face has the vertex as corner i, ascending within each vertex.  Run once per layout.
+ * ga_posmap_fill_backward: d_verts [B,V,3] = sum over each vertex's entries of bary[t,i] d_out[b,:,t], for d_out [B,3,S,S], 1 <= B <= 8.
+ *   No atomics; every element of d_verts is written (0 for a vertex no texel uses). */
+size_t ga_smpl_vertices_backward_workspace_bytes(int32_t B, int32_t V);
+size_t ga_smplx_vertices_backward_workspace_bytes(int32_t B, int32_t V);
+int ga_smpl_vertices_backward(int32_t B, int32_t V, const float *pose, const float *rest_joints, const float *v_shaped,
+                              const float *posedirs, const float *weights, const float *d_verts, void *workspace, size_t workspace_bytes,
+                              float *d_pose, float *d_transl, void *stream);
+int ga_smplx_vertices_backward(int32_t B, int32_t V, const float *pose, const float *rest_pose, const float *rest_joints,
+                               const float *v_shaped, const float *posedirs, const float *weights, const float *d_verts, void *workspace,
+                               size_t workspace_bytes, float *d_pose, float *d_transl, void *stream);
+int ga_posmap_vertex_csr(int32_t S, int32_t V, const int32_t *faces, const int32_t *face_id, int32_t *offsets, int32_t *entries,
+                         void *stream);
+int ga_posmap_fill_backward(int32_t B, int32_t S, int32_t V, const int32_t *csr_offsets, const int32_t *csr_entries, const float *bary,
+                            const float *d_out, float *d_verts, void *stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Fused Gaussian LBS + attribute assembly (model/avatar_model.py:308-326).  dec_out [S*S,8] pixel-major packed decoder
  * output (res.xyz, scale, rgb, pad); valid_index [N] int32 = flat UV index of the n-th valid pixel; query_points [N,3];
