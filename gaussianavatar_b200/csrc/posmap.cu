@@ -1,4 +1,5 @@
-// Stage-2 input position maps on the device: posed SMPL mesh vertices, the UV-space coverage layout, and the per-frame fill.
+// Stage-2 input position maps on the device: posed SMPL / SMPL-X mesh vertices and their backward, the UV-space coverage layout, and
+// the per-frame fill and its backward.
 //
 // Replaces the reference's offline pipeline scripts/gen_pose_map_our_smpl.py (smplx forward -> OBJ per frame -> PosRender in a GLUT
 // window, shaders pos_uv.vs / pos_uv.fs).  The rasterization happens in UV space (gl_Position = 2 (uv - 0.5)), so which face
@@ -24,8 +25,6 @@
 namespace ga {
 namespace {
 
-constexpr int kJoints = 24;
-constexpr int kPoseFeat = 9 * (kJoints - 1);     // 207 pose blend-shape coefficients
 constexpr int kMaxB = 8;
 constexpr int kVertsPerCta = 32;
 constexpr int kCols = 3 * kVertsPerCta;          // posedirs columns per CTA
@@ -34,55 +33,73 @@ constexpr int kVertThreads = kCols * kRowGroups;
 constexpr int kNoFace = 0x7f7f7f7f;                // face_id before the raster pass: every byte 0x7f (one memset)
 constexpr int kMaxS = 512;
 
-__constant__ int c_parents_v[kJoints] = {-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21};
-
-// Posed vertices of B <= 8 frames.  Every CTA first forms the B frames' pose features and joint transforms A (joint j's global
-// transform is the product of its ancestors' local transforms, one lane per joint, so no chain walk), then streams its 96 columns
-// of posedirs [207, 3V] ONCE for all B frames (four row groups, reduced in shared memory), then skins its 32 vertices.
-__global__ void __launch_bounds__(kVertThreads)
-smpl_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,72]*/, const float *__restrict__ transl /*[B,3]*/,
-                     const float *__restrict__ J /*[24,3]*/, const float *__restrict__ v_shaped /*[V,3]*/,
-                     const float *__restrict__ posedirs /*[207,3V]*/, const float *__restrict__ weights /*[V,24]*/,
-                     float *__restrict__ verts /*[B,V,3]*/)
+// The pose phase of vertex posing, forward and backward alike: the pose features feat[b] (R_j - I of every joint but the root) and
+// the rest-relative joint transforms A[b] of B <= 8 frames.  The B x kJ (frame, joint) pairs are spread over the CTA's kThreads
+// threads, and each pair forms its own product of ancestors, so a frame's result does not depend on the batch it is in.  L holds
+// the local transforms; it is dead on return.
+template <int kJ, int kThreads>
+__device__ __forceinline__ void pose_phase(int B, const float *__restrict__ pose, const float *__restrict__ rest_pose,
+                                           const float *__restrict__ J, float (*L)[kJ][12], float (*A)[kJ][12],
+                                           float (*feat)[Body<kJ>::kFeat])
 {
-    __shared__ float sL[kMaxB][kJoints][12], sA[kMaxB][kJoints][12];
-    __shared__ float sFeat[kMaxB][kPoseFeat];
-    __shared__ float sPart[kRowGroups][kMaxB][kCols];
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    if (warp < B && lane < kJoints) {
-        const int b = warp, j = lane;
-        const float r[3] = {pose[b * 72 + j * 3], pose[b * 72 + j * 3 + 1], pose[b * 72 + j * 3 + 2]};
-        float R[9], th;
+    for (int i = threadIdx.x; i < B * kJ; i += kThreads) {
+        const int b = i / kJ, j = i % kJ;
+        float r[3], R[9], th;
+        joint_axis_angle<kJ>(pose, rest_pose, b, j, r);
         rodrigues(r, R, &th);
-        const int p = c_parents_v[j];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            sL[b][j][k * 4 + 0] = R[k * 3 + 0]; sL[b][j][k * 4 + 1] = R[k * 3 + 1]; sL[b][j][k * 4 + 2] = R[k * 3 + 2];
-            sL[b][j][k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
-        }
+        local_transform<kJ>(R, J, j, L[b][j]);
         if (j > 0) {
 #pragma unroll
-            for (int k = 0; k < 9; ++k) sFeat[b][(j - 1) * 9 + k] = R[k] - ((k % 4 == 0) ? 1.f : 0.f);
+            for (int k = 0; k < 9; ++k) feat[b][(j - 1) * 9 + k] = R[k] - ((k % 4 == 0) ? 1.f : 0.f);
         }
     }
     __syncthreads();
-    if (warp < B && lane < kJoints) {
-        const int b = warp, j = lane;
-        float G[12], T[12];
-#pragma unroll
-        for (int k = 0; k < 12; ++k) G[k] = sL[b][j][k];
-        for (int p = c_parents_v[j]; p >= 0; p = c_parents_v[p]) {
-            aff_mul(sL[b][p], G, T);
-#pragma unroll
-            for (int k = 0; k < 12; ++k) G[k] = T[k];
-        }
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-            sA[b][j][r * 4 + 0] = G[r * 4 + 0]; sA[b][j][r * 4 + 1] = G[r * 4 + 1]; sA[b][j][r * 4 + 2] = G[r * 4 + 2];
-            sA[b][j][r * 4 + 3] = G[r * 4 + 3] - (G[r * 4 + 0] * J[j * 3] + G[r * 4 + 1] * J[j * 3 + 1] + G[r * 4 + 2] * J[j * 3 + 2]);
-        }
+    for (int i = threadIdx.x; i < B * kJ; i += kThreads) {
+        const int b = i / kJ, j = i % kJ;
+        float G[12];
+        chain_product<kJ>(L[b], j, G);
+        rest_relative(G, J, j, A[b][j]);
     }
     __syncthreads();
+}
+
+// T_v = sum_j w_vj A_j: the blended transform of a vertex with skinning weights w [kJ], from one frame's A
+template <int kJ>
+__device__ __forceinline__ void blend_transform(const float *__restrict__ w, const float (*A)[12], float T[12])
+{
+#pragma unroll
+    for (int q = 0; q < 12; ++q) T[q] = 0.f;
+    for (int j = 0; j < kJ; ++j) {
+        const float wj = w[j];
+#pragma unroll
+        for (int q = 0; q < 12; ++q) T[q] = fmaf(wj, A[j][q], T[q]);
+    }
+}
+
+// 28.1 KB for SMPL, 56.4 KB for SMPL-X (above the 48 KB of static shared memory: dynamic, with the opt-in).  The local transforms
+// are dead once A is formed, so the row-group partial sums reuse their space.
+template <int kJ> struct VertSmem {
+    float A[kMaxB][kJ][12];
+    float feat[kMaxB][Body<kJ>::kFeat];
+    union {
+        float L[kMaxB][kJ][12];
+        float part[kRowGroups][kMaxB][kCols];
+    } u;
+};
+
+// Posed vertices of B <= 8 frames.  Every CTA forms the B frames' pose features and joint transforms A (pose_phase), then streams its
+// 96 columns of posedirs [kFeat, 3V] ONCE for all B frames (four row groups, reduced in shared memory), then skins its 32 vertices.
+template <int kJ>
+__global__ void __launch_bounds__(kVertThreads)
+vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,3 kTrained]*/, const float *__restrict__ rest_pose /*[B,3 (kJ-kTrained)]*/,
+                const float *__restrict__ transl /*[B,3]*/, const float *__restrict__ J /*[kJ,3]*/,
+                const float *__restrict__ v_shaped /*[V,3]*/, const float *__restrict__ posedirs /*[kFeat,3V]*/,
+                const float *__restrict__ weights /*[V,kJ]*/, float *__restrict__ verts /*[B,V,3]*/)
+{
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    VertSmem<kJ> &sm = *reinterpret_cast<VertSmem<kJ> *>(smem_raw);
+    const int tid = threadIdx.x;
+    pose_phase<kJ, kVertThreads>(B, pose, rest_pose, J, sm.u.L, sm.A, sm.feat);     // L is dead from here on: part may overwrite it
 
     // pose blend shapes: column k of posedirs, rows rg, rg + 4, ...; one accumulator per frame
     const int col = tid % kCols, rg = tid / kCols;
@@ -93,125 +110,7 @@ smpl_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,72]*/, co
     for (int b = 0; b < kMaxB; ++b) acc[b] = 0.f;
     if (k < ncol) {
 #pragma unroll 4
-        for (int r = rg; r < kPoseFeat; r += kRowGroups) {
-            const float pd = __ldg(posedirs + (long long)r * ncol + k);
-#pragma unroll
-            for (int b = 0; b < kMaxB; ++b)
-                if (b < B) acc[b] = fmaf(sFeat[b][r], pd, acc[b]);
-        }
-    }
-#pragma unroll
-    for (int b = 0; b < kMaxB; ++b)
-        if (b < B) sPart[rg][b][col] = acc[b];
-    __syncthreads();
-
-    // skinning: T = sum_j w_vj A_j, x = T [v_posed; 1] + transl
-    for (int i = tid; i < kVertsPerCta * B; i += kVertThreads) {
-        const int vl = i % kVertsPerCta, b = i / kVertsPerCta;
-        const int v = blockIdx.x * kVertsPerCta + vl;
-        if (v >= V) continue;
-        float x[3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            float off = 0.f;
-#pragma unroll
-            for (int g = 0; g < kRowGroups; ++g) off += sPart[g][b][vl * 3 + c];
-            x[c] = v_shaped[(size_t)v * 3 + c] + off;
-        }
-        float T[12];
-#pragma unroll
-        for (int q = 0; q < 12; ++q) T[q] = 0.f;
-        const float *w = weights + (size_t)v * kJoints;
-        for (int j = 0; j < kJoints; ++j) {
-            const float wj = w[j];
-#pragma unroll
-            for (int q = 0; q < 12; ++q) T[q] = fmaf(wj, sA[b][j][q], T[q]);
-        }
-        float *o = verts + ((size_t)b * V + v) * 3;
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-            o[r] = T[r * 4 + 0] * x[0] + T[r * 4 + 1] * x[1] + T[r * 4 + 2] * x[2] + T[r * 4 + 3] + transl[b * 3 + r];
-    }
-}
-
-// ---- SMPL-X (55 joints: global, 21 body, jaw, eyes, 2 x 15 finger joints; kintree_table[0] of SMPLX_*.npz)
-constexpr int kJointsX = 55;
-constexpr int kTrainX = 22;                      // joints taken from pose [B,66]; the other 33 from rest_pose [B,99]
-constexpr int kPoseFeatX = 9 * (kJointsX - 1);   // 486 pose blend-shape coefficients
-
-__constant__ int c_parents_vx[kJointsX] = {-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 15, 15, 15, 20,
-                                           25, 26, 20, 28, 29, 20, 31, 32, 20, 34, 35, 20, 37, 38, 21, 40, 41, 21, 43, 44, 21, 46, 47,
-                                           21, 49, 50, 21, 52, 53};
-
-// 56.4 KB, above the 48 KB of static shared memory: dynamic, with the opt-in.  The local transforms are dead once A is formed, so
-// the row-group partial sums reuse their space.
-struct SmplxVertSmem {
-    float A[kMaxB][kJointsX][12];
-    float feat[kMaxB][kPoseFeatX];
-    union {
-        float L[kMaxB][kJointsX][12];
-        float part[kRowGroups][kMaxB][kCols];
-    } u;
-};
-
-// The SMPL-X counterpart of smpl_vertices_kernel, same three phases.  55 joints do not fit one lane each in a warp per frame, so
-// the B x 55 (frame, joint) pairs are spread over the whole CTA; each pair still forms its own product of ancestors, so a frame's
-// result does not depend on the batch it is in.
-__global__ void __launch_bounds__(kVertThreads)
-smplx_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,66]*/, const float *__restrict__ rest_pose /*[B,99]*/,
-                      const float *__restrict__ transl /*[B,3]*/, const float *__restrict__ J /*[55,3]*/,
-                      const float *__restrict__ v_shaped /*[V,3]*/, const float *__restrict__ posedirs /*[486,3V]*/,
-                      const float *__restrict__ weights /*[V,55]*/, float *__restrict__ verts /*[B,V,3]*/)
-{
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    SmplxVertSmem &sm = *reinterpret_cast<SmplxVertSmem *>(smem_raw);
-    const int tid = threadIdx.x;
-    for (int i = tid; i < B * kJointsX; i += kVertThreads) {
-        const int b = i / kJointsX, j = i % kJointsX;
-        const float *src = (j < kTrainX) ? pose + (size_t)b * (3 * kTrainX) + j * 3
-                                         : rest_pose + (size_t)b * (3 * (kJointsX - kTrainX)) + (j - kTrainX) * 3;
-        const float r[3] = {src[0], src[1], src[2]};
-        float R[9], th;
-        rodrigues(r, R, &th);
-        const int p = c_parents_vx[j];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            sm.u.L[b][j][k * 4 + 0] = R[k * 3 + 0]; sm.u.L[b][j][k * 4 + 1] = R[k * 3 + 1]; sm.u.L[b][j][k * 4 + 2] = R[k * 3 + 2];
-            sm.u.L[b][j][k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
-        }
-        if (j > 0) {
-#pragma unroll
-            for (int k = 0; k < 9; ++k) sm.feat[b][(j - 1) * 9 + k] = R[k] - ((k % 4 == 0) ? 1.f : 0.f);
-        }
-    }
-    __syncthreads();
-    for (int i = tid; i < B * kJointsX; i += kVertThreads) {
-        const int b = i / kJointsX, j = i % kJointsX;
-        float G[12], T[12];
-#pragma unroll
-        for (int k = 0; k < 12; ++k) G[k] = sm.u.L[b][j][k];
-        for (int p = c_parents_vx[j]; p >= 0; p = c_parents_vx[p]) {
-            aff_mul(sm.u.L[b][p], G, T);
-#pragma unroll
-            for (int k = 0; k < 12; ++k) G[k] = T[k];
-        }
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-            sm.A[b][j][r * 4 + 0] = G[r * 4 + 0]; sm.A[b][j][r * 4 + 1] = G[r * 4 + 1]; sm.A[b][j][r * 4 + 2] = G[r * 4 + 2];
-            sm.A[b][j][r * 4 + 3] = G[r * 4 + 3] - (G[r * 4 + 0] * J[j * 3] + G[r * 4 + 1] * J[j * 3 + 1] + G[r * 4 + 2] * J[j * 3 + 2]);
-        }
-    }
-    __syncthreads();        // L is dead from here on: part may overwrite it
-
-    const int col = tid % kCols, rg = tid / kCols;
-    const long long ncol = 3LL * V;
-    const long long k = (long long)blockIdx.x * kCols + col;
-    float acc[kMaxB];
-#pragma unroll
-    for (int b = 0; b < kMaxB; ++b) acc[b] = 0.f;
-    if (k < ncol) {
-#pragma unroll 4
-        for (int r = rg; r < kPoseFeatX; r += kRowGroups) {
+        for (int r = rg; r < Body<kJ>::kFeat; r += kRowGroups) {
             const float pd = __ldg(posedirs + (long long)r * ncol + k);
 #pragma unroll
             for (int b = 0; b < kMaxB; ++b)
@@ -223,6 +122,7 @@ smplx_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,66]*/, c
         if (b < B) sm.u.part[rg][b][col] = acc[b];
     __syncthreads();
 
+    // skinning: x = T_v [v_posed; 1] + transl
     for (int i = tid; i < kVertsPerCta * B; i += kVertThreads) {
         const int vl = i % kVertsPerCta, b = i / kVertsPerCta;
         const int v = blockIdx.x * kVertsPerCta + vl;
@@ -236,14 +136,7 @@ smplx_vertices_kernel(int B, int V, const float *__restrict__ pose /*[B,66]*/, c
             x[c] = v_shaped[(size_t)v * 3 + c] + off;
         }
         float T[12];
-#pragma unroll
-        for (int q = 0; q < 12; ++q) T[q] = 0.f;
-        const float *w = weights + (size_t)v * kJointsX;
-        for (int j = 0; j < kJointsX; ++j) {
-            const float wj = w[j];
-#pragma unroll
-            for (int q = 0; q < 12; ++q) T[q] = fmaf(wj, sm.A[b][j][q], T[q]);
-        }
+        blend_transform<kJ>(weights + (size_t)v * kJ, sm.A[b], T);
         float *o = verts + ((size_t)b * V + v) * 3;
 #pragma unroll
         for (int r = 0; r < 3; ++r)
@@ -378,22 +271,12 @@ posmap_fill_kernel(int S, int V, const float *__restrict__ verts, const int *__r
 constexpr int kBwdThreads = 256;
 constexpr int kBwdWarps = kBwdThreads / 32;
 
-template <int kJ> struct BodyDims;
-template <> struct BodyDims<kJoints> {
-    static constexpr int kFeat = kPoseFeat, kTrained = kJoints;
-    static __device__ __forceinline__ int parent(int j) { return c_parents_v[j]; }
-};
-template <> struct BodyDims<kJointsX> {
-    static constexpr int kFeat = kPoseFeatX, kTrained = kTrainX;
-    static __device__ __forceinline__ int parent(int j) { return c_parents_vx[j]; }
-};
-
 // per-frame sums of one CTA: d_A [J,12], d_feat [kFeat], d_transl [3]
-template <int kJ> constexpr int bwd_sums() { return kJ * 12 + BodyDims<kJ>::kFeat + 3; }
+template <int kJ> constexpr int bwd_sums() { return kJ * 12 + Body<kJ>::kFeat + 3; }
 
 template <int kJ> struct VertBwdSmem {
     float A[kMaxB][kJ][12];
-    float feat[kMaxB][BodyDims<kJ>::kFeat];
+    float feat[kMaxB][Body<kJ>::kFeat];
     float g[kMaxB][kCols];           // d_verts of the CTA's 32 vertices
     float dx[kMaxB][kCols];          // T_v[:, :3]^T g_v
     float x[kMaxB][kCols];           // blend-shaped vertices
@@ -409,48 +292,13 @@ template <int kJ> struct VertFinishSmem {
     float L[kJ][12], G[kJ][12], dG[kJ][12], dR[kJ][9];
 };
 
-// axis-angle of joint j of frame b: SMPL takes all 24 from pose [B,72]; SMPL-X the first 22 from pose [B,66], the rest from rest_pose
-template <int kJ>
-__device__ __forceinline__ void joint_axis_angle(const float *__restrict__ pose, const float *__restrict__ rest_pose, int b, int j, float r[3])
-{
-    constexpr int kT = BodyDims<kJ>::kTrained;
-    const float *src = (j < kT) ? pose + (size_t)b * (3 * kT) + j * 3 : rest_pose + (size_t)b * (3 * (kJ - kT)) + (j - kT) * 3;
-    r[0] = src[0]; r[1] = src[1]; r[2] = src[2];
-}
-
-// local transform of joint j (rotation | offset to its parent) from its rotation R
-template <int kJ>
-__device__ __forceinline__ void local_transform(const float R[9], const float *__restrict__ J, int j, float *L)
-{
-    const int p = BodyDims<kJ>::parent(j);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        L[k * 4 + 0] = R[k * 3 + 0]; L[k * 4 + 1] = R[k * 3 + 1]; L[k * 4 + 2] = R[k * 3 + 2];
-        L[k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
-    }
-}
-
-// global transform of joint j: the product of its ancestors' local transforms, root first (the forwards' order)
-template <int kJ>
-__device__ __forceinline__ void chain_product(const float (*L)[12], int j, float G[12])
-{
-    float T[12];
-#pragma unroll
-    for (int k = 0; k < 12; ++k) G[k] = L[j][k];
-    for (int p = BodyDims<kJ>::parent(j); p >= 0; p = BodyDims<kJ>::parent(p)) {
-        aff_mul(L[p], G, T);
-#pragma unroll
-        for (int k = 0; k < 12; ++k) G[k] = T[k];
-    }
-}
-
 template <int kJ>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 vertices_bwd_kernel(int B, int V, const float *__restrict__ pose, const float *__restrict__ rest_pose, const float *__restrict__ J,
                     const float *__restrict__ v_shaped, const float *__restrict__ posedirs, const float *__restrict__ weights,
                     const float *__restrict__ d_verts, float *__restrict__ sums /*[ctas][B][bwd_sums]*/)
 {
-    constexpr int kF = BodyDims<kJ>::kFeat, kN = bwd_sums<kJ>();
+    constexpr int kF = Body<kJ>::kFeat, kN = bwd_sums<kJ>();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     VertBwdSmem<kJ> &sm = *reinterpret_cast<VertBwdSmem<kJ> *>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -461,29 +309,7 @@ vertices_bwd_kernel(int B, int V, const float *__restrict__ pose, const float *_
         const int b = i / kCols, col = i % kCols;
         sm.g[b][col] = (k0 + col < ncol) ? d_verts[(size_t)b * ncol + k0 + col] : 0.f;
     }
-    for (int i = tid; i < B * kJ; i += kBwdThreads) {
-        const int b = i / kJ, j = i % kJ;
-        float r[3], R[9], th;
-        joint_axis_angle<kJ>(pose, rest_pose, b, j, r);
-        rodrigues(r, R, &th);
-        local_transform<kJ>(R, J, j, sm.u.L[b][j]);
-        if (j > 0) {
-#pragma unroll
-            for (int k = 0; k < 9; ++k) sm.feat[b][(j - 1) * 9 + k] = R[k] - ((k % 4 == 0) ? 1.f : 0.f);
-        }
-    }
-    __syncthreads();
-    for (int i = tid; i < B * kJ; i += kBwdThreads) {
-        const int b = i / kJ, j = i % kJ;
-        float G[12];
-        chain_product<kJ>(sm.u.L[b], j, G);
-#pragma unroll
-        for (int r = 0; r < 3; ++r) {
-            sm.A[b][j][r * 4 + 0] = G[r * 4 + 0]; sm.A[b][j][r * 4 + 1] = G[r * 4 + 1]; sm.A[b][j][r * 4 + 2] = G[r * 4 + 2];
-            sm.A[b][j][r * 4 + 3] = G[r * 4 + 3] - (G[r * 4 + 0] * J[j * 3] + G[r * 4 + 1] * J[j * 3 + 1] + G[r * 4 + 2] * J[j * 3 + 2]);
-        }
-    }
-    __syncthreads();        // L is dead from here on
+    pose_phase<kJ, kBwdThreads>(B, pose, rest_pose, J, sm.u.L, sm.A, sm.feat);     // L is dead from here on
 
     // dx_v = T_v[:, :3]^T g_v
     for (int i = tid; i < B * kVertsPerCta; i += kBwdThreads) {
@@ -492,14 +318,7 @@ vertices_bwd_kernel(int B, int V, const float *__restrict__ pose, const float *_
         float d[3] = {0.f, 0.f, 0.f};
         if (v < V) {
             float T[12];
-#pragma unroll
-            for (int q = 0; q < 12; ++q) T[q] = 0.f;
-            const float *w = weights + (size_t)v * kJ;
-            for (int j = 0; j < kJ; ++j) {
-                const float wj = w[j];
-#pragma unroll
-                for (int q = 0; q < 12; ++q) T[q] = fmaf(wj, sm.A[b][j][q], T[q]);
-            }
+            blend_transform<kJ>(weights + (size_t)v * kJ, sm.A[b], T);
             const float *g = sm.g[b] + vl * 3;
 #pragma unroll
             for (int c = 0; c < 3; ++c) d[c] = T[c] * g[0] + T[4 + c] * g[1] + T[8 + c] * g[2];
@@ -577,46 +396,13 @@ vertices_bwd_kernel(int B, int V, const float *__restrict__ pose, const float *_
     }
 }
 
-// Backward of rodrigues(): R = I + s K + (1 - c) K^2 with K the cross matrix of d = r / theta, theta = |r + 1e-8|.
-__device__ __forceinline__ void rodrigues_bwd(const float r[3], const float gR[9], float gr[3])
-{
-    const float n[3] = {r[0] + 1e-8f, r[1] + 1e-8f, r[2] + 1e-8f};
-    const float theta = sqrtf(n[0] * n[0] + n[1] * n[1] + n[2] * n[2]);
-    const float dx = r[0] / theta, dy = r[1] / theta, dz = r[2] / theta;
-    float s, c;
-    sincosf(theta, &s, &c);
-    const float K[9] = {0.f, -dz, dy, dz, 0.f, -dx, -dy, dx, 0.f};
-    float K2[9], gK[9];
-    float gs = 0.f, g1c = 0.f;
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) K2[i * 3 + j] = K[i * 3] * K[j] + K[i * 3 + 1] * K[3 + j] + K[i * 3 + 2] * K[6 + j];
-#pragma unroll
-    for (int i = 0; i < 9; ++i) { gs = fmaf(gR[i], K[i], gs); g1c = fmaf(gR[i], K2[i], g1c); }
-    // d(K^2) = dK K + K dK: gK = s gR + (1 - c) (gR K^T + K^T gR)
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-            float t = 0.f;
-#pragma unroll
-            for (int k = 0; k < 3; ++k) t += gR[i * 3 + k] * K[j * 3 + k] + K[k * 3 + i] * gR[k * 3 + j];
-            gK[i * 3 + j] = s * gR[i * 3 + j] + (1.f - c) * t;
-        }
-    const float gd[3] = {gK[7] - gK[5], gK[2] - gK[6], gK[3] - gK[1]};
-    float gth = gs * c + g1c * s - (gd[0] * r[0] + gd[1] * r[1] + gd[2] * r[2]) / (theta * theta);
-#pragma unroll
-    for (int k = 0; k < 3; ++k) gr[k] = gd[k] / theta + gth * n[k] / theta;
-}
-
 // One CTA per frame: add the CTAs' sums in order, then d_A -> d_G -> (joint chain, leaves first) d_L -> d_R (+ d_feat) -> d_pose.
 template <int kJ>
 __global__ void __launch_bounds__(kBwdThreads)
 vertices_bwd_finish_kernel(int B, int ctas, const float *__restrict__ pose, const float *__restrict__ rest_pose,
                            const float *__restrict__ J, const float *__restrict__ sums, float *__restrict__ d_pose, float *__restrict__ d_transl)
 {
-    constexpr int kF = BodyDims<kJ>::kFeat, kN = bwd_sums<kJ>(), kT = BodyDims<kJ>::kTrained;
+    constexpr int kF = Body<kJ>::kFeat, kN = bwd_sums<kJ>(), kT = Body<kJ>::kTrained;
     __shared__ VertFinishSmem<kJ> sm;
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
     for (int e = tid; e < kN; e += kBwdThreads) {
@@ -642,7 +428,7 @@ vertices_bwd_finish_kernel(int B, int ctas, const float *__restrict__ pose, cons
     if (tid < 32) {
         // G_j = G_p L_j, leaves first (every parent index is below its child's); lane q owns element q of d_G_p, lane < 9 of d_L_j
         for (int j = kJ - 1; j >= 0; --j) {
-            const int p = BodyDims<kJ>::parent(j);
+            const int p = Body<kJ>::parent(j);
             const float *dG = sm.dG[j];
             if (lane < 9) {
                 const int rr = lane / 3, k = lane % 3;
@@ -790,6 +576,26 @@ posmap_fill_bwd_kernel(int S, int V, const int *__restrict__ offsets, const int 
     if (lane < 3) d_verts[((size_t)b * V + v) * 3 + lane] = a[lane];
 }
 
+template <int kJ>
+int vertices_forward(const char *name, int B, int V, const float *pose, const float *rest_pose, const float *transl, const float *rest_joints,
+                     const float *v_shaped, const float *posedirs, const float *weights, float *verts, cudaStream_t stream)
+{
+    GA_REQUIRE(B >= 0 && B <= kMaxB, "%s: batch %d outside [0, %d]", name, B, kMaxB);
+    GA_REQUIRE(V > 0 && V <= (1 << 24), "%s: bad vertex count %d", name, V);
+    if (B == 0) return GA_OK;
+    GA_REQUIRE(pose && (kJ == kSmplJoints || rest_pose) && transl && rest_joints && v_shaped && posedirs && weights && verts,
+               "NULL pointer argument");
+    static PerDeviceOnce attr_set;
+    if (attr_set.first())
+        GA_CHECK_CUDA(cudaFuncSetAttribute(vertices_kernel<kJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VertSmem<kJ>)));
+    const char *kernel = kJ == kSmplJoints ? "smpl_vertices_kernel" : "smplx_vertices_kernel";
+    { ProfScope _ps(kernel, stream);
+      vertices_kernel<kJ><<<cdiv(V, kVertsPerCta), kVertThreads, sizeof(VertSmem<kJ>), stream>>>(B, V, pose, rest_pose, transl, rest_joints,
+                                                                                               v_shaped, posedirs, weights, verts); }
+    GA_CHECK_LAUNCH(kernel);
+    return GA_OK;
+}
+
 template <int kJ> size_t vertices_bwd_workspace(int B, int V)
 {
     if (B < 1 || B > kMaxB || V < 1 || V > (1 << 24)) return 0;
@@ -803,7 +609,7 @@ int vertices_backward(const char *name, int B, int V, const float *pose, const f
 {
     GA_REQUIRE(B >= 1 && B <= kMaxB, "%s: batch %d outside [1, %d]", name, B, kMaxB);
     GA_REQUIRE(V > 0 && V <= (1 << 24), "%s: bad vertex count %d", name, V);
-    GA_REQUIRE(pose && (kJ == kJoints || rest_pose) && rest_joints && v_shaped && posedirs && weights && d_verts && workspace && d_pose && d_transl,
+    GA_REQUIRE(pose && (kJ == kSmplJoints || rest_pose) && rest_joints && v_shaped && posedirs && weights && d_verts && workspace && d_pose && d_transl,
                "%s: NULL pointer argument", name);
     const size_t need = vertices_bwd_workspace<kJ>(B, V);
     GA_REQUIRE(workspace_bytes >= need, "%s: workspace of %zu bytes, %zu needed", name, workspace_bytes, need);
@@ -813,11 +619,11 @@ int vertices_backward(const char *name, int B, int V, const float *pose, const f
         GA_CHECK_CUDA(cudaFuncSetAttribute(vertices_bwd_kernel<kJ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VertBwdSmem<kJ>)));
     const int ctas = cdiv(V, kVertsPerCta);
     float *sums = static_cast<float *>(workspace);
-    { ProfScope _ps(kJ == kJoints ? "smpl_vertices_bwd_kernel" : "smplx_vertices_bwd_kernel", stream);
+    { ProfScope _ps(kJ == kSmplJoints ? "smpl_vertices_bwd_kernel" : "smplx_vertices_bwd_kernel", stream);
       vertices_bwd_kernel<kJ><<<ctas, kBwdThreads, sizeof(VertBwdSmem<kJ>), stream>>>(B, V, pose, rest_pose, rest_joints, v_shaped,
                                                                                       posedirs, weights, d_verts, sums); }
     GA_CHECK_LAUNCH("vertices_bwd_kernel");
-    { ProfScope _ps(kJ == kJoints ? "smpl_vertices_bwd_finish_kernel" : "smplx_vertices_bwd_finish_kernel", stream);
+    { ProfScope _ps(kJ == kSmplJoints ? "smpl_vertices_bwd_finish_kernel" : "smplx_vertices_bwd_finish_kernel", stream);
       vertices_bwd_finish_kernel<kJ><<<B, kBwdThreads, 0, stream>>>(B, ctas, pose, rest_pose, rest_joints, sums, d_pose, d_transl); }
     GA_CHECK_LAUNCH("vertices_bwd_finish_kernel");
     return GA_OK;
@@ -831,41 +637,22 @@ using namespace ga;
 extern "C" int ga_smpl_vertices(int32_t B, int32_t V, const float *pose, const float *transl, const float *rest_joints,
                                 const float *v_shaped, const float *posedirs, const float *weights, float *verts, void *stream_)
 {
-    GA_REQUIRE(B >= 0 && B <= kMaxB, "ga_smpl_vertices: batch %d outside [0, %d]", B, kMaxB);
-    GA_REQUIRE(V > 0 && V <= (1 << 24), "ga_smpl_vertices: bad vertex count %d", V);
-    if (B == 0) return GA_OK;
-    GA_REQUIRE(pose && transl && rest_joints && v_shaped && posedirs && weights && verts, "NULL pointer argument");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    { ProfScope _ps("smpl_vertices_kernel", stream);
-      smpl_vertices_kernel<<<cdiv(V, kVertsPerCta), kVertThreads, 0, stream>>>(B, V, pose, transl, rest_joints, v_shaped, posedirs,
-               weights, verts); }
-    GA_CHECK_LAUNCH("smpl_vertices_kernel");
-    return GA_OK;
+    return vertices_forward<kSmplJoints>("ga_smpl_vertices", B, V, pose, nullptr, transl, rest_joints, v_shaped, posedirs, weights, verts,
+                                         static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ga_smplx_vertices(int32_t B, int32_t V, const float *pose, const float *rest_pose, const float *transl, const float *rest_joints,
                                  const float *v_shaped, const float *posedirs, const float *weights, float *verts, void *stream_)
 {
-    GA_REQUIRE(B >= 0 && B <= kMaxB, "ga_smplx_vertices: batch %d outside [0, %d]", B, kMaxB);
-    GA_REQUIRE(V > 0 && V <= (1 << 24), "ga_smplx_vertices: bad vertex count %d", V);
-    if (B == 0) return GA_OK;
-    GA_REQUIRE(pose && rest_pose && transl && rest_joints && v_shaped && posedirs && weights && verts, "NULL pointer argument");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    static PerDeviceOnce attr_set;
-    if (attr_set.first())
-        GA_CHECK_CUDA(cudaFuncSetAttribute(smplx_vertices_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmplxVertSmem)));
-    { ProfScope _ps("smplx_vertices_kernel", stream);
-      smplx_vertices_kernel<<<cdiv(V, kVertsPerCta), kVertThreads, sizeof(SmplxVertSmem), stream>>>(B, V, pose, rest_pose, transl, rest_joints,
-               v_shaped, posedirs, weights, verts); }
-    GA_CHECK_LAUNCH("smplx_vertices_kernel");
-    return GA_OK;
+    return vertices_forward<kSmplxJoints>("ga_smplx_vertices", B, V, pose, rest_pose, transl, rest_joints, v_shaped, posedirs, weights, verts,
+                                          static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ga_posmap_weights(int32_t S, int32_t J, const float *weights, const int32_t *faces, const int32_t *face_id, const float *bary,
                                  float *out, void *stream_)
 {
     GA_REQUIRE(S >= 1 && S <= kMaxS, "ga_posmap_weights: map size %d outside [1, %d]", S, kMaxS);
-    GA_REQUIRE(J == kJoints || J == kJointsX, "ga_posmap_weights: joint count %d is neither %d (SMPL) nor %d (SMPL-X)", J, kJoints, kJointsX);
+    GA_REQUIRE(J == kSmplJoints || J == kSmplxJoints, "ga_posmap_weights: joint count %d is neither %d (SMPL) nor %d (SMPL-X)", J, kSmplJoints, kSmplxJoints);
     GA_REQUIRE(weights && faces && face_id && bary && out, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const int n = S * S * J;
@@ -905,14 +692,14 @@ extern "C" int ga_posmap_fill(int32_t B, int32_t S, int32_t V, const float *vert
     return GA_OK;
 }
 
-extern "C" size_t ga_smpl_vertices_backward_workspace_bytes(int32_t B, int32_t V) { return vertices_bwd_workspace<kJoints>(B, V); }
-extern "C" size_t ga_smplx_vertices_backward_workspace_bytes(int32_t B, int32_t V) { return vertices_bwd_workspace<kJointsX>(B, V); }
+extern "C" size_t ga_smpl_vertices_backward_workspace_bytes(int32_t B, int32_t V) { return vertices_bwd_workspace<kSmplJoints>(B, V); }
+extern "C" size_t ga_smplx_vertices_backward_workspace_bytes(int32_t B, int32_t V) { return vertices_bwd_workspace<kSmplxJoints>(B, V); }
 
 extern "C" int ga_smpl_vertices_backward(int32_t B, int32_t V, const float *pose, const float *rest_joints, const float *v_shaped,
                                          const float *posedirs, const float *weights, const float *d_verts, void *workspace,
                                          size_t workspace_bytes, float *d_pose, float *d_transl, void *stream_)
 {
-    return vertices_backward<kJoints>("ga_smpl_vertices_backward", B, V, pose, nullptr, rest_joints, v_shaped, posedirs, weights, d_verts,
+    return vertices_backward<kSmplJoints>("ga_smpl_vertices_backward", B, V, pose, nullptr, rest_joints, v_shaped, posedirs, weights, d_verts,
                                       workspace, workspace_bytes, d_pose, d_transl, static_cast<cudaStream_t>(stream_));
 }
 
@@ -920,7 +707,7 @@ extern "C" int ga_smplx_vertices_backward(int32_t B, int32_t V, const float *pos
                                           const float *v_shaped, const float *posedirs, const float *weights, const float *d_verts,
                                           void *workspace, size_t workspace_bytes, float *d_pose, float *d_transl, void *stream_)
 {
-    return vertices_backward<kJointsX>("ga_smplx_vertices_backward", B, V, pose, rest_pose, rest_joints, v_shaped, posedirs, weights,
+    return vertices_backward<kSmplxJoints>("ga_smplx_vertices_backward", B, V, pose, rest_pose, rest_joints, v_shaped, posedirs, weights,
                                        d_verts, workspace, workspace_bytes, d_pose, d_transl, static_cast<cudaStream_t>(stream_));
 }
 

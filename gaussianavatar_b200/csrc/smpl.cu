@@ -17,18 +17,8 @@
 namespace ga {
 namespace {
 
-__constant__ int c_parents[24] = {-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21};
-// SMPL-X kintree_table[0] (the asset loader checks the model file against this table)
-__constant__ int c_parents_x[55] = {-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 15, 15, 15, 20, 25,
-                                    26, 20, 28, 29, 20, 31, 32, 20, 34, 35, 20, 37, 38, 21, 40, 41, 21, 43, 44, 21, 46, 47, 21, 49, 50,
-                                    21, 52, 53};
-
-// kJ joints, the first kTrain of them from `pose` [B, 3 kTrain], the rest from `rest` [B, 3 (kJ - kTrain)]; kThreads per CTA
-template <int kJ> struct Body;
-template <> struct Body<24> { static constexpr int kTrain = 24, kThreads = 32; };
-template <> struct Body<55> { static constexpr int kTrain = 22, kThreads = 64; };
-
-template <int kJ> __device__ __forceinline__ int parent_of(int j) { return kJ == 24 ? c_parents[j] : c_parents_x[j]; }
+// threads per CTA: one warp for SMPL; SMPL-X's 55 joints need two
+template <int kJ> constexpr int kCtaThreads = (kJ == kSmplJoints) ? 32 : 64;
 
 template <int kThreads> __device__ __forceinline__ void cta_sync()
 {
@@ -36,42 +26,24 @@ template <int kThreads> __device__ __forceinline__ void cta_sync()
     else __syncthreads();
 }
 
-// axis-angle of joint j of pose b
-template <int kJ> __device__ __forceinline__ void load_axis_angle(const float *__restrict__ pose, const float *__restrict__ rest, int b, int j, float r[3])
-{
-    constexpr int kT = Body<kJ>::kTrain;
-    if (kT == kJ || j < kT) {
-        r[0] = pose[(size_t)b * (kT * 3) + j * 3]; r[1] = pose[(size_t)b * (kT * 3) + j * 3 + 1]; r[2] = pose[(size_t)b * (kT * 3) + j * 3 + 2];
-    } else {
-        const int k = j - kT;
-        r[0] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3]; r[1] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3 + 1];
-        r[2] = rest[(size_t)b * ((kJ - kT) * 3) + k * 3 + 2];
-    }
-}
-
 // One block (kThreads) per pose.  Thread j < kJ owns joint j for the per-joint steps; the chain itself is walked
 // in index order through shared memory (children always have a larger index than their parent).
 template <int kJ>
-__global__ void __launch_bounds__(Body<kJ>::kThreads)
+__global__ void __launch_bounds__(kCtaThreads<kJ>)
 smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__ transl, const float *__restrict__ J,
                 const float *__restrict__ inv_cano /*[kJ,4,4]*/, float *__restrict__ C /*[B,kJ,12]*/,
                 float *__restrict__ G_out /*[B,kJ,12] saved for backward*/, const float *__restrict__ rest /*[B,99] (SMPL-X)*/)
 {
-    constexpr int kThreads = Body<kJ>::kThreads;
+    constexpr int kThreads = kCtaThreads<kJ>;
     __shared__ float sL[kJ][12], sG[kJ][12];
     const int b = blockIdx.x, j = threadIdx.x;
     if (b >= B) return;
     if (j < kJ) {
         float r[3];
-        load_axis_angle<kJ>(pose, rest, b, j, r);
+        joint_axis_angle<kJ>(pose, rest, b, j, r);
         float R[9], th;
         rodrigues(r, R, &th);
-        const int p = parent_of<kJ>(j);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            sL[j][k * 4 + 0] = R[k * 3 + 0]; sL[j][k * 4 + 1] = R[k * 3 + 1]; sL[j][k * 4 + 2] = R[k * 3 + 2];
-            sL[j][k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
-        }
+        local_transform<kJ>(R, J, j, sL[j]);
         if (j == 0) {
 #pragma unroll
             for (int k = 0; k < 12; ++k) sG[0][k] = sL[0][k];
@@ -80,17 +52,14 @@ smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
     cta_sync<kThreads>();
     // kJ - 1 dependent 3x4 products: thread 0 walks the chain (latency ~ a few microseconds, B poses run in parallel CTAs)
     for (int i = 1; i < kJ; ++i) {
-        if (j == 0) aff_mul(sG[parent_of<kJ>(i)], sL[i], sG[i]);
+        if (j == 0) aff_mul(sG[Body<kJ>::parent(i)], sL[i], sG[i]);
         cta_sync<kThreads>();
     }
     if (j < kJ) {
         float A[12];
+        rest_relative(sG[j], J, j, A);
 #pragma unroll
-        for (int r = 0; r < 3; ++r) {
-            A[r * 4 + 0] = sG[j][r * 4 + 0]; A[r * 4 + 1] = sG[j][r * 4 + 1]; A[r * 4 + 2] = sG[j][r * 4 + 2];
-            A[r * 4 + 3] = sG[j][r * 4 + 3] - (sG[j][r * 4 + 0] * J[j * 3] + sG[j][r * 4 + 1] * J[j * 3 + 1] + sG[j][r * 4 + 2] * J[j * 3 + 2]) +
-                           transl[(size_t)b * 3 + r];
-        }
+        for (int r = 0; r < 3; ++r) A[r * 4 + 3] += transl[(size_t)b * 3 + r];
         // cano2live = A * inv(A_cano)  (both affine)
         const float *Ic = inv_cano + j * 16;
         float *Cj = C + ((size_t)b * kJ + j) * 12;
@@ -109,25 +78,20 @@ smpl_fwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
 
 // d_pose [B, 3 kTrain] only: the rest_pose joints of SMPL-X are data.
 template <int kJ>
-__global__ void __launch_bounds__(Body<kJ>::kThreads)
+__global__ void __launch_bounds__(kCtaThreads<kJ>)
 smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__ J, const float *__restrict__ inv_cano,
                 const float *__restrict__ G_saved, const float *__restrict__ dC /*[B,kJ,12]*/,
-                float *__restrict__ d_pose /*[B,3 kTrain]*/, float *__restrict__ d_transl /*[B,3]*/, const float *__restrict__ rest)
+                float *__restrict__ d_pose /*[B,3 kTrained]*/, float *__restrict__ d_transl /*[B,3]*/, const float *__restrict__ rest)
 {
-    constexpr int kThreads = Body<kJ>::kThreads, kT = Body<kJ>::kTrain;
+    constexpr int kThreads = kCtaThreads<kJ>, kT = Body<kJ>::kTrained;
     __shared__ float sL[kJ][12], sG[kJ][12], sdG[kJ][12], sdL[kJ][9];
     const int b = blockIdx.x, j = threadIdx.x;
     if (b >= B) return;
     float r[3] = {0.f, 0.f, 0.f}, R[9], theta = 1.f;
     if (j < kJ) {
-        load_axis_angle<kJ>(pose, rest, b, j, r);
+        joint_axis_angle<kJ>(pose, rest, b, j, r);
         rodrigues(r, R, &theta);
-        const int p = parent_of<kJ>(j);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            sL[j][k * 4 + 0] = R[k * 3 + 0]; sL[j][k * 4 + 1] = R[k * 3 + 1]; sL[j][k * 4 + 2] = R[k * 3 + 2];
-            sL[j][k * 4 + 3] = (p < 0) ? J[j * 3 + k] : (J[j * 3 + k] - J[p * 3 + k]);
-        }
+        local_transform<kJ>(R, J, j, sL[j]);
         const float *Gj = G_saved + ((size_t)b * kJ + j) * 12;
 #pragma unroll
         for (int k = 0; k < 12; ++k) sG[j][k] = Gj[k];
@@ -160,7 +124,7 @@ smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
     // reverse chain: G_i = G_p * L_i
     if (j == 0) {
         for (int i = kJ - 1; i >= 1; --i) {
-            const int p = parent_of<kJ>(i);
+            const int p = Body<kJ>::parent(i);
             const float *Gp = sG[p], *Li = sL[i], *dGi = sdG[i];
             // dL_R = Gp_R^T dGi_R ; (dL_t not needed: J is constant)
 #pragma unroll
@@ -184,7 +148,8 @@ smpl_bwd_kernel(int B, const float *__restrict__ pose, const float *__restrict__
     }
     cta_sync<kThreads>();
     if (j < kT) {
-        // Rodrigues backward.  R = I + s K + (1-c) K^2, K = skew(d), d = r/theta, theta = |r + 1e-8|
+        // Rodrigues backward.  R = I + s K + (1-c) K^2, K = skew(d), d = r/theta, theta = |r + 1e-8|.  Not rodrigues_bwd: the two
+        // differ in the last bits (DESIGN.md §7).
         const float *dR = sdL[j];
         const float dx = r[0] / theta, dy = r[1] / theta, dz = r[2] / theta;
         float s, c;
@@ -232,7 +197,7 @@ extern "C" int ga_smpl_forward(int32_t B, const float *pose, const float *transl
     GA_REQUIRE(B >= 0, "bad batch %d", B);
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && transl && rest_joints && inv_cano && cano2live && saved_G, "NULL pointer argument");
-    { ProfScope _ps("smpl_fwd_kernel", static_cast<cudaStream_t>(stream_)); smpl_fwd_kernel<24><<<B, 32, 0, static_cast<cudaStream_t>(stream_)>>>(B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, nullptr); }
+    { ProfScope _ps("smpl_fwd_kernel", static_cast<cudaStream_t>(stream_)); smpl_fwd_kernel<kSmplJoints><<<B, kCtaThreads<kSmplJoints>, 0, static_cast<cudaStream_t>(stream_)>>>(B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, nullptr); }
     GA_CHECK_LAUNCH("smpl_fwd_kernel");
     return GA_OK;
 }
@@ -243,7 +208,7 @@ extern "C" int ga_smpl_backward(int32_t B, const float *pose, const float *rest_
     GA_REQUIRE(B >= 0, "bad batch %d", B);
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && rest_joints && inv_cano && saved_G && d_cano2live && d_pose && d_transl, "NULL pointer argument");
-    { ProfScope _ps("smpl_bwd_kernel", static_cast<cudaStream_t>(stream_)); smpl_bwd_kernel<24><<<B, 32, 0, static_cast<cudaStream_t>(stream_)>>>(B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, nullptr); }
+    { ProfScope _ps("smpl_bwd_kernel", static_cast<cudaStream_t>(stream_)); smpl_bwd_kernel<kSmplJoints><<<B, kCtaThreads<kSmplJoints>, 0, static_cast<cudaStream_t>(stream_)>>>(B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, nullptr); }
     GA_CHECK_LAUNCH("smpl_bwd_kernel");
     return GA_OK;
 }
@@ -255,7 +220,7 @@ extern "C" int ga_smplx_forward(int32_t B, const float *pose, const float *rest_
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && rest_pose && transl && rest_joints && inv_cano && cano2live && saved_G, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    { ProfScope _ps("smplx_fwd_kernel", stream); smpl_fwd_kernel<55><<<B, Body<55>::kThreads, 0, stream>>>(B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, rest_pose); }
+    { ProfScope _ps("smplx_fwd_kernel", stream); smpl_fwd_kernel<kSmplxJoints><<<B, kCtaThreads<kSmplxJoints>, 0, stream>>>(B, pose, transl, rest_joints, inv_cano, cano2live, saved_G, rest_pose); }
     GA_CHECK_LAUNCH("smplx_fwd_kernel");
     return GA_OK;
 }
@@ -267,7 +232,7 @@ extern "C" int ga_smplx_backward(int32_t B, const float *pose, const float *rest
     if (B == 0) return GA_OK;
     GA_REQUIRE(pose && rest_pose && rest_joints && inv_cano && saved_G && d_cano2live && d_pose && d_transl, "NULL pointer argument");
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    { ProfScope _ps("smplx_bwd_kernel", stream); smpl_bwd_kernel<55><<<B, Body<55>::kThreads, 0, stream>>>(B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, rest_pose); }
+    { ProfScope _ps("smplx_bwd_kernel", stream); smpl_bwd_kernel<kSmplxJoints><<<B, kCtaThreads<kSmplxJoints>, 0, stream>>>(B, pose, rest_joints, inv_cano, saved_G, d_cano2live, d_pose, d_transl, rest_pose); }
     GA_CHECK_LAUNCH("smplx_bwd_kernel");
     return GA_OK;
 }

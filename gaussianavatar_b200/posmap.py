@@ -26,7 +26,7 @@ from . import _lib
 from ._lib import ptr
 
 SMPL_MESH_FIELDS = ("v_template", "shapedirs", "posedirs", "weights", "f", "J_regressor")
-MAX_FRAMES_PER_CALL = 8          # ga_smpl_vertices
+MAX_FRAMES_PER_CALL = 8          # ga_smpl_vertices / ga_smplx_vertices and their backward
 
 
 def load_uv_template_obj(path):
@@ -80,6 +80,9 @@ class BodyPoser:
     stream under no_grad."""
 
     BODY, JOINTS, POSE_FEATURES, POSE_WIDTH = "SMPL", 24, 207, 72
+    # the C entry points of vertex posing, its backward and the backward's workspace size
+    _VERTICES, _VERTICES_BWD, _VERTICES_BWD_WS = ("ga_smpl_vertices", "ga_smpl_vertices_backward",
+                                                  "ga_smpl_vertices_backward_workspace_bytes")
 
     def __init__(self, smpl, betas, device="cuda"):
         missing = [k for k in SMPL_MESH_FIELDS if k not in smpl]
@@ -126,18 +129,27 @@ class BodyPoser:
             raise ValueError(f"pose {tuple(pose.shape)} and transl {tuple(transl.shape)} have different frame counts")
         return pose, transl
 
+    @staticmethod
+    def _poses(pose, rest_pose):
+        """The pose arguments the entry points take: pose (SMPL has no rest_pose)."""
+        return (pose,)
+
+    def _vertices(self, poses, transl) -> torch.Tensor:
+        """Posed vertices [B,V,3] of checked poses, (pose,) or (pose, rest_pose), and transl: MAX_FRAMES_PER_CALL frames per call."""
+        B = transl.shape[0]
+        out = torch.empty(B, self.V, 3, dtype=torch.float32, device=self.device)
+        fn = getattr(_lib.lib(), self._VERTICES)
+        for s in range(0, B, MAX_FRAMES_PER_CALL):
+            e = min(B, s + MAX_FRAMES_PER_CALL)
+            _lib.check(fn(e - s, self.V, *(ptr(p[s:e]) for p in poses), ptr(transl[s:e]), ptr(self.rest_joints), ptr(self.v_shaped),
+                          ptr(self.posedirs), ptr(self.weights), ptr(out[s:e]), self._stream()), self._VERTICES)
+        return out
+
     @torch.no_grad()
     def vertices(self, pose, transl) -> torch.Tensor:
         """Posed SMPL vertices [B,V,3] for pose [B,72] and transl [B,3] (the reference's `SMPL.forward(...).vertices`)."""
         pose, transl = self._inputs(pose, transl)
-        B = pose.shape[0]
-        out = torch.empty(B, self.V, 3, dtype=torch.float32, device=self.device)
-        L = _lib.lib()
-        for s in range(0, B, MAX_FRAMES_PER_CALL):
-            e = min(B, s + MAX_FRAMES_PER_CALL)
-            _lib.check(L.ga_smpl_vertices(e - s, self.V, ptr(pose[s:e]), ptr(transl[s:e]), ptr(self.rest_joints), ptr(self.v_shaped),
-                                          ptr(self.posedirs), ptr(self.weights), ptr(out[s:e]), self._stream()), "ga_smpl_vertices")
-        return out
+        return self._vertices((pose,), transl)
 
 
 class SmplxBodyPoser(BodyPoser):
@@ -147,6 +159,8 @@ class SmplxBodyPoser(BodyPoser):
     split: pose [B,66] (global + 21 body joints) and rest_pose [B,99] (jaw, left / right eye, 15 + 15 finger joints)."""
 
     BODY, JOINTS, POSE_FEATURES, POSE_WIDTH = "SMPL-X", 55, 486, 66
+    _VERTICES, _VERTICES_BWD, _VERTICES_BWD_WS = ("ga_smplx_vertices", "ga_smplx_vertices_backward",
+                                                  "ga_smplx_vertices_backward_workspace_bytes")
 
     def _check_model(self, smplx):
         from .synthetic import SMPLX_PARENTS
@@ -156,6 +170,10 @@ class SmplxBodyPoser(BodyPoser):
         kt[0] = -1
         if kt.shape != (len(SMPLX_PARENTS),) or not np.array_equal(kt, np.asarray(SMPLX_PARENTS)):
             raise ValueError("SMPL-X model: kintree_table[0] is not the 55-joint SMPL-X tree this library is built for")
+
+    @staticmethod
+    def _poses(pose, rest_pose):
+        return (pose, rest_pose)
 
     def _inputs(self, pose, rest_pose, transl):
         pose, transl = super()._inputs(pose, transl)
@@ -168,15 +186,7 @@ class SmplxBodyPoser(BodyPoser):
     def vertices(self, pose, rest_pose, transl) -> torch.Tensor:
         """Posed SMPL-X vertices [B,V,3] for pose [B,66], rest_pose [B,99] and transl [B,3] (`SMPLX.forward(...).vertices`)."""
         pose, rest_pose, transl = self._inputs(pose, rest_pose, transl)
-        B = pose.shape[0]
-        out = torch.empty(B, self.V, 3, dtype=torch.float32, device=self.device)
-        L = _lib.lib()
-        for s in range(0, B, MAX_FRAMES_PER_CALL):
-            e = min(B, s + MAX_FRAMES_PER_CALL)
-            _lib.check(L.ga_smplx_vertices(e - s, self.V, ptr(pose[s:e]), ptr(rest_pose[s:e]), ptr(transl[s:e]), ptr(self.rest_joints),
-                                           ptr(self.v_shaped), ptr(self.posedirs), ptr(self.weights), ptr(out[s:e]), self._stream()),
-                       "ga_smplx_vertices")
-        return out
+        return self._vertices((pose, rest_pose), transl)
 
 
 class PoseMapper(BodyPoser):
@@ -277,22 +287,18 @@ def _wants_grad(*ts) -> bool:
 def vertices_backward(poser, pose, rest_pose, d_verts):
     """(d_pose [B,72|66], d_transl [B,3]) of vertex gradients d_verts [B,V,3] at pose (and SMPL-X rest_pose), through
     `ga_smpl_vertices_backward` / `ga_smplx_vertices_backward`."""
-    smplx = isinstance(poser, SmplxBodyPoser)
     d_verts = d_verts.to(device=poser.device, dtype=torch.float32).contiguous()
     B = pose.shape[0]
     d_pose = torch.empty(B, poser.POSE_WIDTH, dtype=torch.float32, device=poser.device)
     d_transl = torch.empty(B, 3, dtype=torch.float32, device=poser.device)
     L = _lib.lib()
-    ws_fn = L.ga_smplx_vertices_backward_workspace_bytes if smplx else L.ga_smpl_vertices_backward_workspace_bytes
-    ws = torch.empty(ws_fn(min(B, MAX_FRAMES_PER_CALL), poser.V), dtype=torch.uint8, device=poser.device)
+    ws = torch.empty(getattr(L, poser._VERTICES_BWD_WS)(min(B, MAX_FRAMES_PER_CALL), poser.V), dtype=torch.uint8, device=poser.device)
+    fn, poses = getattr(L, poser._VERTICES_BWD), poser._poses(pose, rest_pose)
     for s in range(0, B, MAX_FRAMES_PER_CALL):
         e = min(B, s + MAX_FRAMES_PER_CALL)
-        common = (ptr(poser.rest_joints), ptr(poser.v_shaped), ptr(poser.posedirs), ptr(poser.weights), ptr(d_verts[s:e]), ptr(ws), ws.numel(),
-                  ptr(d_pose[s:e]), ptr(d_transl[s:e]), poser._stream())
-        if smplx:
-            _lib.check(L.ga_smplx_vertices_backward(e - s, poser.V, ptr(pose[s:e]), ptr(rest_pose[s:e]), *common), "ga_smplx_vertices_backward")
-        else:
-            _lib.check(L.ga_smpl_vertices_backward(e - s, poser.V, ptr(pose[s:e]), *common), "ga_smpl_vertices_backward")
+        _lib.check(fn(e - s, poser.V, *(ptr(p[s:e]) for p in poses), ptr(poser.rest_joints), ptr(poser.v_shaped), ptr(poser.posedirs),
+                      ptr(poser.weights), ptr(d_verts[s:e]), ptr(ws), ws.numel(), ptr(d_pose[s:e]), ptr(d_transl[s:e]), poser._stream()),
+                   poser._VERTICES_BWD)
     return d_pose, d_transl
 
 
