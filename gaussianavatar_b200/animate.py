@@ -18,7 +18,6 @@ and BatchNorm statistics are left exactly as they were.
 """
 from __future__ import annotations
 
-import contextlib
 import math
 import os
 from dataclasses import dataclass
@@ -28,10 +27,11 @@ import torch
 
 from . import _lib
 from ._lib import ptr
+from .avatar_model import kept_state
 from .camera import Camera, make_camera
 from .dataset import _rodrigues, rotate_camera_by_frame_idx
+from .rasterizer import MAX_FRAMES_PER_CALL, RasterBatchPlan, rasterize_batch
 
-MAX_CHUNK = 8          # ga_frame_pack / the batched rasterizer per call
 POSE_WIDTH = {"smpl": 72, "smplx": 165}
 IDENTITY_ALIGN = np.array([1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0], np.float64)
 
@@ -181,26 +181,6 @@ class Schedule:
     cams: torch.Tensor       # [n,40] camera block (host fp32)
 
 
-@contextlib.contextmanager
-def kept_state(model):
-    """Restores the model's BatchNorm statistics (running buffers and batch counts) on exit: animating must not change what
-    `save()` writes."""
-    net = model.net
-    run = net.bn_running.detach().clone()
-    counts = {k: st.num_batches_tracked for k, st in net._states.items()}
-    enc = getattr(model, "pose_encoder", None)
-    bufs = [(b, b.detach().clone()) for b in enc.buffers()] if enc is not None else []
-    try:
-        yield
-    finally:
-        with torch.no_grad():
-            net.bn_running.copy_(run)
-            for k, st in net._states.items():
-                st.num_batches_tracked = counts.get(k, 0)
-            for b, v in bufs:
-                b.copy_(v)
-
-
 # ---- the player -------------------------------------------------------------------------------------------------------------------
 class Animator:
     """Renders an inference `AvatarModel` (stage 1 or 2) along motion clips.
@@ -210,14 +190,14 @@ class Animator:
     `SmplxPoseMapper` (default: the model's own).  capacity: initial binning capacity of the rasterizer (instances); it grows on
     overflow.  graphs: replay CUDA graphs in stage 1 (False runs the same launches eagerly, e.g. for per-kernel profiling)."""
 
-    def __init__(self, model, cameras, H: int, W: int, chunk: int = 8, channels: int = 3, pose_mapper=None, capacity=None,
-                 graphs: bool = True):
+    def __init__(self, model, cameras, H: int, W: int, chunk: int = MAX_FRAMES_PER_CALL, channels: int = 3, pose_mapper=None,
+                 capacity=None, graphs: bool = True):
         self.model = model
         self.H, self.W = int(H), int(W)
         if not (1 <= self.H <= 16384 and 1 <= self.W <= 16384):
             raise ValueError(f"frame {self.H} x {self.W} outside [1, 16384]^2")
-        if not 1 <= int(chunk) <= MAX_CHUNK:
-            raise ValueError(f"chunk {chunk} outside 1..{MAX_CHUNK}")
+        if not 1 <= int(chunk) <= MAX_FRAMES_PER_CALL:
+            raise ValueError(f"chunk {chunk} outside 1..{MAX_FRAMES_PER_CALL}")
         if int(channels) not in (3, 4):
             raise ValueError(f"channels {channels}: 3 (RGB) or 4 (RGBA)")
         self.chunk, self.channels = int(chunk), int(channels)
@@ -241,14 +221,14 @@ class Animator:
         self.overflows = 0         # chunks rendered again after an overflow
         self._plans, self._graphs, self._clip_key = {}, {}, None
         C, dev = self.channels, self.dev
-        self._out_dev = [torch.empty(MAX_CHUNK, self.H, self.W, C, dtype=torch.uint8, device=dev) for _ in range(2)]
-        self._out_host = [torch.empty(MAX_CHUNK, self.H, self.W, C, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self._out_dev = [torch.empty(MAX_FRAMES_PER_CALL, self.H, self.W, C, dtype=torch.uint8, device=dev) for _ in range(2)]
+        self._out_host = [torch.empty(MAX_FRAMES_PER_CALL, self.H, self.W, C, dtype=torch.uint8).pin_memory() for _ in range(2)]
         self._status_dev = [torch.zeros(16, dtype=torch.int32, device=dev) for _ in range(2)]      # stage 2 leaves them at 0
         self._status_host = [torch.zeros(16, dtype=torch.int32).pin_memory() for _ in range(2)]
         self._keys_pose = self._keys_trans = self._dec = None
         self._align = torch.zeros(12, dtype=torch.float64, device=dev)
-        self._times_dev = torch.zeros(MAX_CHUNK, dtype=torch.float64, device=dev)
-        self._cams_dev = torch.zeros(MAX_CHUNK, 40, dtype=torch.float32, device=dev)
+        self._times_dev = torch.zeros(MAX_FRAMES_PER_CALL, dtype=torch.float64, device=dev)
+        self._cams_dev = torch.zeros(MAX_FRAMES_PER_CALL, 40, dtype=torch.float32, device=dev)
         self._copy_stream = torch.cuda.Stream(device=dev)
         self._rendered = [torch.cuda.Event() for _ in range(2)]
         self._copied = [torch.cuda.Event() for _ in range(2)]
@@ -340,18 +320,12 @@ class Animator:
             self._status_host[slot].copy_(self._status_dev[slot], non_blocking=True)
             self._copied[slot].record(self._copy_stream)
 
-    # ---- stage 1: one graph per (chunk size, slot) -------------------------------------------------------------------------------
-    def _decoder(self):
-        m = self.model
-        if m.cache_decoder and m._dec_cache is not None:
-            return m._dec_cache
-        dec = m.net.forward_packed(m.geo_feature, int(m.model_parms.query_posmap_size), 1)
-        if m.cache_decoder:
-            m._dec_cache = dec.detach()
-        return dec.detach()
+    def _split(self, pose):
+        """Sampled poses [n,72|165] -> (the pose columns the avatar was trained on, SMPL-X's rest_pose [n,99] or None)."""
+        return (pose[:, :66], pose[:, 66:]) if self.body == "smplx" else (pose, None)
 
+    # ---- stage 1: one graph per (chunk size, slot) -------------------------------------------------------------------------------
     def _plan(self, b):
-        from .rasterizer import RasterBatchPlan
         if b not in self._plans:
             self._plans[b] = RasterBatchPlan(b, int(self.model._query_points.shape[0]), self.H, self.W, self.dev, capacity=self.capacity)
         return self._plans[b]
@@ -365,11 +339,9 @@ class Animator:
             self.recaptures += 1
 
     def _stage1_setup(self, clip, sched):
-        from .ops import LbsAssemble
-        from .rasterizer import rasterize_batch
         m = self.model
         T, width = clip.num_keys, int(clip.pose.shape[1])
-        dec = self._decoder()
+        dec = m._stage1_decoder(1)
         if self._keys_pose is None or self._keys_pose.shape[0] < T:
             self._keys_pose = torch.empty(T, width, dtype=torch.float32, device=self.dev)
             self._keys_trans = torch.empty(T, 3, dtype=torch.float32, device=self.dev)
@@ -388,11 +360,8 @@ class Animator:
         def body(b, slot):
             plan = self._plan(b)
             pose, trans = motion_sample(self._keys_pose[:T], self._keys_trans[:T], self._times_dev[:b], self._align)
-            if m.smplx:
-                c2l = m._cano2live(pose[:, :66], trans, pose[:, 66:])
-            else:
-                c2l = m._cano2live(pose, trans)
-            means, scales, colors = LbsAssemble.apply(self._dec, c2l, m.valid_index, m._query_points, m._query_lbs, 1.0)
+            pose, rest = self._split(pose)
+            means, scales, colors = m._assemble(self._dec, pose, trans, rest)
             img = rasterize_batch(means, colors, scales, m.fix_rotation, m.fix_opacity, self._cams_dev[:b], m.background, plan)
             frame_pack(img, final_transmittance(plan), m.background, self.channels, self._out_dev[slot][:b])
             self._status_dev[slot].copy_(plan.status_dev)
@@ -423,15 +392,9 @@ class Animator:
 
         def render(s, e, slot):
             for i in range(s, e):
-                p, t = pose[i:i + 1], trans[i:i + 1]
+                p, rest = self._split(pose[i:i + 1])
+                means, scales, colors, _, _ = m._stage2_from_pose(self.pose_mapper, p, trans[i:i + 1], rest)
                 batch = {"_cams": cams_all[i:i + 1], "height": [self.H], "width": [self.W]}
-                if m.smplx:
-                    batch["rest_pose"] = p[:, 66:]
-                    batch["inp_pos_map"] = self.pose_mapper(p[:, :66], p[:, 66:], t)
-                    p = p[:, :66]
-                else:
-                    batch["inp_pos_map"] = self.pose_mapper(p, t)
-                means, scales, colors, _, _ = m._stage2_gaussians(batch, pose=p, transl=t)
                 img = m._render_frames(batch, means, scales, colors)
                 frame_pack(img, final_transmittance(m._last_plan), m.background, self.channels, self._out_dev[slot][i - s:i - s + 1])
         return render

@@ -15,6 +15,7 @@ Two ways to construct:
 """
 from __future__ import annotations
 
+import contextlib
 import os
 from os.path import join
 
@@ -25,6 +26,7 @@ import torch.nn as nn
 from .config import ModelParams, NetworkParams, OptimizationParams
 from .network import POP_no_unet
 from .ops import LbsAssemble, SmplCano2Live, SmplxCano2Live
+from .rasterizer import MAX_FRAMES_PER_CALL
 from .renderer import render_batch
 
 
@@ -342,6 +344,23 @@ class AvatarModel:
         rest_pose = rest_pose.to(device=self.device, dtype=torch.float32)
         return SmplxCano2Live.apply(pose_batch, rest_pose, transl_batch, self._rest_joints, self._inv_cano)
 
+    def _assemble(self, dec, pose, transl, rest_pose=None, scale_mul=1.0, per_frame=False):
+        """Decoder output `dec` posed by pose / transl (and SMPL-X's rest_pose): cano2live, then the fused LBS / attribute assembly.
+        Returns means3D, scales, colors [B,N,3].  per_frame: `dec` holds one [S*S,8] block per frame (stage 2)."""
+        cano2live = self._cano2live(pose, transl, rest_pose)                                              # [B,J,12]
+        return LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, scale_mul, per_frame)
+
+    def _stage1_decoder(self, batch):
+        """Stage 1's frame-invariant decoder output [S*S,8], its BatchNorm statistics taken over `batch` frames.  With `cache_decoder`
+        set and grad off it is evaluated once and reused until parameters are loaded again."""
+        cache = self.cache_decoder and not torch.is_grad_enabled()
+        if cache and self._dec_cache is not None:
+            return self._dec_cache
+        dec = self.net.forward_packed(self.geo_feature, int(self.model_parms.query_posmap_size), batch)
+        if cache:
+            self._dec_cache = dec.detach()
+        return dec
+
     def _posed_gaussians(self, idx, iteration, ramp=True, rest_pose=None):
         """SMPL / SMPL-X -> cano2live -> net (once) -> fused LBS/assembly.  Returns means3D, scales, colors [B,N,3] and dec_out."""
         if getattr(self, "_detach_pose", False):      # pose optimisation inactive (epoch <= pose_op_start_iter): its gradients are never read
@@ -349,12 +368,10 @@ class AvatarModel:
         else:
             pose_batch = self.pose(idx)
             transl_batch = self.transl(idx)
-        B = pose_batch.shape[0]
-        cano2live = self._cano2live(pose_batch, transl_batch, rest_pose)                                  # [B,J,12]
         S = int(self.model_parms.query_posmap_size)
-        dec = self.net.forward_packed(self.geo_feature, S, B)                                             # [S*S, 8]
+        dec = self.net.forward_packed(self.geo_feature, S, pose_batch.shape[0])                           # [S*S, 8]
         scale_mul = 1e-3 * iteration if (ramp and iteration < 1000) else 1.0                              # avatar_model.py:316-319
-        means, scales, colors = LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, scale_mul)
+        means, scales, colors = self._assemble(dec, pose_batch, transl_batch, rest_pose, scale_mul)
         return means, scales, colors, dec
 
     def _render_one(self, batch_data, means, scales, colors, b):
@@ -430,7 +447,7 @@ class AvatarModel:
         return len(set(h)) == 1 and len(set(w)) == 1
 
     def _render_frames(self, batch_data, means, scales, colors):
-        if means.is_cuda and means.shape[0] <= 8 and self._uniform_frames(batch_data, means.shape[0]):
+        if means.is_cuda and means.shape[0] <= MAX_FRAMES_PER_CALL and self._uniform_frames(batch_data, means.shape[0]):
             return self._render_batched(batch_data, means, scales, colors)
         return self._render_frames_one_by_one(batch_data, means, scales, colors)
 
@@ -484,12 +501,17 @@ class AvatarModel:
         if pose is None:
             idx = batch_data["pose_idx"]
             pose, transl = self.pose(idx), self.transl(idx)
-        cano2live = self._cano2live(pose, transl, batch_data.get("rest_pose"))
         S = int(self.model_parms.query_posmap_size)
         pose_featmap = self.pose_encoder(inp)                                                         # [B,64,h,h]
         dec = self.net.forward_packed_frames(self.geo_feature, pose_featmap, S)                      # [B*S*S, 8]
-        means, scales, colors = LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, 1.0, True)
+        means, scales, colors = self._assemble(dec, pose, transl, batch_data.get("rest_pose"), per_frame=True)
         return means, scales, colors, dec, pose_featmap
+
+    def _stage2_from_pose(self, mapper, pose, transl, rest_pose=None):
+        """`_stage2_gaussians` of explicit poses [B,72|66] / transl [B,3] (and SMPL-X's rest_pose [B,99]): the input position maps are
+        built from the same pose by `mapper` (a posmap.PoseMapper / SmplxPoseMapper, differentiable in pose and transl)."""
+        inp = mapper(pose, rest_pose, transl) if self.smplx else mapper(pose, transl)
+        return self._stage2_gaussians({"inp_pos_map": inp, "rest_pose": rest_pose}, pose=pose, transl=transl)
 
     def _pose_map(self, batch_data):
         """Input position maps [B,3,s,s] of a batch that carries none: from its `pose_data` / `transl_data` when it has them (test,
@@ -521,23 +543,14 @@ class AvatarModel:
         render_novel_pose.py construct) evaluates the net ONCE and reuses the packed output until parameters are loaded again
         (`cache_decoder`).  Per frame that leaves SMPL -> LBS -> rasterizer.  Only the BatchNorm running statistics (never used for
         normalisation by the reference's scripts) stop being updated by the skipped evaluations."""
-        S = int(self.model_parms.query_posmap_size)
         if "pose_data" in batch_data:      # novel-pose datasets carry the pose instead of an embedding index
             pose_batch, transl_batch = batch_data["pose_data"].float(), batch_data["transl_data"].float()
         else:
             idx = batch_data["pose_idx"]
             pose_batch, transl_batch = self.pose(idx), self.transl(idx)
-        B = pose_batch.shape[0]
-        cano2live = self._cano2live(pose_batch, transl_batch, batch_data.get("rest_pose"))
-        cached = getattr(self, "_dec_cache", None)
-        if self.cache_decoder and not torch.is_grad_enabled() and cached is not None:
-            dec = cached
-        else:
-            dec = self.net.forward_packed(self.geo_feature, S, B)
-            if self.cache_decoder and not torch.is_grad_enabled():
-                self._dec_cache = dec.detach()
+        dec = self._stage1_decoder(pose_batch.shape[0])
         scale_mul = 1e-3 * iteration if iteration < 1000 else 1.0
-        means, scales, colors = LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, scale_mul)
+        means, scales, colors = self._assemble(dec, pose_batch, transl_batch, batch_data.get("rest_pose"), scale_mul)
         return self._render_frames(batch_data, means, scales, colors)
 
     def invalidate_decoder_cache(self):
@@ -547,6 +560,26 @@ class AvatarModel:
         """model/avatar_model.py:557-649: the stage-2 forward without the losses."""
         means, scales, colors, _, _ = self._stage2_gaussians(batch_data)
         return self._render_frames(batch_data, means, scales, colors)
+
+
+@contextlib.contextmanager
+def kept_state(model):
+    """Restores the model's BatchNorm statistics (running buffers and batch counts) on exit: rendering or fitting poses through a
+    trained avatar must not change what `save()` writes."""
+    net = model.net
+    run = net.bn_running.detach().clone()
+    counts = {k: st.num_batches_tracked for k, st in net._states.items()}
+    enc = getattr(model, "pose_encoder", None)
+    bufs = [(b, b.detach().clone()) for b in enc.buffers()] if enc is not None else []
+    try:
+        yield
+    finally:
+        with torch.no_grad():
+            net.bn_running.copy_(run)
+            for k, st in net._states.items():
+                st.num_batches_tracked = counts.get(k, 0)
+            for b, v in bufs:
+                b.copy_(v)
 
 
 def smplx_rest_joints(npz_path, beta, parents) -> torch.Tensor:

@@ -26,12 +26,10 @@ import torch
 
 from . import _lib
 from ._lib import ptr
-from .animate import kept_state
+from .avatar_model import kept_state
 from .losses import image_loss
-from .ops import LbsAssemble
-from .rasterizer import RasterBatchPlan, rasterize_batch
+from .rasterizer import MAX_FRAMES_PER_CALL, RasterBatchPlan, rasterize_batch
 
-MAX_CHUNK = 8          # frames per batched-rasterizer call
 BETAS = (0.9, 0.999)   # torch.optim.Adam's defaults, as the training pose optimiser uses them
 EPS = 1e-8
 
@@ -41,13 +39,13 @@ class PoseFitter:
     by default).  pose_mapper: stage 2's `posmap.PoseMapper` / `SmplxPoseMapper` (default: the model's own).  chunk: frames per
     stage-1 rasterizer call (1..8).  capacity: initial binning capacity of the rasterizer (instances); it grows on overflow."""
 
-    def __init__(self, model, iters: int = 100, lr: float = 5e-3, pose_mapper=None, chunk: int = MAX_CHUNK, capacity=None):
+    def __init__(self, model, iters: int = 100, lr: float = 5e-3, pose_mapper=None, chunk: int = MAX_FRAMES_PER_CALL, capacity=None):
         if int(iters) < 0:
             raise ValueError(f"iters {iters} is negative")
         if not (lr > 0 and math.isfinite(lr)):
             raise ValueError(f"lr {lr} is not a positive number")
-        if not 1 <= int(chunk) <= MAX_CHUNK:
-            raise ValueError(f"chunk {chunk} outside 1..{MAX_CHUNK}")
+        if not 1 <= int(chunk) <= MAX_FRAMES_PER_CALL:
+            raise ValueError(f"chunk {chunk} outside 1..{MAX_FRAMES_PER_CALL}")
         self.model = model
         self.iters, self.lr, self.chunk, self.capacity = int(iters), float(lr), int(chunk), capacity
         self.stage = 2 if int(model.model_parms.train_stage) == 2 else 1
@@ -79,7 +77,7 @@ class PoseFitter:
         with kept_state(m):
             if self.stage == 1:
                 with torch.no_grad():
-                    dec = _decoder(m)
+                    dec = m._stage1_decoder(1)
                 groups = self._chunks(frames)
             else:
                 dec = None
@@ -173,22 +171,19 @@ class PoseFitter:
         plan = self._plan(len(items), H, W)
 
         def objective(pose, transl):
-            c2l = m._cano2live(pose, transl, rest)
-            means, scales, colors = LbsAssemble.apply(dec, c2l, m.valid_index, m._query_points, m._query_lbs, 1.0)
+            means, scales, colors = m._assemble(dec, pose, transl, rest)
             img = rasterize_batch(means, colors, scales, m.fix_rotation, m.fix_opacity, cams, m.background, plan)
             return torch.stack([image_loss(img[i:i + 1], gt[i:i + 1], self.lam) for i in range(len(items))]), plan
         return objective
 
     def _stage2_objective(self, item):
-        m, mapper = self.model, self.pose_mapper
+        m = self.model
         cams, H, W = self._cameras([item])
         gt, rest = self._targets([item]), self._rest([item])
         plan = self._plan(1, H, W)
 
         def objective(pose, transl):
-            inp = mapper(pose, rest, transl) if m.smplx else mapper(pose, transl)
-            batch = {"inp_pos_map": inp, "rest_pose": rest, "_cams": cams, "height": [H], "width": [W]}
-            means, scales, colors, _, _ = m._stage2_gaussians(batch, pose=pose, transl=transl)
+            means, scales, colors, _, _ = m._stage2_from_pose(self.pose_mapper, pose, transl, rest)
             img = rasterize_batch(means, colors, scales, m.fix_rotation, m.fix_opacity, cams, m.background, plan)
             return image_loss(img, gt, self.lam).reshape(1), plan
         return objective
@@ -196,13 +191,3 @@ class PoseFitter:
 
 def _size(item):
     return int(item["height"]), int(item["width"])
-
-
-def _decoder(m):
-    """Stage 1's frame-invariant decoder output, evaluated once (kept in the model's cache when it has one)."""
-    if m.cache_decoder and m._dec_cache is not None:
-        return m._dec_cache
-    dec = m.net.forward_packed(m.geo_feature, int(m.model_parms.query_posmap_size), 1).detach()
-    if m.cache_decoder:
-        m._dec_cache = dec
-    return dec

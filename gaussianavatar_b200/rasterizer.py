@@ -232,6 +232,7 @@ def rasterize_backward(ctx: RasterContext, means3D, colors, scales, rotations, r
 # Batched path: all frames of a step in one set of launches, no host read-back (model/avatar_model.py:332-365 loops frames)
 # ----------------------------------------------------------------------------------------------------------------------
 CAM_STRIDE = 40
+MAX_FRAMES_PER_CALL = 8          # ga_rasterb_*
 
 
 def pack_cameras(view, proj, tanfovx, tanfovy, device):

@@ -282,7 +282,7 @@ def test_forced_overflow_gives_the_same_fit(stage):
 def test_stage2_map_gradient_is_live(body):
     """The pose gradient of the stage-2 loss with the map built from the pose differs from the one with the map held constant."""
     from gaussianavatar_b200.losses import image_loss
-    from gaussianavatar_b200.animate import kept_state
+    from gaussianavatar_b200.avatar_model import kept_state
     m, mapper, frames, _, _ = _problem(body, 2, n=1)
     it = frames[0]
     cams = m._batch_cameras({k: [it[k]] for k in ("FovX", "FovY", "world_view_transform", "full_proj_transform")}, 1, DEV)
