@@ -20,7 +20,8 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
                   const float *Yprev, int ldp, const float *pa, const float *pb, const float *pmu, const float *prstd, const float *W, int ldw,
                   float *dW, int lddw, float *dZprev, int ldo, int mode, double *s1, double *s2, int M, int kin, int x_raw, cudaStream_t st);
 int launch_tc_fwd(const float *X, int ldx, int K, const float *a, const float *b, const float *W, int ldw, const float *bias, float *Y,
-                  int ldy, int accumulate, double *sum, double *sumsq, int M, cudaStream_t st);
+                  int ldy, int accumulate, double *sum, double *sumsq, int M, cudaStream_t st, int heads = 1, size_t w_hstride = 0,
+                  size_t y_hstride = 0, int v_hstride = 0);
 int launch_conv_tc(int mode, const float *in, const float *w, float *out, int Hf, int round_out, cudaStream_t st);
 int launch_round_tf32(const float *in, float *out, size_t n, cudaStream_t st);
 namespace {
@@ -658,9 +659,9 @@ extern "C" int ga_decoder_forward(const GaDecoderDesc *d, const float *params, c
         if (int rc = launch_tc_fwd(w.Y[3], kH, kH, cf.a + kBnOff[3], cf.b + kBnOff[3], params + L.w[4] + kFeatLd, kK5, params + L.b[4], w.Y[4], kH, 1,
                                    sum + kBnOff[4], sumsq + kBnOff[4], M, st)) return rc;
         if (int rc = finalize(4, kH)) return rc;
-        for (int h = 0; h < 3; ++h)
-            if (int rc = launch_tc_fwd(w.Y[4], kH, kH, cf.a + kBnOff[4], cf.b + kBnOff[4], params + L.w[5] + (size_t)h * kH * kH, kH,
-                                       params + L.b[5] + h * kH, w.Y6 + h * kH, 3 * kH, 0, sum + kBnOff[5] + h * kH, sumsq + kBnOff[5] + h * kH, M, st)) return rc;
+        // layer 6: the three heads in one launch, whose CTAs of one tile run side by side and share the reads of layer 5's output in L2
+        if (int rc = launch_tc_fwd(w.Y[4], kH, kH, cf.a + kBnOff[4], cf.b + kBnOff[4], params + L.w[5], kH, params + L.b[5], w.Y6, 3 * kH, 0,
+                                   sum + kBnOff[5], sumsq + kBnOff[5], M, st, 3, (size_t)kH * kH, kH, kH)) return rc;
         if (int rc = finalize(5, 3 * kH)) return rc;
         for (int h = 0; h < 3; ++h)
             if (int rc = launch_tc_fwd(w.Y6 + h * kH, 3 * kH, kH, cf.a + kBnOff[5] + h * kH, cf.b + kBnOff[5] + h * kH,

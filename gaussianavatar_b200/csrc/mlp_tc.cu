@@ -74,6 +74,13 @@ struct TcFwdParams {
     double *sum, *sumsq;           // nullable
     int M;
 };
+// One launch computes up to three heads that read the same X: CTA b works for head b % heads on the tiles of group b / heads, so the
+// heads' CTAs of a tile run side by side and two of the three X reads are served from L2.
+constexpr int kMaxHeads = 3;
+struct TcFwdHeads {
+    TcFwdParams h[kMaxHeads];
+    int heads;
+};
 
 struct alignas(1024) TcFwdSmem {
     unsigned char x[kTStages][kTStageBytes];         // X tile: [4 chunks][64 px rows][128 B], K-major, 128-byte swizzle
@@ -85,14 +92,16 @@ struct alignas(1024) TcFwdSmem {
 static_assert(sizeof(TcFwdSmem) + 1024 <= kMaxSmemPerBlock, "forward shared memory");
 
 __global__ void __launch_bounds__(kTcThreads, 1)
-tc_fwd_kernel(const __grid_constant__ TcFwdParams p)
+tc_fwd_kernel(const __grid_constant__ TcFwdHeads ph)
 {
     extern __shared__ unsigned char smem_raw[];
     TcFwdSmem &sm = *reinterpret_cast<TcFwdSmem *>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
+    const TcFwdParams &p = ph.h[blockIdx.x % ph.heads];
+    const int cta = blockIdx.x / ph.heads;                                    // tile group
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int num_tiles = (p.M + kTPx - 1) / kTPx;
-    const int gstep = gridDim.x;
-    const int ntl = (num_tiles - (int)blockIdx.x + gstep - 1) / gstep;       // tiles of this CTA (grid <= tiles: >= 1)
+    const int gstep = gridDim.x / ph.heads;
+    const int ntl = (num_tiles - cta + gstep - 1) / gstep;                   // tiles of this CTA (groups <= tiles: >= 1)
     const int M = p.M;
     if (tid < kTStages) { mbar_init(smem_u32(&sm.full[tid]), 128); mbar_init(smem_u32(&sm.empty[tid]), 256); }
     if (tid < 2) { mbar_init(smem_u32(&sm.yload[tid]), 1); fence_proxy_async(); }   // completed by TMA loads (async proxy)
@@ -129,7 +138,7 @@ tc_fwd_kernel(const __grid_constant__ TcFwdParams p)
             // every producer thread waits (also those without copies): none may arrive on a stage's `full` barrier a round early
             if (j < ntl && j >= kTStages) mbar_wait(smem_u32(&sm.empty[st]), ((j / kTStages) & 1) ^ 1);   // tile j - kTStages is read
             if (j < ntl) {
-                const int t = blockIdx.x + j * gstep;
+                const int t = cta + j * gstep;
                 const uint32_t dst = x0s + (uint32_t)st * kTStageBytes;
                 const float *src = x0 + (size_t)t * kTPx * ldx;
                 const bool whole = (t + 1) * kTPx <= M;
@@ -194,7 +203,7 @@ tc_fwd_kernel(const __grid_constant__ TcFwdParams p)
     const uint32_t ys_u = smem_u32(ys), yload = smem_u32(&sm.yload[wg]);
     double dsum[2] = {0.0, 0.0}, dsq[2] = {0.0, 0.0};
     for (int j = 0; j < ntl; ++j) {
-        const int tile = blockIdx.x + j * gstep, st = j % kTStages;
+        const int tile = cta + j * gstep, st = j % kTStages;
         const uint32_t xs_u = x0s + (uint32_t)st * kTStageBytes;
         if (leader) {
             bulk_wait_read<0>();                       // the stores of tile j - 1 have read the staging half
@@ -264,23 +273,33 @@ tc_fwd_kernel(const __grid_constant__ TcFwdParams p)
 
 }  // namespace
 
-// Host-side launcher shared by the decoder orchestration and the unit-test entry point.
+// Host-side launcher shared by the decoder orchestration and the unit-test entry points.  heads > 1: head h computes with W, Y, bias
+// and the statistics advanced by h times w_hstride, y_hstride (floats) and v_hstride (elements of bias / sum / sumsq); X is shared.
 int launch_tc_fwd(const float *X, int ldx, int K, const float *a, const float *b, const float *W, int ldw, const float *bias, float *Y,
-                  int ldy, int accumulate, double *sum, double *sumsq, int M, cudaStream_t st)
+                  int ldy, int accumulate, double *sum, double *sumsq, int M, cudaStream_t st, int heads, size_t w_hstride, size_t y_hstride,
+                  int v_hstride)
 {
     GA_REQUIRE(K % 8 == 0 && K >= 8 && K <= 128, "tensor-core layer: K=%d must be a multiple of 8 in [8,128]", K);
     GA_REQUIRE(ldx % 4 == 0 && ldw % 4 == 0 && ldy % 4 == 0, "tensor-core layer: leading dimensions must be multiples of 4");
-    TcFwdParams p{{}, X, ldx, K, a, b, W, ldw, bias, accumulate, sum, sumsq, M};
-    if (int rc = make_tmap(&p.ymap, Y, 128, M, ldy, kTPx)) return rc;
+    GA_REQUIRE(heads >= 1 && heads <= kMaxHeads, "tensor-core layer: %d heads (1 .. %d)", heads, kMaxHeads);
+    TcFwdHeads ph{};
+    ph.heads = heads;
+    for (int h = 0; h < heads; ++h, W += w_hstride, Y += y_hstride) {
+        TcFwdParams &p = ph.h[h];
+        const int v = h * v_hstride;
+        p = TcFwdParams{{}, X, ldx, K, a, b, W, ldw, bias ? bias + v : nullptr, accumulate, sum ? sum + v : nullptr, sumsq ? sumsq + v : nullptr, M};
+        if (int rc = make_tmap(&p.ymap, Y, 128, M, ldy, kTPx)) return rc;
+    }
     static PerDeviceOnce attr_t_set;
     if (attr_t_set.first()) {
         GA_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcFwdSmem) + 1024));
     }
-    const int tiles = cdiv(M, kTPx), sms = num_sms();
-    const int grid = tiles < sms ? tiles : sms;
+    // one CTA per SM in all; each head gets the same number of tile groups
+    const int tiles = cdiv(M, kTPx), groups = num_sms() / heads;
+    const int grid = heads * (tiles < groups ? tiles : groups);
     {
         ProfScope _ps("mlp_tc_fwd", st);
-        tc_fwd_kernel<<<grid, kTcThreads, sizeof(TcFwdSmem) + 1024, st>>>(p);
+        tc_fwd_kernel<<<grid, kTcThreads, sizeof(TcFwdSmem) + 1024, st>>>(ph);
     }
     GA_CHECK_LAUNCH("tc_fwd_kernel");
     return GA_OK;
@@ -288,13 +307,24 @@ int launch_tc_fwd(const float *X, int ldx, int K, const float *a, const float *b
 
 }  // namespace ga
 
+// Unit-test / building-block entry of the multi-head form: head h (< heads <= 3) computes
+// Y[:, h y_hstride ...][M,128] (+)= act(bn(X)) W_h^T + bias_h with W_h = W + h w_hstride, bias_h / sum_h / sumsq_h advanced by h v_hstride.
+extern "C" int ga_tc_linear_forward_heads(int32_t M, int32_t heads, int32_t K, const float *X, int32_t ldx, const float *bn_a, const float *bn_b,
+                                          const float *W, int32_t ldw, int64_t w_hstride, const float *bias, float *Y, int32_t ldy, int64_t y_hstride,
+                                          int32_t accumulate, double *sum, double *sumsq, int32_t v_hstride, void *stream)
+{
+    GA_REQUIRE(M > 0 && X && W && Y && w_hstride >= 0 && y_hstride >= 0 && v_hstride >= 0, "bad arguments");
+    return ga::launch_tc_fwd(X, ldx, K, bn_a, bn_b, W, ldw, bias, Y, ldy, accumulate, sum, sumsq, M, static_cast<cudaStream_t>(stream), heads,
+                             (size_t)w_hstride, (size_t)y_hstride, v_hstride);
+}
+
 // Unit-test / building-block entry: Y[M,128] (+)= act(bn(X))[M,K] W[128,K]^T + bias on the tensor cores.
 extern "C" int ga_tc_linear_forward(int32_t M, int32_t K, const float *X, int32_t ldx, const float *bn_a, const float *bn_b, const float *W,
                                     int32_t ldw, const float *bias, float *Y, int32_t ldy, int32_t accumulate, double *sum, double *sumsq,
                                     void *stream)
 {
     GA_REQUIRE(M > 0 && X && W && Y, "bad arguments");
-    return ga::launch_tc_fwd(X, ldx, K, bn_a, bn_b, W, ldw, bias, Y, ldy, accumulate, sum, sumsq, M, static_cast<cudaStream_t>(stream));
+    return ga::launch_tc_fwd(X, ldx, K, bn_a, bn_b, W, ldw, bias, Y, ldy, accumulate, sum, sumsq, M, static_cast<cudaStream_t>(stream), 1, 0, 0, 0);
 }
 
 // =====================================================================================================================
@@ -354,6 +384,9 @@ struct alignas(1024) TcBwdSmem {
 };
 static_assert(sizeof(TcBwdSmem) + 1024 <= kMaxSmemPerBlock, "backward shared memory");
 
+// MODE3: the launch is mode 3, the only one that loads the existing output tile; a separate instantiation keeps that load and its
+// barrier wait out of the other modes' epilogue (measured: a mode-0 launch 10 % faster, DESIGN.md §7).
+template <bool MODE3>
 __global__ void __launch_bounds__(kTcThreads, 1)
 tc_bwd_kernel(const __grid_constant__ TcBwdParams p)
 {
@@ -511,7 +544,7 @@ tc_bwd_kernel(const __grid_constant__ TcBwdParams p)
     // never moved.  Thread 0 of the warpgroup moves the half.
     const int wg = (warp - 4) >> 2, icl = ic - 64 * wg;
     const int nchunks = max(0, min(2, (p.kin - 64 * wg + 31) / 32));
-    const bool load_existing = p.mode == 3 && nchunks > 0;   // mode 2 adds in L2 (TMA reduce-add): the SM reads nothing
+    const bool load_existing = MODE3 && nchunks > 0;   // mode 2 adds in L2 (TMA reduce-add): the SM reads nothing
     const bool leader = (tid & 127) == 0;
     unsigned char *os = sm.os[wg];
     const uint32_t os_u = smem_u32(os), oload = smem_u32(&sm.oload[wg]);
@@ -643,17 +676,19 @@ int launch_tc_bwd(const float *dZ, const float *Y, int ldg, const float *ga, con
     GA_REQUIRE(kin == 128 || mode == 1 || mode == 2, "tensor-core backward: mode %d needs kin = 128 (kin = %d)", mode, kin);
     GA_REQUIRE(ldg % 4 == 0 && ldp % 4 == 0 && ldw % 4 == 0 && ldo % 4 == 0, "tensor-core backward: leading dimensions must be multiples of 4");
     GA_REQUIRE(lddw % 4 == 0 && (reinterpret_cast<uintptr_t>(dW) & 15) == 0, "tensor-core backward: dW must be 16-byte aligned with lddw a multiple of 4");
-    static PerDeviceOnce attr_set;
-    if (attr_set.first()) {
-        GA_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcBwdSmem) + 1024));
-    }
     TcBwdParams p{{}, dZ, Y, ldg, ga, m1, m2, mu, rstd, Yprev, ldp, pa, pb, pmu, prstd, W, ldw, dW, lddw, mode, s1, s2, M, kin, x_raw};
     if (int rc = make_tmap(&p.omap, dZprev, kin, M, ldo, kPx)) return rc;
     const int tiles = cdiv(M, kPx), sms = num_sms();
     const int grid = tiles < sms ? tiles : sms;
+    static PerDeviceOnce attr_set;
+    if (attr_set.first()) {
+        GA_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcBwdSmem) + 1024));
+        GA_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TcBwdSmem) + 1024));
+    }
     {
         ProfScope _ps("mlp_tc_bwd", st);
-        tc_bwd_kernel<<<grid, kTcThreads, sizeof(TcBwdSmem) + 1024, st>>>(p);
+        if (mode == 3) tc_bwd_kernel<true><<<grid, kTcThreads, sizeof(TcBwdSmem) + 1024, st>>>(p);
+        else tc_bwd_kernel<false><<<grid, kTcThreads, sizeof(TcBwdSmem) + 1024, st>>>(p);
     }
     GA_CHECK_LAUNCH("tc_bwd_kernel");
     return GA_OK;

@@ -318,6 +318,11 @@ int ga_decoder_views(const GaDecoderDesc *d, void *workspace, GaDecoderViews *ou
 int ga_tc_linear_forward(int32_t M, int32_t K, const float *X, int32_t ldx, const float *bn_a, const float *bn_b, const float *W,
                          int32_t ldw, const float *bias, float *Y, int32_t ldy, int32_t accumulate, double *sum, double *sumsq,
                          void *stream);
+/* The same for `heads` (1..3) layers that share X, in one launch: head h uses W + h w_hstride, writes Y + h y_hstride (floats) and
+ * takes bias / sum / sumsq advanced by h v_hstride.  Each head's result is that of its own ga_tc_linear_forward. */
+int ga_tc_linear_forward_heads(int32_t M, int32_t heads, int32_t K, const float *X, int32_t ldx, const float *bn_a, const float *bn_b,
+                               const float *W, int32_t ldw, int64_t w_hstride, const float *bias, float *Y, int32_t ldy, int64_t y_hstride,
+                               int32_t accumulate, double *sum, double *sumsq, int32_t v_hstride, void *stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Fused image loss (utils/loss_utils.py:7-8,23-53 as combined at train.py:74-77):
