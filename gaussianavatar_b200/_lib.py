@@ -137,6 +137,9 @@ _SIGNATURES = {
     "ga_mesh_render": (ctypes.c_int, [ctypes.c_int32] * 5 + [c_vp] * 5 + [ctypes.c_float] * 3 + [c_vp] * 6),
     "ga_motion_sample": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 2 + [ctypes.c_int32] + [c_vp] * 5),
     "ga_frame_pack": (ctypes.c_int, [ctypes.c_int32] * 4 + [c_vp] * 5),
+    "ga_silhouette_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 5),
+    "ga_silhouette_forward": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float] + [c_vp] * 8),
+    "ga_silhouette_backward": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float] + [c_vp] * 10),
 }
 
 _lib = None

@@ -23,15 +23,14 @@
 // op by oracle/mesh_oracle.py, so face_id and depth are bit-reproducible and do not depend on the batch a frame is drawn in.
 #include "common.cuh"
 #include "fixed_raster.cuh"
+#include "mesh_project.cuh"
 
 namespace ga {
 namespace {
 
 constexpr int kMaxB = 8;
 constexpr int kMaxSide = 16384;
-constexpr int kCamStride = 40;                   // the ga_rasterb_* camera block: view 0..15, proj 16..31, tan(fov/2) 32..33
-constexpr float kZnear = 0.01f;
-constexpr float kGuard = 1048576.f;              // 2^20 pixels: |fixed-point coordinate| <= 2^28, edge products < 2^59
+using mesh::kCamStride;
 constexpr int kSmallFacePixels = 256;
 constexpr int kTile = 16;
 constexpr unsigned long long kEmpty = ~0ull;
@@ -42,15 +41,6 @@ __device__ __forceinline__ float mul_(float a, float b) { return __fmul_rn(a, b)
 __device__ __forceinline__ float add_(float a, float b) { return __fadd_rn(a, b); }
 __device__ __forceinline__ float sub_(float a, float b) { return __fsub_rn(a, b); }
 __device__ __forceinline__ float div_(float a, float b) { return __fdiv_rn(a, b); }
-
-// the op order of raster.cu's xf_row (row r of the transposed 4x4 M applied to (x, y, z, 1))
-__device__ __forceinline__ float xf_row(const float *__restrict__ M, int r, float x, float y, float z)
-{
-    float t = mul_(M[r], x);
-    t = __fmaf_rn(M[4 + r], y, t);
-    t = __fmaf_rn(M[8 + r], z, t);
-    return add_(t, M[12 + r]);
-}
 
 __device__ __forceinline__ float dot3(const float a[3], const float b[3]) { return add_(add_(mul_(a[0], b[0]), mul_(a[1], b[1])), mul_(a[2], b[2])); }
 
@@ -155,16 +145,10 @@ mesh_vertex_kernel(int V, int H, int W, const float *__restrict__ verts, const i
     float *no = normals + ((size_t)b * V + v) * 3;
     no[0] = n[0]; no[1] = n[1]; no[2] = n[2];
 
-    const float *view = cams + (size_t)b * kCamStride, *proj = view + 16;
-    const float px = X[3 * (size_t)v], py = X[3 * (size_t)v + 1], pz = X[3 * (size_t)v + 2];
-    const float tvz = xf_row(view, 2, px, py, pz);
-    const float hx = xf_row(proj, 0, px, py, pz), hy = xf_row(proj, 1, px, py, pz), hw = xf_row(proj, 3, px, py, pz);
-    const float p_w = div_(1.f, add_(hw, 0.0000001f));
-    const float ndc_x = mul_(hx, p_w), ndc_y = mul_(hy, p_w);
-    const float pixx = (float)__dmul_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)ndc_x, 1.0), (double)W), -1.0), 0.5);
-    const float pixy = (float)__dmul_rn(__dadd_rn(__dmul_rn(__dadd_rn((double)ndc_y, 1.0), (double)H), -1.0), 0.5);
+    float pixx, pixy, tvz;
+    mesh::project(cams + (size_t)b * kCamStride, H, W, X[3 * (size_t)v], X[3 * (size_t)v + 1], X[3 * (size_t)v + 2], pixx, pixy, tvz);
     ScreenVert s;
-    s.ok = tvz > kZnear && fabsf(pixx) <= kGuard && fabsf(pixy) <= kGuard;      // false for NaN
+    s.ok = mesh::drawable(pixx, pixy, tvz);
     s.x = s.ok ? snap_fixed((double)pixx * 256.0) : 0;
     s.y = s.ok ? -snap_fixed((double)pixy * 256.0) : 0;
     s.z = tvz;

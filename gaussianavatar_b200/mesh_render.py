@@ -45,6 +45,13 @@ def vertex_face_csr(faces: np.ndarray, V: int):
     return offsets.astype(np.int32), face[order].astype(np.int32)
 
 
+def coverage_iou(drawn, mask) -> float:
+    """IoU of a drawn silhouette (face_id >= 0) and a subject mask (byte >= 128), boolean [H,W] numpy arrays or tensors; 1 when
+    both are empty.  Integer counts, so the value does not depend on where it is computed."""
+    union = int((mask | drawn).sum())
+    return int((mask & drawn).sum()) / union if union else 1.0
+
+
 def cameras(cams) -> torch.Tensor:
     """[B,40] camera block (ga_rasterb_* layout) of a list of `camera.Camera`."""
     view = torch.stack([c.world_view_transform.float().cpu() for c in cams])

@@ -460,6 +460,29 @@ int ga_motion_sample(int32_t T, int32_t J, const float *key_pose, const float *k
 int ga_frame_pack(int32_t B, int32_t H, int32_t W, int32_t channels, const float *image, const float *final_T, const float *bg,
                   uint8_t *out, void *stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Soft silhouette (pose refinement against masks).  B in [1, 8] frames of verts [B,V,3] (fp32), faces [F,3] (int32, each in
+ * [0, V)), cams [B,40] (the ga_rasterb_* camera block), H, W in [1, 16384], sigma > 0 in pixels^2.  Vertices are projected as
+ * ga_mesh_render projects them, in fp32, not snapped; pixel (c, r) is centred at (c, r).  For face f and pixel centre p, d_f the
+ * distance from p to the projected triangle: D_f = sigmoid(+-d_f^2 / sigma) (+ inside, - outside), 0 outside beyond
+ * d_f^2 > sigma ln(1/1e-4 - 1); S = 1 - prod_f (1 - D_f).  A face with a corner at view depth <= 0.01 or beyond the 2^20-pixel
+ * guard band, or with zero projected area, contributes nothing; no culling.
+ * ga_silhouette_forward: sil [B,H,W]; with mask_u8 [B,H,W] (subject where the byte is >= 128) also loss [B] = mean_p (S - M)^2.
+ *   mask_u8 may be NULL (then loss is not written and may be NULL).
+ * ga_silhouette_backward: from the same inputs, mask_u8 required, and per-frame weights w [B] (device): d_verts [B,V,3] of
+ *   sum_b w_b loss_b, through the projection, ready for ga_smpl(x)_vertices_backward.  adj_offsets [V+1] / adj_faces [3F]: the
+ *   vertex -> face CSR of ga_mesh_render.
+ * workspace: ga_silhouette_workspace_bytes(B, V, F, H, W) bytes, 256-byte aligned, sized by the shapes alone (no capacity).
+ * Every output element is written.  No floating-point atomics and no host read-back: the outputs are bit-reproducible and a
+ * frame's do not depend on the batch it is in.
+ * ---------------------------------------------------------------------------------------------------------------- */
+size_t ga_silhouette_workspace_bytes(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W);
+int ga_silhouette_forward(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, float sigma, const float *verts, const int32_t *faces,
+                          const float *cams, const uint8_t *mask_u8, void *workspace, float *sil, float *loss, void *stream);
+int ga_silhouette_backward(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, float sigma, const float *verts, const int32_t *faces,
+                           const int32_t *adj_offsets, const int32_t *adj_faces, const float *cams, const uint8_t *mask_u8, const float *w,
+                           void *workspace, float *d_verts, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

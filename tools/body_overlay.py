@@ -22,7 +22,7 @@ from PIL import Image
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from gaussianavatar_b200.camera import make_camera  # noqa: E402
-from gaussianavatar_b200.mesh_render import COLORS, MAX_FRAMES_PER_CALL, MeshRenderer, cameras  # noqa: E402
+from gaussianavatar_b200.mesh_render import COLORS, MAX_FRAMES_PER_CALL, MeshRenderer, cameras, coverage_iou  # noqa: E402
 from gaussianavatar_b200.posmap import BodyPoser, SmplxBodyPoser, load_body_model  # noqa: E402
 
 
@@ -76,8 +76,7 @@ def main(argv=None):
                     mname = next(n for n in sorted(os.listdir(mdir)) if os.path.splitext(n)[0] == stem)
                     m = np.array(Image.open(os.path.join(mdir, mname)))
                     m = (m if m.ndim == 2 else m[..., 0]) >= 128
-                    union = int((m | drawn[j]).sum())
-                    ious.append((s + i, int((m & drawn[j]).sum()) / union if union else 1.0))
+                    ious.append((s + i, coverage_iou(drawn[j], m)))
     if a.iou:
         ious.sort()
         per = [v for _, v in ious]
