@@ -33,6 +33,11 @@ class GaRasterBatchDesc(ctypes.Structure):
                 ("scale_modifier", ctypes.c_float)]
 
 
+class GaRasterScene(ctypes.Structure):
+    _fields_ = [("Ps", ctypes.c_int32), ("sh_degree", ctypes.c_int32), ("sh_coeffs", ctypes.c_int32), ("means3D", c_vp), ("scales", c_vp),
+                ("rotations", c_vp), ("opacities", c_vp), ("shs", c_vp), ("rgb", c_vp)]
+
+
 class GaRasterViews(ctypes.Structure):
     _fields_ = [(n, c_vp) for n in ("depth", "xy", "conic_opacity", "cov3d", "tiles_touched", "rect", "point_list", "ranges",
                                     "tile_count", "final_T", "n_contrib", "status")]
@@ -124,6 +129,7 @@ _SIGNATURES = {
     "ga_rasterb_status_to_host": (ctypes.c_int, [ctypes.c_int32] * 3 + [c_vp] * 4),
     "ga_rasterb_forward": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc)] + [c_vp] * 13),
     "ga_rasterb_backward": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc)] + [c_vp] * 19),
+    "ga_rasterb_forward_scene": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc), ctypes.POINTER(GaRasterScene)] + [c_vp] * 13),
     "ga_tc_conv5x5": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, c_vp, c_vp, c_vp, ctypes.c_int32, c_vp]),
     "ga_round_tf32": (ctypes.c_int, [c_vp, c_vp, ctypes.c_int64, c_vp]),
     "ga_lpips_weights_floats": (ctypes.c_size_t, []),

@@ -15,6 +15,9 @@ j+1 renders while the caller consumes chunk j; the rasterizer's overflow status 
 buffer overflowed is re-rendered after the buffer has grown (and the graphs are re-captured) before it is yielded.  Stage 2 runs
 eagerly, one frame per forward, with the sampled pose for both the input position map and the skeleton.  The model's parameters
 and BatchNorm statistics are left exactly as they were.
+
+With a scene (`scene.GaussianScene`) both stages render through the composite forward instead, which splats the avatar and the
+scene in one sort per tile; a `scene.Placement` moves the avatar (and the cameras given around it) into the scene.
 """
 from __future__ import annotations
 
@@ -30,9 +33,11 @@ from ._lib import ptr
 from .avatar_model import kept_state
 from .camera import Camera, make_camera
 from .dataset import _rodrigues, rotate_camera_by_frame_idx
-from .rasterizer import MAX_FRAMES_PER_CALL, RasterBatchPlan, rasterize_batch
+from .rasterizer import MAX_FRAMES_PER_CALL, RasterBatchPlan, rasterize_batch, rasterize_batch_scene
+from .scene import SceneCamera
 
 POSE_WIDTH = {"smpl": 72, "smplx": 165}
+SCENE_CHUNK = 2                 # the player's default chunk with a scene
 IDENTITY_ALIGN = np.array([1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0], np.float64)
 
 
@@ -185,17 +190,23 @@ class Schedule:
 class Animator:
     """Renders an inference `AvatarModel` (stage 1 or 2) along motion clips.
 
-    cameras: a `dataset.camera_item` dict (one camera for every frame) or an `OrbitCamera`.  H, W: frame size.  chunk: frames per
-    rasterizer call (1..8).  channels: 3 (RGB) or 4 (straight-alpha RGBA).  pose_mapper: stage 2's `posmap.PoseMapper` /
+    cameras: a `dataset.camera_item` dict (one camera for every frame), an `OrbitCamera`, or with a scene a `scene.SceneCamera` (one of
+    the scene's own cameras, in the scene's world).  H, W: frame size.  chunk: frames per
+    rasterizer call (1..8; default 8, with a scene SCENE_CHUNK).  channels: 3 (RGB) or 4 (straight-alpha RGBA).  pose_mapper: stage 2's `posmap.PoseMapper` /
     `SmplxPoseMapper` (default: the model's own).  capacity: initial binning capacity of the rasterizer (instances); it grows on
-    overflow.  graphs: replay CUDA graphs in stage 1 (False runs the same launches eagerly, e.g. for per-kernel profiling)."""
+    overflow.  graphs: replay CUDA graphs in stage 1 (False runs the same launches eagerly, e.g. for per-kernel profiling).
+    scene: a `scene.GaussianScene` the avatar is rendered in, splatted together with it (`rasterize_batch_scene`) so that either
+    hides the other; placement: the `scene.Placement` of the avatar's world in it.  The cameras are given in the avatar's world
+    and carried into the scene through the placement; alpha (channels=4) is 1 - final transmittance over both sets."""
 
-    def __init__(self, model, cameras, H: int, W: int, chunk: int = MAX_FRAMES_PER_CALL, channels: int = 3, pose_mapper=None,
-                 capacity=None, graphs: bool = True):
+    def __init__(self, model, cameras, H: int, W: int, chunk: int | None = None, channels: int = 3, pose_mapper=None,
+                 capacity=None, graphs: bool = True, scene=None, placement=None):
         self.model = model
         self.H, self.W = int(H), int(W)
         if not (1 <= self.H <= 16384 and 1 <= self.W <= 16384):
             raise ValueError(f"frame {self.H} x {self.W} outside [1, 16384]^2")
+        if chunk is None:        # with a scene, chunks beyond 2 frames render no faster (DESIGN.md §7) and need far more memory
+            chunk = MAX_FRAMES_PER_CALL if scene is None else SCENE_CHUNK
         if not 1 <= int(chunk) <= MAX_FRAMES_PER_CALL:
             raise ValueError(f"chunk {chunk} outside 1..{MAX_FRAMES_PER_CALL}")
         if int(channels) not in (3, 4):
@@ -205,8 +216,11 @@ class Animator:
             h, w = int(cameras.get("height", self.H)), int(cameras.get("width", self.W))
             if (h, w) != (self.H, self.W):
                 raise ValueError(f"the camera was built for {w} x {h}, the frames are {self.W} x {self.H}")
+        elif isinstance(cameras, SceneCamera):
+            if scene is None:
+                raise ValueError("a scene camera (cameras.json) needs the scene")
         elif not isinstance(cameras, OrbitCamera):
-            raise TypeError("cameras: a camera_item dict or an OrbitCamera")
+            raise TypeError("cameras: a camera_item dict, an OrbitCamera or a scene.SceneCamera")
         self.cameras = cameras
         self.stage = 2 if int(model.model_parms.train_stage) == 2 else 1
         self.body = "smplx" if model.smplx else "smpl"
@@ -214,6 +228,8 @@ class Animator:
         if self.stage == 2 and self.pose_mapper is None:
             raise ValueError("stage 2 needs a pose_mapper (posmap.PoseMapper / SmplxPoseMapper) for the input position maps")
         self.dev = model.device
+        self.scene = None if scene is None else scene.to(self.dev)
+        self.placement = placement
         self.capacity = capacity
         self.use_graphs = bool(graphs)
         self.captures = 0          # CUDA graphs captured
@@ -254,15 +270,18 @@ class Animator:
     def _camera_rows(self, n, clip, align):
         from .mesh_render import cameras as camera_block
         cam = self.cameras
+        place = (lambda c: c) if self.placement is None else self.placement.carry
+        if isinstance(cam, SceneCamera):                  # already in the scene's world
+            return camera_block([cam.camera(self.H, self.W)]).expand(n, -1).contiguous()
         if isinstance(cam, dict):
             one = Camera(float(cam["FovX"]), float(cam["FovY"]), self.H, self.W, torch.as_tensor(cam["world_view_transform"]),
                          torch.as_tensor(cam["full_proj_transform"]), torch.as_tensor(cam["camera_center"]))
-            return camera_block([one]).expand(n, -1).contiguous()
+            return camera_block([place(one)]).expand(n, -1).contiguous()
         R, c = align[:9].reshape(3, 3), align[9:]
         t0 = R @ clip.trans[0].double().numpy() + c
         pelvis = self.model._rest_joints[0].double().cpu().numpy() + t0        # the root rotates about the rest pelvis
-        rows = [make_camera(cam.K, rotate_camera_by_frame_idx(cam.extrinsic, k, trans=pelvis, rotate_axis=cam.rotate_axis, period=n,
-                                                             inv_angle=cam.inv_angle), self.H, self.W) for k in range(n)]
+        rows = [place(make_camera(cam.K, rotate_camera_by_frame_idx(cam.extrinsic, k, trans=pelvis, rotate_axis=cam.rotate_axis, period=n,
+                                                                   inv_angle=cam.inv_angle), self.H, self.W)) for k in range(n)]
         return camera_block(rows)
 
     def _check_clip(self, clip):
@@ -327,8 +346,15 @@ class Animator:
     # ---- stage 1: one graph per (chunk size, slot) -------------------------------------------------------------------------------
     def _plan(self, b):
         if b not in self._plans:
-            self._plans[b] = RasterBatchPlan(b, int(self.model._query_points.shape[0]), self.H, self.W, self.dev, capacity=self.capacity)
+            self._plans[b] = RasterBatchPlan(b, int(self.model._query_points.shape[0]), self.H, self.W, self.dev, capacity=self.capacity,
+                                             static_P=0 if self.scene is None else len(self.scene))
         return self._plans[b]
+
+    def _raster(self, means, scales, colors, cams, plan):
+        m = self.model
+        if self.scene is None:
+            return rasterize_batch(means, colors, scales, m.fix_rotation, m.fix_opacity, cams, m.background, plan)
+        return rasterize_batch_scene(means, colors, scales, m.fix_rotation, m.fix_opacity, cams, m.background, plan, self.scene)
 
     def _grow(self, b, needed):
         if self._graphs:
@@ -361,8 +387,8 @@ class Animator:
             plan = self._plan(b)
             pose, trans = motion_sample(self._keys_pose[:T], self._keys_trans[:T], self._times_dev[:b], self._align)
             pose, rest = self._split(pose)
-            means, scales, colors = m._assemble(self._dec, pose, trans, rest)
-            img = rasterize_batch(means, colors, scales, m.fix_rotation, m.fix_opacity, self._cams_dev[:b], m.background, plan)
+            means, scales, colors = m._assemble(self._dec, pose, trans, rest, placement=self.placement)
+            img = self._raster(means, scales, colors, self._cams_dev[:b], plan)
             frame_pack(img, final_transmittance(plan), m.background, self.channels, self._out_dev[slot][:b])
             self._status_dev[slot].copy_(plan.status_dev)
 
@@ -393,8 +419,18 @@ class Animator:
         def render(s, e, slot):
             for i in range(s, e):
                 p, rest = self._split(pose[i:i + 1])
-                means, scales, colors, _, _ = m._stage2_from_pose(self.pose_mapper, p, trans[i:i + 1], rest)
-                batch = {"_cams": cams_all[i:i + 1], "height": [self.H], "width": [self.W]}
-                img = m._render_frames(batch, means, scales, colors)
-                frame_pack(img, final_transmittance(m._last_plan), m.background, self.channels, self._out_dev[slot][i - s:i - s + 1])
+                means, scales, colors, _, _ = m._stage2_from_pose(self.pose_mapper, p, trans[i:i + 1], rest, placement=self.placement)
+                if self.scene is None:
+                    batch = {"_cams": cams_all[i:i + 1], "height": [self.H], "width": [self.W]}
+                    img = m._render_frames(batch, means, scales, colors)
+                    plan = m._last_plan
+                else:                # as _render_batched: a frame whose binning buffer overflowed is rendered again after it grew
+                    plan = self._plan(1)
+                    img = self._raster(means, scales, colors, cams_all[i:i + 1], plan)
+                    if not plan.check(wait=True):
+                        self.overflows += 1
+                        img = self._raster(means, scales, colors, cams_all[i:i + 1], plan)
+                        if not plan.check(wait=True):
+                            raise RuntimeError("animation: the rasterizer's binning buffer overflowed again after growing")
+                frame_pack(img, final_transmittance(plan), m.background, self.channels, self._out_dev[slot][i - s:i - s + 1])
         return render

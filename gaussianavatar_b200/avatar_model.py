@@ -344,10 +344,14 @@ class AvatarModel:
         rest_pose = rest_pose.to(device=self.device, dtype=torch.float32)
         return SmplxCano2Live.apply(pose_batch, rest_pose, transl_batch, self._rest_joints, self._inv_cano)
 
-    def _assemble(self, dec, pose, transl, rest_pose=None, scale_mul=1.0, per_frame=False):
+    def _assemble(self, dec, pose, transl, rest_pose=None, scale_mul=1.0, per_frame=False, placement=None):
         """Decoder output `dec` posed by pose / transl (and SMPL-X's rest_pose): cano2live, then the fused LBS / attribute assembly.
-        Returns means3D, scales, colors [B,N,3].  per_frame: `dec` holds one [S*S,8] block per frame (stage 2)."""
+        Returns means3D, scales, colors [B,N,3].  per_frame: `dec` holds one [S*S,8] block per frame (stage 2).  placement: a
+        `scene.Placement` folded into cano2live, its scale into the LBS scale multiplier (the Gaussians are isotropic)."""
         cano2live = self._cano2live(pose, transl, rest_pose)                                              # [B,J,12]
+        if placement is not None:
+            cano2live = placement.fold(cano2live)
+            scale_mul = scale_mul * placement.scale
         return LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, scale_mul, per_frame)
 
     def _stage1_decoder(self, batch):
@@ -491,7 +495,7 @@ class AvatarModel:
         images = self._render_frames(batch_data, means, scales, colors)
         return images, means, offset_loss, geo_loss, scale_loss
 
-    def _stage2_gaussians(self, batch_data, pose=None, transl=None):
+    def _stage2_gaussians(self, batch_data, pose=None, transl=None, placement=None):
         """Stage 2 (model/avatar_model.py:369-420 / :557-612): the pose encoder turns each frame's posed-body position map into a
         feature map that is ADDED to the geometry features, so the decoder runs per frame (B*S*S rows, BatchNorm statistics over all of
         them); no scale ramp in this stage.  The skeleton is posed with the model's pose / transl rows at `pose_idx`, as the reference
@@ -504,14 +508,15 @@ class AvatarModel:
         S = int(self.model_parms.query_posmap_size)
         pose_featmap = self.pose_encoder(inp)                                                         # [B,64,h,h]
         dec = self.net.forward_packed_frames(self.geo_feature, pose_featmap, S)                      # [B*S*S, 8]
-        means, scales, colors = self._assemble(dec, pose, transl, batch_data.get("rest_pose"), per_frame=True)
+        means, scales, colors = self._assemble(dec, pose, transl, batch_data.get("rest_pose"), per_frame=True, placement=placement)
         return means, scales, colors, dec, pose_featmap
 
-    def _stage2_from_pose(self, mapper, pose, transl, rest_pose=None):
+    def _stage2_from_pose(self, mapper, pose, transl, rest_pose=None, placement=None):
         """`_stage2_gaussians` of explicit poses [B,72|66] / transl [B,3] (and SMPL-X's rest_pose [B,99]): the input position maps are
-        built from the same pose by `mapper` (a posmap.PoseMapper / SmplxPoseMapper, differentiable in pose and transl)."""
+        built from the same pose by `mapper` (a posmap.PoseMapper / SmplxPoseMapper, differentiable in pose and transl).  placement
+        moves the posed Gaussians into a scene (`_assemble`); the position maps stay in the body's own frame."""
         inp = mapper(pose, rest_pose, transl) if self.smplx else mapper(pose, transl)
-        return self._stage2_gaussians({"inp_pos_map": inp, "rest_pose": rest_pose}, pose=pose, transl=transl)
+        return self._stage2_gaussians({"inp_pos_map": inp, "rest_pose": rest_pose}, pose=pose, transl=transl, placement=placement)
 
     def _pose_map(self, batch_data):
         """Input position maps [B,3,s,s] of a batch that carries none: from its `pose_data` / `transl_data` when it has them (test,

@@ -172,8 +172,10 @@ __device__ __forceinline__ void quat_to_rot(float qr, float qx, float qy, float 
 }
 
 // Where a frame's camera comes from: a device array of kCamStride floats per frame (batched path: view 0..15, proj 16..31,
-// tanfovx 32, tanfovy 33) or two device matrices plus host scalars (per-frame API, stride 0).
+// tanfovx 32, tanfovy 33, camera centre 34..36, read only by the composite forward) or two device matrices plus host scalars
+// (per-frame API, stride 0).
 constexpr int kCamStride = 40;
+constexpr int kCamPos = 34;
 struct CamSrc {
     const float *view, *proj, *tan;
     int stride;
@@ -252,28 +254,45 @@ __device__ __forceinline__ void sh_row_store(float *__restrict__ row, int nrow, 
     }
 }
 
-// K1's SH colour of Gaussian i: rgb = max(sum_k basis_k(dir) sh_k + 0.5, 0), dir = (mean - campos) / |mean - campos|.  Culled
-// Gaussians (live = false) get rgb 0 and no clamp bits; ordinary fp32, no integer decision depends on it.
+// The SH colour of one Gaussian's row of degree D seen from campos: r = max(sum_k basis_k(dir) sh_k + 0.5, 0) with
+// dir = (mean - campos) / |mean - campos|; r must come in zeroed.  Returns the clamp bits (bit c: channel c was clamped at 0).
+__device__ __forceinline__ uint32_t sh_eval(const float *__restrict__ row, int D, bool vec4, const float *__restrict__ campos, float px,
+                                            float py, float pz, float r[3])
+{
+    uint32_t cl = 0;
+    const float vx = px - __ldg(campos), vy = py - __ldg(campos + 1), vz = pz - __ldg(campos + 2);
+    const float inv = 1.f / sqrtf(vx * vx + vy * vy + vz * vz);
+    float b[16];
+    sh_basis(vx * inv, vy * inv, vz * inv, b);
+    const int n = 3 * (D + 1) * (D + 1);
+    sh_row_load(row, n, vec4, [&](int e, float v) { if (e < n) r[e % 3] += b[e / 3] * v; });
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        r[ch] += 0.5f;
+        if (r[ch] < 0.f) { cl |= 1u << ch; r[ch] = 0.f; }
+    }
+    return cl;
+}
+
+// K1's SH colour of Gaussian i (sh_eval from cc.campos).  Culled Gaussians (live = false) get rgb 0 and no clamp bits; ordinary fp32,
+// no integer decision depends on it.
 __device__ __forceinline__ void sh_color_fwd(const ColorCov &cc, size_t i, float px, float py, float pz, bool live)
 {
     float r[3] = {0.f, 0.f, 0.f};
     uint32_t cl = 0;
-    if (live) {
-        const float vx = px - __ldg(cc.campos), vy = py - __ldg(cc.campos + 1), vz = pz - __ldg(cc.campos + 2);
-        const float inv = 1.f / sqrtf(vx * vx + vy * vy + vz * vz);
-        float b[16];
-        sh_basis(vx * inv, vy * inv, vz * inv, b);
-        const int n = 3 * (cc.D + 1) * (cc.D + 1);
-        sh_row_load(cc.shs + i * 3 * cc.M, n, cc.vec4, [&](int e, float v) { if (e < n) r[e % 3] += b[e / 3] * v; });
-#pragma unroll
-        for (int ch = 0; ch < 3; ++ch) {
-            r[ch] += 0.5f;
-            if (r[ch] < 0.f) { cl |= 1u << ch; r[ch] = 0.f; }
-        }
-    }
+    if (live) cl = sh_eval(cc.shs + i * 3 * cc.M, cc.D, cc.vec4, cc.campos, px, py, pz, r);
     cc.rgb[3 * i] = r[0]; cc.rgb[3 * i + 1] = r[1]; cc.rgb[3 * i + 2] = r[2];
     cc.clamped[i] = (uint8_t)cl;
 }
+
+// The static set of the composite forward (GaRasterScene): Ps Gaussians shared by every frame (read with frame stride 0) that
+// follow each frame's P dynamic ones in its index space.  K1 evaluates their SH colours for each frame's camera centre into rgb.
+struct SceneSet {
+    const float *means3D, *scales, *rotations, *opacities, *shs;   // [Ps,3] [Ps,3] [Ps,4] [Ps] [Ps,M,3]
+    int Ps, D, M;
+    bool vec4;               // as ColorCov::vec4
+    float *rgb;              // [B, Ps, 3]
+};
 
 // Backward of sh_color_fwd for a visible Gaussian: writes the whole d_sh row (basis_k * dL/drgb, 0 on clamped channels and for
 // k >= (D+1)^2) and adds the direction term, pushed through the normalisation, to dmean.
@@ -313,9 +332,10 @@ __device__ __forceinline__ void sh_color_bwd(const ColorCov &cc, size_t i, float
 
 // Per-Gaussian part of K1; returns the tile rect (zero area if the Gaussian is culled).  kCov: Sigma is read from cov_pre (this
 // Gaussian's six values) instead of being built from scales / rotations / mod; everything after Sigma is the same op sequence.
+// i indexes the outputs, src the rows of means3D / scales.
 template <bool kCov>
 __device__ __forceinline__ ushort4
-preprocess_one(int il, size_t i, int H, int W, int gx, int gy, const float *view, const float *proj, float tanfovx, float tanfovy,
+preprocess_one(int il, size_t i, size_t src, int H, int W, int gx, int gy, const float *view, const float *proj, float tanfovx, float tanfovy,
                float mod, const float *__restrict__ means3D, const float *__restrict__ scales, const float *__restrict__ rq,
                const float *__restrict__ cov_pre, float opacity, float *__restrict__ depth, float2 *__restrict__ xy,
                float4 *__restrict__ conic_o, float *__restrict__ cov3d, uint32_t *__restrict__ tiles, ushort4 *__restrict__ rect,
@@ -331,7 +351,7 @@ preprocess_one(int il, size_t i, int H, int W, int gx, int gy, const float *view
 #pragma unroll
     for (int k = 0; k < 6; ++k) cov3d[6 * (size_t)i + k] = 0.f;
 
-    const float px = means3D[3 * (size_t)i], py = means3D[3 * (size_t)i + 1], pz = means3D[3 * (size_t)i + 2];
+    const float px = means3D[3 * src], py = means3D[3 * src + 1], pz = means3D[3 * src + 2];
     const float tvx = xf_row(view, 0, px, py, pz), tvy = xf_row(view, 1, px, py, pz), tvz = xf_row(view, 2, px, py, pz);
     if (tvz <= 0.2f) return none;
 
@@ -343,7 +363,7 @@ preprocess_one(int il, size_t i, int H, int W, int gx, int gy, const float *view
     if constexpr (kCov) {
         S00 = cov_pre[0]; S01 = cov_pre[1]; S02 = cov_pre[2]; S11 = cov_pre[3]; S12 = cov_pre[4]; S22 = cov_pre[5];
     } else {
-        const float sv[3] = {mul_(mod, scales[3 * (size_t)i]), mul_(mod, scales[3 * (size_t)i + 1]), mul_(mod, scales[3 * (size_t)i + 2])};
+        const float sv[3] = {mul_(mod, scales[3 * src]), mul_(mod, scales[3 * src + 1]), mul_(mod, scales[3 * src + 2])};
         float Rm[3][3];
         quat_to_rot(rq[0], rq[1], rq[2], rq[3], Rm);
         float Mm[3][3];
@@ -476,14 +496,16 @@ __device__ __forceinline__ int tile_slot_find(const uint32_t *s_key, uint32_t ti
 // one global atomic per (CTA, touched tile) instead of one per instance, which would put a few hundred thousand atomics on a few
 // hundred hot addresses that serialise in L2.
 // kSH / kCov (per-frame API only, B = 1): SH colours into cc.rgb / cc.clamped, Sigma from cc.cov3D.
-template <bool kSH = false, bool kCov = false>
+// kScene (composite forward): frame b holds P + sc.Ps Gaussians, the dynamic P first (per-frame means / scales, strided rotations /
+// opacities, as without it), then the static set; a static Gaussian's SH colour for frame b's camera centre goes to sc.rgb[b].
+template <bool kSH = false, bool kCov = false, bool kScene = false>
 __global__ void __launch_bounds__(256)
 preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod, const float *__restrict__ means3D,
                       const float *__restrict__ scales, const float *__restrict__ rots, long long rot_stride,
                       const float *__restrict__ opac, long long opac_stride, float *__restrict__ depth,
                       float2 *__restrict__ xy, float4 *__restrict__ conic_o, float *__restrict__ cov3d,
                       uint32_t *__restrict__ tiles, ushort4 *__restrict__ rect, int32_t *__restrict__ radii,
-                      uint32_t *__restrict__ tile_count, ColorCov cc)
+                      uint32_t *__restrict__ tile_count, ColorCov cc, SceneSet sc)
 {
     const int b = blockIdx.y;
     __shared__ float view[16], proj[16];
@@ -494,8 +516,25 @@ preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod
     const float tanfovy = cam.tan ? cam.tan[(size_t)b * cam.stride + 1] : cam.tany;
     const int il = blockIdx.x * blockDim.x + threadIdx.x;
     ushort4 rc = make_ushort4(0, 0, 0, 0);
-    if (il < P) {
-        rc = preprocess_one<kCov>(il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, means3D, scales,
+    if constexpr (kScene) {
+        const int Pf = P + sc.Ps;
+        if (il < P) {
+            rc = preprocess_one<false>(il, (size_t)b * Pf + il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod,
+                                       means3D, scales, rots + (size_t)b * rot_stride + 4 * (size_t)il, nullptr,
+                                       opac[(size_t)b * opac_stride + il], depth, xy, conic_o, cov3d, tiles, rect, radii);
+        } else if (il < Pf) {
+            const size_t j = (size_t)(il - P);
+            rc = preprocess_one<false>(il, (size_t)b * Pf + il, j, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, sc.means3D, sc.scales,
+                                       sc.rotations + 4 * j, nullptr, sc.opacities[j], depth, xy, conic_o, cov3d, tiles, rect, radii);
+            float r[3] = {0.f, 0.f, 0.f};
+            if (rc.z > rc.x)
+                sh_eval(sc.shs + j * 3 * sc.M, sc.D, sc.vec4, cam.view + (size_t)b * cam.stride + kCamPos, sc.means3D[3 * j],
+                        sc.means3D[3 * j + 1], sc.means3D[3 * j + 2], r);
+            float *o = sc.rgb + 3 * ((size_t)b * sc.Ps + j);
+            o[0] = r[0]; o[1] = r[1]; o[2] = r[2];
+        }
+    } else if (il < P) {
+        rc = preprocess_one<kCov>(il, (size_t)b * P + il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, means3D, scales,
                                   rots + (size_t)b * rot_stride + 4 * (size_t)il, cc.cov3D + 6 * (size_t)il,
                                   opac[(size_t)b * opac_stride + il], depth, xy, conic_o, cov3d, tiles, rect, radii);
         if constexpr (kSH)
@@ -672,14 +711,16 @@ __device__ __forceinline__ void bitonic_sort_smem(uint64_t *keys, int n2)
 // order, the Gaussian index and the packed record the compositing kernels stream.  Buckets longer than kSortMax are sorted
 // kSortMax keys at a time (written back in place) and merged by rank: keys are unique, so an element's final position is
 // the number of smaller keys, i.e. the sum of its lower bounds in the sorted runs.
-template <int kThreads, int kMax, bool kLong>
+// kScene (composite forward, P = Pd + Ps per frame): colours of indices below Pd come from colors [B,Pd,3], the others from K1's
+// per-frame scene rgb [B,Ps,3].
+template <int kThreads, int kMax, bool kLong, bool kScene = false>
 __global__ void __launch_bounds__(kThreads)
 tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const uint32_t *__restrict__ order,
                  const uint2 *__restrict__ ranges, const uint32_t *__restrict__ seg_start,
                  uint64_t *__restrict__ bucket, const float2 *__restrict__ xy, const float4 *__restrict__ conic_o,
                  const float *__restrict__ colors, uint32_t *__restrict__ point_list, float4 *__restrict__ recA,
                  float4 *__restrict__ recB, float4 *__restrict__ recC, uint32_t *__restrict__ seg_tile,
-                 uint32_t *__restrict__ tile_maxc)
+                 uint32_t *__restrict__ tile_maxc, const float *__restrict__ scene_rgb, int Pd)
 {
     extern __shared__ uint64_t s_keys[];
     using BinScan = cub::BlockScan<uint32_t, kThreads>;
@@ -698,6 +739,11 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
         const size_t gbase = (size_t)(blk / T) * P;      // this frame's Gaussians
         const uint32_t s0 = seg_start[blk];
         for (int i = threadIdx.x; i < (n + kSeg - 1) / kSeg; i += blockDim.x) seg_tile[s0 + i] = (uint32_t)blk;
+        // kScene: colour row of this frame's Gaussian idx
+        auto scene_col = [&](uint32_t idx) {
+            const size_t f = (size_t)(blk / T);
+            return idx < (uint32_t)Pd ? colors + 3 * (f * Pd + idx) : scene_rgb + 3 * (f * (P - Pd) + (idx - Pd));
+        };
 
         auto emit = [&](int rank, uint64_t key) {
             const uint32_t idx = (uint32_t)key;
@@ -707,7 +753,12 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
             point_list[o] = idx;
             recA[o] = make_float4(c.x, c.y, cull_radius2(co), __uint_as_float(idx));
             recB[o] = co;
-            recC[o] = make_float4(colors[3 * g], colors[3 * g + 1], colors[3 * g + 2], 0.f);
+            if constexpr (kScene) {
+                const float *cp = scene_col(idx);
+                recC[o] = make_float4(cp[0], cp[1], cp[2], 0.f);
+            } else {
+                recC[o] = make_float4(colors[3 * g], colors[3 * g + 1], colors[3 * g + 2], 0.f);
+            }
         };
 
         if (n <= kMax) {
@@ -799,7 +850,12 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
                 for (int u = 0; u < 4; ++u) {
                     const size_t g = gbase + (uint32_t)kk[u];
                     c[u] = xy[g]; co[u] = conic_o[g];
-                    col[u][0] = colors[3 * g]; col[u][1] = colors[3 * g + 1]; col[u][2] = colors[3 * g + 2];
+                    if constexpr (kScene) {
+                        const float *cp = scene_col((uint32_t)kk[u]);
+                        col[u][0] = cp[0]; col[u][1] = cp[1]; col[u][2] = cp[2];
+                    } else {
+                        col[u][0] = colors[3 * g]; col[u][1] = colors[3 * g + 1]; col[u][2] = colors[3 * g + 2];
+                    }
                 }
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
@@ -1310,18 +1366,21 @@ struct FwdArgs {
     float mod;
 };
 
-// K1 + K2 for all frames.  cc selects the K1 variant (all zero: precomputed colours, Sigma from scales / rotations).
+// K1 + K2 for all frames.  cc selects the K1 variant (all zero: precomputed colours, Sigma from scales / rotations); a scene
+// selects the composite K1, with d.P = P + Ps Gaussians per frame.
 int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const ColorCov &cc, long long capacity, const GeomViews &g,
-                      const ImgViews &iv, int32_t *radii, cudaStream_t stream)
+                      const ImgViews &iv, int32_t *radii, cudaStream_t stream, const SceneSet *scene = nullptr)
 {
     const size_t BT = (size_t)d.B * d.T;
     GA_CHECK_CUDA(cudaMemsetAsync(iv.count, 0, sizeof(uint32_t) * BT, stream));
     if (d.P > 0) {
         ProfScope _ps("preprocess_fwd_kernel", stream);
-        auto *k1 = cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true> : preprocess_fwd_kernel<true, false>)
+        auto *k1 = scene ? preprocess_fwd_kernel<false, false, true>
+                 : cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true> : preprocess_fwd_kernel<true, false>)
                           : (cc.cov3D ? preprocess_fwd_kernel<false, true> : preprocess_fwd_kernel<>);
-        k1<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D, a.scales, a.rotations,
-                 a.rot_stride, a.opacities, a.opac_stride, g.depth, g.xy, g.conic_o, g.cov3d, g.tiles, g.rect, radii, iv.count, cc);
+        k1<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(scene ? d.P - scene->Ps : d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D,
+                 a.scales, a.rotations, a.rot_stride, a.opacities, a.opac_stride, g.depth, g.xy, g.conic_o, g.cov3d, g.tiles, g.rect, radii,
+                 iv.count, cc, scene ? *scene : SceneSet{});
         GA_CHECK_LAUNCH("preprocess_fwd_kernel");
     }
     {
@@ -1332,15 +1391,22 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
     return GA_OK;
 }
 
-// K3 + K4 + K6 for all frames.
+// K3 + K4 + K6 for all frames (a scene: the composite K4, d.P = P + Ps).
 int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacity, const GeomViews &g, const ImgViews &iv, const BinViews &bv,
-                              float *out_color, cudaStream_t stream)
+                              float *out_color, cudaStream_t stream, const SceneSet *scene = nullptr)
 {
     static PerDeviceOnce attr_set;
     if (attr_set.first()) {
         GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            kSortMax * (int)sizeof(uint64_t)));
+        GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           kSortMax * (int)sizeof(uint64_t)));
     }
+    const float *scene_rgb = scene ? scene->rgb : nullptr;
+    const int Pd = scene ? d.P - scene->Ps : d.P;
+    auto *sort_long = scene ? tile_sort_kernel<kSortThreads, kSortMax, true, true> : tile_sort_kernel<kSortThreads, kSortMax, true>;
+    auto *sort_short = scene ? tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, true>
+                             : tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false>;
     const int BT = d.B * d.T;
     if (d.P > 0) {
         {
@@ -1352,13 +1418,13 @@ int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacit
     }
     {
         ProfScope _ps("tile_sort_kernel", stream);
-        tile_sort_kernel<kSortThreads, kSortMax, true><<<min(BT, 3 * num_sms()), kSortThreads, kSortMax * sizeof(uint64_t), stream>>>(
+        sort_long<<<min(BT, 3 * num_sms()), kSortThreads, kSortMax * sizeof(uint64_t), stream>>>(
                  d.P, d.T, BT, iv.status, iv.order, iv.ranges, iv.seg_start, bv.bucket, g.xy, g.conic_o, a.colors, bv.point_list, bv.recA, bv.recB,
-                 bv.recC, bv.seg_tile, iv.tile_maxc);
+                 bv.recC, bv.seg_tile, iv.tile_maxc, scene_rgb, Pd);
         count_launch();
-        tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false><<<min(BT, 12 * num_sms()), kSortSmallThreads, kSortSmallMax * sizeof(uint64_t), stream>>>(
+        sort_short<<<min(BT, 12 * num_sms()), kSortSmallThreads, kSortSmallMax * sizeof(uint64_t), stream>>>(
                  d.P, d.T, BT, iv.status, iv.order, iv.ranges, iv.seg_start, bv.bucket, g.xy, g.conic_o, a.colors, bv.point_list, bv.recA, bv.recB,
-                 bv.recC, bv.seg_tile, iv.tile_maxc);
+                 bv.recC, bv.seg_tile, iv.tile_maxc, scene_rgb, Pd);
     }
     GA_CHECK_LAUNCH("tile_sort_kernel");
     {
@@ -1607,6 +1673,40 @@ extern "C" int ga_rasterb_forward(const GaRasterBatchDesc *bd, const float *cams
     const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
     if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
     return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream);
+}
+
+extern "C" int ga_rasterb_forward_scene(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const float *cams, const float *bg,
+                                        const float *means3D, const float *colors, const float *scales, const float *rotations,
+                                        const float *opacities, void *geom, void *img, void *binning, int32_t *radii, float *out_color,
+                                        void *stream_)
+{
+    if (int rc = check_batch(bd)) return rc;
+    GA_REQUIRE(scene != nullptr, "scene descriptor is NULL");
+    GA_REQUIRE(scene->Ps >= 0 && (long long)bd->P + scene->Ps <= 0x7fffffffll, "bad static count Ps=%d (P=%d)", (int)scene->Ps, (int)bd->P);
+    const int Pt = bd->P + scene->Ps;
+    if (int rc = check_dims(bd->B, Pt, bd->H, bd->W)) return rc;
+    GA_REQUIRE(cams && bg && img && binning && out_color, "NULL pointer argument");
+    GA_REQUIRE(bd->P == 0 || (means3D && colors && scales && rotations && opacities), "NULL pointer argument");
+    GA_REQUIRE(Pt == 0 || (geom && radii), "NULL pointer argument");
+    SceneSet sc{};
+    if (scene->Ps > 0) {
+        GA_REQUIRE(scene->means3D && scene->scales && scene->rotations && scene->opacities && scene->shs && scene->rgb,
+                   "NULL pointer in the scene descriptor");
+        GA_REQUIRE(scene->sh_degree >= 0 && scene->sh_degree <= 3, "scene sh_degree %d outside 0..3", (int)scene->sh_degree);
+        GA_REQUIRE(scene->sh_coeffs >= (scene->sh_degree + 1) * (scene->sh_degree + 1), "scene sh_coeffs %d < (sh_degree + 1)^2 = %d",
+                   (int)scene->sh_coeffs, (int)((scene->sh_degree + 1) * (scene->sh_degree + 1)));
+        sc = SceneSet{scene->means3D, scene->scales, scene->rotations, scene->opacities, scene->shs, scene->Ps, scene->sh_degree,
+                      scene->sh_coeffs, scene->sh_coeffs % 4 == 0 && reinterpret_cast<uintptr_t>(scene->shs) % 16 == 0, scene->rgb};
+    }
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const Dims d = make_dims(bd->B, Pt, bd->H, bd->W);
+    GeomViews g = carve_geom(geom, (size_t)d.B * d.P);
+    ImgViews iv = carve_img(img, d);
+    BinViews bv = carve_bin(binning, bd->capacity, d);
+    const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
+    const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
+    if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream, &sc)) return rc;
+    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, &sc);
 }
 
 extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,

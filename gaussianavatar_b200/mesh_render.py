@@ -56,7 +56,8 @@ def cameras(cams) -> torch.Tensor:
     """[B,40] camera block (ga_rasterb_* layout) of a list of `camera.Camera`."""
     view = torch.stack([c.world_view_transform.float().cpu() for c in cams])
     proj = torch.stack([c.full_proj_transform.float().cpu() for c in cams])
-    return pack_cameras(view, proj, [math.tan(c.FovX * 0.5) for c in cams], [math.tan(c.FovY * 0.5) for c in cams], "cpu")
+    center = torch.stack([c.camera_center.float().cpu() for c in cams])
+    return pack_cameras(view, proj, [math.tan(c.FovX * 0.5) for c in cams], [math.tan(c.FovY * 0.5) for c in cams], "cpu", campos=center)
 
 
 class MeshRenderer:

@@ -235,8 +235,9 @@ CAM_STRIDE = 40
 MAX_FRAMES_PER_CALL = 8          # ga_rasterb_*
 
 
-def pack_cameras(view, proj, tanfovx, tanfovy, device):
-    """[B,40] device floats: viewmatrix 0..15, projmatrix 16..31 (the reference's transposed 4x4s), tanfovx 32, tanfovy 33."""
+def pack_cameras(view, proj, tanfovx, tanfovy, device, campos=None):
+    """[B,40] device floats: viewmatrix 0..15, projmatrix 16..31 (the reference's transposed 4x4s), tanfovx 32, tanfovy 33 and,
+    when campos [B,3] is given, the camera centre 34..36 (upstream's `campos`, which the composite forward's SH colours need)."""
     B = view.shape[0]
     cams = torch.zeros(B, CAM_STRIDE, dtype=torch.float32, device=device)
     cams[:, 0:16] = view.reshape(B, 16).to(device=device, dtype=torch.float32)
@@ -246,6 +247,8 @@ def pack_cameras(view, proj, tanfovx, tanfovy, device):
         cams[:, 33] = tanfovy.to(device=device, dtype=torch.float32)
     else:
         cams[:, 32:34] = torch.tensor([list(map(float, tanfovx)), list(map(float, tanfovy))], dtype=torch.float32).t().to(device)
+    if campos is not None:
+        cams[:, 34:37] = torch.as_tensor(campos).reshape(B, 3).to(device=device, dtype=torch.float32)
     return cams
 
 
@@ -254,16 +257,22 @@ class RasterBatchPlan:
     scratch, reused every step.  `capacity` is the number of (Gaussian, tile) instances the binning buffer holds; the device
     raises status[1] when a step needs more (nothing is overrun) and `check()` then grows the buffer — the caller re-runs
     the step.  The status words of every forward are copied to pinned host memory asynchronously; reading them never
-    blocks the enqueueing thread unless asked to."""
+    blocks the enqueueing thread unless asked to.
 
-    def __init__(self, B, P, H, W, device, capacity=None):
+    static_P: the size of a static scene set the plan's forwards composite with (`rasterize_batch_scene`): geom and radii then
+    cover P + static_P Gaussians per frame, and `scene_rgb` [B,static_P,3] receives the scene's per-frame SH colours."""
+
+    def __init__(self, B, P, H, W, device, capacity=None, static_P=0):
         L = _lib.lib()
         self.B, self.P, self.H, self.W, self.device = int(B), int(P), int(H), int(W), device
-        self.capacity = int(capacity) if capacity else max(1 << 16, 6 * self.B * self.P)
-        self.geom = torch.empty(L.ga_rasterb_geom_bytes(self.B, self.P), dtype=torch.uint8, device=device)
+        self.static_P = int(static_P)
+        Pt = self.P + self.static_P
+        self.capacity = int(capacity) if capacity else max(1 << 16, 6 * self.B * Pt)
+        self.geom = torch.empty(L.ga_rasterb_geom_bytes(self.B, Pt), dtype=torch.uint8, device=device)
         self.img = torch.empty(L.ga_rasterb_img_bytes(self.B, self.H, self.W), dtype=torch.uint8, device=device)
         self.scratch = torch.empty(L.ga_rasterb_bwd_scratch_bytes(self.B, self.P), dtype=torch.uint8, device=device)
-        self.radii = torch.empty(self.B, self.P, dtype=torch.int32, device=device)
+        self.radii = torch.empty(self.B, Pt, dtype=torch.int32, device=device)
+        self.scene_rgb = torch.empty(self.B, self.static_P, 3, dtype=torch.float32, device=device) if self.static_P else None
         self.binning = None
         self._alloc_binning()
         off = L.ga_rasterb_status(self.B, self.H, self.W, ptr(self.img)) - self.img.data_ptr()
@@ -320,7 +329,7 @@ class RasterBatchPlan:
         self._alloc_binning()
 
     def views(self):
-        return _views(self.B, self.P, self.H, self.W, self.capacity, self.geom, self.binning, self.img, self.radii)
+        return _views(self.B, self.P + self.static_P, self.H, self.W, self.capacity, self.geom, self.binning, self.img, self.radii)
 
 
 class _RasterizeBatch(torch.autograd.Function):
@@ -360,6 +369,34 @@ class _RasterizeBatch(torch.autograd.Function):
 
 def rasterize_batch(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan):
     return _RasterizeBatch.apply(means3D, colors, scales, rotations, opacities, cams, bg, plan)
+
+
+def rasterize_batch_scene(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan, scene):
+    """`rasterize_batch`'s dynamic set splatted together with a static scene set in one sort per tile (correct occlusion both
+    ways); forward only, images [B,3,H,W].  scene: a `scene.GaussianScene` on the device (means3D, scales, rotations, opacities
+    [Ps], shs [Ps,M,3], sh_degree), with Ps = plan.static_P; cams rows must carry the camera centre (words 34..36).  Frame b's
+    index space is the dynamic P, then the scene's Ps (plan.radii [B,P+Ps]); the scene's colours land in plan.scene_rgb."""
+    if not means3D.is_cuda:
+        raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
+    if torch.is_grad_enabled() and any(t.requires_grad for t in (means3D, colors, scales, rotations, opacities, scene.means3D, scene.shs,
+                                                                  scene.scales, scene.rotations, scene.opacities)):
+        raise RuntimeError("rasterize_batch_scene is forward only: it has no backward (run it under torch.no_grad())")
+    Ps = int(scene.means3D.shape[0])
+    if Ps != plan.static_P:
+        raise ValueError(f"the scene has {Ps} Gaussians, the plan was sized for static_P={plan.static_P}")
+    _on_device(means3D.device, scene_means3D=scene.means3D, scene_shs=scene.shs, cams=cams)
+    L = _lib.lib()
+    means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
+    opacities = _c(opacities).reshape(-1)
+    d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
+    sc = _lib.GaRasterScene(Ps, int(scene.sh_degree), int(scene.shs.shape[1]), ptr(scene.means3D), ptr(scene.scales), ptr(scene.rotations),
+                            ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb))
+    out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=means3D.device)
+    _lib.check(L.ga_rasterb_forward_scene(ctypes.byref(d), ctypes.byref(sc), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales),
+                                          ptr(rotations), ptr(opacities), ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii),
+                                          ptr(out), _stream()), "ga_rasterb_forward_scene")
+    plan.record_status()
+    return out
 
 
 class _RasterizeGaussians(torch.autograd.Function):

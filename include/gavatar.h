@@ -119,7 +119,7 @@ int ga_raster_backward_ex(const GaRasterSettings *s, const GaRasterColorCov *cc,
  * and WITHOUT any host read-back, so a whole step can be captured in a CUDA graph.  All frames share H, W and P.
  * Arrays are [B,P,*] (rotations / opacities: [P,*] shared by every frame when the stride is 0); out_color [B,3,H,W];
  * radii [B,P]; cams [B,40] device floats per frame: viewmatrix 0..15, projmatrix 16..31 (the reference's transposed 4x4s),
- * tanfovx 32, tanfovy 33.  `capacity` = number of (Gaussian, tile) instances the caller sized `binning` for; if a step needs
+ * tanfovx 32, tanfovy 33, camera centre 34..36 (read by ga_rasterb_forward_scene only).  `capacity` = number of (Gaussian, tile) instances the caller sized `binning` for; if a step needs
  * more, status[1] is set, the tiles that do not fit are rendered as empty and nothing is overrun — the caller re-runs with a
  * larger buffer (status[0] = the count needed).  status (device, 16 x int32, inside `img`): [0] instances, [1] overflow,
  * [2] backward segments, [4+b] first instance of frame b, [4+B] = [0]. */
@@ -146,6 +146,30 @@ int ga_rasterb_backward(const GaRasterBatchDesc *d, const float *cams, const flo
                         const void *geom, const void *img, const void *binning, const float *dL_dout, void *scratch,
                         float *d_means3D, float *d_colors, float *d_scales, float *d_rotations, float *d_opacities,
                         float *d_means2D, void *stream);
+
+/* A static Gaussian set for ga_rasterb_forward_scene: a 3D Gaussian Splatting scene shared by every frame (read with frame stride
+ * 0, never copied per frame).  Its colours are spherical harmonics, evaluated for each frame's camera centre exactly as
+ * GaRasterColorCov's are: rgb = max(sum_k basis_k(dir) shs[k] + 0.5, 0), dir = (mean - campos) / |mean - campos|, 0 for Gaussians
+ * the frame culls.  Forward only: there is no backward of the composite. */
+typedef struct GaRasterScene {
+    int32_t Ps;                  /* static Gaussians (0: the composite renders the dynamic set alone)        */
+    int32_t sh_degree, sh_coeffs;/* active degree 0..3; coefficients per Gaussian >= (sh_degree + 1)^2     */
+    const float *means3D;        /* [Ps, 3]                                                                 */
+    const float *scales;         /* [Ps, 3] activated (times the descriptor's scale_modifier, as the dynamic set) */
+    const float *rotations;      /* [Ps, 4] (w, x, y, z), normalised                                        */
+    const float *opacities;      /* [Ps] activated                                                          */
+    const float *shs;            /* [Ps, sh_coeffs, 3]                                                      */
+    float *rgb;                  /* [B, Ps, 3] written: frame b's evaluated colours                         */
+} GaRasterScene;
+/* ga_rasterb_forward of the dynamic set (d->P, arrays and strides as there) splatted together with a static scene set in one sort
+ * per tile, so that each occludes the other correctly.  Frame b has P + Ps Gaussians, the dynamic P first, then the static set:
+ * that order fixes radii [B, P+Ps], geom (sized by ga_rasterb_geom_bytes(B, P + Ps)), ga_raster_views(B, P + Ps, ...) and
+ * upstream's tie order (depth bits, then index).  cams rows must carry the camera centre in words 34..36 (upstream's `campos`).
+ * Binning, the capacity / overflow status and compositing are ga_rasterb_forward's. */
+int ga_rasterb_forward_scene(const GaRasterBatchDesc *d, const GaRasterScene *scene, const float *cams, const float *bg,
+                             const float *means3D, const float *colors, const float *scales, const float *rotations,
+                             const float *opacities, void *geom, void *img, void *binning, int32_t *radii, float *out_color,
+                             void *stream);
 
 /* Debug / parity accessors into the opaque buffers (device pointers; valid after the forward that filled them).  B = 1 and
  * capacity = num_rendered for buffers of the per-frame API. */

@@ -10,6 +10,11 @@ DATA / MODEL are the reference's -s / -m folders; stage 1 loads net/iteration_N/
 (`stage2_load`).  --motion: an AMASS SMPL+H / SMPL-X .npz, or a smpl_parms.pth (its rate from --clip_fps).  Cameras: DATA/train's
 cam_parms.npz (--camera dataset) or its orbit around the clip's first pelvis (--camera orbit); --size W H scales the intrinsics.
 --png DIR writes DIR/{:05d}.png; --raw FILE (or - for stdout) writes the frames back to back as H x W x 3 (--rgba: 4) bytes.
+
+--scene PLY renders the avatar inside a 3D Gaussian Splatting scene (3DGS's point_cloud.ply), both splatted in one sort so that
+each occludes the other; --place S RX RY RZ TX TY TZ puts the avatar's world into the scene's (x_scene = S R x + T, R an
+axis-angle).  Dataset and orbit cameras are carried along with the avatar; --camera scene:K takes camera K of the cameras.json of
+the 3DGS model folder holding point_cloud/iteration_*/point_cloud.ply (or of --scene_cameras), at its own size unless --size.
 """
 import argparse
 import json
@@ -46,15 +51,31 @@ def main(argv=None):
     ap.add_argument("--fps", type=float, default=30.0, help="output frame rate")
     ap.add_argument("--speed", type=float, default=1.0)
     ap.add_argument("--align_to", type=int, default=None, help="map clip frame 0 onto this training frame")
-    ap.add_argument("--camera", choices=("dataset", "orbit"), default="dataset")
+    ap.add_argument("--camera", default="dataset", help="dataset | orbit | scene:K (camera K of the scene's cameras.json)")
+    ap.add_argument("--scene", default=None, help="a 3DGS point_cloud.ply to render the avatar in")
+    ap.add_argument("--place", type=float, nargs=7, metavar=("S", "RX", "RY", "RZ", "TX", "TY", "TZ"), default=None,
+                    help="the avatar in the scene: x_scene = S R x + T, R from the axis-angle (RX, RY, RZ)")
+    ap.add_argument("--scene_cameras", default=None, help="cameras.json for --camera scene:K (default: the 3DGS model folder's)")
     ap.add_argument("--size", type=int, nargs=2, metavar=("W", "H"), default=None)
-    ap.add_argument("--chunk", type=int, default=8)
+    ap.add_argument("--chunk", type=int, default=None, help="frames per rasterizer call (default 8, with --scene 2)")
     ap.add_argument("--rgba", action="store_true")
     ap.add_argument("--png", default=None)
     ap.add_argument("--raw", default=None)
     a = ap.parse_args(argv)
     if a.png is None and a.raw is None:
         ap.error("nothing to write: give --png DIR and / or --raw FILE")
+    scene_cam = None
+    if a.camera.startswith("scene:"):
+        if a.scene is None:
+            ap.error("--camera scene:K needs --scene")
+        try:
+            scene_cam = int(a.camera[len("scene:"):])
+        except ValueError:
+            ap.error(f"--camera {a.camera}: K must be an integer")
+    elif a.camera not in ("dataset", "orbit"):
+        ap.error(f"--camera {a.camera}: dataset, orbit or scene:K")
+    if a.place is not None and a.scene is None:
+        ap.error("--place needs --scene")
 
     model_dir = os.path.dirname(os.path.abspath(a.smpl_model)) if a.smpl_model else ""
     mp = ModelParams(source_path=a.source_path, model_path=a.model_path, project_path=a.project_path, smpl_model_path=model_dir,
@@ -82,8 +103,23 @@ def main(argv=None):
     K[1, :] *= H / H0
     cameras = camera_item(K, E, H, W) if a.camera == "dataset" else OrbitCamera(K, E)
 
+    scene = placement = None
+    if a.scene is not None:
+        from gaussianavatar_b200.scene import GaussianScene, Placement, load_scene_cameras, scene_cameras_path
+        scene = GaussianScene.load_ply(a.scene)
+        if a.place is not None:
+            placement = Placement.from_axis_angle(a.place[0], a.place[1:4], a.place[4:7])
+        if scene_cam is not None:
+            cams = load_scene_cameras(a.scene_cameras or scene_cameras_path(a.scene))
+            if not 0 <= scene_cam < len(cams):
+                ap.error(f"--camera scene:{scene_cam}: the scene has cameras 0..{len(cams) - 1}")
+            cameras = cams[scene_cam]
+            if not a.size:
+                W, H = cameras.width, cameras.height
+
     clip = MotionClip.load(a.motion, a.body, fps=a.clip_fps)
-    anim = Animator(model, cameras, H, W, chunk=a.chunk if a.stage == 1 else 1, channels=4 if a.rgba else 3, pose_mapper=pose_mapper)
+    anim = Animator(model, cameras, H, W, chunk=a.chunk if a.stage == 1 else 1, channels=4 if a.rgba else 3, pose_mapper=pose_mapper,
+                    scene=scene, placement=placement)
     if a.png:
         os.makedirs(a.png, exist_ok=True)
     raw = None if a.raw is None else (sys.stdout.buffer if a.raw == "-" else open(a.raw, "wb"))
