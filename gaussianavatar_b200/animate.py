@@ -31,12 +31,12 @@ import torch
 from . import _lib
 from ._lib import ptr
 from .avatar_model import kept_state
+from .body import body_of
 from .camera import Camera, make_camera
 from .dataset import _rodrigues, rotate_camera_by_frame_idx
 from .rasterizer import MAX_FRAMES_PER_CALL, RasterBatchPlan, rasterize_batch, rasterize_batch_scene
 from .scene import SceneCamera
 
-POSE_WIDTH = {"smpl": 72, "smplx": 165}
 SCENE_CHUNK = 2                 # the player's default chunk with a scene
 IDENTITY_ALIGN = np.array([1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0], np.float64)
 
@@ -99,8 +99,7 @@ class MotionClip:
         """A reference `smpl_parms.pth` (`body_pose` [T,72|165] and `trans`; fps must be given), an AMASS SMPL+H `.npz` (`poses`
         [T,156], `trans`, `mocap_framerate`) or an AMASS SMPL-X `.npz` (`poses` [T,165], `trans`, `mocap_frame_rate` or
         `mocap_framerate`).  `fps` overrides a file's rate.  The clip's betas are ignored: only rotations and translations transfer."""
-        if body not in POSE_WIDTH:
-            raise ValueError(f"body {body!r} is neither 'smpl' nor 'smplx'")
+        width = body_of(body).full_width
         path = os.fspath(path)
         if path.endswith(".npz"):
             with np.load(path, allow_pickle=False) as z:
@@ -127,8 +126,8 @@ class MotionClip:
                 if key not in d:
                     raise ValueError(f"{path}: no '{key}' entry")
             pose = np.asarray(torch.as_tensor(d["body_pose"]).double().numpy())
-            if pose.ndim != 2 or pose.shape[1] != POSE_WIDTH[body]:
-                raise ValueError(f"{path}: 'body_pose' {pose.shape}; expected [T,{POSE_WIDTH[body]}] for body={body!r}")
+            if pose.ndim != 2 or pose.shape[1] != width:
+                raise ValueError(f"{path}: 'body_pose' {pose.shape}; expected [T,{width}] for body={body!r}")
             trans = np.asarray(torch.as_tensor(d["trans"]).double().numpy())
         if pose.shape[0] < 1 or trans.shape != (pose.shape[0], 3):
             raise ValueError(f"{path}: 'trans' {trans.shape}; expected [{pose.shape[0]},3] (one row per pose, at least one)")
@@ -223,7 +222,7 @@ class Animator:
             raise TypeError("cameras: a camera_item dict, an OrbitCamera or a scene.SceneCamera")
         self.cameras = cameras
         self.stage = 2 if int(model.model_parms.train_stage) == 2 else 1
-        self.body = "smplx" if model.smplx else "smpl"
+        self.body = model.body
         self.pose_mapper = pose_mapper if pose_mapper is not None else getattr(model, "pose_mapper", None)
         if self.stage == 2 and self.pose_mapper is None:
             raise ValueError("stage 2 needs a pose_mapper (posmap.PoseMapper / SmplxPoseMapper) for the input position maps")
@@ -285,8 +284,8 @@ class Animator:
         return camera_block(rows)
 
     def _check_clip(self, clip):
-        if clip.body != self.body or clip.pose.shape[1] != POSE_WIDTH[self.body]:
-            raise ValueError(f"clip for body {clip.body!r} ({tuple(clip.pose.shape)}), the avatar is {self.body!r}")
+        if clip.body != self.body.name or clip.pose.shape[1] != self.body.full_width:
+            raise ValueError(f"clip for body {clip.body!r} ({tuple(clip.pose.shape)}), the avatar is {self.body.name!r}")
 
     @torch.no_grad()
     def sample(self, clip: MotionClip, sched: Schedule):
@@ -339,10 +338,6 @@ class Animator:
             self._status_host[slot].copy_(self._status_dev[slot], non_blocking=True)
             self._copied[slot].record(self._copy_stream)
 
-    def _split(self, pose):
-        """Sampled poses [n,72|165] -> (the pose columns the avatar was trained on, SMPL-X's rest_pose [n,99] or None)."""
-        return (pose[:, :66], pose[:, 66:]) if self.body == "smplx" else (pose, None)
-
     # ---- stage 1: one graph per (chunk size, slot) -------------------------------------------------------------------------------
     def _plan(self, b):
         if b not in self._plans:
@@ -386,7 +381,7 @@ class Animator:
         def body(b, slot):
             plan = self._plan(b)
             pose, trans = motion_sample(self._keys_pose[:T], self._keys_trans[:T], self._times_dev[:b], self._align)
-            pose, rest = self._split(pose)
+            pose, rest = self.body.split(pose)
             means, scales, colors = m._assemble(self._dec, pose, trans, rest, placement=self.placement)
             img = self._raster(means, scales, colors, self._cams_dev[:b], plan)
             frame_pack(img, final_transmittance(plan), m.background, self.channels, self._out_dev[slot][:b])
@@ -418,7 +413,7 @@ class Animator:
 
         def render(s, e, slot):
             for i in range(s, e):
-                p, rest = self._split(pose[i:i + 1])
+                p, rest = self.body.split(pose[i:i + 1])
                 means, scales, colors, _, _ = m._stage2_from_pose(self.pose_mapper, p, trans[i:i + 1], rest, placement=self.placement)
                 if self.scene is None:
                     batch = {"_cams": cams_all[i:i + 1], "height": [self.H], "width": [self.W]}

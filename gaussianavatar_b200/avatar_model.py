@@ -23,9 +23,10 @@ import numpy as np
 import torch
 import torch.nn as nn
 
+from .body import SMPLX, body_of, load_model
 from .config import ModelParams, NetworkParams, OptimizationParams
 from .network import POP_no_unet
-from .ops import LbsAssemble, SmplCano2Live, SmplxCano2Live
+from .ops import Cano2Live, LbsAssemble
 from .rasterizer import MAX_FRAMES_PER_CALL
 from .renderer import render_batch
 
@@ -56,9 +57,7 @@ class AvatarModel:
         if self.device.type != "cuda":
             raise RuntimeError("AvatarModel runs on CUDA only (no CPU fallback)")
         self.batch_size = model_parms.batch_size if train else 1      # avatar_model.py:31-34
-        assert model_parms.smpl_type in ["smplx", "smpl"]
-        self.smplx = model_parms.smpl_type == "smplx"
-        self.num_joints = 55 if self.smplx else 24
+        self.body = body_of(model_parms.smpl_type)
         if model_parms.train_stage not in (0, 1, 2):
             raise ValueError(f"train_stage {model_parms.train_stage} is not one of 1, 2")
         self.posmap_from_pose = model_parms.train_stage == 2 and bool(getattr(model_parms, "inp_posmap_from_pose", False))
@@ -81,12 +80,11 @@ class AvatarModel:
         rots = torch.zeros((N, 4), device=dev)
         rots[:, 0] = 1
         self.fix_rotation = rots
-        J = self.num_joints
+        J = self.body.joints
         lbs = _assets["query_lbs"].to(dev).float()
         if tuple(lbs.shape) != (N, J):
             raise ValueError(f"query_lbs {tuple(lbs.shape)}: expected [{N},{J}] for smpl_type={model_parms.smpl_type!r}")
-        if self.smplx:      # 220-byte rows -> 224: whole float4s for the LBS kernel's TMA copy and row reads (zero last column)
-            lbs = torch.nn.functional.pad(lbs, (0, 1))
+        lbs = torch.nn.functional.pad(lbs, (0, self.body.lbs_ld - J))                  # zero columns up to the LBS kernel's row width
         self._query_lbs = lbs.contiguous()                                              # [N,24] / [N,56], ONE copy for all frames
         self.query_lbs = self._query_lbs[None, :, :J].expand(self.batch_size, -1, -1)  # view only (reference materialises B copies, :86-87)
         cano = _assets["cano_joint_mats"].to(dev).float()
@@ -99,7 +97,7 @@ class AvatarModel:
 
         self.train_dataset = _FrameSet(_frames) if isinstance(_frames, list) else _frames
         num_training_frames = _pose_data.shape[0]
-        pose_dim = 66 if self.smplx else 72          # SMPL-X: global + 21 body joints are trained, the rest comes with the frame
+        pose_dim = self.body.pose_width                 # SMPL-X: global + 21 body joints are trained, the rest comes with the frame
         if _pose_data.shape[1] != pose_dim:
             raise ValueError(f"pose data {tuple(_pose_data.shape)}: expected [F,{pose_dim}] for smpl_type={model_parms.smpl_type!r}")
         self.pose = torch.nn.Embedding(num_training_frames, pose_dim, _weight=_pose_data.clone().float(), sparse=True).to(dev)
@@ -124,75 +122,46 @@ class AvatarModel:
     @classmethod
     def from_assets(cls, assets, frames, pose_data, transl_data, batch_size=2, train=True, opt_parms=None, device="cuda", net_parms=None,
                     **model_fields):
-        """assets: gaussianavatar_b200.synthetic.SyntheticAvatarAssets (or a dict with the same fields).  55 rest joints make an
-        SMPL-X model (its frames then carry `rest_pose`).  model_fields override ModelParams fields (e.g. train_stage=2,
+        """assets: gaussianavatar_b200.synthetic.SyntheticAvatarAssets (or a dict with the same fields; without `smpl_type` the body
+        is SMPL).  An SMPL-X model's frames carry `rest_pose`.  model_fields override ModelParams fields (e.g. train_stage=2,
         inp_posmap_size, inp_posmap_from_pose=True; the last needs the dict keys `smpl_mesh`, the SMPL_{GENDER}.pkl fields, and
         `uv_template`, a path or what posmap.load_uv_template_obj returns)."""
         if not isinstance(assets, dict):
             assets = dict(valid_idx=assets.valid_idx, query_points=assets.query_points, query_lbs=assets.query_lbs,
-                          cano_joint_mats=assets.cano_joint_mats, rest_joints=assets.rest_joints, betas=assets.body.betas[0], S=assets.S)
-        smpl_type = "smplx" if assets["rest_joints"].shape[0] == 55 else "smpl"
-        mp = ModelParams(batch_size=batch_size, query_posmap_size=int(assets["S"]), smpl_type=smpl_type, **model_fields)
+                          cano_joint_mats=assets.cano_joint_mats, rest_joints=assets.rest_joints, betas=assets.body.betas[0], S=assets.S,
+                          smpl_type=assets.smpl_type)
+        mp = ModelParams(batch_size=batch_size, query_posmap_size=int(assets["S"]), smpl_type=assets.get("smpl_type", "smpl"), **model_fields)
         return cls(mp, net_parms or NetworkParams(), opt_parms or OptimizationParams(), train=train, _assets=assets, _frames=frames,
                    _pose_data=pose_data, _transl_data=transl_data, device=device)
 
     def _load_reference_assets(self, mp, train):
         """Folder contract of the reference (model/avatar_model.py:41-98; scene/dataset_mono.py:83-160): the training dataset (always
         built, even for evaluation, avatar_model.py:41), the UV mask / canonical position map / LBS map / canonical joint
-        matrices, and the SMPL model pickle for the rest joints J(beta).  Exercised against a synthetic folder written in the
-        same layout (tests/test_dataset_cpu.py, tests/test_avatar_gpu.py)."""
+        matrices of the body (`uv_mask{S}_with_faceid_{body}.npy`, `query_posemap_{S}_cano_{body}.npz`, `lbs_map_{body}_{S}.npy`,
+        `{body}_cano_joint_mat.pth`), and the body-model file (SMPL_{GENDER}.pkl under smpl_model_path, SMPLX_{GENDER}.npz under
+        smplx_model_path) for the rest joints J(beta).  Exercised against a synthetic folder written in the same layout
+        (tests/test_dataset_cpu.py, tests/test_avatar_gpu.py)."""
         from .dataset import MonoDataset_train
         split = "train" if train else "test"
         dataset = MonoDataset_train(mp)
-        S = int(mp.query_posmap_size)
-        if mp.smpl_type == "smplx":
-            return self._load_reference_assets_smplx(mp, split, dataset, S)
-        mask = np.load(join(mp.project_path, "assets", "uv_masks", f"uv_mask{S}_with_faceid_smpl.npy")).reshape(S, S)
+        S, body = int(mp.query_posmap_size), self.body
+        n, J = body.name, body.joints
+        mask = np.load(join(mp.project_path, "assets", "uv_masks", f"uv_mask{S}_with_faceid_{n}.npy")).reshape(S, S)
         valid = torch.from_numpy(mask != -1).reshape(-1)
-        qmap = torch.from_numpy(np.load(join(mp.source_path, split, f"query_posemap_{S}_cano_smpl.npz"))[f"posmap{S}"]).reshape(-1, 3)
-        lbs = torch.from_numpy(np.load(join(mp.project_path, "assets", f"lbs_map_smpl_{S}.npy"))).reshape(S * S, 24)
-        cano = torch.load(join(mp.source_path, split, "smpl_cano_joint_mat.pth"), weights_only=False).reshape(24, 4, 4)
-        cano = torch.as_tensor(cano).float()
-        smpl_data = dataset.smpl_data
-        beta = torch.as_tensor(smpl_data["beta"][0]).float()
-        import pickle
-        with open(join(mp.smpl_model_path, f"SMPL_{mp.smpl_gender.upper()}.pkl"), "rb") as f:
-            sm = pickle.load(f, encoding="latin1")
-        v_t = torch.as_tensor(np.asarray(sm["v_template"])).double()
-        sd = torch.as_tensor(np.asarray(sm["shapedirs"])[:, :, :10]).double()
-        Jr = torch.as_tensor(np.asarray(sm["J_regressor"].todense() if hasattr(sm["J_regressor"], "todense") else sm["J_regressor"])).double()
-        rest = (Jr @ (v_t + torch.einsum("l,mkl->mk", beta.double(), sd))).float()
-        pose = dataset.pose_data.float()
-        transl = dataset.transl_data.float()
-        assets = dict(valid_idx=valid, query_points=qmap[valid].float(), query_lbs=lbs[valid].float(), cano_joint_mats=cano, rest_joints=rest,
-                      betas=beta, S=S)
+        qmap = torch.from_numpy(np.load(join(mp.source_path, split, f"query_posemap_{S}_cano_{n}.npz"))[f"posmap{S}"]).reshape(-1, 3)
+        lbs = torch.from_numpy(np.load(join(mp.project_path, "assets", f"lbs_map_{n}_{S}.npy"))).reshape(S * S, J)
+        cano = torch.as_tensor(torch.load(join(mp.source_path, split, f"{n}_cano_joint_mat.pth"), weights_only=False)).reshape(J, 4, 4).float()
+        beta = torch.as_tensor(dataset.smpl_data["beta"][0]).float()
+        model = load_model(join(getattr(mp, body.model_dir), body.model_file.format(gender=mp.smpl_gender.upper())))
+        assets = dict(valid_idx=valid, query_points=qmap[valid].float(), query_lbs=lbs[valid].float(), cano_joint_mats=cano,
+                      rest_joints=body.rest_joints(model, beta), betas=beta, S=S)
         if mp.train_stage == 2 and getattr(mp, "inp_posmap_from_pose", False):
-            # the mesh comes from the same SMPL_{GENDER}.pkl as the rest joints; the UV template from where the reference's scripts read it
-            from .posmap import SMPL_MESH_FIELDS
-            missing = [k for k in SMPL_MESH_FIELDS if k not in sm]
-            if missing:
-                raise ValueError(f"{f.name}: no {', '.join(missing)}; inp_posmap_from_pose needs the full SMPL mesh model")
-            template = join(mp.project_path, "assets", "template_mesh_smpl_uv.obj")
+            # the mesh comes from the same model file as the rest joints; the UV template from where the reference's scripts read it
+            body.check_model(model)
+            template = join(mp.project_path, "assets", f"template_mesh_{n}_uv.obj")
             if not os.path.exists(template):
                 raise FileNotFoundError(f"inp_posmap_from_pose: UV template {template} not found")
-            assets.update(smpl_mesh=sm, uv_template=template)
-        return assets, dataset, pose, transl
-
-    def _load_reference_assets_smplx(self, mp, split, dataset, S):
-        """The SMPL-X branch of the folder contract (model/avatar_model.py:45-53): `uv_mask{S}_with_faceid_smplx.npy`,
-        `query_posemap_{S}_cano_smplx.npz`, `lbs_map_smplx_{S}.npy` [S*S,55], `smplx_cano_joint_mat.pth` [55,4,4], and the rest joints
-        from `SMPLX_{GENDER}.npz` under smplx_model_path (the shape directions past the 10 betas are expression: the reference passes
-        none, so they drop out)."""
-        from .synthetic import SMPLX_PARENTS
-        mask = np.load(join(mp.project_path, "assets", "uv_masks", f"uv_mask{S}_with_faceid_smplx.npy")).reshape(S, S)
-        valid = torch.from_numpy(mask != -1).reshape(-1)
-        qmap = torch.from_numpy(np.load(join(mp.source_path, split, f"query_posemap_{S}_cano_smplx.npz"))[f"posmap{S}"]).reshape(-1, 3)
-        lbs = torch.from_numpy(np.load(join(mp.project_path, "assets", f"lbs_map_smplx_{S}.npy"))).reshape(S * S, 55)
-        cano = torch.as_tensor(torch.load(join(mp.source_path, split, "smplx_cano_joint_mat.pth"), weights_only=False)).reshape(55, 4, 4).float()
-        beta = torch.as_tensor(dataset.smpl_data["beta"][0]).float()
-        rest = smplx_rest_joints(join(mp.smplx_model_path, f"SMPLX_{mp.smpl_gender.upper()}.npz"), beta, SMPLX_PARENTS)
-        assets = dict(valid_idx=valid, query_points=qmap[valid].float(), query_lbs=lbs[valid].float(), cano_joint_mats=cano, rest_joints=rest,
-                      betas=beta, S=S)
+            assets.update(smpl_mesh=model, uv_template=template)
         return assets, dataset, dataset.pose_data.float(), dataset.transl_data.float()
 
     # ------------------------------------------------------------------------------------------------------------------
@@ -331,18 +300,13 @@ class AvatarModel:
             self.optimizer_pose.step()
 
     # ------------------------------------------------------------------------------------------------------------------
+    @property
+    def smplx(self) -> bool:
+        return self.body is SMPLX
+
     def _cano2live(self, pose_batch, transl_batch, rest_pose=None):
         """[B,J,12] for the body model: SMPL from pose [B,72]; SMPL-X from pose [B,66] and the frames' rest_pose [B,99]."""
-        if not self.smplx:
-            return SmplCano2Live.apply(pose_batch, transl_batch, self._rest_joints, self._inv_cano)
-        B = pose_batch.shape[0]
-        if rest_pose is None:
-            raise ValueError("smpl_type='smplx': the batch has no 'rest_pose' (jaw, eyes and hands, [B,99])")
-        rest_pose = torch.as_tensor(rest_pose)
-        if rest_pose.dim() != 2 or tuple(rest_pose.shape) != (B, 99):
-            raise ValueError(f"smpl_type='smplx': rest_pose {tuple(rest_pose.shape)}, expected [{B},99] (jaw, eyes, 2 x 15 finger joints)")
-        rest_pose = rest_pose.to(device=self.device, dtype=torch.float32)
-        return SmplxCano2Live.apply(pose_batch, rest_pose, transl_batch, self._rest_joints, self._inv_cano)
+        return Cano2Live.apply(self.body, pose_batch, rest_pose, transl_batch, self._rest_joints, self._inv_cano)
 
     def _assemble(self, dec, pose, transl, rest_pose=None, scale_mul=1.0, per_frame=False, placement=None):
         """Decoder output `dec` posed by pose / transl (and SMPL-X's rest_pose): cano2live, then the fused LBS / attribute assembly.
@@ -515,7 +479,7 @@ class AvatarModel:
         """`_stage2_gaussians` of explicit poses [B,72|66] / transl [B,3] (and SMPL-X's rest_pose [B,99]): the input position maps are
         built from the same pose by `mapper` (a posmap.PoseMapper / SmplxPoseMapper, differentiable in pose and transl).  placement
         moves the posed Gaussians into a scene (`_assemble`); the position maps stay in the body's own frame."""
-        inp = mapper(pose, rest_pose, transl) if self.smplx else mapper(pose, transl)
+        inp = mapper.maps(pose, rest_pose, transl)
         return self._stage2_gaussians({"inp_pos_map": inp, "rest_pose": rest_pose}, pose=pose, transl=transl, placement=placement)
 
     def _pose_map(self, batch_data):
@@ -586,18 +550,3 @@ def kept_state(model):
             for b, v in bufs:
                 b.copy_(v)
 
-
-def smplx_rest_joints(npz_path, beta, parents) -> torch.Tensor:
-    """Rest joints J = J_regressor (v_template + shapedirs[:, :, :10] beta) [55,3] of an SMPLX_{GENDER}.npz.  The file's
-    kintree_table must be the SMPL-X tree the joint-transform kernel is built for."""
-    sm = np.load(npz_path, allow_pickle=True)
-    kt = np.asarray(sm["kintree_table"]).astype(np.int64)[0].copy()
-    kt[0] = -1
-    if kt.shape != (len(parents),) or not np.array_equal(kt, np.asarray(parents)):
-        raise ValueError(f"{npz_path}: kintree_table[0] is not the 55-joint SMPL-X tree this library is built for")
-    beta = torch.as_tensor(beta).double().reshape(-1)
-    v_t = torch.as_tensor(np.asarray(sm["v_template"])).double()
-    sd = torch.as_tensor(np.asarray(sm["shapedirs"])[:, :, :beta.numel()]).double()
-    Jr = sm["J_regressor"]
-    Jr = torch.as_tensor(np.asarray(Jr.todense() if hasattr(Jr, "todense") else Jr)).double()
-    return (Jr @ (v_t + torch.einsum("l,mkl->mk", beta, sd))).float()

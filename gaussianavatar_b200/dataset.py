@@ -24,6 +24,7 @@ import numpy as np
 import torch
 from torch.utils.data import Dataset
 
+from .body import body_of
 from .camera import make_camera, projection_from_K
 
 
@@ -84,10 +85,7 @@ class _MonoFolder(Dataset):
         self._index_frames()
         pose, trans = _as_tensor(self.smpl_data["body_pose"]), _as_tensor(self.smpl_data["trans"])
         n = self.data_length
-        if dataset_parms.smpl_type == "smplx":
-            self.pose_data, self.rest_pose_data = pose[:n, :66], pose[:n, 66:]
-        else:
-            self.pose_data, self.rest_pose_data = pose[:n], None
+        self.pose_data, self.rest_pose_data = body_of(dataset_parms.smpl_type).split(pose[:n])
         self.transl_data = trans[:n, :]
         if dataset_parms.cam_static:
             cam = np.load(join(self.data_folder, "cam_parms.npz"))

@@ -26,63 +26,45 @@ def _f32c(t: torch.Tensor) -> torch.Tensor:
     return t.float().contiguous() if (t.dtype != torch.float32 or not t.is_contiguous()) else t
 
 
-class SmplCano2Live(torch.autograd.Function):
-    """pose [B,72], transl [B,3] -> cano2live [B,24,12] (3x4 per joint).
-    Reference: model/avatar_model.py:291-296 (SMPL.forward(...).A @ inv_mats)."""
+def _rows(t, device) -> torch.Tensor:
+    return torch.as_tensor(t).to(device=device, dtype=torch.float32).contiguous()
+
+
+class Cano2Live(torch.autograd.Function):
+    """body (`body.SMPL` / `body.SMPLX`), pose [B,72], rest_pose None, transl [B,3] -> cano2live [B,24,12] (3x4 per joint); SMPL-X:
+    pose [B,66] (global + 21 body joints), rest_pose [B,99] (jaw, eyes, 2 x 15 finger joints) -> [B,55,12].  Gradients flow to pose
+    and transl only: rest_pose is data.  Reference: model/avatar_model.py:279-296 (SMPL.forward(...).A @ inv_mats)."""
 
     @staticmethod
-    def forward(ctx, pose, transl, rest_joints, inv_cano):
-        _need_cuda(pose, "SmplCano2Live")
-        pose, transl = _f32c(pose), _f32c(transl)
+    def forward(ctx, body, pose, rest_pose, transl, rest_joints, inv_cano):
+        _need_cuda(pose, "Cano2Live")
         B = pose.shape[0]
-        C = torch.empty(B, 24, 12, device=pose.device, dtype=torch.float32)
-        G = torch.empty(B, 24, 12, device=pose.device, dtype=torch.float32)
-        _lib.check(_lib.lib().ga_smpl_forward(B, ptr(pose), ptr(transl), ptr(rest_joints), ptr(inv_cano), ptr(C), ptr(G), _stream()),
-                   "ga_smpl_forward")
-        ctx.save_for_backward(pose, rest_joints, inv_cano, G)
+        got = [None if t is None else tuple(t.shape) for t in (pose, rest_pose, transl)]
+        want = [(B, body.pose_width), (B, body.rest_width) if body.rest_width else None, (B, 3)]
+        if got != want:
+            raise ValueError(f"{body.label} cano2live: (pose, rest_pose, transl) {got}; expected {want}")
+        dev = pose.device
+        poses = [_rows(p, dev) for p in body.pose_args(pose, rest_pose)]
+        transl = _rows(transl, dev)
+        C = torch.empty(B, body.joints, 12, device=dev, dtype=torch.float32)
+        G = torch.empty(B, body.joints, 12, device=dev, dtype=torch.float32)
+        _lib.check(getattr(_lib.lib(), body.cano2live)(B, *(ptr(p) for p in poses), ptr(transl), ptr(rest_joints), ptr(inv_cano), ptr(C),
+                                                       ptr(G), _stream()), body.cano2live)
+        ctx.body = body
+        ctx.save_for_backward(*poses, rest_joints, inv_cano, G)
         return C
 
     @staticmethod
     def backward(ctx, dC):
-        pose, rest_joints, inv_cano, G = ctx.saved_tensors
-        B = pose.shape[0]
+        *poses, rest_joints, inv_cano, G = ctx.saved_tensors
+        body = ctx.body
+        B = poses[0].shape[0]
         dC = _f32c(dC)
-        d_pose = torch.empty_like(pose)
-        d_transl = torch.empty(B, 3, device=pose.device, dtype=torch.float32)
-        _lib.check(_lib.lib().ga_smpl_backward(B, ptr(pose), ptr(rest_joints), ptr(inv_cano), ptr(G), ptr(dC), ptr(d_pose),
-                                               ptr(d_transl), _stream()), "ga_smpl_backward")
-        return d_pose, d_transl, None, None
-
-
-class SmplxCano2Live(torch.autograd.Function):
-    """SMPL-X: pose [B,66] (global + 21 body joints), rest_pose [B,99] (jaw, eyes, 2 x 15 finger joints), transl [B,3]
-    -> cano2live [B,55,12].  Gradients flow to pose and transl only: rest_pose is data (model/avatar_model.py:279-296)."""
-
-    @staticmethod
-    def forward(ctx, pose, rest_pose, transl, rest_joints, inv_cano):
-        _need_cuda(pose, "SmplxCano2Live")
-        pose, rest_pose, transl = _f32c(pose), _f32c(rest_pose), _f32c(transl)
-        B = pose.shape[0]
-        if tuple(pose.shape) != (B, 66) or tuple(rest_pose.shape) != (B, 99) or tuple(transl.shape) != (B, 3):
-            raise ValueError(f"SmplxCano2Live: pose {tuple(pose.shape)}, rest_pose {tuple(rest_pose.shape)}, transl {tuple(transl.shape)}; "
-                             f"expected [B,66], [B,99], [B,3]")
-        C = torch.empty(B, 55, 12, device=pose.device, dtype=torch.float32)
-        G = torch.empty(B, 55, 12, device=pose.device, dtype=torch.float32)
-        _lib.check(_lib.lib().ga_smplx_forward(B, ptr(pose), ptr(rest_pose), ptr(transl), ptr(rest_joints), ptr(inv_cano), ptr(C), ptr(G),
-                                               _stream()), "ga_smplx_forward")
-        ctx.save_for_backward(pose, rest_pose, rest_joints, inv_cano, G)
-        return C
-
-    @staticmethod
-    def backward(ctx, dC):
-        pose, rest_pose, rest_joints, inv_cano, G = ctx.saved_tensors
-        B = pose.shape[0]
-        dC = _f32c(dC)
-        d_pose = torch.empty_like(pose)
-        d_transl = torch.empty(B, 3, device=pose.device, dtype=torch.float32)
-        _lib.check(_lib.lib().ga_smplx_backward(B, ptr(pose), ptr(rest_pose), ptr(rest_joints), ptr(inv_cano), ptr(G), ptr(dC),
-                                                ptr(d_pose), ptr(d_transl), _stream()), "ga_smplx_backward")
-        return d_pose, None, d_transl, None, None
+        d_pose = torch.empty_like(poses[0])
+        d_transl = torch.empty(B, 3, device=dC.device, dtype=torch.float32)
+        _lib.check(getattr(_lib.lib(), body.cano2live_bwd)(B, *(ptr(p) for p in poses), ptr(rest_joints), ptr(inv_cano), ptr(G), ptr(dC),
+                                                           ptr(d_pose), ptr(d_transl), _stream()), body.cano2live_bwd)
+        return None, d_pose, None, d_transl, None, None
 
 
 class LbsAssemble(torch.autograd.Function):

@@ -52,7 +52,7 @@ class PoseFitter:
         self.pose_mapper = pose_mapper if pose_mapper is not None else getattr(model, "pose_mapper", None)
         if self.stage == 2 and self.pose_mapper is None:
             raise ValueError("stage 2 needs a pose_mapper (posmap.PoseMapper / SmplxPoseMapper) for the input position maps")
-        self.width = 66 if model.smplx else 72
+        self.width = model.body.pose_width
         self.lam = float(model.opt_parms.lambda_dssim)
         self.dev = model.device
         self.overflows = 0         # chunks fitted again after a binning overflow
@@ -158,11 +158,13 @@ class PoseFitter:
         return torch.stack([torch.as_tensor(it["original_image"]).float() for it in items]).to(self.dev).contiguous()
 
     def _rest(self, items):
-        if not self.model.smplx:
+        """The frames' rest_pose [b,rest_width] on the device (None for SMPL)."""
+        body = self.model.body
+        if not body.rest_width:
             return None
         if any("rest_pose" not in it for it in items):
-            raise ValueError("smpl_type='smplx': every frame needs its 'rest_pose' (jaw, eyes and hands, [99])")
-        return torch.stack([torch.as_tensor(it["rest_pose"]).float().reshape(99) for it in items]).to(self.dev).contiguous()
+            raise ValueError(f"smpl_type={body.name!r}: every frame needs its 'rest_pose' (jaw, eyes and hands, [{body.rest_width}])")
+        return torch.stack([torch.as_tensor(it["rest_pose"]).float().reshape(body.rest_width) for it in items]).to(self.dev).contiguous()
 
     def _stage1_objective(self, items, dec):
         m = self.model

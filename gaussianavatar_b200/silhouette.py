@@ -168,7 +168,6 @@ class PoseRefiner:
         self.poser, self.renderer = poser, renderer
         self.iters, self.lr = int(iters), float(lr)
         self.lambda_smooth, self.lambda_prior = float(lambda_smooth), float(lambda_prior)
-        self.smplx = poser.POSE_WIDTH == 66
         self.dev = poser.device
         self._mesh = None
         b1, b2 = BETAS
@@ -176,18 +175,6 @@ class PoseRefiner:
         hyper = torch.stack([torch.full_like(k, self.lr), torch.full_like(k, b1), torch.full_like(k, b2), torch.full_like(k, EPS),
                              1.0 - b1 ** k, torch.sqrt(1.0 - b2 ** k), torch.ones_like(k)], 1)
         self._hyper = hyper.float().to(self.dev).contiguous()
-
-    def _split(self, pose):
-        """pose [F,72] (SMPL) or [F,165] (SMPL-X: pose 66 | rest_pose 99) -> (pose, rest_pose or None)."""
-        width = 165 if self.smplx else 72
-        pose = torch.as_tensor(pose).to(device=self.dev, dtype=torch.float32)
-        if pose.dim() != 2 or pose.shape[1] != width:
-            raise ValueError(f"pose {tuple(pose.shape)}: expected [F,{width}]")
-        return (pose[:, :66].contiguous(), pose[:, 66:].contiguous()) if self.smplx else (pose.contiguous(), None)
-
-    def _vertices(self, p, rest, transl):
-        poses = (p, rest) if self.smplx else (p,)
-        return self.poser._vertices(tuple(x.contiguous() for x in poses), transl.contiguous())
 
     def _quadratic(self, theta, theta0):
         """(value, gradient) of the smoothness and prior terms."""
@@ -199,12 +186,16 @@ class PoseRefiner:
         g[:-1] -= 2.0 * self.lambda_smooth * d
         return val, g
 
+    def _chunk(self, theta, rest, s, e):
+        """(pose, rest_pose, transl) of frames s..e-1, from theta = [pose | transl] and the rest poses (None for SMPL)."""
+        W = self.poser.body.pose_width
+        return theta[s:e, :W].contiguous(), None if rest is None else rest[s:e], theta[s:e, W:].contiguous()
+
     def _losses(self, theta, rest, cams, masks):
-        W = self.poser.POSE_WIDTH
         out = []
         for s in range(0, theta.shape[0], MAX_FRAMES_PER_CALL):
             e = min(theta.shape[0], s + MAX_FRAMES_PER_CALL)
-            verts = self._vertices(theta[s:e, :W], None if rest is None else rest[s:e], theta[s:e, W:])
+            verts = self.poser.posed(*self._chunk(theta, rest, s, e))
             out.append(self.renderer.losses(verts, cams[s:e], masks[s:e]))
         return torch.cat(out)
 
@@ -212,11 +203,11 @@ class PoseRefiner:
         """Each frame's hard IoU: ga_mesh_render coverage against mask >= 128 (tools/body_overlay.py --iou's rule)."""
         if self._mesh is None:
             self._mesh = MeshRenderer(self.poser.faces, self.poser.V, device=self.dev)
-        W, (H, Wd) = self.poser.POSE_WIDTH, masks.shape[-2:]
+        H, Wd = masks.shape[-2:]
         ious = []
         for s in range(0, theta.shape[0], MAX_FRAMES_PER_CALL):
             e = min(theta.shape[0], s + MAX_FRAMES_PER_CALL)
-            verts = self._vertices(theta[s:e, :W], None if rest is None else rest[s:e], theta[s:e, W:])
+            verts = self.poser.posed(*self._chunk(theta, rest, s, e))
             _, face_id, _ = self._mesh.render(verts, cams[s:e], H, Wd)
             ious += [coverage_iou(face_id[i] >= 0, masks[s + i] >= 128) for i in range(e - s)]
         return ious
@@ -225,7 +216,7 @@ class PoseRefiner:
         """pose [F,72] / [F,165], transl [F,3], cam: one camera block [40] (or [F,40]), masks [F,H,W] uint8 (>= 128: subject).
         Returns (pose, transl, report) on the host, pose as wide as given (SMPL-X's rest pose unchanged); report holds the objective
         and each frame's IoU before and after."""
-        p, rest = self._split(pose)
+        p, rest = self.poser.body.split(torch.as_tensor(pose).to(device=self.dev, dtype=torch.float32))
         transl = torch.as_tensor(transl).to(device=self.dev, dtype=torch.float32).reshape(-1, 3)
         n = p.shape[0]
         if transl.shape[0] != n:
@@ -236,7 +227,7 @@ class PoseRefiner:
         masks = masks.contiguous()
         cams = torch.as_tensor(cam).to(device=self.dev, dtype=torch.float32)
         cams = (cams.reshape(1, CAM_STRIDE).expand(n, CAM_STRIDE) if cams.numel() == CAM_STRIDE else cams.reshape(n, CAM_STRIDE)).contiguous()
-        W = self.poser.POSE_WIDTH
+        W = self.poser.body.pose_width
         theta0 = torch.cat([p, transl], 1).contiguous()
         theta = theta0.clone()
 
@@ -253,8 +244,8 @@ class PoseRefiner:
             for k in range(self.iters):
                 for s in range(0, n, MAX_FRAMES_PER_CALL):
                     e = min(n, s + MAX_FRAMES_PER_CALL)
-                    tp, r = theta[s:e, :W].contiguous(), None if rest is None else rest[s:e]
-                    verts = self._vertices(tp, r, theta[s:e, W:])
+                    tp, r, tt = self._chunk(theta, rest, s, e)
+                    verts = self.poser.posed(tp, r, tt)
                     d_verts = self.renderer.verts_grad(verts, cams[s:e], masks[s:e], ones[:e - s])
                     d_pose, d_transl = vertices_backward(self.poser, tp, r, d_verts)
                     grad[s:e, :W] = d_pose
@@ -263,7 +254,7 @@ class PoseRefiner:
                 _lib.check(L.ga_adam_step_dev(theta.numel(), ptr(theta), ptr(grad), ptr(exp_avg), ptr(exp_avg_sq), ptr(self._hyper[k]),
                                               None, stream), "ga_adam_step_dev")
         after, iou_after = objective(theta), self._ious(theta, rest, cams, masks)
-        out_pose = theta[:, :W] if rest is None else torch.cat([theta[:, :W], rest], 1)
+        out_pose = self.poser.body.join(theta[:, :W], rest)
         report = dict(objective_before=before, objective_after=after, iou_before=iou_before, iou_after=iou_after,
                       mean_iou_before=float(np.mean(iou_before)), mean_iou_after=float(np.mean(iou_after)))
         return out_pose.cpu(), theta[:, W:].cpu(), report

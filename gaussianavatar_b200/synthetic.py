@@ -25,7 +25,8 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-SMPL_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21]
+from .body import SMPL_PARENTS, SMPLX_PARENTS
+
 NUM_JOINTS = 24
 NUM_VERTS = 6890
 
@@ -42,10 +43,7 @@ _REST_JOINTS = np.array([
 _BONE_RADIUS = np.array([0.12, 0.10, 0.10, 0.13, 0.075, 0.075, 0.14, 0.05, 0.05, 0.14, 0.04, 0.04,
                          0.06, 0.08, 0.08, 0.095, 0.06, 0.06, 0.045, 0.045, 0.035, 0.035, 0.03, 0.03], dtype=np.float64)
 
-# ---- SMPL-X: joint order global, 21 body, jaw, left eye, right eye, 15 left-hand, 15 right-hand (index, middle, pinky, ring,
-# thumb; three segments each), kintree_table[0] of SMPLX_*.npz
-SMPLX_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 15, 15, 15, 20, 25, 26, 20, 28, 29, 20,
-                 31, 32, 20, 34, 35, 20, 37, 38, 21, 40, 41, 21, 43, 44, 21, 46, 47, 21, 49, 50, 21, 52, 53]
+# ---- SMPL-X
 SMPLX_NUM_JOINTS = 55
 SMPLX_NUM_VERTS = 10475      # the reference's vertex-joint selector indexes SMPL-X vertex ids
 
@@ -240,13 +238,14 @@ class SyntheticAvatarAssets:
     query_lbs: torch.Tensor      # [N,24] (SMPL-X: [N,55])
     cano_joint_mats: torch.Tensor  # [24,4,4] A_cano  (smpl_cano_joint_mat.pth; SMPL-X: [55,4,4])
     rest_joints: torch.Tensor    # [24,3] (SMPL-X: [55,3])
+    smpl_type: str = "smpl"      # the body: "smpl" or "smplx"
 
 
 def make_avatar_assets(N: int, S: int, seed: int = 0, body: str = "smpl") -> SyntheticAvatarAssets:
     """body: "smpl" (24 joints) or "smplx" (55 joints, canonical pose = the star pose with zero hand / face pose)."""
     assert N <= S * S and body in _SKELETON
     joints, parents, radius = _SKELETON[body]
-    smplx = body == "smplx"
+    smpl_type, smplx = body, body == "smplx"
     body = make_smplx_body(seed) if smplx else make_body(seed)
     g = torch.Generator().manual_seed(2000 + seed)
     pts, _ = _sample_on_capsules(N, g, joints, parents, radius)
@@ -259,7 +258,7 @@ def make_avatar_assets(N: int, S: int, seed: int = 0, body: str = "smpl") -> Syn
     valid = torch.zeros(S * S, dtype=torch.bool)
     valid[torch.randperm(S * S, generator=g)[:N]] = True
     return SyntheticAvatarAssets(body, S, N, valid, cano.float().contiguous(), W.float().contiguous(),
-                                 torch.tensor(A_cano).float(), torch.tensor(J).float())
+                                 torch.tensor(A_cano).float(), torch.tensor(J).float(), smpl_type)
 
 
 # BASELINE.json configs -> (N, S, image side)   (BASELINE.md §4)

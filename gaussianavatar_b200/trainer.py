@@ -246,7 +246,7 @@ class Stage1Trainer:
                   width=m._scalar_list(batch["width"], B))
         # SMPL-X: the frames' hand / face pose is a step input like pose_idx; a replay must read this step's, not the captured one's
         G.rest = None
-        if getattr(m, "smplx", False) and batch.get("rest_pose") is not None:
+        if batch.get("rest_pose") is not None:
             G.rest = torch.as_tensor(batch["rest_pose"]).to(device=dev, dtype=torch.float32).contiguous().clone()
             sb["rest_pose"] = G.rest
         m._detach_pose = True

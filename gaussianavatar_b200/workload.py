@@ -11,6 +11,7 @@ import torch
 
 from . import synthetic as syn
 from .avatar_model import AvatarModel
+from .body import body_of
 from .camera import TEST_POSE_EXTRINSIC, TEST_POSE_K, make_camera, scaled_intrinsics
 from .config import OptimizationParams
 
@@ -38,10 +39,9 @@ class Stage1Workload:
         assets = syn.make_avatar_assets(self.N, self.S, seed=seed, body=body)
         pose, transl, self.pose_source = load_poses(num_frames)
         self.num_frames = pose.shape[0]
-        self.rest_dev = None
-        if body == "smplx":
-            pose = pose[:, :66].contiguous()
-            self.rest_dev = syn.synthetic_smplx_poses(self.num_frames, seed=seed)[1].to(self.device)
+        b = body_of(body)
+        pose = pose[:, :b.pose_width].contiguous()
+        self.rest_dev = syn.synthetic_smplx_poses(self.num_frames, seed=seed)[1].to(self.device) if b.rest_width else None
         cam = make_camera(scaled_intrinsics(TEST_POSE_K, self.side), TEST_POSE_EXTRINSIC, self.side, self.side)
         self.cam = cam
         frames = [dict(pose_idx=i) for i in range(self.num_frames)]

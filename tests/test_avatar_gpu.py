@@ -19,16 +19,17 @@ def _rel(a, b):
 
 
 # ---------------------------------------------------------------------------------------------------------------- SMPL
-def test_smpl_cano2live_matches_reference_fixture_and_autograd():
+def test_cano2live_smpl_matches_reference_fixture_and_autograd():
     from gaussianavatar_b200 import synthetic as syn
-    from gaussianavatar_b200.ops import SmplCano2Live
+    from gaussianavatar_b200.body import SMPL
+    from gaussianavatar_b200.ops import Cano2Live
     d = np.load(os.path.join(GOLD, "smpl_A.npz"))
     a = syn.make_avatar_assets(100, 16, seed=0)
     J = torch.tensor(d["rest_joints"])
     inv_cano = torch.linalg.inv(a.cano_joint_mats)
     pose = torch.tensor(d["pose"], device=DEV, requires_grad=True)
     transl = torch.tensor(d["transl"], device=DEV, requires_grad=True)
-    C = SmplCano2Live.apply(pose, transl, J.to(DEV), inv_cano.to(DEV).contiguous())
+    C = Cano2Live.apply(SMPL, pose, None, transl, J.to(DEV), inv_cano.to(DEV).contiguous())
     # fixture: A straight from the reference's lbs(); cano2live = A @ inv(A_cano)  (avatar_model.py:296)
     ref = torch.matmul(torch.tensor(d["A"]), inv_cano[None])[:, :, :3, :].reshape(-1, 24, 12)
     assert (C.detach().cpu() - ref).abs().max() < 5e-6

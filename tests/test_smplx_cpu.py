@@ -24,21 +24,21 @@ def test_parent_tables_agree_with_the_reference_model():
     assert all(p < j for j, p in enumerate(syn.SMPLX_PARENTS))          # index order is a valid walk of the chain
 
 
-def test_loader_rest_joints_match_the_reference(tmp_path):
-    from gaussianavatar_b200.avatar_model import smplx_rest_joints
+def test_body_rest_joints_match_the_reference(tmp_path):
+    from gaussianavatar_b200.body import SMPLX, load_model
     d = np.load(os.path.join(GOLD, "smplx_A.npz"))
     body = syn.make_smplx_body(int(d["body_seed"]))
     assert np.array_equal(body.betas[0].numpy(), d["betas"])
     path = str(tmp_path / "SMPLX_NEUTRAL.npz")
     syn.write_smplx_model_npz(path, body, seed=0)
-    J = smplx_rest_joints(path, torch.tensor(d["betas"]), syn.SMPLX_PARENTS)
+    J = SMPLX.rest_joints(load_model(path), torch.tensor(d["betas"]))
     assert J.shape == (55, 3)
     np.testing.assert_allclose(J.numpy(), d["rest_joints"], rtol=0, atol=2e-6)
     np.testing.assert_allclose(body.rest_joints().numpy(), d["rest_joints"], rtol=0, atol=2e-6)
 
 
-def test_wrong_kintree_table_raises(tmp_path):
-    from gaussianavatar_b200.avatar_model import smplx_rest_joints
+def test_body_rejects_a_wrong_kintree_table(tmp_path):
+    from gaussianavatar_b200.body import SMPLX, load_model
     body = syn.make_smplx_body(0)
     path = str(tmp_path / "SMPLX_NEUTRAL.npz")
     syn.write_smplx_model_npz(path, body, seed=0)
@@ -48,7 +48,7 @@ def test_wrong_kintree_table_raises(tmp_path):
     bad = str(tmp_path / "bad.npz")
     np.savez(bad, **m)
     with pytest.raises(ValueError, match="kintree_table"):
-        smplx_rest_joints(bad, body.betas[0], syn.SMPLX_PARENTS)
+        SMPLX.rest_joints(load_model(bad), body.betas[0])
 
 
 def test_oracle_with_smplx_parents_reproduces_the_reference_A():

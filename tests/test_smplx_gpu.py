@@ -27,9 +27,10 @@ def _oracle_C(J, pose66, rest99, transl, inv_cano):
 
 
 # ------------------------------------------------------------------------------------------------------ joint transforms
-def test_smplx_cano2live_matches_reference_fixture_and_autograd():
+def test_cano2live_smplx_matches_reference_fixture_and_autograd():
     from gaussianavatar_b200 import synthetic as syn
-    from gaussianavatar_b200.ops import SmplxCano2Live
+    from gaussianavatar_b200.body import SMPLX
+    from gaussianavatar_b200.ops import Cano2Live
     d = np.load(os.path.join(GOLD, "smplx_A.npz"))
     a = syn.make_avatar_assets(100, 16, seed=0, body="smplx")
     J = torch.tensor(d["rest_joints"])
@@ -37,7 +38,7 @@ def test_smplx_cano2live_matches_reference_fixture_and_autograd():
     pose = torch.tensor(d["pose66"], device=DEV, requires_grad=True)
     rest = torch.tensor(d["rest99"], device=DEV)
     transl = torch.tensor(d["transl"], device=DEV, requires_grad=True)
-    C = SmplxCano2Live.apply(pose, rest, transl, J.to(DEV), inv_cano.to(DEV).contiguous())
+    C = Cano2Live.apply(SMPLX, pose, rest, transl, J.to(DEV), inv_cano.to(DEV).contiguous())
     assert C.shape == (pose.shape[0], 55, 12)
     ref = torch.matmul(torch.tensor(d["A"]), inv_cano[None])[:, :, :3, :].reshape(-1, 55, 12)
     assert (C.detach().cpu() - ref).abs().max() < 5e-6
@@ -52,13 +53,14 @@ def test_smplx_cano2live_matches_reference_fixture_and_autograd():
     assert _rel(transl.grad.cpu(), t64.grad) < 1e-5
 
 
-def test_smplx_cano2live_rejects_bad_shapes():
-    from gaussianavatar_b200.ops import SmplxCano2Live
+def test_cano2live_rejects_bad_smplx_shapes():
+    from gaussianavatar_b200.body import SMPLX
+    from gaussianavatar_b200.ops import Cano2Live
     z = lambda *s: torch.zeros(*s, device=DEV)
     with pytest.raises(ValueError, match="rest_pose"):
-        SmplxCano2Live.apply(z(2, 66), z(2, 6), z(2, 3), z(55, 3), z(55, 4, 4))
+        Cano2Live.apply(SMPLX, z(2, 66), z(2, 6), z(2, 3), z(55, 3), z(55, 4, 4))
     with pytest.raises(ValueError, match="pose"):
-        SmplxCano2Live.apply(z(2, 72), z(2, 99), z(2, 3), z(55, 3), z(55, 4, 4))
+        Cano2Live.apply(SMPLX, z(2, 72), z(2, 99), z(2, 3), z(55, 3), z(55, 4, 4))
 
 
 # ------------------------------------------------------------------------------------------------------------------ LBS

@@ -1110,18 +1110,17 @@ def test_joint_transforms(body, kind, B):
 
 
 @pytest.mark.parametrize("body", ["smpl", "smplx"])
-def test_joint_transforms_through_wrapper(body):
-    """SmplCano2Live / SmplxCano2Live forward and backward at B = 8 random poses, within the same bounds."""
-    from gaussianavatar_b200.ops import SmplCano2Live, SmplxCano2Live
+def test_joint_transforms_through_cano2live(body):
+    """Cano2Live forward and backward at B = 8 random poses of either body, within the same bounds."""
+    from gaussianavatar_b200.body import body_of
+    from gaussianavatar_b200.ops import Cano2Live
     cs = BodyCase(body, "random", 8, seed=31)
     gen = torch.Generator(device=DEV).manual_seed(3)
     B, J, kT = cs.B, cs.J, cs.kT
     pose = cs.full[:, :3 * kT].clone().requires_grad_(True)
     tr = cs.transl.clone().requires_grad_(True)
-    if body == "smpl":
-        C = SmplCano2Live.apply(pose, tr, cs.Jr, cs.inv)
-    else:
-        C = SmplxCano2Live.apply(pose, cs.full[:, 66:].contiguous(), tr, cs.Jr, cs.inv)
+    b = body_of(body)
+    C = Cano2Live.apply(b, pose, b.split(cs.full)[1], tr, cs.Jr, cs.inv)
     dC = torch.randn(B, J, 12, device=DEV, generator=gen)
     (C * dC).sum().backward()
     torch.cuda.synchronize()

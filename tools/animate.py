@@ -89,9 +89,10 @@ def main(argv=None):
         model.stage2_load(a.epoch)
         if not (a.smpl_model and a.uv_template):
             ap.error("--stage 2 needs --smpl_model and --uv_template for the input position maps")
-        from gaussianavatar_b200.posmap import PoseMapper, SmplxPoseMapper, load_body_model
-        mapper_cls = SmplxPoseMapper if a.body == "smplx" else PoseMapper
-        pose_mapper = mapper_cls(load_body_model(a.smpl_model), model.betas[0], a.uv_template, a.inp_posmap_size, device=model.device)
+        from gaussianavatar_b200.body import load_model
+        from gaussianavatar_b200.posmap import PoseMapper
+        pose_mapper = PoseMapper(load_model(a.smpl_model), model.betas[0], a.uv_template, a.inp_posmap_size, device=model.device,
+                                 body=model.body)
 
     cam = np.load(os.path.join(a.source_path, "train", "cam_parms.npz"))
     K, E = np.array(cam["intrinsic"], np.float32).reshape(3, 3), np.asarray(cam["extrinsic"], np.float64)

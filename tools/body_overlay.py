@@ -21,9 +21,10 @@ import torch
 from PIL import Image
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from gaussianavatar_b200.body import body_of, load_model  # noqa: E402
 from gaussianavatar_b200.camera import make_camera  # noqa: E402
 from gaussianavatar_b200.mesh_render import COLORS, MAX_FRAMES_PER_CALL, MeshRenderer, cameras, coverage_iou  # noqa: E402
-from gaussianavatar_b200.posmap import BodyPoser, SmplxBodyPoser, load_body_model  # noqa: E402
+from gaussianavatar_b200.posmap import BodyPoser  # noqa: E402
 
 
 def main(argv=None):
@@ -38,11 +39,11 @@ def main(argv=None):
     a = ap.parse_args(argv)
     params = a.params or ("smpl_parms_pred.pth" if os.path.exists(os.path.join(a.folder, "smpl_parms_pred.pth")) else "smpl_parms.pth")
     prm = torch.load(os.path.join(a.folder, params), map_location="cpu", weights_only=False)
+    body = body_of(a.body)
     pose = torch.as_tensor(prm["body_pose"]).float()
     transl = torch.as_tensor(prm["trans"]).float()
     beta = torch.as_tensor(prm["beta"]).float().reshape(-1, 10)[0]
-    model = load_body_model(a.smpl_model)
-    poser = (SmplxBodyPoser if a.body == "smplx" else BodyPoser)(model, beta)
+    poser = BodyPoser(load_model(a.smpl_model), beta, body=body)
     renderer = MeshRenderer(poser.faces, poser.V, device=poser.device, color=a.color)
     cam_npz = np.load(os.path.join(a.folder, "cam_parms.npz"))
     K, extr = np.asarray(cam_npz["intrinsic"]).reshape(3, 3), np.asarray(cam_npz["extrinsic"])
@@ -54,10 +55,7 @@ def main(argv=None):
     ious = []
     for s in range(0, len(names), MAX_FRAMES_PER_CALL):
         chunk = names[s:s + MAX_FRAMES_PER_CALL]
-        if a.body == "smplx":
-            verts = poser.vertices(pose[s:s + len(chunk), :66], pose[s:s + len(chunk), 66:], transl[s:s + len(chunk)])
-        else:
-            verts = poser.vertices(pose[s:s + len(chunk)], transl[s:s + len(chunk)])
+        verts = poser.posed(*body.split(pose[s:s + len(chunk)]), transl[s:s + len(chunk)])
         images = [np.array(Image.open(os.path.join(a.folder, "images", n)).convert("RGB")) for n in chunk]
         sizes = {im.shape[:2] for im in images}
         # frames of one size go to the device together

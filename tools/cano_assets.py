@@ -28,7 +28,8 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from gaussianavatar_b200.posmap import canonical_assets, load_body_model  # noqa: E402
+from gaussianavatar_b200.body import load_model  # noqa: E402
+from gaussianavatar_b200.posmap import canonical_assets  # noqa: E402
 
 
 def output_paths(folder, assets, body, S):
@@ -62,7 +63,7 @@ def main(argv=None):
         if not os.path.exists(path):
             ap.error(f"{path} not found")
     beta = torch.as_tensor(torch.load(os.path.join(a.folder, "smpl_parms.pth"), weights_only=False)["beta"]).float().reshape(-1, 10)[0]
-    res = canonical_assets(load_body_model(a.model), beta, a.uv_template, S, body=a.body)
+    res = canonical_assets(load_model(a.model), beta, a.uv_template, S, body=a.body)
     got = dict(posmap=res.posmap.cpu().numpy(), joint_mats=res.joint_mats[None].cpu().numpy(), face_id=res.face_id.cpu().numpy(),
                lbs_map=res.lbs_map.cpu().numpy(), bary=res.bary.cpu().numpy())
     paths = output_paths(a.folder, a.assets, a.body, S)

@@ -16,6 +16,9 @@ import sys
 
 import torch
 
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from gaussianavatar_b200.body import body_of  # noqa: E402
+
 
 def export(ckpt_dir, folder, body="smpl"):
     saved = torch.load(os.path.join(ckpt_dir, "net.pth"), map_location="cpu", weights_only=False)
@@ -24,7 +27,7 @@ def export(ckpt_dir, folder, body="smpl"):
     smpl = torch.load(os.path.join(folder, "smpl_parms.pth"), map_location="cpu", weights_only=False)
     bp = torch.as_tensor(smpl["body_pose"]).clone()
     tr = torch.as_tensor(smpl["trans"]).clone()
-    width = 72 if body == "smpl" else 66
+    width = body_of(body).pose_width
     F = pose.shape[0]
     if pose.dim() != 2 or pose.shape[1] != width or tuple(transl.shape) != (F, 3):
         raise ValueError(f"checkpoint pose {tuple(pose.shape)} / transl {tuple(transl.shape)}: expected [F,{width}] / [F,3] for {body}")

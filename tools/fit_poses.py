@@ -92,9 +92,10 @@ def main(argv=None):
         model.load(a.epoch)
     else:
         model.stage2_load(a.epoch)
-        from gaussianavatar_b200.posmap import PoseMapper, SmplxPoseMapper, load_body_model
-        mapper_cls = SmplxPoseMapper if a.body == "smplx" else PoseMapper
-        pose_mapper = mapper_cls(load_body_model(a.smpl_model), model.betas[0], a.uv_template, a.inp_posmap_size, device=model.device)
+        from gaussianavatar_b200.body import load_model
+        from gaussianavatar_b200.posmap import PoseMapper
+        pose_mapper = PoseMapper(load_model(a.smpl_model), model.betas[0], a.uv_template, a.inp_posmap_size, device=model.device,
+                                 body=model.body)
 
     # the maps come from the pose being fitted: the dataset need not read inp_map/
     dmp = ModelParams(**{**vars(mp), "inp_posmap_from_pose": True})

@@ -18,14 +18,14 @@ texels whose face id differs.
 import argparse
 import json
 import os
-import pickle
 import sys
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from gaussianavatar_b200.posmap import PoseMapper, SmplxPoseMapper, load_body_model  # noqa: E402
+from gaussianavatar_b200.body import body_of, load_model  # noqa: E402
+from gaussianavatar_b200.posmap import PoseMapper  # noqa: E402
 
 CHUNK = 64      # frames per device call
 
@@ -44,25 +44,17 @@ def main(argv=None):
     S = a.size
     params = a.params or ("smpl_parms_pred.pth" if os.path.exists(os.path.join(a.folder, "smpl_parms_pred.pth")) else "smpl_parms.pth")
     smpl_data = torch.load(os.path.join(a.folder, params), weights_only=False)
+    body = body_of(a.body)
     pose = torch.as_tensor(smpl_data["body_pose"]).float()
     transl = torch.as_tensor(smpl_data["trans"]).float()
     beta = torch.as_tensor(smpl_data["beta"]).float().reshape(-1, 10)[0]
-    if a.body == "smplx":
-        mapper = SmplxPoseMapper(load_body_model(a.smpl_model), beta, a.uv_template, S)
-        pose, rest_pose = pose[:, :66], pose[:, 66:]
-    else:
-        with open(a.smpl_model, "rb") as fh:
-            sm = pickle.load(fh, encoding="latin1")
-        mapper = PoseMapper(sm, beta, a.uv_template, S)
+    mapper = PoseMapper(load_model(a.smpl_model), beta, a.uv_template, S, body=body)
     out_dir = os.path.join(a.folder, "inp_map")
     if not a.check:
         os.makedirs(out_dir, exist_ok=True)
     max_err, n_missing = 0.0, 0
     for s in range(0, pose.shape[0], CHUNK):
-        if a.body == "smplx":
-            maps = mapper(pose[s:s + CHUNK], rest_pose[s:s + CHUNK], transl[s:s + CHUNK])
-        else:
-            maps = mapper(pose[s:s + CHUNK], transl[s:s + CHUNK])
+        maps = mapper.maps(*body.split(pose[s:s + CHUNK]), transl[s:s + CHUNK])
         maps = maps.permute(0, 2, 3, 1).cpu().numpy()      # [b,S,S,3]
         for i, m in enumerate(maps):
             fn = os.path.join(out_dir, "inp_posemap_%s_%s.npz" % (S, str(s + i).zfill(8)))

@@ -61,12 +61,13 @@ def refine(a, names, poses, theta):
     """Refined theta [N,72] and transl [N,3] and the report of `PoseRefiner`."""
     from gaussianavatar_b200.camera import make_camera
     from gaussianavatar_b200.mesh_render import cameras
-    from gaussianavatar_b200.posmap import BodyPoser, load_body_model
+    from gaussianavatar_b200.body import load_model
+    from gaussianavatar_b200.posmap import BodyPoser
     from gaussianavatar_b200.silhouette import PoseRefiner, SilhouetteRenderer
     cam = np.load(os.path.join(a.capture, "cameras.npz"))
     masks = np.stack([read_mask(os.path.join(a.capture, "masks", n)) for n in names])
     H, W = masks.shape[1:]
-    poser = BodyPoser(load_body_model(a.smpl_model), torch.from_numpy(np.asarray(poses["betas"], np.float32).reshape(-1)[:10].copy()))
+    poser = BodyPoser(load_model(a.smpl_model), torch.from_numpy(np.asarray(poses["betas"], np.float32).reshape(-1)[:10].copy()))
     renderer = SilhouetteRenderer(poser.faces, poser.V, sigma=a.sigma, device=poser.device)
     refiner = PoseRefiner(poser, renderer, iters=a.iters, lr=a.lr, lambda_smooth=a.lambda_smooth, lambda_prior=a.lambda_prior)
     K, extr = np.asarray(cam["intrinsic"]).reshape(3, 3), np.asarray(cam["extrinsic"])
