@@ -56,7 +56,9 @@ class GaDecoderLayout(ctypes.Structure):
 
 
 class GaDecoderViews(ctypes.Structure):
-    _fields_ = [(n, c_vp) for n in ("conv3_nhwc", "feat", "y1", "y5", "bn_mean", "bn_rstd", "d_feat")]
+    _fields_ = [("F", c_vp * 4), ("wr", c_vp), ("dF", c_vp * 2), ("Fp", c_vp), ("dFp", c_vp), ("feat", c_vp), ("d_feat", c_vp),
+                ("Y", c_vp * 5), ("Y6", c_vp), ("Y7", c_vp), ("dZa", c_vp), ("dZb", c_vp), ("dZ6", c_vp), ("dZ7", c_vp),
+                ("stat", c_vp), ("coef", c_vp)]
 
 
 class GaLpipsViews(ctypes.Structure):

@@ -946,19 +946,21 @@ extern "C" int ga_decoder_backward(const GaDecoderDesc *d, const float *params, 
     return GA_OK;
 }
 
-// Parity accessor: copies of internal activations / statistics (device pointers into the workspace).
+// Addresses of every workspace buffer (device pointers; nothing is copied and the device is not touched).
 extern "C" int ga_decoder_views(const GaDecoderDesc *d, void *workspace, GaDecoderViews *out)
 {
     if (int rc = check_desc(d)) return rc;
     GA_REQUIRE(workspace && out, "NULL pointer argument");
     const Workspace w = carve_ws(workspace, d->S, d->feat_res, d->frames ? d->frames : 1);
-    const Coef cf = coef_views(w);
-    out->conv3_nhwc = w.F[3];
-    out->feat = w.feat;
-    out->y1 = w.Y[0];
-    out->y5 = w.Y[4];
-    out->bn_mean = cf.mean;
-    out->bn_rstd = cf.rstd;
-    out->d_feat = w.d_feat;
+    for (int i = 0; i < 4; ++i) out->F[i] = w.F[i];
+    out->wr = w.wr;
+    for (int i = 0; i < 2; ++i) out->dF[i] = w.dF[i];
+    out->Fp = w.Fp; out->dFp = w.dFp;
+    out->feat = w.feat; out->d_feat = w.d_feat;
+    for (int i = 0; i < 5; ++i) out->Y[i] = w.Y[i];
+    out->Y6 = w.Y6; out->Y7 = w.Y7;
+    out->dZa = w.dZa; out->dZb = w.dZb; out->dZ6 = w.dZ6; out->dZ7 = w.dZ7;
+    out->stat = w.stat;
+    out->coef = w.coef;
     return GA_OK;
 }

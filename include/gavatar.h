@@ -324,8 +324,19 @@ typedef struct GaDecoderLayout {
     int64_t w8, b8, total;
     int32_t bn_channels, bn_offset[7];
 } GaDecoderLayout;
+/* Every buffer of the decoder workspace (device pointers; ga_decoder_views only computes addresses).  P = feat_res^2,
+ * M = frames * S * S rows, frames 0 counted as 1.  Fp / dFp hold [frames][P,64] only when frames > 1 (4 floats otherwise). */
 typedef struct GaDecoderViews {
-    const float *conv3_nhwc, *feat, *y1, *y5, *bn_mean, *bn_rstd, *d_feat;
+    const float *F[4];              /* [P,64] NHWC: geo, conv1, conv2, conv3 (tensor-core path: F[0..2] TF32-rounded) */
+    const float *wr;                /* [3][25*64*64] TF32-rounded conv weights (tensor-core path only) */
+    const float *dF[2];             /* [P,64] ping-pong conv gradients */
+    const float *Fp, *dFp;          /* [frames][P,64] stage-2 per-frame input maps and their gradients */
+    const float *feat, *d_feat;     /* [M,72] [up-sampled features | u | v | 0 x 6] and its gradient */
+    const float *Y[5], *Y6, *Y7;    /* [M,128] pre-BN outputs of layers 1-5; [M,384] of layers 6 and 7 (heads xyz, N, SH) */
+    const float *dZa, *dZb;         /* [M,128] ping-pong pre-BN gradients of layers 5..1 */
+    const float *dZ6, *dZ7;         /* [M,384] */
+    const double *stat;             /* [4][1408]: sum, sumsq (forward), s1, s2 (backward) per BatchNorm channel */
+    const float *coef;              /* [7][1408]: mean, rstd, a, b (forward), ga, m1, m2 (backward) */
 } GaDecoderViews;
 int ga_decoder_layout(const GaDecoderDesc *d, GaDecoderLayout *out);
 size_t ga_decoder_workspace_bytes(const GaDecoderDesc *d);
