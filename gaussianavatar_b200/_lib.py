@@ -38,6 +38,10 @@ class GaRasterScene(ctypes.Structure):
                 ("rotations", c_vp), ("opacities", c_vp), ("shs", c_vp), ("rgb", c_vp)]
 
 
+class GaRasterSets(ctypes.Structure):
+    _fields_ = [("K", ctypes.c_int32), ("first", ctypes.c_int32 * 9), ("mattes", c_vp)]
+
+
 class GaRasterViews(ctypes.Structure):
     _fields_ = [(n, c_vp) for n in ("depth", "xy", "conic_opacity", "cov3d", "tiles_touched", "rect", "point_list", "ranges",
                                     "tile_count", "final_T", "n_contrib", "status")]
@@ -132,6 +136,8 @@ _SIGNATURES = {
     "ga_rasterb_forward": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc)] + [c_vp] * 13),
     "ga_rasterb_backward": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc)] + [c_vp] * 19),
     "ga_rasterb_forward_scene": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc), ctypes.POINTER(GaRasterScene)] + [c_vp] * 13),
+    "ga_rasterb_forward_mattes": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc), ctypes.POINTER(GaRasterScene), ctypes.POINTER(GaRasterSets)]
+                                  + [c_vp] * 13),
     "ga_tc_conv5x5": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, c_vp, c_vp, c_vp, ctypes.c_int32, c_vp]),
     "ga_round_tf32": (ctypes.c_int, [c_vp, c_vp, ctypes.c_int64, c_vp]),
     "ga_lpips_weights_floats": (ctypes.c_size_t, []),
@@ -145,6 +151,7 @@ _SIGNATURES = {
     "ga_mesh_render": (ctypes.c_int, [ctypes.c_int32] * 5 + [c_vp] * 5 + [ctypes.c_float] * 3 + [c_vp] * 6),
     "ga_motion_sample": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 2 + [ctypes.c_int32] + [c_vp] * 5),
     "ga_frame_pack": (ctypes.c_int, [ctypes.c_int32] * 4 + [c_vp] * 5),
+    "ga_matte_pack": (ctypes.c_int, [ctypes.c_int64] + [c_vp] * 3),
     "ga_silhouette_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 5),
     "ga_silhouette_forward": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float] + [c_vp] * 8),
     "ga_silhouette_backward": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float] + [c_vp] * 10),

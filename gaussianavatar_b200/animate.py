@@ -18,9 +18,19 @@ and BatchNorm statistics are left exactly as they were.
 
 With a scene (`scene.GaussianScene`) both stages render through the composite forward instead, which splats the avatar and the
 scene in one sort per tile; a `scene.Placement` moves the avatar (and the cameras given around it) into the scene.
+
+Several avatars play together through `Ensemble`, of which `Animator` is the one-actor case:
+
+    cast = [Actor(model_a, walk), Actor(model_b, dance, placement=Placement.from_axis_angle(1, [0, 0, 0], [0.8, 0, 0]))]
+    for first, frames, mattes in Ensemble(cast, cameras, 1080, 1920, mattes=True).frames(fps_out=30):   # mattes: uint8 [b,K,H,W]
+        ...
+
+Their Gaussians are concatenated into one dynamic set and splatted together (and with the scene), so they occlude each other;
+with `mattes` each actor's visible matte comes from the same compositing pass (`rasterizer.rasterize_batch_mattes`).
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import os
 from dataclasses import dataclass
@@ -34,7 +44,7 @@ from .avatar_model import kept_state
 from .body import body_of
 from .camera import Camera, make_camera
 from .dataset import _rodrigues, rotate_camera_by_frame_idx
-from .rasterizer import MAX_FRAMES_PER_CALL, RasterBatchPlan, rasterize_batch, rasterize_batch_scene
+from .rasterizer import MAX_FRAMES_PER_CALL, MAX_SETS, RasterBatchPlan, rasterize_batch, rasterize_batch_mattes, rasterize_batch_scene
 from .scene import SceneCamera
 
 SCENE_CHUNK = 2                 # the player's default chunk with a scene
@@ -67,6 +77,14 @@ def frame_pack(images, final_T=None, bg=None, channels=3, out=None):
     if out is None:
         out = torch.empty(B, H, W, channels, dtype=torch.uint8, device=images.device)
     _lib.check(_lib.lib().ga_frame_pack(B, H, W, int(channels), ptr(images), ptr(final_T), ptr(bg), ptr(out), _stream()), "ga_frame_pack")
+    return out
+
+
+def matte_pack(mattes, out=None):
+    """ga_matte_pack on the current stream: mattes [B,K,H,W] fp32 -> uint8 [B,K,H,W] (ga_frame_pack's quantisation)."""
+    if out is None:
+        out = torch.empty(mattes.shape, dtype=torch.uint8, device=mattes.device)
+    _lib.check(_lib.lib().ga_matte_pack(mattes.numel(), ptr(mattes), ptr(out), _stream()), "ga_matte_pack")
     return out
 
 
@@ -185,22 +203,53 @@ class Schedule:
     cams: torch.Tensor       # [n,40] camera block (host fp32)
 
 
+
+
+def cast_times(num_keys, fps_clip, speeds, fps_out: float) -> np.ndarray:
+    """Fractional key indices [K, n] of K clips played together: actor k samples tau = min(j speed_k fps_k / fps_out, T_k - 1), so a
+    shorter clip holds its last pose, and the playback lasts as long as the longest (n = the most `sample_times` frames)."""
+    steps = [float(v) * float(f) / float(fps_out) for v, f in zip(speeds, fps_clip)]
+    n = max(len(sample_times(T, f, fps_out, v)) for T, f, v in zip(num_keys, fps_clip, speeds))
+    j = np.arange(n, dtype=np.float64)
+    return np.stack([np.minimum(j * st, float(T - 1)) for T, st in zip(num_keys, steps)])
+
+
+@dataclass
+class Actor:
+    """One avatar of an `Ensemble`: an inference `AvatarModel` (stage 1 or 2) driven by `clip` (of the model's body) at `speed`,
+    clip frame 0 mapped onto training frame `align_to` (None: the clip as it is), and `placement` (a `scene.Placement`, None =
+    identity) mapping the avatar's world into the shared one.  pose_mapper: stage 2's position mapper (default: the model's own)."""
+    model: object
+    clip: MotionClip | None
+    placement: object = None
+    align_to: int | None = None
+    speed: float = 1.0
+    pose_mapper: object = None
+
+
 # ---- the player -------------------------------------------------------------------------------------------------------------------
-class Animator:
-    """Renders an inference `AvatarModel` (stage 1 or 2) along motion clips.
+class Ensemble:
+    """Renders up to 8 actors (`Actor`) together, each along its own clip, splatted in one sort per tile so that each hides the
+    others (and the scene) where it is in front.
 
-    cameras: a `dataset.camera_item` dict (one camera for every frame), an `OrbitCamera`, or with a scene a `scene.SceneCamera` (one of
-    the scene's own cameras, in the scene's world).  H, W: frame size.  chunk: frames per
-    rasterizer call (1..8; default 8, with a scene SCENE_CHUNK).  channels: 3 (RGB) or 4 (straight-alpha RGBA).  pose_mapper: stage 2's `posmap.PoseMapper` /
-    `SmplxPoseMapper` (default: the model's own).  capacity: initial binning capacity of the rasterizer (instances); it grows on
-    overflow.  graphs: replay CUDA graphs in stage 1 (False runs the same launches eagerly, e.g. for per-kernel profiling).
-    scene: a `scene.GaussianScene` the avatar is rendered in, splatted together with it (`rasterize_batch_scene`) so that either
-    hides the other; placement: the `scene.Placement` of the avatar's world in it.  The cameras are given in the avatar's world
-    and carried into the scene through the placement; alpha (channels=4) is 1 - final transmittance over both sets."""
+    cameras: a `dataset.camera_item` dict (one camera for every frame), an `OrbitCamera` (around actor 0's aligned frame-0 pelvis),
+    or with a scene a `scene.SceneCamera` (in the scene's world, used as it is).  Dict and orbit cameras are given in actor 0's world
+    and carried through actor 0's placement, so the shared world is the scene's with a scene and otherwise actor 0's.  H, W: frame
+    size.  chunk: frames per rasterizer call (1..8; default 8, with a scene SCENE_CHUNK).  channels: 3 (RGB) or 4 (straight-alpha
+    RGBA, alpha = 1 - final transmittance over everything splatted).  mattes: also return each actor's visibility matte, the weight
+    its Gaussians added to each pixel (`rasterize_batch_mattes`), as bytes.  capacity: initial binning capacity of the rasterizer
+    (instances); it grows on overflow.  graphs: replay CUDA graphs when every actor is in stage 1 (False runs the same launches
+    eagerly).  scene: a `scene.GaussianScene` the actors are rendered in.
 
-    def __init__(self, model, cameras, H: int, W: int, chunk: int | None = None, channels: int = 3, pose_mapper=None,
-                 capacity=None, graphs: bool = True, scene=None, placement=None):
-        self.model = model
+    With every actor in stage 1 each distinct model's decoder is evaluated once and one CUDA graph per (chunk size, output slot)
+    replays sample -> cano2live -> LBS per actor, their concatenation, the rasterizer and the packing.  Any stage-2 actor makes the
+    player render eagerly, one frame per rasterizer call.  Every model's parameters and BatchNorm statistics are left as they were."""
+
+    def __init__(self, actors, cameras, H: int, W: int, chunk: int | None = None, channels: int = 3, mattes: bool = False,
+                 capacity=None, graphs: bool = True, scene=None):
+        self.actors = list(actors)
+        if not 1 <= len(self.actors) <= MAX_SETS:
+            raise ValueError(f"{len(self.actors)} actors: 1..{MAX_SETS}")
         self.H, self.W = int(H), int(W)
         if not (1 <= self.H <= 16384 and 1 <= self.W <= 16384):
             raise ValueError(f"frame {self.H} x {self.W} outside [1, 16384]^2")
@@ -221,28 +270,45 @@ class Animator:
         elif not isinstance(cameras, OrbitCamera):
             raise TypeError("cameras: a camera_item dict, an OrbitCamera or a scene.SceneCamera")
         self.cameras = cameras
-        self.stage = 2 if int(model.model_parms.train_stage) == 2 else 1
-        self.body = model.body
-        self.pose_mapper = pose_mapper if pose_mapper is not None else getattr(model, "pose_mapper", None)
-        if self.stage == 2 and self.pose_mapper is None:
-            raise ValueError("stage 2 needs a pose_mapper (posmap.PoseMapper / SmplxPoseMapper) for the input position maps")
-        self.dev = model.device
+        m0 = self.actors[0].model
+        self.dev = m0.device
+        self._stages, self._mappers = [], []
+        for k, a in enumerate(self.actors):
+            if a.clip is not None:
+                self._check_clip(a.model, a.clip, k)
+            if not torch.equal(a.model.background.to(self.dev), m0.background):
+                raise ValueError(f"actor {k}'s background {a.model.background.tolist()} differs from actor 0's {m0.background.tolist()}")
+            stage = 2 if int(a.model.model_parms.train_stage) == 2 else 1
+            mapper = a.pose_mapper if a.pose_mapper is not None else getattr(a.model, "pose_mapper", None)
+            if stage == 2 and mapper is None:
+                raise ValueError("stage 2 needs a pose_mapper (posmap.PoseMapper / SmplxPoseMapper) for the input position maps")
+            self._stages.append(stage)
+            self._mappers.append(mapper)
+        self._models = list({id(a.model): a.model for a in self.actors}.values())
+        sizes = [int(a.model._query_points.shape[0]) for a in self.actors]
+        self.first = [0] + np.cumsum(sizes).tolist()          # actor k's Gaussians in the concatenated dynamic set
+        one = len(self.actors) == 1                             # rotations / opacities shared by every frame, concatenated
+        self._rot = m0.fix_rotation if one else torch.cat([a.model.fix_rotation for a in self.actors])
+        self._opac = m0.fix_opacity if one else torch.cat([a.model.fix_opacity for a in self.actors])
+        self.mattes = bool(mattes)
         self.scene = None if scene is None else scene.to(self.dev)
-        self.placement = placement
         self.capacity = capacity
         self.use_graphs = bool(graphs)
         self.captures = 0          # CUDA graphs captured
         self.recaptures = 0        # ... of them because a chunk overflowed the binning buffer
         self.overflows = 0         # chunks rendered again after an overflow
         self._plans, self._graphs, self._clip_key = {}, {}, None
-        C, dev = self.channels, self.dev
+        C, K, dev = self.channels, len(self.actors), self.dev
         self._out_dev = [torch.empty(MAX_FRAMES_PER_CALL, self.H, self.W, C, dtype=torch.uint8, device=dev) for _ in range(2)]
         self._out_host = [torch.empty(MAX_FRAMES_PER_CALL, self.H, self.W, C, dtype=torch.uint8).pin_memory() for _ in range(2)]
-        self._status_dev = [torch.zeros(16, dtype=torch.int32, device=dev) for _ in range(2)]      # stage 2 leaves them at 0
+        if self.mattes:
+            self._mattes_dev = [torch.empty(MAX_FRAMES_PER_CALL, K, self.H, self.W, dtype=torch.uint8, device=dev) for _ in range(2)]
+            self._mattes_host = [torch.empty(MAX_FRAMES_PER_CALL, K, self.H, self.W, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self._status_dev = [torch.zeros(16, dtype=torch.int32, device=dev) for _ in range(2)]      # eager rendering leaves them at 0
         self._status_host = [torch.zeros(16, dtype=torch.int32).pin_memory() for _ in range(2)]
-        self._keys_pose = self._keys_trans = self._dec = None
-        self._align = torch.zeros(12, dtype=torch.float64, device=dev)
-        self._times_dev = torch.zeros(MAX_FRAMES_PER_CALL, dtype=torch.float64, device=dev)
+        self._keys_pose, self._keys_trans = [None] * K, [None] * K
+        self._align = [torch.zeros(12, dtype=torch.float64, device=dev) for _ in range(K)]
+        self._times_dev = [torch.zeros(MAX_FRAMES_PER_CALL, dtype=torch.float64, device=dev) for _ in range(K)]
         self._cams_dev = torch.zeros(MAX_FRAMES_PER_CALL, 40, dtype=torch.float32, device=dev)
         self._copy_stream = torch.cuda.Stream(device=dev)
         self._rendered = [torch.cuda.Event() for _ in range(2)]
@@ -250,26 +316,28 @@ class Animator:
         self._slot_used = [False, False]
 
     # ---- host-side schedule ------------------------------------------------------------------------------------------------------
-    def schedule(self, clip: MotionClip, fps_out: float, speed: float = 1.0, align_to=None) -> Schedule:
-        """Sample times, alignment and camera rows of a playback (all built on the host in fp64, cameras narrowed to fp32)."""
-        self._check_clip(clip)
-        times = sample_times(clip.num_keys, clip.fps, fps_out, speed)
+    @staticmethod
+    def _check_clip(model, clip, k=0):
+        if clip.body != model.body.name or clip.pose.shape[1] != model.body.full_width:
+            who = "the avatar" if k == 0 else f"actor {k}'s avatar"
+            raise ValueError(f"clip for body {clip.body!r} ({tuple(clip.pose.shape)}), {who} is {model.body.name!r}")
+
+    @staticmethod
+    def _alignment(model, clip, align_to):
         if align_to is None:
-            align = IDENTITY_ALIGN.copy()
-        else:
-            k = int(align_to)
-            F = int(self.model.pose.weight.shape[0])
-            if not 0 <= k < F:
-                raise ValueError(f"align_to {k}: the model has training frames 0..{F - 1}")
-            align = alignment(clip.pose[0, :3].double().numpy(), clip.trans[0].double().numpy(),
-                              self.model.pose.weight[k, :3].detach().double().cpu().numpy(),
-                              self.model.transl.weight[k].detach().double().cpu().numpy())
-        return Schedule(times, align, self._camera_rows(len(times), clip, align))
+            return IDENTITY_ALIGN.copy()
+        k = int(align_to)
+        F = int(model.pose.weight.shape[0])
+        if not 0 <= k < F:
+            raise ValueError(f"align_to {k}: the model has training frames 0..{F - 1}")
+        return alignment(clip.pose[0, :3].double().numpy(), clip.trans[0].double().numpy(),
+                         model.pose.weight[k, :3].detach().double().cpu().numpy(), model.transl.weight[k].detach().double().cpu().numpy())
 
     def _camera_rows(self, n, clip, align):
+        """[n,40] camera rows (host fp32): dict and orbit cameras from actor 0 (its clip, alignment and placement)."""
         from .mesh_render import cameras as camera_block
-        cam = self.cameras
-        place = (lambda c: c) if self.placement is None else self.placement.carry
+        cam, a0 = self.cameras, self.actors[0]
+        place = (lambda c: c) if a0.placement is None else a0.placement.carry
         if isinstance(cam, SceneCamera):                  # already in the scene's world
             return camera_block([cam.camera(self.H, self.W)]).expand(n, -1).contiguous()
         if isinstance(cam, dict):
@@ -278,32 +346,38 @@ class Animator:
             return camera_block([place(one)]).expand(n, -1).contiguous()
         R, c = align[:9].reshape(3, 3), align[9:]
         t0 = R @ clip.trans[0].double().numpy() + c
-        pelvis = self.model._rest_joints[0].double().cpu().numpy() + t0        # the root rotates about the rest pelvis
+        pelvis = a0.model._rest_joints[0].double().cpu().numpy() + t0        # the root rotates about the rest pelvis
         rows = [place(make_camera(cam.K, rotate_camera_by_frame_idx(cam.extrinsic, k, trans=pelvis, rotate_axis=cam.rotate_axis, period=n,
                                                                    inv_angle=cam.inv_angle), self.H, self.W)) for k in range(n)]
         return camera_block(rows)
 
-    def _check_clip(self, clip):
-        if clip.body != self.body.name or clip.pose.shape[1] != self.body.full_width:
-            raise ValueError(f"clip for body {clip.body!r} ({tuple(clip.pose.shape)}), the avatar is {self.body.name!r}")
+    def _playback(self, fps_out):
+        """Per-actor times [K,n] and alignments [K][12], and the camera rows [n,40] of a playback."""
+        for k, a in enumerate(self.actors):
+            if a.clip is None:
+                raise ValueError(f"actor {k} has no clip")
+            self._check_clip(a.model, a.clip, k)
+        times = cast_times([a.clip.num_keys for a in self.actors], [a.clip.fps for a in self.actors], [a.speed for a in self.actors],
+                           fps_out)
+        aligns = [self._alignment(a.model, a.clip, a.align_to) for a in self.actors]
+        return times, aligns, self._camera_rows(times.shape[1], self.actors[0].clip, aligns[0])
 
-    @torch.no_grad()
-    def sample(self, clip: MotionClip, sched: Schedule):
-        """All sampled poses [n,72|165] and translations [n,3] of a playback, on the device."""
-        keys_p, keys_t = clip.pose.to(self.dev).contiguous(), clip.trans.to(self.dev).contiguous()
-        times = torch.from_numpy(sched.times).to(self.dev)
-        align = torch.from_numpy(sched.align).to(self.dev)
-        return motion_sample(keys_p, keys_t, times, align)
+    def _kept(self):
+        stack = contextlib.ExitStack()
+        for m in self._models:
+            stack.enter_context(kept_state(m))
+        return stack
 
     # ---- playback ---------------------------------------------------------------------------------------------------------------
-    def frames(self, clip: MotionClip, fps_out: float, speed: float = 1.0, align_to=None):
-        """Yields (index of the chunk's first frame, uint8 [b,H,W,C]) in order.  The array lives in one of two pinned buffers and is
-        overwritten two chunks later: copy it to keep it."""
-        sched = self.schedule(clip, fps_out, speed, align_to)
-        n = len(sched.times)
+    def frames(self, fps_out: float):
+        """Yields (index of the chunk's first frame, uint8 [b,H,W,C], uint8 [b,K,H,W] mattes or None) in order.  The arrays live in
+        two pinned buffers and are overwritten two chunks later: copy them to keep them."""
+        times, aligns, cams = self._playback(fps_out)
+        n = times.shape[1]
         starts = list(range(0, n, self.chunk))
-        with torch.no_grad(), kept_state(self.model):
-            render = self._stage1_setup(clip, sched) if self.stage == 1 else self._stage2_setup(clip, sched)
+        with torch.no_grad(), self._kept():
+            setup = self._stage1_setup if all(s == 1 for s in self._stages) else self._eager_setup
+            render = setup(times, aligns, cams)
         self._enqueue(render, starts[0], min(n, starts[0] + self.chunk), 0)
         for j, s in enumerate(starts):
             e = min(n, s + self.chunk)
@@ -320,36 +394,50 @@ class Animator:
                 self._grow(e - s, int(self._status_host[slot][0]))
                 self._enqueue(render, s, e, slot)
                 self._copied[slot].synchronize()
-            yield s, self._out_host[slot][:e - s]
+            yield s, self._out_host[slot][:e - s], self._mattes_host[slot][:e - s] if self.mattes else None
         torch.cuda.current_stream().wait_stream(self._copy_stream)
 
     def _enqueue(self, render, s, e, slot):
-        """Renders frames s..e-1 into the slot's device buffer and copies them, with the overflow status, to its pinned buffers."""
+        """Renders frames s..e-1 into the slot's device buffers and copies them, with the overflow status, to its pinned buffers."""
         main = torch.cuda.current_stream()
         if self._slot_used[slot]:
             main.wait_event(self._copied[slot])          # the previous copy out of this slot has finished reading it
-        with torch.no_grad(), kept_state(self.model):
+        with torch.no_grad(), self._kept():
             render(s, e, slot)
         self._rendered[slot].record(main)
         self._slot_used[slot] = True
         with torch.cuda.stream(self._copy_stream):
             self._copy_stream.wait_event(self._rendered[slot])
             self._out_host[slot][:e - s].copy_(self._out_dev[slot][:e - s], non_blocking=True)
+            if self.mattes:
+                self._mattes_host[slot][:e - s].copy_(self._mattes_dev[slot][:e - s], non_blocking=True)
             self._status_host[slot].copy_(self._status_dev[slot], non_blocking=True)
             self._copied[slot].record(self._copy_stream)
 
-    # ---- stage 1: one graph per (chunk size, slot) -------------------------------------------------------------------------------
     def _plan(self, b):
         if b not in self._plans:
-            self._plans[b] = RasterBatchPlan(b, int(self.model._query_points.shape[0]), self.H, self.W, self.dev, capacity=self.capacity,
+            self._plans[b] = RasterBatchPlan(b, self.first[-1], self.H, self.W, self.dev, capacity=self.capacity,
                                              static_P=0 if self.scene is None else len(self.scene))
         return self._plans[b]
 
-    def _raster(self, means, scales, colors, cams, plan):
-        m = self.model
-        if self.scene is None:
-            return rasterize_batch(means, colors, scales, m.fix_rotation, m.fix_opacity, cams, m.background, plan)
-        return rasterize_batch_scene(means, colors, scales, m.fix_rotation, m.fix_opacity, cams, m.background, plan, self.scene)
+    def _render(self, parts, cams, plan):
+        """Concatenates the actors' (means, scales, colours) and rasterizes them: (images, mattes or None)."""
+        means, scales, colors = parts[0] if len(parts) == 1 else [torch.cat(t, 1) for t in zip(*parts)]
+        bg = self.actors[0].model.background
+        mattes = None
+        if self.mattes:
+            img, mattes = rasterize_batch_mattes(means, colors, scales, self._rot, self._opac, cams, bg, plan, self.first, self.scene)
+        elif self.scene is None:
+            img = rasterize_batch(means, colors, scales, self._rot, self._opac, cams, bg, plan)
+        else:
+            img = rasterize_batch_scene(means, colors, scales, self._rot, self._opac, cams, bg, plan, self.scene)
+        return img, mattes
+
+    def _pack(self, img, mattes, plan, slot, lo, hi):
+        """Packs images (and mattes) into frames lo..hi-1 of the slot's device buffers."""
+        frame_pack(img, final_transmittance(plan), self.actors[0].model.background, self.channels, self._out_dev[slot][lo:hi])
+        if mattes is not None:
+            matte_pack(mattes, self._mattes_dev[slot][lo:hi])
 
     def _grow(self, b, needed):
         if self._graphs:
@@ -359,37 +447,44 @@ class Animator:
             del self._graphs[key]
             self.recaptures += 1
 
-    def _stage1_setup(self, clip, sched):
-        m = self.model
-        T, width = clip.num_keys, int(clip.pose.shape[1])
-        dec = m._stage1_decoder(1)
-        if self._keys_pose is None or self._keys_pose.shape[0] < T:
-            self._keys_pose = torch.empty(T, width, dtype=torch.float32, device=self.dev)
-            self._keys_trans = torch.empty(T, 3, dtype=torch.float32, device=self.dev)
-            self._graphs = {}
-        # the graphs take the clip's key count as a kernel argument and the decoder output by address
-        key = (T, dec.data_ptr())
+    # ---- every actor in stage 1: one graph per (chunk size, slot) ----------------------------------------------------------------
+    def _stage1_setup(self, times, aligns, cams):
+        decs = {}
+        for m in self._models:
+            decs[id(m)] = m._stage1_decoder(1)
+        key = []
+        for k, a in enumerate(self.actors):
+            T, width = a.clip.num_keys, int(a.clip.pose.shape[1])
+            if self._keys_pose[k] is None or self._keys_pose[k].shape[0] < T or self._keys_pose[k].shape[1] != width:
+                self._keys_pose[k] = torch.empty(T, width, dtype=torch.float32, device=self.dev)
+                self._keys_trans[k] = torch.empty(T, 3, dtype=torch.float32, device=self.dev)
+                self._graphs = {}
+            self._keys_pose[k][:T].copy_(a.clip.pose)
+            self._keys_trans[k][:T].copy_(a.clip.trans)
+            self._align[k].copy_(torch.from_numpy(aligns[k]))
+            key.append((T, decs[id(a.model)].data_ptr()))
+        # the graphs take each clip's key count as a kernel argument and the decoder outputs by address
         if key != self._clip_key:
             self._graphs, self._clip_key = {}, key
-        self._dec = dec
-        self._keys_pose[:T].copy_(clip.pose)
-        self._keys_trans[:T].copy_(clip.trans)
-        self._align.copy_(torch.from_numpy(sched.align))
-        times_all = torch.from_numpy(sched.times).to(self.dev)
-        cams_all = sched.cams.to(self.dev)
+        times_all = torch.from_numpy(times).to(self.dev)
+        cams_all = cams.to(self.dev)
 
         def body(b, slot):
             plan = self._plan(b)
-            pose, trans = motion_sample(self._keys_pose[:T], self._keys_trans[:T], self._times_dev[:b], self._align)
-            pose, rest = self.body.split(pose)
-            means, scales, colors = m._assemble(self._dec, pose, trans, rest, placement=self.placement)
-            img = self._raster(means, scales, colors, self._cams_dev[:b], plan)
-            frame_pack(img, final_transmittance(plan), m.background, self.channels, self._out_dev[slot][:b])
+            parts = []
+            for k, a in enumerate(self.actors):
+                T = a.clip.num_keys
+                pose, trans = motion_sample(self._keys_pose[k][:T], self._keys_trans[k][:T], self._times_dev[k][:b], self._align[k])
+                pose, rest = a.model.body.split(pose)
+                parts.append(a.model._assemble(decs[id(a.model)], pose, trans, rest, placement=a.placement))
+            img, mattes = self._render(parts, self._cams_dev[:b], plan)
+            self._pack(img, mattes, plan, slot, 0, b)
             self._status_dev[slot].copy_(plan.status_dev)
 
         def render(s, e, slot):
             b = e - s
-            self._times_dev[:b].copy_(times_all[s:e])
+            for k in range(len(self.actors)):
+                self._times_dev[k][:b].copy_(times_all[k, s:e])
             self._cams_dev[:b].copy_(cams_all[s:e])
             if not self.use_graphs:
                 body(b, slot)
@@ -405,27 +500,75 @@ class Animator:
             g.replay()
         return render
 
-    # ---- stage 2: eager, one frame per forward ------------------------------------------------------------------------------------
-    def _stage2_setup(self, clip, sched):
-        m = self.model
-        pose, trans = self.sample(clip, sched)
-        cams_all = sched.cams.to(self.dev)
+    # ---- any actor in stage 2: eager, one frame per forward -----------------------------------------------------------------------
+    def _eager_setup(self, times, aligns, cams):
+        sampled, decs = [], {}
+        for k, a in enumerate(self.actors):
+            sampled.append(motion_sample(a.clip.pose.to(self.dev).contiguous(), a.clip.trans.to(self.dev).contiguous(),
+                                         torch.from_numpy(times[k]).to(self.dev), torch.from_numpy(aligns[k]).to(self.dev)))
+            if self._stages[k] == 1 and id(a.model) not in decs:
+                decs[id(a.model)] = a.model._stage1_decoder(1)
+        cams_all = cams.to(self.dev)
 
         def render(s, e, slot):
             for i in range(s, e):
-                p, rest = self.body.split(pose[i:i + 1])
-                means, scales, colors, _, _ = m._stage2_from_pose(self.pose_mapper, p, trans[i:i + 1], rest, placement=self.placement)
-                if self.scene is None:
-                    batch = {"_cams": cams_all[i:i + 1], "height": [self.H], "width": [self.W]}
-                    img = m._render_frames(batch, means, scales, colors)
-                    plan = m._last_plan
-                else:                # as _render_batched: a frame whose binning buffer overflowed is rendered again after it grew
-                    plan = self._plan(1)
-                    img = self._raster(means, scales, colors, cams_all[i:i + 1], plan)
+                parts = []
+                for k, a in enumerate(self.actors):
+                    m = a.model
+                    p, rest = m.body.split(sampled[k][0][i:i + 1])
+                    t = sampled[k][1][i:i + 1]
+                    if self._stages[k] == 2:
+                        parts.append(m._stage2_from_pose(self._mappers[k], p, t, rest, placement=a.placement)[:3])
+                    else:
+                        parts.append(m._assemble(decs[id(m)], p, t, rest, placement=a.placement))
+                plan = self._plan(1)       # as _render_batched: a frame whose binning buffer overflowed is rendered again after it grew
+                img, mattes = self._render(parts, cams_all[i:i + 1], plan)
+                if not plan.check(wait=True):
+                    self.overflows += 1
+                    img, mattes = self._render(parts, cams_all[i:i + 1], plan)
                     if not plan.check(wait=True):
-                        self.overflows += 1
-                        img = self._raster(means, scales, colors, cams_all[i:i + 1], plan)
-                        if not plan.check(wait=True):
-                            raise RuntimeError("animation: the rasterizer's binning buffer overflowed again after growing")
-                frame_pack(img, final_transmittance(plan), m.background, self.channels, self._out_dev[slot][i - s:i - s + 1])
+                        raise RuntimeError("animation: the rasterizer's binning buffer overflowed again after growing")
+                self._pack(img, mattes, plan, slot, i - s, i - s + 1)
         return render
+
+
+class Animator(Ensemble):
+    """Renders one inference `AvatarModel` (stage 1 or 2) along motion clips: the one-actor `Ensemble`.
+
+    cameras, H, W, chunk, channels, capacity, graphs and scene as for `Ensemble`; pose_mapper: stage 2's `posmap.PoseMapper` /
+    `SmplxPoseMapper` (default: the model's own).  scene: a `scene.GaussianScene` the avatar is rendered in, splatted together
+    with it (`rasterize_batch_scene`) so that either hides the other; placement: the `scene.Placement` of the avatar's world in
+    it.  The cameras are given in the avatar's world and carried into the scene through the placement; alpha (channels=4) is
+    1 - final transmittance over both sets."""
+
+    def __init__(self, model, cameras, H: int, W: int, chunk: int | None = None, channels: int = 3, pose_mapper=None,
+                 capacity=None, graphs: bool = True, scene=None, placement=None):
+        super().__init__([Actor(model, None, placement, pose_mapper=pose_mapper)], cameras, H, W, chunk=chunk, channels=channels,
+                         capacity=capacity, graphs=graphs, scene=scene)
+        self.model, self.body, self.placement = model, model.body, placement
+        self.stage, self.pose_mapper = self._stages[0], self._mappers[0]
+
+    def schedule(self, clip: MotionClip, fps_out: float, speed: float = 1.0, align_to=None) -> Schedule:
+        """Sample times, alignment and camera rows of a playback (all built on the host in fp64, cameras narrowed to fp32)."""
+        self._cast(clip, speed, align_to)
+        times, aligns, cams = self._playback(fps_out)
+        return Schedule(times[0], aligns[0], cams)
+
+    @torch.no_grad()
+    def sample(self, clip: MotionClip, sched: Schedule):
+        """All sampled poses [n,72|165] and translations [n,3] of a playback, on the device."""
+        keys_p, keys_t = clip.pose.to(self.dev).contiguous(), clip.trans.to(self.dev).contiguous()
+        times = torch.from_numpy(sched.times).to(self.dev)
+        align = torch.from_numpy(sched.align).to(self.dev)
+        return motion_sample(keys_p, keys_t, times, align)
+
+    def frames(self, clip: MotionClip, fps_out: float, speed: float = 1.0, align_to=None):
+        """Yields (index of the chunk's first frame, uint8 [b,H,W,C]) in order.  The array lives in one of two pinned buffers and is
+        overwritten two chunks later: copy it to keep it."""
+        self._cast(clip, speed, align_to)
+        for s, frames, _ in super().frames(fps_out):
+            yield s, frames
+
+    def _cast(self, clip, speed, align_to):
+        self.actors[0] = Actor(self.model, clip, self.placement, align_to, speed, self.actors[0].pose_mapper)
+        self._check_clip(self.model, clip)

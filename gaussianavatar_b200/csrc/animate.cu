@@ -143,6 +143,12 @@ __global__ void frame_pack_kernel(long long HW, const float *__restrict__ image,
     }
 }
 
+__global__ void matte_pack_kernel(long long n, const float *__restrict__ mattes, uint8_t *__restrict__ out)
+{
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        out[i] = quant8(mattes[i]);
+}
+
 }  // namespace
 }  // namespace ga
 
@@ -179,5 +185,16 @@ extern "C" int ga_frame_pack(int32_t B, int32_t H, int32_t W, int32_t channels, 
       if (channels == 3) frame_pack_kernel<3><<<grid, 256, 0, stream>>>(HW, image, final_T, bg, out);
       else frame_pack_kernel<4><<<grid, 256, 0, stream>>>(HW, image, final_T, bg, out); }
     GA_CHECK_LAUNCH("frame_pack_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_matte_pack(int64_t n, const float *mattes, uint8_t *out, void *stream_)
+{
+    GA_REQUIRE(n >= 1, "ga_matte_pack: %lld values", (long long)n);
+    GA_REQUIRE(mattes && out, "ga_matte_pack: NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    { ProfScope _ps("matte_pack_kernel", stream);
+      matte_pack_kernel<<<min(cdiv(n, 256), 1 << 20), 256, 0, stream>>>(n, mattes, out); }
+    GA_CHECK_LAUNCH("matte_pack_kernel");
     return GA_OK;
 }

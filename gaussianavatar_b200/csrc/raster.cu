@@ -928,7 +928,7 @@ __device__ __forceinline__ float entry_alpha(const float4 a, const float4 co, fl
     return alpha;
 }
 
-__device__ __forceinline__ void blend(PixState &p, float alpha, bool ok, const float4 rgb, uint32_t pos1)
+__device__ __forceinline__ float blend(PixState &p, float alpha, bool ok, const float4 rgb, uint32_t pos1)
 {
     const float test_T = p.T * (1.f - alpha);
     const bool live = ok && !p.done;
@@ -939,6 +939,24 @@ __device__ __forceinline__ void blend(PixState &p, float alpha, bool ok, const f
     p.T = take ? test_T : p.T;
     p.last = take ? pos1 : p.last;
     p.done = p.done || stop;
+    return w;
+}
+
+// The sets of ga_rasterb_forward_mattes: entry idx of a frame belongs to set k when first[k] <= idx < first[k+1]; sets k >= K
+// are empty (first[k] = first[K]), and so is every index at or above first[K] (the rest of the dynamic set, the scene's).
+constexpr int kMaxSets = 8;
+struct MatteSets {
+    uint32_t first[kMaxSets + 1];
+    int K;
+    float *out;              // [B, K, H, W]
+};
+
+// Adds an entry's blending weight to the accumulator of its set: unrolled selects keep the accumulators in registers.  The add
+// is never contracted with the product that formed w, so matte k equals the colour channel an indicator colour of set k gives.
+__device__ __forceinline__ void matte_add(float (&mt)[kMaxSets], const MatteSets &ms, uint32_t idx, float w)
+{
+#pragma unroll
+    for (int k = 0; k < kMaxSets; ++k) mt[k] = __fadd_rn(mt[k], (idx >= ms.first[k] && idx < ms.first[k + 1]) ? w : 0.f);
 }
 
 // K6: one CTA per (frame, 16x16 tile), one warp per 8x4-pixel sub-tile, one lane per pixel.  The warps of a CTA do not
@@ -946,13 +964,16 @@ __device__ __forceinline__ void blend(PixState &p, float alpha, bool ok, const f
 // registers), tests the 32 against its sub-tile in parallel (one per lane, cull_radius2 precomputed by the sort kernel),
 // stages them in its own slice of shared memory and composites the ballot's survivors in list order, two at a time.
 // At every 256th list position it stores each pixel's (T, C) — the state the backward's segment CTAs start from.
+// kMattes: also sums, per pixel and per set of `ms`, the weights alpha T its set's entries add, and writes them to ms.out; every
+// other output is the same.
+template <bool kMattes>
 __global__ void __launch_bounds__(kBlock)
 render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict__ order, const uint2 *__restrict__ ranges,
                   const uint32_t *__restrict__ seg_start,
                   const float4 *__restrict__ recA, const float4 *__restrict__ recB, const float4 *__restrict__ recC,
                   const float *__restrict__ bg, float4 *__restrict__ ckpt, float *__restrict__ final_T,
                   uint32_t *__restrict__ n_contrib, float4 *__restrict__ final_state, uint32_t *__restrict__ tile_maxc,
-                  float *__restrict__ out)
+                  float *__restrict__ out, const MatteSets ms)
 {
     __shared__ float4 s_a[kBlock / 32][32], s_b[kBlock / 32][32], s_c[kBlock / 32][32];
 
@@ -971,6 +992,11 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
     float4 *ck = ckpt + (size_t)seg_start[blk] * kBlock + tid;
 
     PixState p{1.f, 0.f, 0.f, 0.f, 0u, !inside};
+    float mt[kMaxSets];
+    if constexpr (kMattes) {
+#pragma unroll
+        for (int k = 0; k < kMaxSets; ++k) mt[k] = 0.f;
+    }
     float4 fa = make_float4(0.f, 0.f, -1.f, 0.f), fb = fa, fc = fa;
     if (lane < n) { fa = recA[range.x + lane]; fb = recB[range.x + lane]; fc = recC[range.x + lane]; }
 
@@ -996,8 +1022,12 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
                 bool ok0, ok1;
                 const float al0 = entry_alpha(s_a[warp][j0], s_b[warp][j0], pxf, pyf, ok0);
                 const float al1 = entry_alpha(s_a[warp][j1], s_b[warp][j1], pxf, pyf, ok1);
-                blend(p, al0, ok0, s_c[warp][j0], base1 + j0);
-                blend(p, al1, ok1 && two, s_c[warp][j1], base1 + j1);
+                const float w0 = blend(p, al0, ok0, s_c[warp][j0], base1 + j0);
+                const float w1 = blend(p, al1, ok1 && two, s_c[warp][j1], base1 + j1);
+                if constexpr (kMattes) {
+                    matte_add(mt, ms, __float_as_uint(s_a[warp][j0].w), w0);
+                    matte_add(mt, ms, __float_as_uint(s_a[warp][j1].w), w1);
+                }
             }
             all_done = __all_sync(0xffffffffu, p.done);
         }
@@ -1011,6 +1041,12 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
         o[0] = p.C0 + p.T * bg[0];
         o[HW] = p.C1 + p.T * bg[1];
         o[2 * HW] = p.C2 + p.T * bg[2];
+        if constexpr (kMattes) {
+            float *mo = ms.out + (size_t)b * ms.K * HW + (size_t)py * W + px;
+#pragma unroll
+            for (int k = 0; k < kMaxSets; ++k)
+                if (k < ms.K) mo[(size_t)k * HW] = mt[k];
+        }
     }
     final_state[(size_t)blk * kBlock + tid] = make_float4(p.T, p.C0, p.C1, p.C2);
     uint32_t m = p.last;
@@ -1391,9 +1427,9 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
     return GA_OK;
 }
 
-// K3 + K4 + K6 for all frames (a scene: the composite K4, d.P = P + Ps).
+// K3 + K4 + K6 for all frames (a scene: the composite K4, d.P = P + Ps; mattes: K6's matte variant).
 int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacity, const GeomViews &g, const ImgViews &iv, const BinViews &bv,
-                              float *out_color, cudaStream_t stream, const SceneSet *scene = nullptr)
+                              float *out_color, cudaStream_t stream, const SceneSet *scene = nullptr, const MatteSets *mattes = nullptr)
 {
     static PerDeviceOnce attr_set;
     if (attr_set.first()) {
@@ -1427,10 +1463,16 @@ int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacit
                  bv.recC, bv.seg_tile, iv.tile_maxc, scene_rgb, Pd);
     }
     GA_CHECK_LAUNCH("tile_sort_kernel");
-    {
+    if (mattes) {
+        ProfScope _ps("render_fwd_mattes_kernel", stream);
+        render_fwd_kernel<true><<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC,
+                                                          a.bg, bv.ckpt, iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color,
+                                                          *mattes);
+    } else {
         ProfScope _ps("render_fwd_kernel", stream);
-        render_fwd_kernel<<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC, a.bg, bv.ckpt,
-                                                    iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color);
+        render_fwd_kernel<false><<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC,
+                                                           a.bg, bv.ckpt, iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color,
+                                                           MatteSets{});
     }
     GA_CHECK_LAUNCH("render_fwd_kernel");
     return GA_OK;
@@ -1657,31 +1699,25 @@ extern "C" int ga_rasterb_status_to_host(int32_t B, int32_t H, int32_t W, void *
     return GA_OK;
 }
 
-extern "C" int ga_rasterb_forward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,
-                                  const float *colors, const float *scales, const float *rotations, const float *opacities,
-                                  void *geom, void *img, void *binning, int32_t *radii, float *out_color, void *stream_)
+// The batched forward (bd checked by the caller): scene NULL renders the dynamic set alone, a scene (even with Ps = 0) through the
+// composite kernels; mattes NULL writes no mattes.  Every check runs before the first launch.
+static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const MatteSets *mattes, const float *cams,
+                         const float *bg, const float *means3D, const float *colors, const float *scales, const float *rotations,
+                         const float *opacities, void *geom, void *img, void *binning, int32_t *radii, float *out_color,
+                         cudaStream_t stream)
 {
-    if (int rc = check_batch(bd)) return rc;
-    GA_REQUIRE(cams && bg && img && binning && out_color, "NULL pointer argument");
-    GA_REQUIRE(bd->P == 0 || (means3D && colors && scales && rotations && opacities && geom && radii), "NULL pointer argument");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
-    GeomViews g = carve_geom(geom, (size_t)d.B * d.P);
-    ImgViews iv = carve_img(img, d);
-    BinViews bv = carve_bin(binning, bd->capacity, d);
-    const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
-    const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
-    if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
-    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream);
-}
-
-extern "C" int ga_rasterb_forward_scene(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const float *cams, const float *bg,
-                                        const float *means3D, const float *colors, const float *scales, const float *rotations,
-                                        const float *opacities, void *geom, void *img, void *binning, int32_t *radii, float *out_color,
-                                        void *stream_)
-{
-    if (int rc = check_batch(bd)) return rc;
-    GA_REQUIRE(scene != nullptr, "scene descriptor is NULL");
+    if (scene == nullptr) {
+        GA_REQUIRE(cams && bg && img && binning && out_color, "NULL pointer argument");
+        GA_REQUIRE(bd->P == 0 || (means3D && colors && scales && rotations && opacities && geom && radii), "NULL pointer argument");
+        const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
+        GeomViews g = carve_geom(geom, (size_t)d.B * d.P);
+        ImgViews iv = carve_img(img, d);
+        BinViews bv = carve_bin(binning, bd->capacity, d);
+        const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
+        const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
+        if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
+        return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, nullptr, mattes);
+    }
     GA_REQUIRE(scene->Ps >= 0 && (long long)bd->P + scene->Ps <= 0x7fffffffll, "bad static count Ps=%d (P=%d)", (int)scene->Ps, (int)bd->P);
     const int Pt = bd->P + scene->Ps;
     if (int rc = check_dims(bd->B, Pt, bd->H, bd->W)) return rc;
@@ -1698,7 +1734,6 @@ extern "C" int ga_rasterb_forward_scene(const GaRasterBatchDesc *bd, const GaRas
         sc = SceneSet{scene->means3D, scene->scales, scene->rotations, scene->opacities, scene->shs, scene->Ps, scene->sh_degree,
                       scene->sh_coeffs, scene->sh_coeffs % 4 == 0 && reinterpret_cast<uintptr_t>(scene->shs) % 16 == 0, scene->rgb};
     }
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const Dims d = make_dims(bd->B, Pt, bd->H, bd->W);
     GeomViews g = carve_geom(geom, (size_t)d.B * d.P);
     ImgViews iv = carve_img(img, d);
@@ -1706,7 +1741,51 @@ extern "C" int ga_rasterb_forward_scene(const GaRasterBatchDesc *bd, const GaRas
     const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
     const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
     if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream, &sc)) return rc;
-    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, &sc);
+    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, &sc, mattes);
+}
+
+extern "C" int ga_rasterb_forward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,
+                                  const float *colors, const float *scales, const float *rotations, const float *opacities,
+                                  void *geom, void *img, void *binning, int32_t *radii, float *out_color, void *stream_)
+{
+    if (int rc = check_batch(bd)) return rc;
+    return forward_batch(bd, nullptr, nullptr, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii, out_color,
+                         static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ga_rasterb_forward_scene(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const float *cams, const float *bg,
+                                        const float *means3D, const float *colors, const float *scales, const float *rotations,
+                                        const float *opacities, void *geom, void *img, void *binning, int32_t *radii, float *out_color,
+                                        void *stream_)
+{
+    if (int rc = check_batch(bd)) return rc;
+    GA_REQUIRE(scene != nullptr, "scene descriptor is NULL");
+    return forward_batch(bd, scene, nullptr, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii,
+                         out_color, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ga_rasterb_forward_mattes(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const GaRasterSets *sets,
+                                         const float *cams, const float *bg, const float *means3D, const float *colors, const float *scales,
+                                         const float *rotations, const float *opacities, void *geom, void *img, void *binning,
+                                         int32_t *radii, float *out_color, void *stream_)
+{
+    if (int rc = check_batch(bd)) return rc;
+    GA_REQUIRE(sets != nullptr, "sets descriptor is NULL");
+    GA_REQUIRE(sets->K >= 1 && sets->K <= kMaxSets, "bad set count K=%d (1..%d)", (int)sets->K, kMaxSets);
+    GA_REQUIRE(sets->first[0] == 0, "sets: first[0] = %d, must be 0", (int)sets->first[0]);
+    for (int k = 0; k < sets->K; ++k)
+        GA_REQUIRE(sets->first[k + 1] >= sets->first[k], "sets: first[%d] = %d < first[%d] = %d (must not decrease)", k + 1,
+                   (int)sets->first[k + 1], k, (int)sets->first[k]);
+    GA_REQUIRE(sets->first[sets->K] <= bd->P, "sets: first[K=%d] = %d > P = %d (the sets index the dynamic set)", (int)sets->K,
+               (int)sets->first[sets->K], (int)bd->P);
+    GA_REQUIRE(sets->mattes != nullptr, "sets: mattes is NULL");
+    MatteSets ms{};
+    for (int k = 0; k <= kMaxSets; ++k) ms.first[k] = (uint32_t)sets->first[k < sets->K ? k : sets->K];
+    ms.K = sets->K;
+    ms.out = sets->mattes;
+    if (scene != nullptr && scene->Ps == 0) scene = nullptr;
+    return forward_batch(bd, scene, &ms, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii, out_color,
+                         static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,

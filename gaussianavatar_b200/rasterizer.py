@@ -399,6 +399,49 @@ def rasterize_batch_scene(means3D, colors, scales, rotations, opacities, cams, b
     return out
 
 
+MAX_SETS = 8                     # ga_rasterb_forward_mattes
+
+
+def rasterize_batch_mattes(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan, first, scene=None):
+    """`rasterize_batch` (scene None) or `rasterize_batch_scene` that also returns each set's visibility matte; forward only.
+    first: K+1 nondecreasing dynamic indices, first[0] = 0 and first[K] <= plan.P; set k is Gaussians first[k]..first[k+1]-1.
+    Returns (images [B,3,H,W], mattes [B,K,H,W]): matte k is the weight set k's Gaussians added to each pixel (sum of alpha T
+    over its blended entries), so the mattes sum to 1 - final transmittance where every splatted Gaussian is in a set."""
+    if not means3D.is_cuda:
+        raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
+    given = [means3D, colors, scales, rotations, opacities]
+    if scene is not None:
+        given += [scene.means3D, scene.shs, scene.scales, scene.rotations, scene.opacities]
+    if torch.is_grad_enabled() and any(t.requires_grad for t in given):
+        raise RuntimeError("rasterize_batch_mattes is forward only: it has no backward (run it under torch.no_grad())")
+    first = [int(f) for f in first]
+    K = len(first) - 1
+    if not 1 <= K <= MAX_SETS:
+        raise ValueError(f"first has {len(first)} entries: 2..{MAX_SETS + 1} (1..{MAX_SETS} sets)")
+    Ps = 0 if scene is None else int(scene.means3D.shape[0])
+    if Ps != plan.static_P:
+        raise ValueError(f"the scene has {Ps} Gaussians, the plan was sized for static_P={plan.static_P}")
+    L = _lib.lib()
+    dev = means3D.device
+    means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
+    opacities = _c(opacities).reshape(-1)
+    d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
+    sc = None
+    if scene is not None:
+        _on_device(dev, scene_means3D=scene.means3D, scene_shs=scene.shs, cams=cams)
+        sc = _lib.GaRasterScene(Ps, int(scene.sh_degree), int(scene.shs.shape[1]), ptr(scene.means3D), ptr(scene.scales),
+                                ptr(scene.rotations), ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb))
+    out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=dev)
+    mattes = torch.empty(plan.B, K, plan.H, plan.W, dtype=torch.float32, device=dev)
+    sets = _lib.GaRasterSets(K, (ctypes.c_int32 * 9)(*(first + [0] * (9 - len(first)))), ptr(mattes))
+    _lib.check(L.ga_rasterb_forward_mattes(ctypes.byref(d), None if sc is None else ctypes.byref(sc), ctypes.byref(sets), ptr(cams),
+                                           ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(opacities),
+                                           ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii), ptr(out), _stream()),
+               "ga_rasterb_forward_mattes")
+    plan.record_status()
+    return out, mattes
+
+
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings):

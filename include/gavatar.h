@@ -171,6 +171,24 @@ int ga_rasterb_forward_scene(const GaRasterBatchDesc *d, const GaRasterScene *sc
                              const float *opacities, void *geom, void *img, void *binning, int32_t *radii, float *out_color,
                              void *stream);
 
+/* Index ranges of the dynamic set for ga_rasterb_forward_mattes, e.g. several avatars concatenated into one [B, P1+...+PK, *]
+ * set.  Entry idx of a frame belongs to set k when first[k] <= idx < first[k+1]; indices at or above first[K] (the rest of the
+ * dynamic set, and the scene's) belong to no set. */
+typedef struct GaRasterSets {
+    int32_t K;                   /* 1..8 sets                                                               */
+    int32_t first[9];            /* first[0] = 0, nondecreasing up to first[K] <= d->P; entries past K unread */
+    float *mattes;               /* [B, K, H, W] written                                                    */
+} GaRasterSets;
+/* ga_rasterb_forward_scene (scene NULL or Ps = 0: ga_rasterb_forward of the dynamic set alone) that also writes, for each set
+ * and pixel, the weight its Gaussians added to the pixel: matte_k = sum over set k's blended entries of alpha T, the same
+ * weights the colour is blended with, so sum_k matte_k = 1 - final T where every entry belongs to a set.  Binning, the capacity
+ * / overflow status, tie order and every other output are the composite's, bit for bit.  Bad K or first, or a NULL mattes,
+ * are refused before anything launches.  Forward only. */
+int ga_rasterb_forward_mattes(const GaRasterBatchDesc *d, const GaRasterScene *scene, const GaRasterSets *sets, const float *cams,
+                              const float *bg, const float *means3D, const float *colors, const float *scales,
+                              const float *rotations, const float *opacities, void *geom, void *img, void *binning,
+                              int32_t *radii, float *out_color, void *stream);
+
 /* Debug / parity accessors into the opaque buffers (device pointers; valid after the forward that filled them).  B = 1 and
  * capacity = num_rendered for buffers of the per-frame API. */
 typedef struct GaRasterViews {
@@ -494,6 +512,8 @@ int ga_motion_sample(int32_t T, int32_t J, const float *key_pose, const float *k
                      const double *align, float *pose_out, float *trans_out, void *stream);
 int ga_frame_pack(int32_t B, int32_t H, int32_t W, int32_t channels, const float *image, const float *final_T, const float *bg,
                   uint8_t *out, void *stream);
+/* ga_matte_pack: out[i] = q(mattes[i]) for n >= 1 values (ga_frame_pack's q; the mattes of ga_rasterb_forward_mattes as bytes). */
+int ga_matte_pack(int64_t n, const float *mattes, uint8_t *out, void *stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Soft silhouette (pose refinement against masks).  B in [1, 8] frames of verts [B,V,3] (fp32), faces [F,3] (int32, each in

@@ -91,7 +91,7 @@ def main():
         fps, n = sustained(anim, long_clip)
         sched = anim.schedule(long_clip, 30.0)
         with torch.no_grad():
-            render = anim._stage1_setup(long_clip, sched)
+            render = anim._stage1_setup(sched.times[None], [sched.align], sched.cams)
             render(0, b, 0)
             dev_ms, dev_rounds = events_ms(lambda: render(0, b, 0), 20)
         lat = []

@@ -89,7 +89,7 @@ def one_chunk(m, cam, c, scene, P, Ps, M, b):
             pass
         sched = anim.schedule(c, 30.0)
         with torch.no_grad():
-            render = anim._stage1_setup(c, sched)
+            render = anim._stage1_setup(sched.times[None], [sched.align], sched.cams)
             render(0, b, 0)
         players[key] = (anim, render)
     rounds = {"scene": [], "avatar": []}
