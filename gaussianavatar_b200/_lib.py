@@ -138,6 +138,8 @@ _SIGNATURES = {
     "ga_rasterb_forward_scene": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc), ctypes.POINTER(GaRasterScene)] + [c_vp] * 13),
     "ga_rasterb_forward_mattes": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc), ctypes.POINTER(GaRasterScene), ctypes.POINTER(GaRasterSets)]
                                   + [c_vp] * 13),
+    "ga_rasterb_forward_depth": (ctypes.c_int, [ctypes.POINTER(GaRasterBatchDesc), ctypes.POINTER(GaRasterScene), ctypes.POINTER(GaRasterSets)]
+                                 + [c_vp] * 14),
     "ga_tc_conv5x5": (ctypes.c_int, [ctypes.c_int32, ctypes.c_int32, c_vp, c_vp, c_vp, ctypes.c_int32, c_vp]),
     "ga_round_tf32": (ctypes.c_int, [c_vp, c_vp, ctypes.c_int64, c_vp]),
     "ga_lpips_weights_floats": (ctypes.c_size_t, []),

@@ -26,7 +26,11 @@ Several avatars play together through `Ensemble`, of which `Animator` is the one
         ...
 
 Their Gaussians are concatenated into one dynamic set and splatted together (and with the scene), so they occlude each other;
-with `mattes` each actor's visible matte comes from the same compositing pass (`rasterizer.rasterize_batch_mattes`).
+with `mattes` each actor's visible matte comes from the same compositing pass (`rasterizer.rasterize_batch_mattes`).  With
+`depth` the same pass also writes each frame's mean and median view depth (`rasterizer.rasterize_batch_depth`):
+
+    for first, frames, mattes, depth in Ensemble(cast, cameras, 1080, 1920, depth=True).frames(fps_out=30):  # depth: fp32 [b,2,H,W]
+        ...
 """
 from __future__ import annotations
 
@@ -44,7 +48,8 @@ from .avatar_model import kept_state
 from .body import body_of
 from .camera import Camera, make_camera
 from .dataset import _rodrigues, rotate_camera_by_frame_idx
-from .rasterizer import MAX_FRAMES_PER_CALL, MAX_SETS, RasterBatchPlan, rasterize_batch, rasterize_batch_mattes, rasterize_batch_scene
+from .rasterizer import (MAX_FRAMES_PER_CALL, MAX_SETS, RasterBatchPlan, rasterize_batch, rasterize_batch_depth, rasterize_batch_mattes,
+                         rasterize_batch_scene)
 from .scene import SceneCamera
 
 SCENE_CHUNK = 2                 # the player's default chunk with a scene
@@ -239,14 +244,17 @@ class Ensemble:
     RGBA, alpha = 1 - final transmittance over everything splatted).  mattes: also return each actor's visibility matte, the weight
     its Gaussians added to each pixel (`rasterize_batch_mattes`), as bytes.  capacity: initial binning capacity of the rasterizer
     (instances); it grows on overflow.  graphs: replay CUDA graphs when every actor is in stage 1 (False runs the same launches
-    eagerly).  scene: a `scene.GaussianScene` the actors are rendered in.
+    eagerly).  scene: a `scene.GaussianScene` the actors are rendered in.  depth: also return each frame's depth pass, fp32
+    [b,2,H,W] (`rasterize_batch_depth`: plane 0 the mean, plane 1 the median view depth in the shared world's units, 0 where there
+    is no surface), from the same compositing launch; it leaves through two pinned slots of 8 x 2 x H x W floats each, about 265 MB
+    of pinned host memory at 1920 x 1080 (and as much on the device).
 
     With every actor in stage 1 each distinct model's decoder is evaluated once and one CUDA graph per (chunk size, output slot)
     replays sample -> cano2live -> LBS per actor, their concatenation, the rasterizer and the packing.  Any stage-2 actor makes the
     player render eagerly, one frame per rasterizer call.  Every model's parameters and BatchNorm statistics are left as they were."""
 
     def __init__(self, actors, cameras, H: int, W: int, chunk: int | None = None, channels: int = 3, mattes: bool = False,
-                 capacity=None, graphs: bool = True, scene=None):
+                 capacity=None, graphs: bool = True, scene=None, depth: bool = False):
         self.actors = list(actors)
         if not 1 <= len(self.actors) <= MAX_SETS:
             raise ValueError(f"{len(self.actors)} actors: 1..{MAX_SETS}")
@@ -290,7 +298,7 @@ class Ensemble:
         one = len(self.actors) == 1                             # rotations / opacities shared by every frame, concatenated
         self._rot = m0.fix_rotation if one else torch.cat([a.model.fix_rotation for a in self.actors])
         self._opac = m0.fix_opacity if one else torch.cat([a.model.fix_opacity for a in self.actors])
-        self.mattes = bool(mattes)
+        self.mattes, self.depth = bool(mattes), bool(depth)
         self.scene = None if scene is None else scene.to(self.dev)
         self.capacity = capacity
         self.use_graphs = bool(graphs)
@@ -304,6 +312,9 @@ class Ensemble:
         if self.mattes:
             self._mattes_dev = [torch.empty(MAX_FRAMES_PER_CALL, K, self.H, self.W, dtype=torch.uint8, device=dev) for _ in range(2)]
             self._mattes_host = [torch.empty(MAX_FRAMES_PER_CALL, K, self.H, self.W, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        if self.depth:
+            self._depth_dev = [torch.empty(MAX_FRAMES_PER_CALL, 2, self.H, self.W, dtype=torch.float32, device=dev) for _ in range(2)]
+            self._depth_host = [torch.empty(MAX_FRAMES_PER_CALL, 2, self.H, self.W, dtype=torch.float32).pin_memory() for _ in range(2)]
         self._status_dev = [torch.zeros(16, dtype=torch.int32, device=dev) for _ in range(2)]      # eager rendering leaves them at 0
         self._status_host = [torch.zeros(16, dtype=torch.int32).pin_memory() for _ in range(2)]
         self._keys_pose, self._keys_trans = [None] * K, [None] * K
@@ -370,8 +381,9 @@ class Ensemble:
 
     # ---- playback ---------------------------------------------------------------------------------------------------------------
     def frames(self, fps_out: float):
-        """Yields (index of the chunk's first frame, uint8 [b,H,W,C], uint8 [b,K,H,W] mattes or None) in order.  The arrays live in
-        two pinned buffers and are overwritten two chunks later: copy them to keep them."""
+        """Yields (index of the chunk's first frame, uint8 [b,H,W,C], uint8 [b,K,H,W] mattes or None) in order, and with depth a
+        fourth item, the fp32 [b,2,H,W] depth pass.  The arrays live in two pinned buffers and are overwritten two chunks later: copy
+        them to keep them."""
         times, aligns, cams = self._playback(fps_out)
         n = times.shape[1]
         starts = list(range(0, n, self.chunk))
@@ -394,7 +406,8 @@ class Ensemble:
                 self._grow(e - s, int(self._status_host[slot][0]))
                 self._enqueue(render, s, e, slot)
                 self._copied[slot].synchronize()
-            yield s, self._out_host[slot][:e - s], self._mattes_host[slot][:e - s] if self.mattes else None
+            out = (s, self._out_host[slot][:e - s], self._mattes_host[slot][:e - s] if self.mattes else None)
+            yield out + (self._depth_host[slot][:e - s],) if self.depth else out
         torch.cuda.current_stream().wait_stream(self._copy_stream)
 
     def _enqueue(self, render, s, e, slot):
@@ -411,6 +424,8 @@ class Ensemble:
             self._out_host[slot][:e - s].copy_(self._out_dev[slot][:e - s], non_blocking=True)
             if self.mattes:
                 self._mattes_host[slot][:e - s].copy_(self._mattes_dev[slot][:e - s], non_blocking=True)
+            if self.depth:
+                self._depth_host[slot][:e - s].copy_(self._depth_dev[slot][:e - s], non_blocking=True)
             self._status_host[slot].copy_(self._status_dev[slot], non_blocking=True)
             self._copied[slot].record(self._copy_stream)
 
@@ -421,23 +436,30 @@ class Ensemble:
         return self._plans[b]
 
     def _render(self, parts, cams, plan):
-        """Concatenates the actors' (means, scales, colours) and rasterizes them: (images, mattes or None)."""
+        """Concatenates the actors' (means, scales, colours) and rasterizes them: (images, mattes or None, depth or None)."""
         means, scales, colors = parts[0] if len(parts) == 1 else [torch.cat(t, 1) for t in zip(*parts)]
         bg = self.actors[0].model.background
-        mattes = None
-        if self.mattes:
+        mattes = depth = None
+        if self.depth:
+            out = rasterize_batch_depth(means, colors, scales, self._rot, self._opac, cams, bg, plan, self.scene,
+                                        self.first if self.mattes else None)
+            img, depth = out[0], out[-1]
+            mattes = out[1] if self.mattes else None
+        elif self.mattes:
             img, mattes = rasterize_batch_mattes(means, colors, scales, self._rot, self._opac, cams, bg, plan, self.first, self.scene)
         elif self.scene is None:
             img = rasterize_batch(means, colors, scales, self._rot, self._opac, cams, bg, plan)
         else:
             img = rasterize_batch_scene(means, colors, scales, self._rot, self._opac, cams, bg, plan, self.scene)
-        return img, mattes
+        return img, mattes, depth
 
-    def _pack(self, img, mattes, plan, slot, lo, hi):
-        """Packs images (and mattes) into frames lo..hi-1 of the slot's device buffers."""
+    def _pack(self, img, mattes, depth, plan, slot, lo, hi):
+        """Packs images (and mattes) into frames lo..hi-1 of the slot's device buffers, and copies depth there."""
         frame_pack(img, final_transmittance(plan), self.actors[0].model.background, self.channels, self._out_dev[slot][lo:hi])
         if mattes is not None:
             matte_pack(mattes, self._mattes_dev[slot][lo:hi])
+        if depth is not None:
+            self._depth_dev[slot][lo:hi].copy_(depth)
 
     def _grow(self, b, needed):
         if self._graphs:
@@ -477,8 +499,7 @@ class Ensemble:
                 pose, trans = motion_sample(self._keys_pose[k][:T], self._keys_trans[k][:T], self._times_dev[k][:b], self._align[k])
                 pose, rest = a.model.body.split(pose)
                 parts.append(a.model._assemble(decs[id(a.model)], pose, trans, rest, placement=a.placement))
-            img, mattes = self._render(parts, self._cams_dev[:b], plan)
-            self._pack(img, mattes, plan, slot, 0, b)
+            self._pack(*self._render(parts, self._cams_dev[:b], plan), plan, slot, 0, b)
             self._status_dev[slot].copy_(plan.status_dev)
 
         def render(s, e, slot):
@@ -522,29 +543,29 @@ class Ensemble:
                     else:
                         parts.append(m._assemble(decs[id(m)], p, t, rest, placement=a.placement))
                 plan = self._plan(1)       # as _render_batched: a frame whose binning buffer overflowed is rendered again after it grew
-                img, mattes = self._render(parts, cams_all[i:i + 1], plan)
+                out = self._render(parts, cams_all[i:i + 1], plan)
                 if not plan.check(wait=True):
                     self.overflows += 1
-                    img, mattes = self._render(parts, cams_all[i:i + 1], plan)
+                    out = self._render(parts, cams_all[i:i + 1], plan)
                     if not plan.check(wait=True):
                         raise RuntimeError("animation: the rasterizer's binning buffer overflowed again after growing")
-                self._pack(img, mattes, plan, slot, i - s, i - s + 1)
+                self._pack(*out, plan, slot, i - s, i - s + 1)
         return render
 
 
 class Animator(Ensemble):
     """Renders one inference `AvatarModel` (stage 1 or 2) along motion clips: the one-actor `Ensemble`.
 
-    cameras, H, W, chunk, channels, capacity, graphs and scene as for `Ensemble`; pose_mapper: stage 2's `posmap.PoseMapper` /
+    cameras, H, W, chunk, channels, capacity, graphs, scene and depth as for `Ensemble`; pose_mapper: stage 2's `posmap.PoseMapper` /
     `SmplxPoseMapper` (default: the model's own).  scene: a `scene.GaussianScene` the avatar is rendered in, splatted together
     with it (`rasterize_batch_scene`) so that either hides the other; placement: the `scene.Placement` of the avatar's world in
     it.  The cameras are given in the avatar's world and carried into the scene through the placement; alpha (channels=4) is
     1 - final transmittance over both sets."""
 
     def __init__(self, model, cameras, H: int, W: int, chunk: int | None = None, channels: int = 3, pose_mapper=None,
-                 capacity=None, graphs: bool = True, scene=None, placement=None):
+                 capacity=None, graphs: bool = True, scene=None, placement=None, depth: bool = False):
         super().__init__([Actor(model, None, placement, pose_mapper=pose_mapper)], cameras, H, W, chunk=chunk, channels=channels,
-                         capacity=capacity, graphs=graphs, scene=scene)
+                         capacity=capacity, graphs=graphs, scene=scene, depth=depth)
         self.model, self.body, self.placement = model, model.body, placement
         self.stage, self.pose_mapper = self._stages[0], self._mappers[0]
 
@@ -563,11 +584,11 @@ class Animator(Ensemble):
         return motion_sample(keys_p, keys_t, times, align)
 
     def frames(self, clip: MotionClip, fps_out: float, speed: float = 1.0, align_to=None):
-        """Yields (index of the chunk's first frame, uint8 [b,H,W,C]) in order.  The array lives in one of two pinned buffers and is
-        overwritten two chunks later: copy it to keep it."""
+        """Yields (index of the chunk's first frame, uint8 [b,H,W,C]) in order, with depth (..., fp32 [b,2,H,W] depth).  The arrays
+        live in two pinned buffers and are overwritten two chunks later: copy them to keep them."""
         self._cast(clip, speed, align_to)
-        for s, frames, _ in super().frames(fps_out):
-            yield s, frames
+        for s, frames, _, *depth in super().frames(fps_out):
+            yield (s, frames, *depth)
 
     def _cast(self, clip, speed, align_to):
         self.actors[0] = Actor(self.model, clip, self.placement, align_to, speed, self.actors[0].pose_mapper)

@@ -113,7 +113,8 @@ ImgViews carve_img(void *buf, const Dims &d)
 struct BinViews {
     uint64_t *bucket;        // [cap] (depth bits << 32 | Gaussian index), grouped by tile, unsorted inside a tile
     uint32_t *point_list;    // [cap] Gaussian index in upstream's sorted order
-    float4 *recA, *recB, *recC;   // [cap] packed records in list order: (x, y, cull r^2, idx) (conic xyz, opacity) (r, g, b, -)
+    float4 *recA, *recB, *recC;   // [cap] packed records in list order: (x, y, cull r^2, idx) (conic xyz, opacity) (r, g, b, z)
+                                  // (z: the view depth when the forward writes depth, else 0)
     float4 *ckpt;            // [max_segments][256] per-pixel (T, C) at the start of each 256-entry segment
     uint32_t *seg_tile;      // [max_segments] segment -> tile
     size_t max_segments;
@@ -713,7 +714,9 @@ __device__ __forceinline__ void bitonic_sort_smem(uint64_t *keys, int n2)
 // the number of smaller keys, i.e. the sum of its lower bounds in the sorted runs.
 // kScene (composite forward, P = Pd + Ps per frame): colours of indices below Pd come from colors [B,Pd,3], the others from K1's
 // per-frame scene rgb [B,Ps,3].
-template <int kThreads, int kMax, bool kLong, bool kScene = false>
+// kZ (for K6's depth variant, the only reader of recC.w): recC.w is the entry's view depth z, the key's high word (K1's depth,
+// exact); otherwise 0.  A template parameter because holding the high word changes the short instance's register allocation.
+template <int kThreads, int kMax, bool kLong, bool kScene = false, bool kZ = false>
 __global__ void __launch_bounds__(kThreads)
 tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const uint32_t *__restrict__ order,
                  const uint2 *__restrict__ ranges, const uint32_t *__restrict__ seg_start,
@@ -745,6 +748,7 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
             return idx < (uint32_t)Pd ? colors + 3 * (f * Pd + idx) : scene_rgb + 3 * (f * (P - Pd) + (idx - Pd));
         };
 
+        auto rec_z = [](uint64_t key) { return kZ ? __uint_as_float((uint32_t)(key >> 32)) : 0.f; };
         auto emit = [&](int rank, uint64_t key) {
             const uint32_t idx = (uint32_t)key;
             const size_t g = gbase + idx, o = (size_t)r.x + rank;
@@ -755,9 +759,9 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
             recB[o] = co;
             if constexpr (kScene) {
                 const float *cp = scene_col(idx);
-                recC[o] = make_float4(cp[0], cp[1], cp[2], 0.f);
+                recC[o] = make_float4(cp[0], cp[1], cp[2], rec_z(key));
             } else {
-                recC[o] = make_float4(colors[3 * g], colors[3 * g + 1], colors[3 * g + 2], 0.f);
+                recC[o] = make_float4(colors[3 * g], colors[3 * g + 1], colors[3 * g + 2], rec_z(key));
             }
         };
 
@@ -865,7 +869,8 @@ tile_sort_kernel(int P, int T, int BT, const int32_t *__restrict__ status, const
                         point_list[o] = (uint32_t)kk[u];
                         recA[o] = make_float4(c[u].x, c[u].y, cull_radius2(co[u]), __uint_as_float((uint32_t)kk[u]));
                         recB[o] = co[u];
-                        recC[o] = make_float4(col[u][0], col[u][1], col[u][2], 0.f);
+                        // kZ: the depth word is re-read from shared memory rather than held through the gathers (no spill)
+                        recC[o] = make_float4(col[u][0], col[u][1], col[u][2], rec_z(kZ ? s_keys[i] : 0ull));
                     }
                 }
             }
@@ -966,14 +971,19 @@ __device__ __forceinline__ void matte_add(float (&mt)[kMaxSets], const MatteSets
 // At every 256th list position it stores each pixel's (T, C) — the state the backward's segment CTAs start from.
 // kMattes: also sums, per pixel and per set of `ms`, the weights alpha T its set's entries add, and writes them to ms.out; every
 // other output is the same.
-template <bool kMattes>
+// kDepth: also writes depth [B,2,H,W] over the blended entries (z = recC.w): plane 0 the mean D / (1 - T), D = sum of w z
+// accumulated as the colour channels are (so D is the red channel a colour (z, 0, 0) gives), 0 where nothing was blended;
+// plane 1 the median, the z of the entry whose blend takes T from above 0.5 to at most 0.5, 0 where the final T > 0.5.  An
+// entry that is not blended leaves T unchanged, so the T crossing alone selects a blended one; the 1e-4 stop cannot pre-empt
+// the crossing, since alpha <= 0.99 puts T below 0.01 before it can fire.
+template <bool kMattes, bool kDepth>
 __global__ void __launch_bounds__(kBlock)
 render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict__ order, const uint2 *__restrict__ ranges,
                   const uint32_t *__restrict__ seg_start,
                   const float4 *__restrict__ recA, const float4 *__restrict__ recB, const float4 *__restrict__ recC,
                   const float *__restrict__ bg, float4 *__restrict__ ckpt, float *__restrict__ final_T,
                   uint32_t *__restrict__ n_contrib, float4 *__restrict__ final_state, uint32_t *__restrict__ tile_maxc,
-                  float *__restrict__ out, const MatteSets ms)
+                  float *__restrict__ out, const MatteSets ms, float *__restrict__ depth)
 {
     __shared__ float4 s_a[kBlock / 32][32], s_b[kBlock / 32][32], s_c[kBlock / 32][32];
 
@@ -997,6 +1007,7 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
 #pragma unroll
         for (int k = 0; k < kMaxSets; ++k) mt[k] = 0.f;
     }
+    float dsum = 0.f, dmed = 0.f;
     float4 fa = make_float4(0.f, 0.f, -1.f, 0.f), fb = fa, fc = fa;
     if (lane < n) { fa = recA[range.x + lane]; fb = recB[range.x + lane]; fc = recC[range.x + lane]; }
 
@@ -1022,8 +1033,17 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
                 bool ok0, ok1;
                 const float al0 = entry_alpha(s_a[warp][j0], s_b[warp][j0], pxf, pyf, ok0);
                 const float al1 = entry_alpha(s_a[warp][j1], s_b[warp][j1], pxf, pyf, ok1);
+                const float T0 = p.T;
                 const float w0 = blend(p, al0, ok0, s_c[warp][j0], base1 + j0);
+                const float T1 = p.T;
                 const float w1 = blend(p, al1, ok1 && two, s_c[warp][j1], base1 + j1);
+                if constexpr (kDepth) {
+                    const float z0 = s_c[warp][j0].w, z1 = s_c[warp][j1].w;
+                    dsum += z0 * w0;
+                    dsum += z1 * w1;
+                    dmed = (T0 > 0.5f && T1 <= 0.5f) ? z0 : dmed;
+                    dmed = (T1 > 0.5f && p.T <= 0.5f) ? z1 : dmed;
+                }
                 if constexpr (kMattes) {
                     matte_add(mt, ms, __float_as_uint(s_a[warp][j0].w), w0);
                     matte_add(mt, ms, __float_as_uint(s_a[warp][j1].w), w1);
@@ -1046,6 +1066,11 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
 #pragma unroll
             for (int k = 0; k < kMaxSets; ++k)
                 if (k < ms.K) mo[(size_t)k * HW] = mt[k];
+        }
+        if constexpr (kDepth) {
+            float *dp = depth + (size_t)b * 2 * HW + (size_t)py * W + px;
+            dp[0] = p.last ? __fdiv_rn(dsum, __fsub_rn(1.f, p.T)) : 0.f;
+            dp[HW] = dmed;
         }
     }
     final_state[(size_t)blk * kBlock + tid] = make_float4(p.T, p.C0, p.C1, p.C2);
@@ -1427,9 +1452,10 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
     return GA_OK;
 }
 
-// K3 + K4 + K6 for all frames (a scene: the composite K4, d.P = P + Ps; mattes: K6's matte variant).
+// K3 + K4 + K6 for all frames (a scene: the composite K4, d.P = P + Ps; mattes and / or depth: K6's variant that writes them).
 int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacity, const GeomViews &g, const ImgViews &iv, const BinViews &bv,
-                              float *out_color, cudaStream_t stream, const SceneSet *scene = nullptr, const MatteSets *mattes = nullptr)
+                              float *out_color, cudaStream_t stream, const SceneSet *scene = nullptr, const MatteSets *mattes = nullptr,
+                              float *depth = nullptr)
 {
     static PerDeviceOnce attr_set;
     if (attr_set.first()) {
@@ -1437,12 +1463,20 @@ int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacit
                                            kSortMax * (int)sizeof(uint64_t)));
         GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            kSortMax * (int)sizeof(uint64_t)));
+        GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true, false, true>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, kSortMax * (int)sizeof(uint64_t)));
+        GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true, true, true>,
+                                           cudaFuncAttributeMaxDynamicSharedMemorySize, kSortMax * (int)sizeof(uint64_t)));
     }
     const float *scene_rgb = scene ? scene->rgb : nullptr;
     const int Pd = scene ? d.P - scene->Ps : d.P;
-    auto *sort_long = scene ? tile_sort_kernel<kSortThreads, kSortMax, true, true> : tile_sort_kernel<kSortThreads, kSortMax, true>;
-    auto *sort_short = scene ? tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, true>
-                             : tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false>;
+    auto *sort_long = depth ? (scene ? tile_sort_kernel<kSortThreads, kSortMax, true, true, true>
+                                     : tile_sort_kernel<kSortThreads, kSortMax, true, false, true>)
+                            : (scene ? tile_sort_kernel<kSortThreads, kSortMax, true, true> : tile_sort_kernel<kSortThreads, kSortMax, true>);
+    auto *sort_short = depth ? (scene ? tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, true, true>
+                                      : tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, false, true>)
+                             : (scene ? tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, true>
+                                      : tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false>);
     const int BT = d.B * d.T;
     if (d.P > 0) {
         {
@@ -1463,17 +1497,16 @@ int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacit
                  bv.recC, bv.seg_tile, iv.tile_maxc, scene_rgb, Pd);
     }
     GA_CHECK_LAUNCH("tile_sort_kernel");
-    if (mattes) {
-        ProfScope _ps("render_fwd_mattes_kernel", stream);
-        render_fwd_kernel<true><<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC,
-                                                          a.bg, bv.ckpt, iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color,
-                                                          *mattes);
-    } else {
-        ProfScope _ps("render_fwd_kernel", stream);
-        render_fwd_kernel<false><<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC,
-                                                           a.bg, bv.ckpt, iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color,
-                                                           MatteSets{});
-    }
+    auto render = [&](auto kernel, const char *name) {
+        ProfScope _ps(name, stream);
+        kernel<<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC, a.bg, bv.ckpt,
+                                          iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color, mattes ? *mattes : MatteSets{},
+                                          depth);
+    };
+    if (mattes && depth) render(render_fwd_kernel<true, true>, "render_fwd_mattes_depth_kernel");
+    else if (mattes) render(render_fwd_kernel<true, false>, "render_fwd_mattes_kernel");
+    else if (depth) render(render_fwd_kernel<false, true>, "render_fwd_depth_kernel");
+    else render(render_fwd_kernel<false, false>, "render_fwd_kernel");
     GA_CHECK_LAUNCH("render_fwd_kernel");
     return GA_OK;
 }
@@ -1700,11 +1733,11 @@ extern "C" int ga_rasterb_status_to_host(int32_t B, int32_t H, int32_t W, void *
 }
 
 // The batched forward (bd checked by the caller): scene NULL renders the dynamic set alone, a scene (even with Ps = 0) through the
-// composite kernels; mattes NULL writes no mattes.  Every check runs before the first launch.
-static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const MatteSets *mattes, const float *cams,
-                         const float *bg, const float *means3D, const float *colors, const float *scales, const float *rotations,
-                         const float *opacities, void *geom, void *img, void *binning, int32_t *radii, float *out_color,
-                         cudaStream_t stream)
+// composite kernels; mattes NULL writes no mattes, depth NULL no depth.  Every check runs before the first launch.
+static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const MatteSets *mattes, float *depth,
+                         const float *cams, const float *bg, const float *means3D, const float *colors, const float *scales,
+                         const float *rotations, const float *opacities, void *geom, void *img, void *binning, int32_t *radii,
+                         float *out_color, cudaStream_t stream)
 {
     if (scene == nullptr) {
         GA_REQUIRE(cams && bg && img && binning && out_color, "NULL pointer argument");
@@ -1716,7 +1749,7 @@ static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene
         const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
         const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
         if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
-        return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, nullptr, mattes);
+        return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, nullptr, mattes, depth);
     }
     GA_REQUIRE(scene->Ps >= 0 && (long long)bd->P + scene->Ps <= 0x7fffffffll, "bad static count Ps=%d (P=%d)", (int)scene->Ps, (int)bd->P);
     const int Pt = bd->P + scene->Ps;
@@ -1741,7 +1774,7 @@ static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene
     const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
     const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
     if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream, &sc)) return rc;
-    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, &sc, mattes);
+    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, &sc, mattes, depth);
 }
 
 extern "C" int ga_rasterb_forward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,
@@ -1749,7 +1782,7 @@ extern "C" int ga_rasterb_forward(const GaRasterBatchDesc *bd, const float *cams
                                   void *geom, void *img, void *binning, int32_t *radii, float *out_color, void *stream_)
 {
     if (int rc = check_batch(bd)) return rc;
-    return forward_batch(bd, nullptr, nullptr, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii, out_color,
+    return forward_batch(bd, nullptr, nullptr, nullptr, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii, out_color,
                          static_cast<cudaStream_t>(stream_));
 }
 
@@ -1760,8 +1793,26 @@ extern "C" int ga_rasterb_forward_scene(const GaRasterBatchDesc *bd, const GaRas
 {
     if (int rc = check_batch(bd)) return rc;
     GA_REQUIRE(scene != nullptr, "scene descriptor is NULL");
-    return forward_batch(bd, scene, nullptr, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii,
+    return forward_batch(bd, scene, nullptr, nullptr, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii,
                          out_color, static_cast<cudaStream_t>(stream_));
+}
+
+// Checks a GaRasterSets descriptor against the batch (bd checked) and unpacks it into the kernel's form.
+static int unpack_sets(const GaRasterBatchDesc *bd, const GaRasterSets *sets, MatteSets &ms)
+{
+    GA_REQUIRE(sets->K >= 1 && sets->K <= kMaxSets, "bad set count K=%d (1..%d)", (int)sets->K, kMaxSets);
+    GA_REQUIRE(sets->first[0] == 0, "sets: first[0] = %d, must be 0", (int)sets->first[0]);
+    for (int k = 0; k < sets->K; ++k)
+        GA_REQUIRE(sets->first[k + 1] >= sets->first[k], "sets: first[%d] = %d < first[%d] = %d (must not decrease)", k + 1,
+                   (int)sets->first[k + 1], k, (int)sets->first[k]);
+    GA_REQUIRE(sets->first[sets->K] <= bd->P, "sets: first[K=%d] = %d > P = %d (the sets index the dynamic set)", (int)sets->K,
+               (int)sets->first[sets->K], (int)bd->P);
+    GA_REQUIRE(sets->mattes != nullptr, "sets: mattes is NULL");
+    ms = MatteSets{};
+    for (int k = 0; k <= kMaxSets; ++k) ms.first[k] = (uint32_t)sets->first[k < sets->K ? k : sets->K];
+    ms.K = sets->K;
+    ms.out = sets->mattes;
+    return GA_OK;
 }
 
 extern "C" int ga_rasterb_forward_mattes(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const GaRasterSets *sets,
@@ -1771,21 +1822,26 @@ extern "C" int ga_rasterb_forward_mattes(const GaRasterBatchDesc *bd, const GaRa
 {
     if (int rc = check_batch(bd)) return rc;
     GA_REQUIRE(sets != nullptr, "sets descriptor is NULL");
-    GA_REQUIRE(sets->K >= 1 && sets->K <= kMaxSets, "bad set count K=%d (1..%d)", (int)sets->K, kMaxSets);
-    GA_REQUIRE(sets->first[0] == 0, "sets: first[0] = %d, must be 0", (int)sets->first[0]);
-    for (int k = 0; k < sets->K; ++k)
-        GA_REQUIRE(sets->first[k + 1] >= sets->first[k], "sets: first[%d] = %d < first[%d] = %d (must not decrease)", k + 1,
-                   (int)sets->first[k + 1], k, (int)sets->first[k]);
-    GA_REQUIRE(sets->first[sets->K] <= bd->P, "sets: first[K=%d] = %d > P = %d (the sets index the dynamic set)", (int)sets->K,
-               (int)sets->first[sets->K], (int)bd->P);
-    GA_REQUIRE(sets->mattes != nullptr, "sets: mattes is NULL");
-    MatteSets ms{};
-    for (int k = 0; k <= kMaxSets; ++k) ms.first[k] = (uint32_t)sets->first[k < sets->K ? k : sets->K];
-    ms.K = sets->K;
-    ms.out = sets->mattes;
+    MatteSets ms;
+    if (int rc = unpack_sets(bd, sets, ms)) return rc;
     if (scene != nullptr && scene->Ps == 0) scene = nullptr;
-    return forward_batch(bd, scene, &ms, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii, out_color,
-                         static_cast<cudaStream_t>(stream_));
+    return forward_batch(bd, scene, &ms, nullptr, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii,
+                         out_color, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int ga_rasterb_forward_depth(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const GaRasterSets *sets, float *depth,
+                                        const float *cams, const float *bg, const float *means3D, const float *colors, const float *scales,
+                                        const float *rotations, const float *opacities, void *geom, void *img, void *binning,
+                                        int32_t *radii, float *out_color, void *stream_)
+{
+    if (int rc = check_batch(bd)) return rc;
+    GA_REQUIRE(depth != nullptr, "depth is NULL");
+    MatteSets ms;
+    if (sets != nullptr)
+        if (int rc = unpack_sets(bd, sets, ms)) return rc;
+    if (scene != nullptr && scene->Ps == 0) scene = nullptr;
+    return forward_batch(bd, scene, sets ? &ms : nullptr, depth, cams, bg, means3D, colors, scales, rotations, opacities, geom, img,
+                         binning, radii, out_color, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,

@@ -407,17 +407,33 @@ def rasterize_batch_mattes(means3D, colors, scales, rotations, opacities, cams, 
     first: K+1 nondecreasing dynamic indices, first[0] = 0 and first[K] <= plan.P; set k is Gaussians first[k]..first[k+1]-1.
     Returns (images [B,3,H,W], mattes [B,K,H,W]): matte k is the weight set k's Gaussians added to each pixel (sum of alpha T
     over its blended entries), so the mattes sum to 1 - final transmittance where every splatted Gaussian is in a set."""
+    return _forward_passes("rasterize_batch_mattes", means3D, colors, scales, rotations, opacities, cams, bg, plan, first, scene, False)
+
+
+def rasterize_batch_depth(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan, scene=None, first=None):
+    """`rasterize_batch` (scene None) or `rasterize_batch_scene` that also returns a depth pass, and with `first` the mattes of
+    `rasterize_batch_mattes`, all from the one compositing launch; forward only.  Returns (images [B,3,H,W], depth [B,2,H,W]), or
+    (images, mattes [B,K,H,W], depth) with `first`.  Depths are view-space z in world units over the entries each pixel blends,
+    with the weights its colour uses: plane 0 the mean sum(w z) / (1 - T) (0 where nothing was blended), plane 1 the median, the z
+    of the first blended entry after which T <= 0.5 (0 where the final T > 0.5).  0 means no surface (z <= 0.2 is culled)."""
+    return _forward_passes("rasterize_batch_depth", means3D, colors, scales, rotations, opacities, cams, bg, plan, first, scene, True)
+
+
+def _forward_passes(name, means3D, colors, scales, rotations, opacities, cams, bg, plan, first, scene, depth):
+    """The batched forward with mattes (first not None) and / or depth: ga_rasterb_forward_mattes or ga_rasterb_forward_depth."""
     if not means3D.is_cuda:
         raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
     given = [means3D, colors, scales, rotations, opacities]
     if scene is not None:
         given += [scene.means3D, scene.shs, scene.scales, scene.rotations, scene.opacities]
     if torch.is_grad_enabled() and any(t.requires_grad for t in given):
-        raise RuntimeError("rasterize_batch_mattes is forward only: it has no backward (run it under torch.no_grad())")
-    first = [int(f) for f in first]
-    K = len(first) - 1
-    if not 1 <= K <= MAX_SETS:
-        raise ValueError(f"first has {len(first)} entries: 2..{MAX_SETS + 1} (1..{MAX_SETS} sets)")
+        raise RuntimeError(f"{name} is forward only: it has no backward (run it under torch.no_grad())")
+    K = 0
+    if first is not None:
+        first = [int(f) for f in first]
+        K = len(first) - 1
+        if not 1 <= K <= MAX_SETS:
+            raise ValueError(f"first has {len(first)} entries: 2..{MAX_SETS + 1} (1..{MAX_SETS} sets)")
     Ps = 0 if scene is None else int(scene.means3D.shape[0])
     if Ps != plan.static_P:
         raise ValueError(f"the scene has {Ps} Gaussians, the plan was sized for static_P={plan.static_P}")
@@ -432,14 +448,21 @@ def rasterize_batch_mattes(means3D, colors, scales, rotations, opacities, cams, 
         sc = _lib.GaRasterScene(Ps, int(scene.sh_degree), int(scene.shs.shape[1]), ptr(scene.means3D), ptr(scene.scales),
                                 ptr(scene.rotations), ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb))
     out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=dev)
-    mattes = torch.empty(plan.B, K, plan.H, plan.W, dtype=torch.float32, device=dev)
-    sets = _lib.GaRasterSets(K, (ctypes.c_int32 * 9)(*(first + [0] * (9 - len(first)))), ptr(mattes))
-    _lib.check(L.ga_rasterb_forward_mattes(ctypes.byref(d), None if sc is None else ctypes.byref(sc), ctypes.byref(sets), ptr(cams),
-                                           ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(opacities),
-                                           ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii), ptr(out), _stream()),
-               "ga_rasterb_forward_mattes")
+    mattes = sets = dmap = None
+    if first is not None:
+        mattes = torch.empty(plan.B, K, plan.H, plan.W, dtype=torch.float32, device=dev)
+        sets = _lib.GaRasterSets(K, (ctypes.c_int32 * 9)(*(first + [0] * (9 - len(first)))), ptr(mattes))
+    rest = (ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(opacities), ptr(plan.geom), ptr(plan.img),
+            ptr(plan.binning), ptr(plan.radii), ptr(out), _stream())
+    sc = None if sc is None else ctypes.byref(sc)
+    sets = None if sets is None else ctypes.byref(sets)
+    if depth:
+        dmap = torch.empty(plan.B, 2, plan.H, plan.W, dtype=torch.float32, device=dev)
+        _lib.check(L.ga_rasterb_forward_depth(ctypes.byref(d), sc, sets, ptr(dmap), *rest), "ga_rasterb_forward_depth")
+    else:
+        _lib.check(L.ga_rasterb_forward_mattes(ctypes.byref(d), sc, sets, *rest), "ga_rasterb_forward_mattes")
     plan.record_status()
-    return out, mattes
+    return tuple(t for t in (out, mattes, dmap) if t is not None)
 
 
 class _RasterizeGaussians(torch.autograd.Function):

@@ -188,6 +188,18 @@ int ga_rasterb_forward_mattes(const GaRasterBatchDesc *d, const GaRasterScene *s
                               const float *bg, const float *means3D, const float *colors, const float *scales,
                               const float *rotations, const float *opacities, void *geom, void *img, void *binning,
                               int32_t *radii, float *out_color, void *stream);
+/* ga_rasterb_forward_mattes (sets NULL: no mattes; scene NULL or Ps = 0: no scene) that also writes a depth pass, depth
+ * [B, 2, H, W] fp32, over the entries each pixel blends, with the weights w_i = alpha_i T_i its colour uses.  z_i is the entry's
+ * view-space depth in world units (the scene's units after its placement; K1 culls z <= 0.2, so 0 means no surface):
+ *   plane 0, mean depth:   D / (1 - T) with D = sum_i w_i z_i (accumulated as the colour channels are, so D is bit for bit the
+ *                          red channel a colour (z_i, 0, 0) with bg = 0 gives) and T the final transmittance; 0 where n_contrib = 0;
+ *   plane 1, median depth: z of the first blended entry after which T <= 0.5; 0 where the final T > 0.5.
+ * Every other output (and the mattes, with sets) is the call without depth's, bit for bit.  A NULL depth, or bad sets when sets
+ * are given, are refused before anything launches.  Forward only. */
+int ga_rasterb_forward_depth(const GaRasterBatchDesc *d, const GaRasterScene *scene, const GaRasterSets *sets, float *depth,
+                             const float *cams, const float *bg, const float *means3D, const float *colors, const float *scales,
+                             const float *rotations, const float *opacities, void *geom, void *img, void *binning, int32_t *radii,
+                             float *out_color, void *stream);
 
 /* Debug / parity accessors into the opaque buffers (device pointers; valid after the forward that filled them).  B = 1 and
  * capacity = num_rendered for buffers of the per-frame API. */

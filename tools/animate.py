@@ -27,6 +27,9 @@ first actor's placed world).  The output, camera and scene flags are shared; the
 shorter one holding its last pose.
 --mattes DIR writes DIR/{:05d}_{k}.png, actor k's visible matte (8-bit greyscale: the weight its Gaussians add to each pixel),
 with --cast or for the single avatar (its visible mask inside a scene).
+--depth DIR writes DIR/{:05d}.npy, float32 [2,H,W]: plane 0 the mean, plane 1 the median view depth of the composited frame (the
+shared world's units, 0 where there is no surface), from the same compositing pass as the frame; with --cast, --scene, --mattes
+or for the single avatar.
 """
 import argparse
 import json
@@ -143,9 +146,10 @@ def main(argv=None):
     ap.add_argument("--png", default=None)
     ap.add_argument("--raw", default=None)
     ap.add_argument("--mattes", default=None, help="DIR: each avatar's visible matte as DIR/{:05d}_{k}.png")
+    ap.add_argument("--depth", default=None, help="DIR: each frame's mean and median depth as DIR/{:05d}.npy, float32 [2,H,W]")
     a = ap.parse_args(argv)
-    if a.png is None and a.raw is None and a.mattes is None:
-        ap.error("nothing to write: give --png DIR and / or --raw FILE")
+    if a.png is None and a.raw is None and a.mattes is None and a.depth is None:
+        ap.error("nothing to write: give --png DIR, --raw FILE, --mattes DIR and / or --depth DIR")
     if a.cast is not None:
         given = [f for f, v in (("-s", a.source_path), ("-m", a.model_path), ("--epoch", a.epoch), ("--motion", a.motion), ("--body", a.body),
                                 ("--stage", a.stage)) if v is not None]
@@ -212,15 +216,16 @@ def main(argv=None):
     if a.cast is None and a.mattes is None:
         x = actors[0]
         anim = Animator(x.model, cameras, H, W, chunk=chunk, channels=channels, pose_mapper=x.pose_mapper, scene=scene,
-                        placement=x.placement)
-        playback = ((first, frames, None) for first, frames in anim.frames(x.clip, a.fps, x.speed, x.align_to))
+                        placement=x.placement, depth=a.depth is not None)
+        playback = ((first, frames, None, *depth) for first, frames, *depth in anim.frames(x.clip, a.fps, x.speed, x.align_to))
     else:
         try:
-            ens = Ensemble(actors, cameras, H, W, chunk=chunk, channels=channels, mattes=a.mattes is not None, scene=scene)
+            ens = Ensemble(actors, cameras, H, W, chunk=chunk, channels=channels, mattes=a.mattes is not None, scene=scene,
+                           depth=a.depth is not None)
         except ValueError as e:
             ap.error(str(e))
         playback = ens.frames(a.fps)
-    for d in (a.png, a.mattes):
+    for d in (a.png, a.mattes, a.depth):
         if d:
             os.makedirs(d, exist_ok=True)
     raw = None if a.raw is None else (sys.stdout.buffer if a.raw == "-" else open(a.raw, "wb"))
@@ -228,7 +233,7 @@ def main(argv=None):
     n = 0
     t0 = time.perf_counter()
     try:
-        for first, frames, mattes in playback:
+        for first, frames, mattes, *depth in playback:
             arr = frames.numpy()
             if raw is not None:
                 raw.write(arr.tobytes())
@@ -240,6 +245,10 @@ def main(argv=None):
                 for k in range(mt.shape[0]):
                     for j in range(mt.shape[1]):
                         Image.fromarray(mt[k, j], "L").save(os.path.join(a.mattes, "{:05d}_{}.png".format(first + k, j)))
+            if depth:
+                dp = depth[0].numpy()
+                for k in range(dp.shape[0]):
+                    np.save(os.path.join(a.depth, "{:05d}.npy".format(first + k)), dp[k])
             n += arr.shape[0]
     finally:
         if raw is not None and raw is not sys.stdout.buffer:

@@ -1,14 +1,17 @@
-"""Cost of rendering several avatars together (animate.Ensemble) and of their visibility mattes: 1, 2 and 4 actors of the synthetic
-avatar at 200k Gaussians (S = 512, the same model on its own clip per actor, placed side by side), 1920 x 1080 frames, the shipped
-test-pose camera, with no scene and with the 1M-Gaussian synthetic scene of tools/time_scene.py.  Run on the GPU box:
-    python tools/time_cast.py > cast.json
+"""Cost of rendering several avatars together (animate.Ensemble), of their visibility mattes and of the depth pass: 1, 2 and 4
+actors of the synthetic avatar at 200k Gaussians (S = 512, the same model on its own clip per actor, placed side by side),
+1920 x 1080 frames, the shipped test-pose camera, with no scene and with the 1M-Gaussian synthetic scene of tools/time_scene.py.
+Run on the GPU box:
+    python tools/time_cast.py [--actors 1 2] > cast.json
 For each scene, actor count and chunk = 2, 8, stage 1 (graph replays, RGB):
-  device_ms_per_frame         CUDA events around back-to-back replays of the chunk's graph, mattes off
-  mattes_ms_per_frame         the same with mattes on; the two players alternate round by round in this process
-  render_fwd_ms / render_fwd_mattes_ms   the compositing kernel alone per frame, without and with mattes (library event profiler,
-                              eager launches)
+  device_ms_per_frame         CUDA events around back-to-back replays of the chunk's graph, mattes and depth off
+  mattes_ms_per_frame         the same with mattes on
+  depth_ms_per_frame          the same with depth on (mattes off); the three players alternate round by round in this process
+  render_fwd_ms / render_fwd_mattes_ms / render_fwd_depth_ms   the compositing kernel alone per frame, plain, with mattes and with
+                              depth (library event profiler, eager launches)
 The card's name, power limit and clocks are read in the same run.
 """
+import argparse
 import json
 import os
 import statistics
@@ -45,8 +48,12 @@ def actors(m, n):
     return out
 
 
-def player(cast, cam, b, scene, mattes, capacity=None):
-    ens = an.Ensemble(cast, cam, H, W, chunk=b, mattes=mattes, scene=scene, capacity=capacity)
+VARIANTS = {"plain": {}, "mattes": dict(mattes=True), "depth": dict(depth=True)}
+KERNELS = {"plain": "render_fwd_kernel", "mattes": "render_fwd_mattes_kernel", "depth": "render_fwd_depth_kernel"}
+
+
+def player(cast, cam, b, scene, variant, capacity=None):
+    ens = an.Ensemble(cast, cam, H, W, chunk=b, scene=scene, capacity=capacity, **VARIANTS[variant])
     for _ in ens.frames(30.0):                        # warm-up: graphs captured, binning grown to what the chunks need
         pass
     times, aligns, cams = ens._playback(30.0)
@@ -57,8 +64,8 @@ def player(cast, cam, b, scene, mattes, capacity=None):
 
 
 def one(cast, cam, b, scene):
-    players = {key: player(cast, cam, b, scene, key == "mattes") for key in ("plain", "mattes")}
-    rounds = {"plain": [], "mattes": []}
+    players = {key: player(cast, cam, b, scene, key) for key in VARIANTS}
+    rounds = {key: [] for key in VARIANTS}
     with torch.no_grad():
         for _ in range(5):
             for key, (_, render) in players.items():
@@ -68,27 +75,31 @@ def one(cast, cam, b, scene):
     del players
     torch.cuda.empty_cache()
     kernels = {}
-    for key in ("plain", "mattes"):
-        ens = an.Ensemble(cast, cam, H, W, chunk=b, mattes=key == "mattes", scene=scene, graphs=False, capacity=capacity)
+    for key in VARIANTS:
+        ens = an.Ensemble(cast, cam, H, W, chunk=b, scene=scene, graphs=False, capacity=capacity, **VARIANTS[key])
         for _ in ens.frames(30.0):
             pass
         torch.cuda.synchronize()
         _lib.profile(True)
         n = 0
-        for _, f, _ in ens.frames(30.0):
+        for _, f, *_ in ens.frames(30.0):
             n += f.shape[0]
         rep = _lib.profile_report()
         _lib.profile(False)
-        name = "render_fwd_mattes_kernel" if key == "mattes" else "render_fwd_kernel"
-        kernels[key] = rep.get(name, (0, 0.0))[1] / n
+        kernels[key] = rep.get(KERNELS[key], (0, 0.0))[1] / n
         del ens
         torch.cuda.empty_cache()
     return dict(device_ms_per_frame=statistics.median(rounds["plain"]), device_rounds_ms=rounds["plain"],
                 mattes_ms_per_frame=statistics.median(rounds["mattes"]), mattes_rounds_ms=rounds["mattes"],
-                render_fwd_ms=kernels["plain"], render_fwd_mattes_ms=kernels["mattes"], overflows_while_warming=overflows)
+                depth_ms_per_frame=statistics.median(rounds["depth"]), depth_rounds_ms=rounds["depth"],
+                render_fwd_ms=kernels["plain"], render_fwd_mattes_ms=kernels["mattes"], render_fwd_depth_ms=kernels["depth"],
+                overflows_while_warming=overflows)
 
 
 def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument("--actors", type=int, nargs="+", default=list(ACTORS), help="actor counts to time (default 1 2 4)")
+    args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("no CUDA device: nothing to time")
     res = card()
@@ -99,7 +110,7 @@ def main():
     m, _ = model(1)
     for Ps in (0, 1_000_000):
         scene = synthetic_scene(Ps).to(m.device) if Ps else None
-        for n in ACTORS:
+        for n in args.actors:
             cast = actors(m, n)
             for b in CHUNKS:
                 key = f"scene{Ps}_actors{n}_chunk{b}"
@@ -114,6 +125,10 @@ def main():
     res["peak_memory_gb"] = torch.cuda.max_memory_allocated() / 1e9
     res["mattes_over_plain"] = {k: v["mattes_ms_per_frame"] / v["device_ms_per_frame"] for k, v in res.items()
                                 if isinstance(v, dict) and "mattes_ms_per_frame" in v}
+    res["depth_over_plain"] = {k: v["depth_ms_per_frame"] / v["device_ms_per_frame"] for k, v in res.items()
+                               if isinstance(v, dict) and "depth_ms_per_frame" in v}
+    res["depth_kernel_over_plain"] = {k: v["render_fwd_depth_ms"] / v["render_fwd_ms"] for k, v in res.items()
+                                      if isinstance(v, dict) and v.get("render_fwd_ms")}
     res["card_after"] = card()["nvidia_smi"]
     print(json.dumps(res, indent=1))
 
