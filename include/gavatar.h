@@ -141,6 +141,8 @@ int ga_rasterb_status_to_host(int32_t B, int32_t H, int32_t W, void *img, const 
 int ga_rasterb_forward(const GaRasterBatchDesc *d, const float *cams, const float *bg, const float *means3D,
                        const float *colors, const float *scales, const float *rotations, const float *opacities, void *geom,
                        void *img, void *binning, int32_t *radii, float *out_color, void *stream);
+/* d_rotations [B,P,4], d_opacities [B,P] and d_means2D [B,P,3] (each may be NULL) are written per frame whatever rot_stride /
+ * opac_stride are: with shared rotations / opacities the caller sums the frames. */
 int ga_rasterb_backward(const GaRasterBatchDesc *d, const float *cams, const float *bg, const float *means3D,
                         const float *colors, const float *scales, const float *rotations, const int32_t *radii,
                         const void *geom, const void *img, const void *binning, const float *dL_dout, void *scratch,

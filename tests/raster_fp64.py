@@ -1,4 +1,5 @@
-"""fp64 reference of the rasterizer's compositing (K6) and its backward (K7), with a running error bound (test helper).
+"""fp64 reference of the rasterizer's compositing (K6) and its backward (K7), with a running error bound (test helper);
+the fused preprocess backward (K8/K9) and K1's SH colour are restated with the same bound in the section at the end.
 
 It starts from what the kernels themselves stage: one frame's `xy`, `conic_opacity`, per-tile sorted Gaussian list and tile
 ranges, plus the colours, `bg` and dL/dout.  It returns, per pixel, the image, final_T and n_contrib, and per Gaussian d_colors,
@@ -327,4 +328,337 @@ def backward(fr: Frame, fw, dL_dout, restart=True, use_bg_dot=True, swap_hw=Fals
         out[name] = (acc_v[rows].T.contiguous(), bound[rows].T.contiguous())
     out["excluded"] = excluded
     out["active"] = active_n
+    return out
+
+
+# ============================================================================================ K8/K9: preprocess_bwd_kernel
+# fp64 restatement of the fused K8/K9 (preprocess_bwd_kernel) with the same running bound, from one launch's own inputs.
+#
+# Inputs (`preprocess_backward`): one frame's means3D, scales, rotations, scale_modifier, view / proj matrices and tanfov, the radii
+# and the STAGED cov3d K1 left in the geom buffer, the d_mean2D / d_conic_op K7 left in the backward scratch, and with SH the
+# coefficients, campos, K1's clamp bits and dL/drgb (K7's d_colors).  Every input is an fp32 value, so it enters with error 0.
+#
+# Exact part.  K1 and K8 both evaluate tvx, tvy, tvz, hx, hy, hw with xf_row, which uses __fmul_rn / __fmaf_rn / __fadd_rn; quat_to_rot
+# uses __fmul_rn / __fadd_rn / __fsub_rn; txtz = tvx / tvz and limx = 1.3f * tanfovx are single correctly rounded operations (the
+# library is built without fast-math).  They are reproduced bit for bit: an fp32 +, -, *, / of fp32 operands evaluated in fp64 and
+# rounded to fp32 is correctly rounded (53 >= 2 * 24 + 2, so the double rounding is innocuous), and fma32 rounds the exact a * b + c
+# once (TwoSum, with the one case where the fp64 sum lands on an fp32 midpoint resolved by the sign of the residual).  So the
+# guard-band gates x_grad_mul / y_grad_mul and the clamped tx / ty are the kernel's own, with no marginal band, and tvz must equal
+# K1's staged depth bit for bit.
+#
+# Bounded part.  Everything else is ordinary fp32 that nvcc may contract: each operation is counted as one rounding (u |result|,
+# the model of the K6 / K7 reference above), a contracted multiply-add as two, which bounds the FMA's single rounding.  The kernel's
+# left-to-right order is restated exactly, e.g. -fx * tx * tz2 = ((-fx) tx) tz2; products of compile-time constants (6.f * kShC3_0)
+# are folded in fp32 and exact here; 1.f / sqrtf(.) is a correctly rounded sqrt (sqrt_ below) and a correctly rounded division.
+# The one floating decision left is denom2inv != 0 (denom^2 + 1e-7f overflowing fp32): `marg_overflow` flags a Gaussian whose
+# bound reaches within a factor 2 of that overflow, and callers assert there is none.
+#
+# Upstream's three deviations from true autograd (oracle/raster_twin.py) are encoded as the kernel has them: a clamped tx / ty is
+# constant w.r.t. tz (dL_dtz uses the clamped value, dL_dtx / dL_dty are gated), the conic backward uses 1 / (det^2 + 1e-7), and
+# the off-diagonal dL/dB comes in the half convention (d_conic_op.y).  The quaternion is not normalised (as upstream).
+#
+# `bug` names corruptions for the self-checks: gate (dL_dtx / dL_dty ungated), tz_unclamped (dL_dtz from txtz tz), scale_mod
+# (d_scales without the outer scale_modifier), full_offdiag (dL/dB taken as the full off-diagonal), no_proj_w (the proj[4k+3] mul
+# terms dropped), norm_quat (d_rotations of the normalised quaternion), no_sh_dir (the SH direction term missing from d_means3D),
+# no_clamp_mask (d_sh ignoring the clamp bits), sh_extra (coefficient (D+1)^2 not zeroed).
+F32_MAX = 3.4028234663852886e38
+
+
+def f32(x):
+    return x.float().double()
+
+
+def fma32(a, b, c):
+    """fp32 fmaf(a, b, c) of fp32 values held in float64 tensors, rounded once."""
+    p = a * b                                   # exact: 24 + 24 bits
+    s = p + c
+    bb = s - p
+    err = (p - (s - bb)) + (c - bb)             # TwoSum: p + c = s + err exactly
+    r = f32(s)
+    inf = torch.full_like(s, math.inf).float()
+    o = torch.nextafter(r.float(), torch.where(s > r, inf, -inf)).double()
+    tie = (r != s) & ((r + o) * 0.5 == s)
+    hi, lo = torch.maximum(r, o), torch.minimum(r, o)
+    return torch.where(tie & (err != 0), torch.where(err > 0, hi, lo), r)
+
+
+def xf_row32(M, r, x, y, z):
+    t = f32(M[r] * x)
+    t = fma32(M[4 + r], y, t)
+    t = fma32(M[8 + r], z, t)
+    return f32(t + M[12 + r])
+
+
+def xf_row64(M, r, x, y, z):
+    return ((M[r] * x + M[4 + r] * y) + M[8 + r] * z) + M[12 + r]
+
+
+def quat_to_rot32(q, rn):
+    qr, qx, qy, qz = q.unbind(-1)
+    m = lambda a, b: rn(a * b)
+    R00 = rn(1.0 - m(2.0, rn(m(qy, qy) + m(qz, qz))))
+    R01 = m(2.0, rn(m(qx, qy) - m(qr, qz)))
+    R02 = m(2.0, rn(m(qx, qz) + m(qr, qy)))
+    R10 = m(2.0, rn(m(qx, qy) + m(qr, qz)))
+    R11 = rn(1.0 - m(2.0, rn(m(qx, qx) + m(qz, qz))))
+    R12 = m(2.0, rn(m(qy, qz) - m(qr, qx)))
+    R20 = m(2.0, rn(m(qx, qz) - m(qr, qy)))
+    R21 = m(2.0, rn(m(qy, qz) + m(qr, qx)))
+    R22 = rn(1.0 - m(2.0, rn(m(qx, qx) + m(qy, qy))))
+    return [[R00, R01, R02], [R10, R11, R12], [R20, R21, R22]]
+
+
+def sqrt_(a):
+    """Correctly rounded sqrtf: |sqrt(v') - sqrt(v)| <= e / (sqrt(v) + sqrt(v - e)) for |v' - v| <= e."""
+    av, ae = a
+    v = av.clamp_min(0).sqrt()
+    return _round(v, ae / (v + (av - ae).clamp_min(0).sqrt()).clamp_min(1e-300))
+
+
+def lsum(*terms):
+    """Left-to-right sum of tracked terms (a + b + c = (a + b) + c)."""
+    s = terms[0]
+    for t in terms[1:]:
+        s = add(s, t)
+    return s
+
+
+def cf32(x):
+    """A float constant as the fp32 value the kernel holds."""
+    import numpy as np
+    return float(np.float32(x))
+
+
+SH_C64 = dict(C0=0.28209479177387814, C1=0.4886025119029199, C2_0=1.0925484305920792, C2_1=-1.0925484305920792,
+            C2_2=0.31539156525252005, C2_3=-1.0925484305920792, C2_4=0.5462742152960396, C3_0=-0.5900435899266435,
+            C3_1=2.890611442640554, C3_2=-0.4570457994644658, C3_3=0.3731763325901154, C3_4=-0.4570457994644658,
+            C3_5=1.445305721320277, C3_6=-0.5900435899266435)
+SH_C32 = {k: cf32(v) for k, v in SH_C64.items()}      # the kernel's kSh* constants; the fp64 oracle uses SH_C64
+
+
+def kc(a, name, C):
+    """A constant product folded at compile time (in fp32 for the kernel's constants): a * kSh<name>."""
+    v = a * C[name]
+    return cf32(v) if C is SH_C32 else v
+
+
+def sh_dir(means, campos):
+    """sh_eval / sh_color_bwd: dir = (mean - campos) * (1 / sqrtf(|v|^2)); returns (x, y, z), inv."""
+    v = [sub((means[:, k], 0.0), (campos[k], 0.0)) for k in range(3)]
+    n2 = lsum(mul(v[0], v[0]), mul(v[1], v[1]), mul(v[2], v[2]))
+    inv = div(1.0, sqrt_(n2))
+    return [mul(v[k], inv) for k in range(3)], inv
+
+
+def sh_basis(x, y, z, C=SH_C32):
+    xx, yy, zz = mul(x, x), mul(y, y), mul(z, z)
+    one = torch.ones_like(x[0])
+    b = [(C["C0"] * one, torch.zeros_like(x[0]))]
+    b += [mul(-C["C1"], y), mul(C["C1"], z), mul(-C["C1"], x)]
+    b += [mul(mul(C["C2_0"], x), y), mul(mul(C["C2_1"], y), z), mul(C["C2_2"], sub(sub(scale(zz, 2.0), xx), yy)),
+          mul(mul(C["C2_3"], x), z), mul(C["C2_4"], sub(xx, yy))]
+    b += [mul(mul(C["C3_0"], y), sub(mul(3.0, xx), yy)), mul(mul(mul(C["C3_1"], x), y), z),
+          mul(mul(C["C3_2"], y), sub(sub(scale(zz, 4.0), xx), yy)),
+          mul(mul(C["C3_3"], z), sub(sub(scale(zz, 2.0), mul(3.0, xx)), mul(3.0, yy))),
+          mul(mul(C["C3_4"], x), sub(sub(scale(zz, 4.0), xx), yy)), mul(mul(C["C3_5"], z), sub(xx, yy)),
+          mul(mul(C["C3_6"], x), sub(xx, mul(3.0, yy)))]
+    return b
+
+
+def sh_forward(means, shs, D, campos):
+    """K1's SH colour (sh_eval) of fp32 inputs: (pre-clamp value per channel as (v, e) [P,3], rgb after the clamp)."""
+    dev = means.device if torch.is_tensor(means) else "cpu"
+    f = lambda t: torch.as_tensor(t).to(device=dev, dtype=torch.float64)
+    means, shs, campos = f(means), f(shs), f(campos).reshape(3)
+    (x, y, z), _ = sh_dir(means, campos)
+    b = sh_basis(x, y, z)
+    pre = []
+    for ch in range(3):
+        r = None
+        for k in range((D + 1) ** 2):
+            t = mul(b[k], (shs[:, k, ch], 0.0))
+            r = t if r is None else add(r, t)
+        pre.append(add(r, 0.5))
+    v = torch.stack([p[0] for p in pre], 1)
+    e = torch.stack([p[1] for p in pre], 1)
+    return (v, e), v.clamp_min(0)
+
+
+def preprocess_backward(means, view, proj, tanfovx, tanfovy, H, W, mod, radii, cov3d, d_mean2D, d_conic_op, scales=None,
+                        rots=None, depth=None, shs=None, D=0, campos=None, clamped=None, d_rgb=None, exact32=True, bug=()):
+    """preprocess_bwd_kernel for one frame's P Gaussians (tensors of fp32 values; any device, computed in float64).  Returns a
+    dict of (value, bound) pairs: d_means3D [P,3], d_cov3D [P,6], and without cov mode (scales given) d_scales [P,3] and
+    d_rotations [P,4]; with SH d_sh [P,M,3].  Culled Gaussians (radii <= 0) get exact zeros with bound 0.  `vis`, `xgm` / `ygm`
+    (the guard-band gates), `tvz` and `marg_overflow` describe the Gaussians.  exact32=False evaluates the exact part in plain
+    fp64 instead (to match the fp64 oracle)."""
+    dev = means.device
+    f = lambda t: torch.as_tensor(t).to(device=dev, dtype=torch.float64)
+    means, view, proj = f(means), f(view).reshape(16), f(proj).reshape(16)
+    radii, cov3d, d_mean2D, d_conic_op = torch.as_tensor(radii).to(dev), f(cov3d), f(d_mean2D), f(d_conic_op)
+    P = means.shape[0]
+    vis = radii > 0
+    rn = f32 if exact32 else (lambda t: t)
+    xf = xf_row32 if exact32 else xf_row64
+    px, py, pz = means[:, 0], means[:, 1], means[:, 2]
+    tvx, tvy, tvz = xf(view, 0, px, py, pz), xf(view, 1, px, py, pz), xf(view, 2, px, py, pz)
+    tanx, tany = cf32(tanfovx), cf32(tanfovy)
+    limx, limy = rn(torch.tensor(cf32(1.3) * tanx, dtype=torch.float64)), rn(torch.tensor(cf32(1.3) * tany, dtype=torch.float64))
+    limx, limy = float(limx), float(limy)
+    txtz, tytz = rn(tvx / tvz), rn(tvy / tvz)
+    xgm = ~((txtz < -limx) | (txtz > limx))
+    ygm = ~((tytz < -limy) | (tytz > limy))
+    if "gate" in bug:
+        xgm, ygm = torch.ones_like(xgm), torch.ones_like(ygm)
+    txc, tyc = txtz.clamp(-limx, limx), tytz.clamp(-limy, limy)
+    tv = (tvz, 0.0)
+    fx = div(float(W), (torch.tensor(2.0 * tanx, dtype=torch.float64, device=dev), 0.0))
+    fy = div(float(H), (torch.tensor(2.0 * tany, dtype=torch.float64, device=dev), 0.0))
+    tx, ty = mul((txc, 0.0), tv), mul((tyc, 0.0), tv)
+    tz = div(1.0, tv)
+    tz2 = mul(tz, tz)
+    tz3 = mul(tz2, tz)
+    J00, J02 = mul(fx, tz), mul(mul(neg(fx), tx), tz2)
+    J11, J12 = mul(fy, tz), mul(mul(neg(fy), ty), tz2)
+    V = lambda k: (view[k], 0.0)
+    m0 = [add(mul(V(k * 4 + 0), J00), mul(V(k * 4 + 2), J02)) for k in range(3)]
+    m1 = [add(mul(V(k * 4 + 1), J11), mul(V(k * 4 + 2), J12)) for k in range(3)]
+    c3 = [(cov3d[:, k], 0.0) for k in range(6)]
+    Sg = [[c3[0], c3[1], c3[2]], [c3[1], c3[3], c3[4]], [c3[2], c3[4], c3[5]]]
+    v0 = [lsum(mul(Sg[k][0], m0[0]), mul(Sg[k][1], m0[1]), mul(Sg[k][2], m0[2])) for k in range(3)]
+    v1 = [lsum(mul(Sg[k][0], m1[0]), mul(Sg[k][1], m1[1]), mul(Sg[k][2], m1[2])) for k in range(3)]
+    c03 = cf32(0.3)
+    a = add(lsum(mul(m0[0], v0[0]), mul(m0[1], v0[1]), mul(m0[2], v0[2])), c03)
+    b = lsum(mul(m0[0], v1[0]), mul(m0[1], v1[1]), mul(m0[2], v1[2]))
+    c = add(lsum(mul(m1[0], v1[0]), mul(m1[1], v1[1]), mul(m1[2], v1[2])), c03)
+    gA, gBh, gC = (d_conic_op[:, 0], 0.0), (d_conic_op[:, 1], 0.0), (d_conic_op[:, 2], 0.0)
+    if "full_offdiag" in bug:
+        gBh = scale(gBh, 2.0)
+    denom = sub(mul(a, c), mul(b, b))
+    dd = add(mul(denom, denom), cf32(1e-7))
+    marg_overflow = vis & (dd[0] + dd[1] >= 0.5 * F32_MAX)
+    d2i = div(1.0, dd)
+    ac = mul(a, c)
+    dL_da = mul(d2i, lsum(mul(mul(neg(c), c), gA), mul(mul(scale(b, 2.0), c), gBh), mul(sub(denom, ac), gC)))
+    dL_dc = mul(d2i, lsum(mul(mul(neg(a), a), gC), mul(mul(scale(a, 2.0), b), gBh), mul(sub(denom, ac), gA)))
+    dL_db = mul(scale(d2i, 2.0), lsum(sub(mul(mul(b, c), gA), mul(add(denom, mul(scale(b, 2.0), b)), gBh)), mul(mul(a, b), gC)))
+    dc = [None] * 6
+    for k, (i, j) in ((0, (0, 0)), (3, (1, 1)), (5, (2, 2))):
+        dc[k] = lsum(mul(mul(m0[i], m0[i]), dL_da), mul(mul(m0[i], m1[i]), dL_db), mul(mul(m1[i], m1[i]), dL_dc))
+    for k, (i, j) in ((1, (0, 1)), (2, (0, 2))):
+        dc[k] = lsum(mul(mul(scale(m0[i], 2.0), m0[j]), dL_da), mul(add(mul(m0[i], m1[j]), mul(m0[j], m1[i])), dL_db),
+                     mul(mul(scale(m1[i], 2.0), m1[j]), dL_dc))
+    dc[4] = lsum(mul(mul(scale(m0[2], 2.0), m0[1]), dL_da), mul(add(mul(m0[1], m1[2]), mul(m0[2], m1[1])), dL_db),
+                 mul(mul(scale(m1[1], 2.0), m1[2]), dL_dc))
+    dm0 = [add(mul(scale(v0[k], 2.0), dL_da), mul(v1[k], dL_db)) for k in range(3)]
+    dm1 = [add(mul(scale(v1[k], 2.0), dL_dc), mul(v0[k], dL_db)) for k in range(3)]
+    dJ00 = lsum(*[mul(V(k * 4 + 0), dm0[k]) for k in range(3)])
+    dJ02 = lsum(*[mul(V(k * 4 + 2), dm0[k]) for k in range(3)])
+    dJ11 = lsum(*[mul(V(k * 4 + 1), dm1[k]) for k in range(3)])
+    dJ12 = lsum(*[mul(V(k * 4 + 2), dm1[k]) for k in range(3)])
+    dL_dtx = mul(mul(mul((xgm.double(), 0.0), neg(fx)), tz2), dJ02)
+    dL_dty = mul(mul(mul((ygm.double(), 0.0), neg(fy)), tz2), dJ12)
+    txz, tyz = (tx, ty) if "tz_unclamped" not in bug else (mul((txtz, 0.0), tv), mul((tytz, 0.0), tv))
+    dL_dtz = lsum(sub(mul(mul(neg(fx), tz2), dJ00), mul(mul(fy, tz2), dJ11)), mul(mul(mul(scale(fx, 2.0), txz), tz3), dJ02),
+                  mul(mul(mul(scale(fy, 2.0), tyz), tz3), dJ12))
+    dmean = [lsum(mul(V(k * 4 + 0), dL_dtx), mul(V(k * 4 + 1), dL_dty), mul(V(k * 4 + 2), dL_dtz)) for k in range(3)]
+    hx, hy, hw = xf(proj, 0, px, py, pz), xf(proj, 1, px, py, pz), xf(proj, 3, px, py, pz)
+    m_w = div(1.0, add((hw, 0.0), cf32(1e-7)))
+    mul1, mul2 = mul(mul((hx, 0.0), m_w), m_w), mul(mul((hy, 0.0), m_w), m_w)
+    g2x, g2y = (d_mean2D[:, 0], 0.0), (d_mean2D[:, 1], 0.0)
+    Pm = lambda k: (proj[k], 0.0)
+    for k in range(3):
+        if "no_proj_w" in bug:
+            tx_, ty_ = mul(Pm(4 * k + 0), m_w), mul(Pm(4 * k + 1), m_w)
+        else:
+            tx_ = sub(mul(Pm(4 * k + 0), m_w), mul(Pm(4 * k + 3), mul1))
+            ty_ = sub(mul(Pm(4 * k + 1), m_w), mul(Pm(4 * k + 3), mul2))
+        dmean[k] = add(dmean[k], add(mul(tx_, g2x), mul(ty_, g2y)))
+    out = {}
+    if shs is not None:
+        shs, campos, d_rgb = f(shs), f(campos).reshape(3), f(d_rgb)
+        cl = torch.as_tensor(clamped).to(dev).long()
+        M = shs.shape[1]
+        g = [(torch.where((cl >> ch) & 1 == 1, 0.0, d_rgb[:, ch]) if "no_clamp_mask" not in bug else d_rgb[:, ch], 0.0)
+             for ch in range(3)]
+        (x, y, z), inv = sh_dir(means, campos)
+        C = SH_C32 if exact32 else SH_C64
+        bs = sh_basis(x, y, z, C)
+        nk = (D + 1) ** 2
+        s = []
+        for k in range(16):
+            if k < nk:
+                s.append(lsum(*[mul((shs[:, k, ch], 0.0), g[ch]) for ch in range(3)]))
+            else:
+                s.append((torch.zeros(P, dtype=torch.float64, device=dev), torch.zeros(P, dtype=torch.float64, device=dev)))
+        dsh_v = torch.zeros(P, M, 3, dtype=torch.float64, device=dev)
+        dsh_e = torch.zeros_like(dsh_v)
+        for k in range(min(nk + (1 if "sh_extra" in bug else 0), 16, M)):
+            for ch in range(3):
+                dsh_v[:, k, ch], dsh_e[:, k, ch] = mul(bs[k], g[ch])
+        xx, yy, zz = mul(x, x), mul(y, y), mul(z, z)
+        xy, yz, xz = mul(x, y), mul(y, z), mul(x, z)
+        kc_ = lambda a, n: kc(a, n, C)
+        ddx = lsum(mul(-C["C1"], s[3]), mul(mul(C["C2_0"], y), s[4]))
+        ddx = sub(ddx, mul(mul(kc_(2, "C2_2"), x), s[6]))
+        ddx = lsum(ddx, mul(mul(C["C2_3"], z), s[7]), mul(mul(kc_(2, "C2_4"), x), s[8]), mul(mul(kc_(6, "C3_0"), xy), s[9]),
+                   mul(mul(C["C3_1"], yz), s[10]))
+        ddx = sub(sub(ddx, mul(mul(kc_(2, "C3_2"), xy), s[11])), mul(mul(kc_(6, "C3_3"), xz), s[12]))
+        ddx = lsum(ddx, mul(mul(C["C3_4"], sub(sub(scale(zz, 4.0), mul(3.0, xx)), yy)), s[13]), mul(mul(kc_(2, "C3_5"), xz), s[14]),
+                   mul(mul(kc_(3, "C3_6"), sub(xx, yy)), s[15]))
+        ddy = lsum(mul(-C["C1"], s[1]), mul(mul(C["C2_0"], x), s[4]), mul(mul(C["C2_1"], z), s[5]))
+        ddy = sub(sub(ddy, mul(mul(kc_(2, "C2_2"), y), s[6])), mul(mul(kc_(2, "C2_4"), y), s[8]))
+        ddy = lsum(ddy, mul(mul(kc_(3, "C3_0"), sub(xx, yy)), s[9]), mul(mul(C["C3_1"], xz), s[10]),
+                   mul(mul(C["C3_2"], sub(sub(scale(zz, 4.0), xx), mul(3.0, yy))), s[11]))
+        ddy = sub(sub(sub(sub(ddy, mul(mul(kc_(6, "C3_3"), yz), s[12])), mul(mul(kc_(2, "C3_4"), xy), s[13])),
+                      mul(mul(kc_(2, "C3_5"), yz), s[14])), mul(mul(kc_(6, "C3_6"), xy), s[15]))
+        ddz = lsum(mul(C["C1"], s[2]), mul(mul(C["C2_1"], y), s[5]), mul(mul(kc_(4, "C2_2"), z), s[6]), mul(mul(C["C2_3"], x), s[7]),
+                   mul(mul(C["C3_1"], xy), s[10]), mul(mul(kc_(8, "C3_2"), yz), s[11]),
+                   mul(mul(C["C3_3"], sub(sub(mul(6.0, zz), mul(3.0, xx)), mul(3.0, yy))), s[12]), mul(mul(kc_(8, "C3_4"), xz), s[13]),
+                   mul(mul(C["C3_5"], sub(xx, yy)), s[14]))
+        dot = lsum(mul(x, ddx), mul(y, ddy), mul(z, ddz))
+        if "no_sh_dir" not in bug:
+            for k, (dk, ck) in enumerate(((ddx, x), (ddy, y), (ddz, z))):
+                dmean[k] = add(dmean[k], mul(sub(dk, mul(ck, dot)), inv))
+        out["d_sh"] = (dsh_v, dsh_e)
+    out["d_means3D"] = (torch.stack([d[0] for d in dmean], 1), torch.stack([d[1] for d in dmean], 1))
+    out["d_cov3D"] = (torch.stack([d[0] for d in dc], 1), torch.stack([d[1] for d in dc], 1))
+    if scales is not None:
+        scales, rots = f(scales), f(rots)
+        modf = cf32(mod)
+        sv = [mul(modf, (scales[:, k], 0.0)) for k in range(3)]
+        q = rots
+        if "norm_quat" in bug:
+            q = rn(q / q.norm(dim=1, keepdim=True))
+        Rm = quat_to_rot32(q, rn)
+        Rm = [[(Rm[i][j], 0.0) for j in range(3)] for i in range(3)]
+        dS = [[dc[0], scale(dc[1], 0.5), scale(dc[2], 0.5)], [scale(dc[1], 0.5), dc[3], scale(dc[4], 0.5)],
+              [scale(dc[2], 0.5), scale(dc[4], 0.5), dc[5]]]
+        dM = [[scale(lsum(*[mul(mul(sv[a2], Rm[j][a2]), dS[j][k]) for j in range(3)]), 2.0) for k in range(3)] for a2 in range(3)]
+        dsc = []
+        for a2 in range(3):
+            t = lsum(*[mul(Rm[k][a2], dM[a2][k]) for k in range(3)])
+            dsc.append(t if "scale_mod" in bug else mul(modf, t))
+        dR = [[mul(sv[a2], dM[a2][k]) for a2 in range(3)] for k in range(3)]
+        qr, qx, qy, qz = [(q[:, k], 0.0) for k in range(4)]
+        m2 = lambda t: scale(t, 2.0)
+        dqr = lsum(mul(neg(qz), dR[0][1]), mul(qy, dR[0][2]), mul(qz, dR[1][0]))
+        dqr = add(sub(sub(dqr, mul(qx, dR[1][2])), mul(qy, dR[2][0])), mul(qx, dR[2][1]))
+        dqx = lsum(mul(qy, dR[0][1]), mul(qz, dR[0][2]), mul(qy, dR[1][0]))
+        dqx = add(add(sub(sub(dqx, mul(m2(qx), dR[1][1])), mul(qr, dR[1][2])), mul(qz, dR[2][0])), mul(qr, dR[2][1]))
+        dqx = sub(dqx, mul(m2(qx), dR[2][2]))
+        dqy = lsum(mul(neg(m2(qy)), dR[0][0]), mul(qx, dR[0][1]), mul(qr, dR[0][2]), mul(qx, dR[1][0]), mul(qz, dR[1][2]))
+        dqy = sub(add(sub(dqy, mul(qr, dR[2][0])), mul(qz, dR[2][1])), mul(m2(qy), dR[2][2]))
+        dqz = sub(mul(neg(m2(qz)), dR[0][0]), mul(qr, dR[0][1]))
+        dqz = lsum(dqz, mul(qx, dR[0][2]), mul(qr, dR[1][0]))
+        dqz = lsum(sub(dqz, mul(m2(qz), dR[1][1])), mul(qy, dR[1][2]), mul(qx, dR[2][0]), mul(qy, dR[2][1]))
+        dq = [m2(t) for t in (dqr, dqx, dqy, dqz)]
+        out["d_scales"] = (torch.stack([d[0] for d in dsc], 1), torch.stack([d[1] for d in dsc], 1))
+        out["d_rotations"] = (torch.stack([d[0] for d in dq], 1), torch.stack([d[1] for d in dq], 1))
+    for k, (v, e) in out.items():
+        m = vis.reshape(-1, *([1] * (v.dim() - 1)))
+        out[k] = (torch.where(m, v, 0.0), torch.where(m, e, 0.0))
+    out.update(vis=vis, xgm=xgm & vis, ygm=ygm & vis, tvz=tvz, marg_overflow=marg_overflow)
+    if depth is not None and exact32:
+        dz = f(depth)
+        assert torch.equal(tvz[vis], dz[vis]), "K8's tvz differs from K1's staged depth"
     return out
