@@ -70,6 +70,11 @@ class GaLpipsViews(ctypes.Structure):
                 ("dz", c_vp * 5), ("dnext", c_vp * 4), ("dpool", c_vp * 2)]
 
 
+class GaTsdfDesc(ctypes.Structure):
+    _fields_ = [("nx", ctypes.c_int32), ("ny", ctypes.c_int32), ("nz", ctypes.c_int32), ("origin", ctypes.c_float * 3),
+                ("voxel", ctypes.c_float), ("trunc", ctypes.c_float)]
+
+
 # name -> (restype, argtypes); every symbol include/gavatar.h declares must be listed here (tests check both ways)
 _SIGNATURES = {
     "ga_version": (ctypes.c_int, []),
@@ -157,6 +162,13 @@ _SIGNATURES = {
     "ga_silhouette_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 5),
     "ga_silhouette_forward": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float] + [c_vp] * 8),
     "ga_silhouette_backward": (ctypes.c_int, [ctypes.c_int32] * 5 + [ctypes.c_float] + [c_vp] * 10),
+    "ga_tsdf_state_bytes": (ctypes.c_size_t, [ctypes.POINTER(GaTsdfDesc)]),
+    "ga_tsdf_reset": (ctypes.c_int, [ctypes.POINTER(GaTsdfDesc), c_vp, c_vp]),
+    "ga_tsdf_integrate": (ctypes.c_int, [ctypes.POINTER(GaTsdfDesc)] + [ctypes.c_int32] * 3 + [c_vp] * 6),
+    "ga_tsdf_mesh_workspace_bytes": (ctypes.c_size_t, [ctypes.POINTER(GaTsdfDesc)]),
+    "ga_tsdf_mesh_count": (ctypes.c_int, [ctypes.POINTER(GaTsdfDesc), c_vp, ctypes.c_int32, c_vp, ctypes.c_size_t, c_vp, c_vp]),
+    "ga_tsdf_mesh_emit": (ctypes.c_int, [ctypes.POINTER(GaTsdfDesc), c_vp, ctypes.c_int32, c_vp, ctypes.c_size_t, ctypes.c_int64,
+                                         ctypes.c_int64] + [c_vp] * 4),
 }
 
 _lib = None

@@ -552,6 +552,47 @@ int ga_silhouette_backward(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W
                            const int32_t *adj_offsets, const int32_t *adj_faces, const float *cams, const uint8_t *mask_u8, const float *w,
                            void *workspace, float *d_verts, void *stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Mesh extraction: truncated signed distance (TSDF) fusion of depth passes, then marching tetrahedra.  The grid holds samples at
+ * origin + voxel (i, j, k), 0 <= i < nx etc., each side in [2, 512].  Its state is one caller buffer of ga_tsdf_state_bytes(d) =
+ * 28 nx ny nz bytes: seven planes of nx ny nz 4-byte words, x fastest, in the order
+ *   sdf (fp32, units of trunc, in [-1, 1]), weight (int32: views that observed the sample), carve (int32: views that saw no surface
+ *   through it), r, g, b (fp32 sums of un-premultiplied colour), colour weight (int32).
+ * ga_tsdf_reset zeroes the state (asynchronously, on `stream`).
+ * ga_tsdf_integrate folds B in [1, 8] views into it, each sample's views in order (so the state does not depend on how views are
+ *   split into calls): cams [B,40] (the ga_rasterb_* camera block), depth [B,2,H,W] (ga_rasterb_forward_depth; plane 1, the median,
+ *   is read), image [B,3,H,W] rendered with bg = 0, final_T [B,H,W].  A sample is projected as the Gaussian preprocess projects a
+ *   mean and reads the nearest pixel (pixel (c, r) centred at (c, r), ties to even); a view with view-space z <= 0.2 or the pixel
+ *   outside the image is skipped.  With d the median depth there: d = 0 increments carve; else eta = d - z; eta < -trunc changes
+ *   nothing; otherwise sdf <- (sdf weight + min(1, eta / trunc)) / (weight + 1), weight + 1, and where |eta| < trunc the colour sums
+ *   gain image / (1 - final_T) and the colour weight 1.  No atomics: bit-reproducible.
+ * ga_tsdf_mesh_count / ga_tsdf_mesh_emit: the zero level set by marching tetrahedra on the Kuhn split (each cube into the six
+ *   tetrahedra (p, p + e_a, p + e_a + e_b, p + (1,1,1))).  A sample is outside (value +1) on the grid's outer layer or where
+ *   carve >= min_carve (>= 1); otherwise inside (value -1) where weight = 0; otherwise inside iff sdf < 0 (value sdf).  count writes
+ *   the vertex and face totals to totals [2] (device int32) and leaves offsets in the workspace (ga_tsdf_mesh_workspace_bytes(d));
+ *   emit, with the same state, min_carve and workspace, writes verts [V,3] (the crossing of edge (p0, p1) at t = s0 / (s0 - s1)),
+ *   colors [V,3] (the endpoints' mean colours interpolated at t; an endpoint without colour takes the other's, 0 if neither has one)
+ *   and faces [F,3] int32 wound from inside to outside.  Vertices are ordered by owning sample p and slot (edges (p, p + d), d = x, y,
+ *   z, xy, xz, yz, xyz), faces by cube, tetrahedron and triangle: the mesh is bit-reproducible, closed and 2-manifold.  emit writes no
+ *   vertex at or past vertex_capacity and no face at or past face_capacity.
+ * Bad sizes, NULL pointers, B outside [1, 8], a voxel or trunc that is not finite and > 0 are refused before anything launches.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct GaTsdfDesc {
+    int32_t nx, ny, nz;          /* samples per axis, each in [2, 512]                                      */
+    float origin[3];             /* world position of sample (0, 0, 0)                                      */
+    float voxel;                 /* sample spacing, world units                                             */
+    float trunc;                 /* truncation distance tau, world units                                    */
+} GaTsdfDesc;
+size_t ga_tsdf_state_bytes(const GaTsdfDesc *d);             /* 0 for a bad descriptor */
+int ga_tsdf_reset(const GaTsdfDesc *d, void *state, void *stream);
+int ga_tsdf_integrate(const GaTsdfDesc *d, int32_t B, int32_t H, int32_t W, const float *cams, const float *depth, const float *image,
+                      const float *final_T, void *state, void *stream);
+size_t ga_tsdf_mesh_workspace_bytes(const GaTsdfDesc *d);    /* 0 for a bad descriptor */
+int ga_tsdf_mesh_count(const GaTsdfDesc *d, const void *state, int32_t min_carve, void *workspace, size_t workspace_bytes, int32_t *totals,
+                       void *stream);
+int ga_tsdf_mesh_emit(const GaTsdfDesc *d, const void *state, int32_t min_carve, const void *workspace, size_t workspace_bytes,
+                      int64_t vertex_capacity, int64_t face_capacity, float *verts, float *colors, int32_t *faces, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
