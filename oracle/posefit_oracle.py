@@ -44,22 +44,22 @@ def rotations(aa):
     z = torch.zeros_like(d[:, 0])
     K = torch.stack([z, -d[:, 2], d[:, 1], d[:, 2], z, -d[:, 0], -d[:, 1], d[:, 0], z], 1).reshape(-1, 3, 3)
     s, c = torch.sin(theta)[:, :, None], torch.cos(theta)[:, :, None]
-    return torch.eye(3, dtype=aa.dtype) + s * K + (1.0 - c) * (K @ K)
+    return torch.eye(3, dtype=aa.dtype, device=aa.device) + s * K + (1.0 - c) * (K @ K)
 
 
 def vertices(body: Body, full_pose, transl):
-    """full_pose [B,3J] (SMPL: 72; SMPL-X: pose 66 | rest_pose 99), transl [B,3] -> [B,V,3], all fp64 torch."""
+    """full_pose [B,3J] (SMPL: 72; SMPL-X: pose 66 | rest_pose 99), transl [B,3] -> [B,V,3], all fp64 torch on the body's device."""
     nj = len(body.parents)
     out = []
     for b in range(full_pose.shape[0]):
         R = rotations(full_pose[b].reshape(nj, 3))
-        feat = (R[1:] - torch.eye(3, dtype=R.dtype)).reshape(-1)
+        feat = (R[1:] - torch.eye(3, dtype=R.dtype, device=R.device)).reshape(-1)
         v_posed = body.v_shaped + body.posedirs @ feat
         G = []
         for j in range(nj):
             p = body.parents[j]
             t = body.J[j] - (body.J[p] if p >= 0 else 0.0)
-            L = torch.cat([torch.cat([R[j], t[:, None]], 1), torch.tensor([[0.0, 0.0, 0.0, 1.0]], dtype=R.dtype)], 0)
+            L = torch.cat([torch.cat([R[j], t[:, None]], 1), torch.tensor([[0.0, 0.0, 0.0, 1.0]], dtype=R.dtype, device=R.device)], 0)
             G.append(L if p < 0 else G[p] @ L)
         G = torch.stack(G)
         A = torch.cat([G[:, :3, :3], (G[:, :3, 3] - torch.einsum("jab,jb->ja", G[:, :3, :3], body.J))[:, :, None]], 2)   # [J,3,4]

@@ -883,8 +883,7 @@ def rod_model(r, rnd):
     return R, (n, th, d, s, c, K, K2)
 
 
-def rod_bwd_model(r, gR, rnd):
-    """The Rodrigues backward of smpl_bwd_kernel op by op (it recomputes theta, d, s, c, K, K^2 as the forward does)."""
+def _rod_bwd(r, gR, rnd, pair_first):
     _, (n, th, d, s, c, K, K2) = rod_model(r, rnd)
     ds = torch.zeros_like(th)
     dcm = torch.zeros_like(th)
@@ -894,7 +893,8 @@ def rod_bwd_model(r, gR, rnd):
         dcm = rnd(dcm + rnd(gRf[:, i] * K2f[:, i]))
     t = torch.zeros_like(gR)
     for k in range(3):
-        t = rnd(rnd(t + rnd(gR[:, :, k, None] * K[:, None, :, k])) + rnd(K[:, k, :, None] * gR[:, None, k, :]))
+        a, b = gR[:, :, k, None] * K[:, None, :, k], K[:, k, :, None] * gR[:, None, k, :]
+        t = rnd(t + rnd(rnd(a) + rnd(b))) if pair_first else rnd(rnd(t + rnd(a)) + rnd(b))
     dK = rnd(rnd(s[:, None, None] * gR) + rnd(rnd(1 - c)[:, None, None] * t)).reshape(-1, 9)
     dd = torch.stack([rnd(dK[:, 7] - dK[:, 5]), rnd(dK[:, 2] - dK[:, 6]), rnd(dK[:, 3] - dK[:, 1])], 1)
     dth = rnd(rnd(ds * c) + rnd(dcm * s))
@@ -904,11 +904,106 @@ def rod_bwd_model(r, gR, rnd):
     return rnd(dr + rnd(rnd(dth[:, None] * n) / th[:, None]))
 
 
+def rod_bwd_model(r, gR, rnd):
+    """The Rodrigues backward of smpl_bwd_kernel op by op (it recomputes theta, d, s, c, K, K^2 as the forward does)."""
+    return _rod_bwd(r, gR, rnd, pair_first=False)
+
+
+def rodrigues_bwd_model(r, gR, rnd):
+    """rodrigues_bwd() of csrc/smpl_math.cuh op by op: as rod_bwd_model, except that the d(K^2) sum adds each pair of products
+    first, t += gR K^T + K^T gR, where smpl_bwd_kernel adds them one at a time."""
+    return _rod_bwd(r, gR, rnd, pair_first=True)
+
+
 def aff_abs(A, B):
     """|A| |B| for 3x4 affine transforms (implicit last row 0 0 0 1), on absolute values: [.., 3, 4]."""
     out = A[..., :3] @ B
     out[..., 3] = out[..., 3] + A[..., 3]
     return out
+
+
+def full_pose(kind, B, J, gen):
+    """Full poses [B, 3 J] fp32 of one POSES kind (or "flat_hands": random, SMPL-X hands, jaw and eyes zero) on gen's device."""
+    dev, nfull = gen.device, 3 * J
+    if kind == "zero":
+        full = torch.zeros(B, nfull, device=dev)
+    elif kind.startswith("tiny"):
+        full = torch.full((B, nfull), float(kind[4:]), device=dev)
+    elif kind in ("pi", "2pi"):
+        axis = torch.randn(B, J, 3, device=dev, generator=gen)
+        axis = axis / axis.norm(dim=-1, keepdim=True)
+        full = (axis * ((1 if kind == "pi" else 2) * math.pi - 1e-3)).view(B, nfull)
+    else:
+        full = 0.4 * torch.randn(B, nfull, device=dev, generator=gen)
+    if J == 55 and kind == "flat_hands":
+        full[:, 66:] = 0.0
+    return full.float()
+
+
+def chain_bounds(R, eR, Jr, parents, any_order=False):
+    """The global transforms G_j = G_p L_j of rotations R [B, J, 3, 3] known within eR, and bounds on their fp32 values.
+
+    L_j = [R_j | J_j - J_p]: R_j within eR, the offset one subtraction.  Each product is three products and two adds, three adds
+    for the translation, counted as gamma(4) on |G_p| |L_j|, so G_j's error is E_p |L_j| + |G_p| dL_j + gamma(4) |G_p| |L_j|.
+    That holds when the kernel forms G_j from its parent's product (smpl.cu).  With any_order, |G_p| is replaced by
+    |L_root| ... |L_p|, which bounds every association of the chain, e.g. chain_product's right to left (posmap.cu).
+    Returns L, dL, G, EG [B, J, 3, 4] in fp64."""
+    B, J = R.shape[:2]
+    rel = Jr.clone()
+    rel[1:] = Jr[1:] - Jr[list(parents[1:])]
+    L = torch.cat([R, rel[None, :, :, None].expand(B, J, 3, 1)], -1)
+    dL = torch.cat([eR, (U * rel.abs())[None, :, :, None].expand(B, J, 3, 1)], -1)
+    G = [None] * J
+    E = [None] * J
+    P = [None] * J                                  # |G| of the association the bound assumes
+    G[0], E[0], P[0] = L[:, 0], dL[:, 0], L[:, 0].abs()
+    for j in range(1, J):
+        pj = parents[j]
+        G[j] = G[pj][..., :3] @ L[:, j]
+        G[j][..., 3] = G[j][..., 3] + G[pj][..., 3]
+        Pp = P[pj] if any_order else G[pj].abs()
+        absG = aff_abs(Pp, L[:, j].abs())
+        E[j] = aff_abs(E[pj], L[:, j].abs()) + Pp[..., :3] @ dL[:, j] + gam(4) * absG
+        P[j] = absG if any_order else None
+    return L, dL, torch.stack(G, 1), torch.stack(E, 1)
+
+
+def rest_relative_bwd_bounds(dA, eA, Jr):
+    """dG of dA [B, J, 3, 4] through A = G - pad(G_R J_j) (rest_relative): dG_R = dA_R - dA_t J^T, two roundings; dG_t = dA_t."""
+    dG = dA.clone()
+    dG[..., :3] = dA[..., :3] - dA[..., 3:] * Jr[None, :, None, :]
+    eG = eA.clone()
+    eG[..., :3] = eA[..., :3] + eA[..., 3:] * Jr.abs()[None, :, None, :] + gam(2) * (dA[..., :3].abs() + dA[..., 3:].abs() * Jr.abs()[None, :, None, :])
+    return dG, eG
+
+
+def reverse_walk_bounds(G, EG, L, dL, dG, eG, parents):
+    """The joint chain run backwards, leaves first, restated on error bounds: dG [B, J, 3, 4] known within eG -> (dR, edR) lists of
+    [B, 3, 3], one per joint.  dL_i = G_p^T dG_i (three products, two adds) takes the forward error EG of G_p and dG_i's;
+    dG_p += dG_i L_i^T (four products, three adds, one accumulate: gamma(5) and u |dG_p|) takes L_i's error dL."""
+    J = len(parents)
+    dG = list(dG.unbind(1))
+    eG = list(eG.unbind(1))
+    dLR = [None] * J
+    eLR = [None] * J
+    for i in range(J - 1, 0, -1):
+        pj = parents[i]
+        GpR, EpR = G[:, pj, :, :3], EG[:, pj, :, :3]
+        dLR[i] = GpR.transpose(-1, -2) @ dG[i][..., :3]
+        eLR[i] = EpR.transpose(-1, -2) @ dG[i][..., :3].abs() + GpR.abs().transpose(-1, -2) @ eG[i][..., :3] \
+            + gam(3) * (GpR.abs().transpose(-1, -2) @ dG[i][..., :3].abs())
+        Li, dLi = L[:, i], dL[:, i]
+        add = dG[i] @ Li.transpose(-1, -2)                                    # [B,3,3]
+        newR = dG[pj][..., :3] + add
+        eG[pj] = eG[pj].clone()
+        eG[pj][..., :3] = eG[pj][..., :3] + eG[i] @ Li.abs().transpose(-1, -2) + dG[i].abs() @ dLi.transpose(-1, -2) \
+            + gam(5) * (dG[i].abs() @ Li.abs().transpose(-1, -2)) + U * newR.abs()
+        newt = dG[pj][..., 3] + dG[i][..., 3]
+        eG[pj][..., 3] = eG[pj][..., 3] + eG[i][..., 3] + U * newt.abs()
+        dG[pj] = dG[pj].clone()
+        dG[pj][..., :3], dG[pj][..., 3] = newR, newt
+    dLR[0], eLR[0] = dG[0][..., :3], eG[0][..., :3]
+    return dLR, eLR
 
 
 class BodyCase:
@@ -923,20 +1018,7 @@ class BodyCase:
         self.Jr = a.rest_joints.to(DEV).contiguous()
         self.inv = torch.linalg.inv(a.cano_joint_mats.double()).float().to(DEV).contiguous()
         gen = torch.Generator(device=DEV).manual_seed(seed)
-        nfull = 3 * self.J
-        if kind == "zero":
-            full = torch.zeros(B, nfull, device=DEV)
-        elif kind.startswith("tiny"):
-            full = torch.full((B, nfull), float(kind[4:]), device=DEV)
-        elif kind in ("pi", "2pi"):
-            axis = torch.randn(B, self.J, 3, device=DEV, generator=gen)
-            axis = axis / axis.norm(dim=-1, keepdim=True)
-            full = (axis * ((1 if kind == "pi" else 2) * math.pi - 1e-3)).view(B, nfull)
-        else:
-            full = 0.4 * torch.randn(B, nfull, device=DEV, generator=gen)
-        if x and kind == "flat_hands":
-            full[:, 66:] = 0.0
-        self.full = full.float()
+        self.full = full_pose(kind, B, self.J, gen)
         self.transl = 0.3 * torch.randn(B, 3, device=DEV, generator=gen)
         self.where = f"{body} {kind} B={B}"
 
@@ -956,21 +1038,7 @@ class BodyCase:
         eR = rnd.bound(R).detach().view(B, J, 3, 3)
         R = R.detach().view(B, J, 3, 3)
         Jr = self.Jr.double()
-        rel = Jr.clone()
-        rel[1:] = Jr[1:] - Jr[P[1:]]
-        L = torch.cat([R, rel[None, :, :, None].expand(B, J, 3, 1)], -1)
-        dL = torch.cat([eR, (U * rel.abs())[None, :, :, None].expand(B, J, 3, 1)], -1)
-        G = [None] * J
-        E = [None] * J
-        G[0], E[0] = L[:, 0], dL[:, 0]
-        for j in range(1, J):
-            pj = P[j]
-            G[j] = G[pj][..., :3] @ L[:, j]
-            G[j][..., 3] = G[j][..., 3] + G[pj][..., 3]
-            absG = aff_abs(G[pj].abs(), L[:, j].abs())
-            E[j] = aff_abs(E[pj], L[:, j].abs()) + G[pj][..., :3].abs() @ dL[:, j] + gam(4) * absG
-        self.G, self.EG = torch.stack(G, 1), torch.stack(E, 1)
-        self.L, self.dL = L, dL
+        self.L, self.dL, self.G, self.EG = chain_bounds(R, eR, Jr, P)
         GR, Gt = self.G[..., :3], self.G[..., 3]
         A = self.G.clone()
         GJ = (GR * Jr[None, :, None, :]).sum(-1)
@@ -1000,34 +1068,10 @@ class BodyCase:
         dA = dC @ inv.transpose(-1, -2)
         eA = gam(4) * (dC.abs() @ inv.abs().transpose(-1, -2))
         Jr = self.Jr.double()
-        dG = dA.clone()
-        dG[..., :3] = dA[..., :3] - dA[..., 3:] * Jr[None, :, None, :]
-        eG = eA.clone()
-        eG[..., :3] = eA[..., :3] + eA[..., 3:] * Jr.abs()[None, :, None, :] + gam(2) * (dA[..., :3].abs() + dA[..., 3:].abs() * Jr.abs()[None, :, None, :])
+        dG, eG = rest_relative_bwd_bounds(dA, eA, Jr)
         dtr = dA[..., 3].sum(1)
         etr = eA[..., 3].sum(1) + gam(J) * dA[..., 3].abs().sum(1)
-        dG = list(dG.unbind(1))
-        eG = list(eG.unbind(1))
-        dLR = [None] * J
-        eLR = [None] * J
-        G, EG, L, dL = self.G, self.EG, self.L, self.dL
-        for i in range(J - 1, 0, -1):
-            pj = P[i]
-            GpR, EpR = G[:, pj, :, :3], EG[:, pj, :, :3]
-            dLR[i] = GpR.transpose(-1, -2) @ dG[i][..., :3]
-            eLR[i] = EpR.transpose(-1, -2) @ dG[i][..., :3].abs() + GpR.abs().transpose(-1, -2) @ eG[i][..., :3] \
-                + gam(3) * (GpR.abs().transpose(-1, -2) @ dG[i][..., :3].abs())
-            Li, dLi = L[:, i], dL[:, i]
-            add = dG[i] @ Li.transpose(-1, -2)                                    # [B,3,3]
-            newR = dG[pj][..., :3] + add
-            eG[pj] = eG[pj].clone()
-            eG[pj][..., :3] = eG[pj][..., :3] + eG[i] @ Li.abs().transpose(-1, -2) + dG[i].abs() @ dLi.transpose(-1, -2) \
-                + gam(5) * (dG[i].abs() @ Li.abs().transpose(-1, -2)) + U * newR.abs()
-            newt = dG[pj][..., 3] + dG[i][..., 3]
-            eG[pj][..., 3] = eG[pj][..., 3] + eG[i][..., 3] + U * newt.abs()
-            dG[pj] = dG[pj].clone()
-            dG[pj][..., :3], dG[pj][..., 3] = newR, newt
-        dLR[0], eLR[0] = dG[0][..., :3], eG[0][..., :3]
+        dLR, eLR = reverse_walk_bounds(self.G, self.EG, self.L, self.dL, dG, eG, P)
         kT = self.kT
         gR = torch.stack(dLR[:kT], 1).reshape(B * kT, 3, 3)
         egR = torch.stack(eLR[:kT], 1).reshape(B * kT, 3, 3)
