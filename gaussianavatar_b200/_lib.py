@@ -169,6 +169,7 @@ _SIGNATURES = {
     "ga_tsdf_mesh_count": (ctypes.c_int, [ctypes.POINTER(GaTsdfDesc), c_vp, ctypes.c_int32, c_vp, ctypes.c_size_t, c_vp, c_vp]),
     "ga_tsdf_mesh_emit": (ctypes.c_int, [ctypes.POINTER(GaTsdfDesc), c_vp, ctypes.c_int32, c_vp, ctypes.c_size_t, ctypes.c_int64,
                                          ctypes.c_int64] + [c_vp] * 4),
+    "ga_skin_weights": (ctypes.c_int, [ctypes.c_int32] * 6 + [c_vp] * 6),
 }
 
 _lib = None

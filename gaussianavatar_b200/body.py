@@ -18,6 +18,11 @@ SMPL_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17
 # three segments each), kintree_table[0] of SMPLX_*.npz
 SMPLX_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 15, 15, 15, 20, 25, 26, 20, 28, 29, 20,
                  31, 32, 20, 34, 35, 20, 37, 38, 21, 40, 41, 21, 43, 44, 21, 46, 47, 21, 49, 50, 21, 52, 53]
+SMPL_JOINT_NAMES = ("pelvis", "left_hip", "right_hip", "spine1", "left_knee", "right_knee", "spine2", "left_ankle", "right_ankle", "spine3",
+                    "left_foot", "right_foot", "neck", "left_collar", "right_collar", "head", "left_shoulder", "right_shoulder",
+                    "left_elbow", "right_elbow", "left_wrist", "right_wrist", "left_hand", "right_hand")
+SMPLX_JOINT_NAMES = SMPL_JOINT_NAMES[:22] + ("jaw", "left_eye", "right_eye") + tuple(
+    f"{side}_{finger}{s}" for side in ("left", "right") for finger in ("index", "middle", "pinky", "ring", "thumb") for s in (1, 2, 3))
 
 MESH_FIELDS = ("v_template", "shapedirs", "posedirs", "weights", "f", "J_regressor")
 

@@ -210,6 +210,14 @@ def extract_mesh(model, pose, transl, rest_pose=None, res: int = 256, views: int
     and truncation trunc_voxels voxels, meshed with `min_carve`.  The model's state is left as it was."""
     with kept_state(model):
         means, scales, colors = posed_gaussians(model, pose, transl, rest_pose, pose_mapper)
+    return mesh_gaussians(model, means, scales, colors, res, views, size, trunc_voxels, min_carve)
+
+
+@torch.no_grad()
+def mesh_gaussians(model, means, scales, colors, res: int = 256, views: int = 64, size: int = 512, trunc_voxels: float = 4,
+                   min_carve: int = 1):
+    """The mesh of a set of the model's Gaussians, means, scales, colors [1,N,3] on the device (rendered with its rotations and
+    opacities), as `extract_mesh` returns it."""
     origin, voxel, dims, trunc = fusion_grid(means, scales, res, trunc_voxels)
     vol = TsdfVolume(origin, voxel, dims, trunc, device=means.device)
     center = np.asarray(vol.origin) + 0.5 * voxel * (np.asarray(dims) - 1)

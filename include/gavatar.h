@@ -593,6 +593,22 @@ int ga_tsdf_mesh_count(const GaTsdfDesc *d, const void *state, int32_t min_carve
 int ga_tsdf_mesh_emit(const GaTsdfDesc *d, const void *state, int32_t min_carve, const void *workspace, size_t workspace_bytes,
                       int64_t vertex_capacity, int64_t face_capacity, float *verts, float *colors, int32_t *faces, void *stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Skin-weight transfer: per mesh vertex v of verts [V,3] (canonical space), the K joints it moves with, taken from the skinning rows
+ * lbs [N,ld] of the N canonical Gaussian means [N,3] around it.
+ *   Nearest means: the k nearest means by the fp32 squared distance d2 = __fadd_rn(__fadd_rn(dx dx, dy dy), dz dz), d = mean - v,
+ *     each product and difference rounded on its own (no fused multiply-add); equal distances go to the lower Gaussian index.
+ *   Blend (fp64, in neighbour order): c_i = 1 / (d2_i + eps^2), eps = 1e-3 world units; w_j = (sum_i c_i lbs_i[j]) / (sum_i c_i)
+ *     for j < J (columns J..ld-1, e.g. SMPL-X's zero 56th, never count).
+ *   Select: the K joints of largest positive w_j (equal weights go to the lower joint), renormalised to sum to 1 (the fp64 sum in
+ *     slot order, each weight then rounded to fp32), written heaviest first as joints [V,K] uint8 and weights [V,K] fp32.  Slots left
+ *     without a joint of positive weight are written (0, 0.0); a vertex whose blend is zero everywhere gets (0, 1.0) in slot 0.
+ * One thread per vertex, no atomics: bit-reproducible.  Sizes outside 1 <= k <= min(16, N), 1 <= K <= min(8, J), 1 <= J <= ld <= 256,
+ * V, N >= 1, and NULL pointers are refused before anything launches.
+ * ---------------------------------------------------------------------------------------------------------------- */
+int ga_skin_weights(int32_t V, int32_t N, int32_t J, int32_t ld, int32_t k, int32_t K, const float *verts, const float *means,
+                    const float *lbs, uint8_t *joints, float *weights, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

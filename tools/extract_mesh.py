@@ -9,6 +9,13 @@ does, --align_to mapping its first frame onto a training frame) and writes OUT/{
 --res samples along the grid's longest side, --views fusion views of --size x --size pixels, --trunc the truncation in voxels,
 --min_carve the views that must see through a sample to carve it.  --iou prints each mesh's silhouette IoU against the avatar's own
 (median depth > 0) from the dataset camera.  One JSON line per mesh goes to stdout.
+
+    python tools/extract_mesh.py -s DATA -m MODEL --epoch N --format glb --motion walk.npz --fps 30 --out rig
+
+--format glb writes one rigged mesh, OUT/avatar.glb (gaussianavatar_b200.rig): the canonical mesh, the body skeleton and
+--influences (4 or 8) skin weights per vertex, with --motion CLIP baked in as an animation at --fps (--up: the clip world's up
+axis, by default -y for a smpl_parms.pth or with --align_to, else z).  --iou poses the rig at every baked frame, or at each --frame K
+without a clip, and prints its silhouette IoUs.  One JSON line goes to stdout.
 """
 import argparse
 import json
@@ -48,11 +55,20 @@ def parse(argv=None):
     ap.add_argument("--size", type=int, default=512)
     ap.add_argument("--trunc", type=float, default=4.0, help="truncation distance in voxels")
     ap.add_argument("--min_carve", type=int, default=1)
-    ap.add_argument("--format", choices=("ply", "obj"), default="ply")
+    ap.add_argument("--format", choices=("ply", "obj", "glb"), default="ply")
+    ap.add_argument("--influences", type=int, choices=(4, 8), default=None, help="glb: joints per vertex (default 4)")
+    ap.add_argument("--up", choices=("y", "z", "-y"), default=None, help="glb: the clip world's up axis")
     ap.add_argument("--out", required=True)
     ap.add_argument("--iou", action="store_true")
     a = ap.parse_args(argv)
-    if (a.frame is None) == (a.motion is None):
+    if a.format != "glb" and (a.influences is not None or a.up is not None):
+        ap.error("--influences and --up go with --format glb")
+    if a.format == "glb":
+        if a.frame is not None and a.motion is not None:
+            ap.error("give --frame K (repeatable) or --motion CLIP, not both")
+        if a.up is not None and a.motion is None:
+            ap.error("--up goes with --motion")
+    elif (a.frame is None) == (a.motion is None):
         ap.error("give --frame K (repeatable) or --motion CLIP, not both")
     if a.motion is None and (a.fps is not None or a.align_to is not None or a.clip_fps is not None):
         ap.error("--fps, --clip_fps and --align_to go with --motion")
@@ -83,6 +99,8 @@ def dataset_camera(src):
 
 def main(argv=None):
     a = parse(argv)
+    if a.format == "glb":
+        return main_glb(a)
     from animate import load_actor
     from gaussianavatar_b200 import animate as an
     from gaussianavatar_b200.mesh_extract import extract_mesh, silhouette_iou, write_obj, write_ply
@@ -125,6 +143,61 @@ def main(argv=None):
         if cam is not None:
             rec["iou"] = round(silhouette_iou(model, pose, transl, verts, faces, cam[0], cam[1], cam[2], rest, actor.pose_mapper)[0], 5)
         print(json.dumps(rec), flush=True)
+    return 0
+
+
+def main_glb(a):
+    from animate import load_actor
+    from gaussianavatar_b200 import animate as an
+    from gaussianavatar_b200 import rig as rg
+    from gaussianavatar_b200.mesh_extract import silhouette_iou
+
+    spec = dict(source_path=a.source_path, model_path=a.model_path, epoch=a.epoch, stage=a.stage, body=a.body, clip=None, speed=1.0,
+                align_to=a.align_to, smpl_model=a.smpl_model, smpl_gender=a.smpl_gender, uv_template=a.uv_template,
+                query_posmap_size=a.query_posmap_size, inp_posmap_size=a.inp_posmap_size, nf=a.nf, white_background=True)
+    actor = load_actor(spec, a.project_path, None)
+    model, body = actor.model, actor.model.body
+    F = int(model.pose.weight.shape[0])
+    for k in a.frame or []:
+        if not 0 <= k < F:
+            raise SystemExit(f"--frame {k}: the model has training frames 0..{F - 1}")
+    t0 = time.perf_counter()
+    rig = rg.extract_rigged_mesh(model, res=a.res, views=a.views, size=a.size, trunc_voxels=a.trunc, min_carve=a.min_carve,
+                                 influences=a.influences or 4, pose_mapper=actor.pose_mapper)
+    motion = None
+    if a.motion is not None:
+        clip = an.MotionClip.load(a.motion, body.name, fps=a.clip_fps)
+        motion = rg.bake_motion(model, clip, a.fps, a.align_to, a.up, clip_path=a.motion)
+    torch.cuda.synchronize()
+    os.makedirs(a.out, exist_ok=True)
+    path = os.path.join(a.out, "avatar.glb")
+    rg.write_glb(path, rig, motion)
+    rec = dict(mesh=path, vertices=int(rig.verts.shape[0]), faces=int(rig.faces.shape[0]), joints=len(rig.parents),
+               frames=0 if motion is None else motion.frames, seconds=round(time.perf_counter() - t0, 4))
+    if a.iou:
+        cam = dataset_camera(a.source_path)
+        if motion is not None:        # the baked frames, carried back from glTF's +Y up into the clip's world
+            poses = [(motion, i) for i in range(motion.frames)]
+            pose, trans = an.motion_sample(clip.pose.to(model.device).contiguous(), clip.trans.to(model.device).contiguous(),
+                                           torch.from_numpy(an.sample_times(clip.num_keys, clip.fps, a.fps)).to(model.device),
+                                           torch.from_numpy(an.Ensemble._alignment(model, clip, a.align_to)).to(model.device))
+            pose, rest = body.split(pose)
+        else:
+            pose, rest = None, None
+            if body.rest_width:
+                train = an.MotionClip.load(os.path.join(a.source_path, "train", "smpl_parms.pth"), body.name, fps=30.0)
+                rest = body.split(train.pose)[1][a.frame or []].to(model.device)
+            pose = model.pose.weight.detach()[a.frame or []]
+            trans = model.transl.weight.detach()[a.frame or []]
+            full = body.join(pose, rest) if body.rest_width else pose
+            poses = [(rg.bake_poses(model._rest_joints, full[i:i + 1], trans[i:i + 1], 1.0, "y"), 0) for i in range(len(a.frame or []))]
+        ious = []
+        for i, (m, f) in enumerate(poses):
+            v = torch.from_numpy(rg.pose_rig(rig, m, f) @ m.up_rotation).float().to(model.device)
+            ious.append(round(silhouette_iou(model, pose[i], trans[i], v, rig.faces, cam[0], cam[1], cam[2],
+                                             None if rest is None else rest[i], actor.pose_mapper)[0], 5))
+        rec["iou"] = ious
+    print(json.dumps(rec), flush=True)
     return 0
 
 
