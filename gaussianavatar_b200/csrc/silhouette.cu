@@ -61,27 +61,35 @@ struct Near {
     bool inside;
 };
 
-// Face f at pixel centre (px, py): false where D_f is truncated to 0.
+// Face f at pixel centre (px, py): false where D_f is truncated to 0.  The per-edge geometry is evaluated in fp64 from the fp32
+// corners: a corner may lie anywhere in the 2^20-pixel guard band, and near an edge of length l, w - t e cancels to an error of
+// ~1e-7 l in fp32, which moved d^2 by up to ~0.3 for a corner 10^6 pixels away (tests/test_silhouette_kernels_gpu.py, long-edge
+// tier).  d^2, t and p - q are rounded to fp32 once; softplus, sigmoid and the sums stay in fp32.
 __device__ __forceinline__ bool eval_face(const FaceXY &f, float px, float py, float inv_sigma, float trunc_d2, Near &n)
 {
-    float best = INFINITY;
+    double best = INFINITY, bt = 0.0, bdx = 0.0, bdy = 0.0;
     bool pos = true, neg = true;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         const int k1 = k == 2 ? 0 : k + 1;
-        const float ex = f.x[k1] - f.x[k], ey = f.y[k1] - f.y[k];
-        const float wx = px - f.x[k], wy = py - f.y[k];
-        const float cr = ex * wy - ey * wx;
-        pos = pos && cr >= 0.f;
-        neg = neg && cr <= 0.f;
-        const float t = fminf(fmaxf((wx * ex + wy * ey) / (ex * ex + ey * ey), 0.f), 1.f);
-        const float dx = wx - t * ex, dy = wy - t * ey;
-        const float d2 = dx * dx + dy * dy;
-        if (d2 < best) { best = d2; n.t = t; n.dx = dx; n.dy = dy; n.edge = k; }
+        const double ax = f.x[k], ay = f.y[k];
+        const double ex = (double)f.x[k1] - ax, ey = (double)f.y[k1] - ay;
+        const double wx = (double)px - ax, wy = (double)py - ay;
+        const double cr = ex * wy - ey * wx;
+        pos = pos && cr >= 0.0;
+        neg = neg && cr <= 0.0;
+        const double t = fmin(fmax((wx * ex + wy * ey) / (ex * ex + ey * ey), 0.0), 1.0);
+        const double dx = wx - t * ex, dy = wy - t * ey;
+        const double d2 = dx * dx + dy * dy;
+        if (d2 < best) { best = d2; bt = t; bdx = dx; bdy = dy; n.edge = k; }
     }
     n.inside = pos || neg;
-    if (!n.inside && best > trunc_d2) return false;
-    n.x = (n.inside ? best : -best) * inv_sigma;
+    if (!n.inside && best > (double)trunc_d2) return false;
+    const float b32 = (float)best;
+    n.x = (n.inside ? b32 : -b32) * inv_sigma;
+    n.t = (float)bt;
+    n.dx = (float)bdx;
+    n.dy = (float)bdy;
     return true;
 }
 
