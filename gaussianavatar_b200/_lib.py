@@ -170,6 +170,10 @@ _SIGNATURES = {
     "ga_tsdf_mesh_emit": (ctypes.c_int, [ctypes.POINTER(GaTsdfDesc), c_vp, ctypes.c_int32, c_vp, ctypes.c_size_t, ctypes.c_int64,
                                          ctypes.c_int64] + [c_vp] * 4),
     "ga_skin_weights": (ctypes.c_int, [ctypes.c_int32] * 6 + [c_vp] * 6),
+    "ga_mesh_shade_unlit": (ctypes.c_int, [ctypes.c_int32] * 5 + [c_vp] * 7 + [ctypes.c_int32] * 2 + [c_vp] * 3),
+    "ga_mesh_laplacian": (ctypes.c_int, [ctypes.c_int32] + [c_vp] * 5),
+    "ga_texture_pushpull_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int32] * 2),
+    "ga_texture_pushpull": (ctypes.c_int, [ctypes.c_int32] * 2 + [c_vp] * 3 + [ctypes.c_size_t, c_vp, c_vp]),
 }
 
 _lib = None

@@ -13,6 +13,8 @@
 //                             covers the whole frame costs one bounded loop per pixel instead of one unbounded loop in one thread.
 //   mesh_shade_kernel         per (pixel, frame): resolves the winner, recomputes its weights and shades it (glTF metallic-roughness
 //                             BRDF, one headlight), or writes the background.
+//   mesh_unlit_kernel         (ga_mesh_shade_unlit, after ga_mesh_render) per (pixel, frame): the drawn face's weights, recomputed
+//                             from its projected corners, interpolate vertex colours or a texture coordinate sampled bilinearly.
 //
 // Coverage: a pixel is covered when its centre is (pixel (c, r) sits at window position (c, r), as the Gaussians' pixels do).  The
 // winner per pixel is the 64-bit atomicMin of (fp32 depth bits << 32) | face: the nearest face, and the lower index at equal
@@ -67,13 +69,27 @@ struct FaceSetup {
     int c0, c1, r0, r1;               // pixel box, inclusive, clipped to the frame
 };
 
-__device__ __forceinline__ bool setup_face(const ScreenVert *__restrict__ sv, const int *__restrict__ faces, int f, int H, int W, FaceSetup &s)
+__device__ __forceinline__ ScreenVert screen_vert(const float *__restrict__ cam, int H, int W, const float *__restrict__ p)
+{
+    float pixx, pixy, tvz;
+    mesh::project(cam, H, W, p[0], p[1], p[2], pixx, pixy, tvz);
+    ScreenVert s;
+    s.ok = mesh::drawable(pixx, pixy, tvz);
+    s.x = s.ok ? snap_fixed((double)pixx * 256.0) : 0;
+    s.y = s.ok ? -snap_fixed((double)pixy * 256.0) : 0;
+    s.z = tvz;
+    return s;
+}
+
+// sv: the screen positions of all vertices, or (sv_local) those of face f's three corners
+__device__ __forceinline__ bool setup_face(const ScreenVert *__restrict__ sv, const int *__restrict__ faces, int f, int H, int W, FaceSetup &s,
+                                           const ScreenVert *sv_local = nullptr)
 {
     s.f = f;
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
         const int vi = faces[3 * (size_t)f + i];
-        const ScreenVert q = sv[vi];
+        const ScreenVert q = sv_local ? sv_local[i] : sv[vi];
         if (!q.ok) return false;
         s.v[i] = vi; s.x[i] = q.x; s.y[i] = q.y; s.z[i] = q.z;
     }
@@ -144,15 +160,7 @@ mesh_vertex_kernel(int V, int H, int W, const float *__restrict__ verts, const i
     normalize3(n);
     float *no = normals + ((size_t)b * V + v) * 3;
     no[0] = n[0]; no[1] = n[1]; no[2] = n[2];
-
-    float pixx, pixy, tvz;
-    mesh::project(cams + (size_t)b * kCamStride, H, W, X[3 * (size_t)v], X[3 * (size_t)v + 1], X[3 * (size_t)v + 2], pixx, pixy, tvz);
-    ScreenVert s;
-    s.ok = mesh::drawable(pixx, pixy, tvz);
-    s.x = s.ok ? snap_fixed((double)pixx * 256.0) : 0;
-    s.y = s.ok ? -snap_fixed((double)pixy * 256.0) : 0;
-    s.z = tvz;
-    sv[(size_t)b * V + v] = s;
+    sv[(size_t)b * V + v] = screen_vert(cams + (size_t)b * kCamStride, H, W, X + 3 * (size_t)v);
 }
 
 __global__ void __launch_bounds__(128)
@@ -296,6 +304,68 @@ mesh_shade_kernel(int V, int H, int W, const float *__restrict__ verts, const in
     for (int ch = 0; ch < 3; ++ch) out[(size_t)ch * n] = c[ch];
 }
 
+// Unlit resolve of a drawn frame: per pixel, the face mesh_shade_kernel resolved there, its perspective-correct weights w_i = q_i / sum
+// recomputed in fp64 from the same snapped corners, and either the interpolated vertex colours or a bilinear texture sample at the
+// interpolated texture coordinate (glTF's: texel (c, r) centred at ((c + 0.5) / Tw, (r + 0.5) / Th), row 0 first, clamped to the edge).
+// Every step is an explicitly rounded fp64 operation, rounded to fp32 once at the end.
+__global__ void __launch_bounds__(256)
+mesh_unlit_kernel(int V, int F, int H, int W, const float *__restrict__ verts, const int *__restrict__ faces, const float *__restrict__ cams,
+                  const int *__restrict__ face_id, const float *__restrict__ colors, const float *__restrict__ uvs, const float *__restrict__ tex,
+                  int Th, int Tw, const float *__restrict__ background, float *__restrict__ rgb)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x, b = blockIdx.y;
+    const int n = H * W;
+    if (t >= n) return;
+    float *out = rgb + (size_t)b * 3 * n + t;
+    const int f = face_id[(size_t)b * n + t];
+    const float *X = verts + (size_t)b * V * 3, *cam = cams + (size_t)b * kCamStride;
+    FaceSetup s;
+    bool drawn = f >= 0 && f < F;
+    if (drawn) {
+        ScreenVert q[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) q[i] = screen_vert(cam, H, W, X + 3 * (size_t)faces[3 * (size_t)f + i]);
+        drawn = setup_face(nullptr, faces, f, H, W, s, q);
+    }
+    if (!drawn) {
+        const float *bgp = background ? background + (size_t)b * 3 * n + t : nullptr;
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) out[(size_t)ch * n] = bgp ? bgp[(size_t)ch * n] : 0.f;
+        return;
+    }
+    long long e[3];
+    covers(s, t % W, t / W, e);
+    double q[3];
+    const double sum = inv_depth(s, e, q);
+    double w[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) w[i] = __ddiv_rn(q[i], sum);
+    const auto lerp3 = [&](const float *a, int stride, int k) {
+        return __dadd_rn(__dadd_rn(__dmul_rn(w[0], (double)a[stride * (size_t)s.v[0] + k]), __dmul_rn(w[1], (double)a[stride * (size_t)s.v[1] + k])),
+                         __dmul_rn(w[2], (double)a[stride * (size_t)s.v[2] + k]));
+    };
+    if (colors) {
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) out[(size_t)ch * n] = __double2float_rn(lerp3(colors, 3, ch));
+        return;
+    }
+    const double x = __dsub_rn(__dmul_rn(lerp3(uvs, 2, 0), (double)Tw), 0.5), y = __dsub_rn(__dmul_rn(lerp3(uvs, 2, 1), (double)Th), 0.5);
+    const double x0 = floor(x), y0 = floor(y);
+    const double fx = __dsub_rn(x, x0), fy = __dsub_rn(y, y0);
+    // NaN or far-off coordinates clamp to the edge too
+    const int c0 = x0 >= 0.0 ? (int)fmin(x0, (double)(Tw - 1)) : 0, c1 = x0 + 1.0 >= 0.0 ? (int)fmin(x0 + 1.0, (double)(Tw - 1)) : 0;
+    const int r0 = y0 >= 0.0 ? (int)fmin(y0, (double)(Th - 1)) : 0, r1 = y0 + 1.0 >= 0.0 ? (int)fmin(y0 + 1.0, (double)(Th - 1)) : 0;
+    const double gx = __dsub_rn(1.0, fx), gy = __dsub_rn(1.0, fy);
+    const float *T00 = tex + 3 * ((size_t)r0 * Tw + c0), *T01 = tex + 3 * ((size_t)r0 * Tw + c1);
+    const float *T10 = tex + 3 * ((size_t)r1 * Tw + c0), *T11 = tex + 3 * ((size_t)r1 * Tw + c1);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        const double top = __dadd_rn(__dmul_rn(gx, (double)T00[ch]), __dmul_rn(fx, (double)T01[ch]));
+        const double bot = __dadd_rn(__dmul_rn(gx, (double)T10[ch]), __dmul_rn(fx, (double)T11[ch]));
+        out[(size_t)ch * n] = __double2float_rn(__dadd_rn(__dmul_rn(gy, top), __dmul_rn(fy, bot)));
+    }
+}
+
 struct MeshWs {
     unsigned long long *keys;
     ScreenVert *sv;
@@ -357,5 +427,25 @@ extern "C" int ga_mesh_render(int32_t B, int32_t V, int32_t F, int32_t H, int32_
       mesh_shade_kernel<<<dim3(cdiv((long long)H * W, 256), B), 256, 0, stream>>>(V, H, W, verts, faces, cams, w.sv, w.normals, w.keys, background,
                                                                                   base_r, base_g, base_b, face_id, depth, rgb); }
     GA_CHECK_LAUNCH("mesh_shade_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_mesh_shade_unlit(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, const float *verts, const int32_t *faces,
+                                   const float *cams, const int32_t *face_id, const float *colors, const float *uvs, const float *texture,
+                                   int32_t Th, int32_t Tw, const float *background, float *rgb, void *stream_)
+{
+    GA_REQUIRE(B >= 1 && B <= kMaxB, "ga_mesh_shade_unlit: batch %d outside [1, %d]", B, kMaxB);
+    GA_REQUIRE(V > 0 && V <= (1 << 24) && F >= 0 && F <= (1 << 24), "ga_mesh_shade_unlit: bad vertex / face count %d / %d", V, F);
+    GA_REQUIRE(H >= 1 && H <= kMaxSide && W >= 1 && W <= kMaxSide, "ga_mesh_shade_unlit: frame %d x %d outside [1, %d]^2", H, W, kMaxSide);
+    GA_REQUIRE((colors != nullptr) != (uvs != nullptr || texture != nullptr),
+               "ga_mesh_shade_unlit: give vertex colours or texture coordinates and a texture, not both");
+    GA_REQUIRE(colors || (uvs && texture && Th >= 1 && Th <= kMaxSide && Tw >= 1 && Tw <= kMaxSide),
+               "ga_mesh_shade_unlit: texture %d x %d outside [1, %d]^2 or a NULL texture / texture coordinates", Th, Tw, kMaxSide);
+    GA_REQUIRE(verts && cams && face_id && rgb && (F == 0 || faces), "ga_mesh_shade_unlit: NULL pointer argument");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    { ProfScope _ps("mesh_unlit_kernel", stream);
+      mesh_unlit_kernel<<<dim3(cdiv((long long)H * W, 256), B), 256, 0, stream>>>(V, F, H, W, verts, faces, cams, face_id, colors, uvs, texture,
+                                                                                  Th, Tw, background, rgb); }
+    GA_CHECK_LAUNCH("mesh_unlit_kernel");
     return GA_OK;
 }

@@ -120,3 +120,43 @@ class MeshRenderer:
                                         None if background is None else ptr(background[s:e]), ptr(ws), ptr(face_id[s:e]),
                                         ptr(depth[s:e]), ptr(rgb[s:e]), stream), "ga_mesh_render")
         return rgb, face_id, depth
+
+    @torch.no_grad()
+    def render_unlit(self, verts, cams, H: int, W: int, colors=None, uvs=None, texture=None, background=None):
+        """The mesh drawn as `render` draws it, coloured without lighting (`ga_mesh_shade_unlit`): colors [V,3] interpolated, or
+        texture [Th,Tw,3] (fp32, row 0 first) sampled bilinearly at uvs [V,2] (glTF's convention), clamped to the edge.  Returns
+        (rgb [B,3,H,W], face_id [B,H,W], depth [B,H,W])."""
+        if (colors is None) == (uvs is None or texture is None):
+            raise ValueError("give colors, or uvs and texture")
+        _, face_id, depth = self.render(verts, cams, H, W)
+        H, W = int(H), int(W)
+        dev = self.device
+        verts = torch.as_tensor(verts).to(device=dev, dtype=torch.float32).contiguous()
+        cams = torch.as_tensor(cams).to(device=dev, dtype=torch.float32).contiguous()
+        B = verts.shape[0]
+        f32 = lambda t, shape: None if t is None else _shaped(t, shape, dev)
+        colors, uvs = f32(colors, (self.V, 3)), f32(uvs, (self.V, 2))
+        Th = Tw = 0
+        if texture is not None:
+            texture = torch.as_tensor(texture).to(device=dev, dtype=torch.float32).contiguous()
+            if texture.dim() != 3 or texture.shape[2] != 3:
+                raise ValueError(f"texture {tuple(texture.shape)}: expected [Th,Tw,3]")
+            Th, Tw = int(texture.shape[0]), int(texture.shape[1])
+        if background is not None:
+            background = _shaped(background, (B, 3, H, W), dev)
+        rgb = torch.empty(B, 3, H, W, dtype=torch.float32, device=dev)
+        stream = torch.cuda.current_stream().cuda_stream
+        for s in range(0, B, MAX_FRAMES_PER_CALL):
+            e = min(B, s + MAX_FRAMES_PER_CALL)
+            _lib.check(_lib.lib().ga_mesh_shade_unlit(e - s, self.V, self.F, H, W, ptr(verts[s:e]), ptr(self.faces), ptr(cams[s:e]),
+                                                      ptr(face_id[s:e]), ptr(colors), ptr(uvs), ptr(texture), Th, Tw,
+                                                      None if background is None else ptr(background[s:e]), ptr(rgb[s:e]), stream),
+                       "ga_mesh_shade_unlit")
+        return rgb, face_id, depth
+
+
+def _shaped(t, shape, device) -> torch.Tensor:
+    t = torch.as_tensor(t).to(device=device, dtype=torch.float32).contiguous()
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"{tuple(t.shape)}: expected {list(shape)}")
+    return t

@@ -505,6 +505,20 @@ size_t ga_mesh_render_workspace_bytes(int32_t B, int32_t V, int32_t F, int32_t H
 int ga_mesh_render(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, const float *verts, const int32_t *faces,
                    const int32_t *adj_offsets, const int32_t *adj_faces, const float *cams, float base_r, float base_g, float base_b,
                    const float *background, void *workspace, int32_t *face_id, float *depth, float *rgb, void *stream);
+/* ga_mesh_shade_unlit: the unlit colour of the frames ga_mesh_render drew, from its face_id [B,H,W] and the same verts, faces, cams,
+ * B in [1, 8].  At each pixel centre the drawn face's perspective-correct weights w_i = (E_i / area / z_i) / sum_k (E_k / area / z_k)
+ * are recomputed in fp64 from the same snapped corners, then either
+ *   colors [V,3] != NULL: rgb = sum_i w_i colors[v_i], or
+ *   uvs [V,2] and texture [Th,Tw,3] (fp32, row 0 first, Th, Tw in [1, 16384]) != NULL: (s, t) = sum_i w_i uvs[v_i] in glTF's
+ *   convention, x = s Tw - 0.5, y = t Th - 0.5 (texel (c, r) centred at (c, r)), and the bilinear blend of the four texels around
+ *   (x, y), indices clamped to the edge.  The texels are blended as stored (display-encoded values, as a glTF viewer that does not
+ *   decode sRGB to linear before filtering would; the unlit preview compares those values with the avatar's rendered ones).
+ * All fp64 steps explicitly rounded, rgb [B,3,H,W] rounded to fp32 once; background [B,3,H,W] (0 if NULL) where face_id is -1 (or
+ * not a face below F).  Exactly one of colors and (uvs, texture) is given.  Every element written, no atomics: bit-reproducible, and
+ * a frame's output does not depend on the batch it is in. */
+int ga_mesh_shade_unlit(int32_t B, int32_t V, int32_t F, int32_t H, int32_t W, const float *verts, const int32_t *faces, const float *cams,
+                        const int32_t *face_id, const float *colors, const float *uvs, const float *texture, int32_t Th, int32_t Tw,
+                        const float *background, float *rgb, void *stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Animation player.
@@ -608,6 +622,26 @@ int ga_tsdf_mesh_emit(const GaTsdfDesc *d, const void *state, int32_t min_carve,
  * ---------------------------------------------------------------------------------------------------------------- */
 int ga_skin_weights(int32_t V, int32_t N, int32_t J, int32_t ld, int32_t k, int32_t K, const float *verts, const float *means,
                     const float *lbs, uint8_t *joints, float *weights, void *stream);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Body-topology rig: the operators of its geometry fit and texture (rig.extract_body_rig).
+ * ga_mesh_laplacian: y [V,3] = deg_v x_v - sum_{u in N(v)} x_u (the uniform graph Laplacian) for x [V,3] (fp32) and the vertex
+ *   adjacency CSR offsets [V+1] / adj (neighbours of v at adj[offsets[v] .. offsets[v+1]), each in [0, V)).  In fp32: s = 0,
+ *   s += x_u in stored order, y = fp32(deg x_v) - s, each step rounded on its own.  V in [1, 2^24].
+ * ga_texture_pushpull: fills the texels of an S x S map, S in [1, 512], that mask [S,S] (uint8, nonzero: covered) leaves out, from
+ *   the covered texels of image [C,S,S] (planar fp32, C in [1, 4]).  Down: level l+1 has side ceil(n_l / 2); its texel (r, c) gets
+ *   weight w = sum of its children's weights (level 0: 1 per covered texel) and value (sum_k w_k v_k) / w over the children (2r + i,
+ *   2c + j) with w_k > 0, in the order (0,0) (0,1) (1,0) (1,1), each product and sum rounded on its own (0 when w = 0); down to 1 x 1.
+ *   Up: a texel of weight 0 takes its parent's (r / 2, c / 2) value, coarsest level first.  out [C,S,S]: covered texels copied from
+ *   image bit for bit (uncovered texels of image are not read).  Every filled value is a convex combination of covered ones (0 when
+ *   nothing is covered).  workspace: ga_texture_pushpull_workspace_bytes(S, C) bytes (0 for S = 1; 0 also for bad sizes), 256-byte
+ *   aligned.
+ * No atomics and no host read-back: bit-reproducible.  Bad sizes and NULL pointers are refused before anything launches.
+ * ---------------------------------------------------------------------------------------------------------------- */
+int ga_mesh_laplacian(int32_t V, const int32_t *offsets, const int32_t *adj, const float *x, float *y, void *stream);
+size_t ga_texture_pushpull_workspace_bytes(int32_t S, int32_t C);
+int ga_texture_pushpull(int32_t S, int32_t C, const float *image, const uint8_t *mask, void *workspace, size_t workspace_bytes, float *out,
+                        void *stream);
 
 #ifdef __cplusplus
 }

@@ -15,7 +15,14 @@ does, --align_to mapping its first frame onto a training frame) and writes OUT/{
 --format glb writes one rigged mesh, OUT/avatar.glb (gaussianavatar_b200.rig): the canonical mesh, the body skeleton and
 --influences (4 or 8) skin weights per vertex, with --motion CLIP baked in as an animation at --fps (--up: the clip world's up
 axis, by default -y for a smpl_parms.pth or with --align_to, else z).  --iou poses the rig at every baked frame, or at each --frame K
-without a clip, and prints its silhouette IoUs.  One JSON line goes to stdout.
+without a clip, and prints its silhouette IoUs; --psnr at the same poses prints the PSNR of the rig drawn unlit (its texture or
+vertex colours) against the avatar's own render, both on black.  One JSON line goes to stdout.
+
+    python tools/extract_mesh.py -s DATA -m MODEL --epoch N --format glb --topology body --subdiv 1 --smpl_model SMPL_NEUTRAL.pkl --out rig
+
+--topology body (default tsdf) writes the rig in the body model's own topology instead (rig.extract_body_rig): the --uv_template
+(default PROJECT/assets/template_mesh_{body}_uv.obj) subdivided --subdiv times (0, 1 or 2; default 1) and fitted through the
+Gaussians, the body model's skin weights and the decoder's colour map as its texture.  It needs --smpl_model.
 """
 import argparse
 import json
@@ -60,9 +67,16 @@ def parse(argv=None):
     ap.add_argument("--up", choices=("y", "z", "-y"), default=None, help="glb: the clip world's up axis")
     ap.add_argument("--out", required=True)
     ap.add_argument("--iou", action="store_true")
+    ap.add_argument("--psnr", action="store_true", help="glb: the unlit rig's PSNR against the avatar's render")
+    ap.add_argument("--topology", choices=("tsdf", "body"), default="tsdf", help="glb: the TSDF mesh or the body model's own topology")
+    ap.add_argument("--subdiv", type=int, choices=(0, 1, 2), default=None, help="--topology body: midpoint subdivisions (default 1)")
     a = ap.parse_args(argv)
-    if a.format != "glb" and (a.influences is not None or a.up is not None):
-        ap.error("--influences and --up go with --format glb")
+    if a.format != "glb" and (a.influences is not None or a.up is not None or a.psnr or a.topology != "tsdf"):
+        ap.error("--influences, --up, --psnr and --topology go with --format glb")
+    if a.subdiv is not None and a.topology != "body":
+        ap.error("--subdiv goes with --topology body")
+    if a.topology == "body" and not a.smpl_model:
+        ap.error("--topology body needs --smpl_model (the body model's skin weights and canonical mesh)")
     if a.format == "glb":
         if a.frame is not None and a.motion is not None:
             ap.error("give --frame K (repeatable) or --motion CLIP, not both")
@@ -162,8 +176,15 @@ def main_glb(a):
         if not 0 <= k < F:
             raise SystemExit(f"--frame {k}: the model has training frames 0..{F - 1}")
     t0 = time.perf_counter()
-    rig = rg.extract_rigged_mesh(model, res=a.res, views=a.views, size=a.size, trunc_voxels=a.trunc, min_carve=a.min_carve,
-                                 influences=a.influences or 4, pose_mapper=actor.pose_mapper)
+    if a.topology == "body":
+        from gaussianavatar_b200.body import load_model
+        from gaussianavatar_b200.posmap import BodyPoser
+        poser = actor.pose_mapper or BodyPoser(load_model(a.smpl_model), model.betas[0].cpu(), device=model.device, body=body)
+        uv = a.uv_template or os.path.join(a.project_path, "assets", f"template_mesh_{body.name}_uv.obj")
+        rig = rg.extract_body_rig(model, uv, 1 if a.subdiv is None else a.subdiv, a.influences or 4, pose_mapper=poser)
+    else:
+        rig = rg.extract_rigged_mesh(model, res=a.res, views=a.views, size=a.size, trunc_voxels=a.trunc, min_carve=a.min_carve,
+                                     influences=a.influences or 4, pose_mapper=actor.pose_mapper)
     motion = None
     if a.motion is not None:
         clip = an.MotionClip.load(a.motion, body.name, fps=a.clip_fps)
@@ -174,7 +195,9 @@ def main_glb(a):
     rg.write_glb(path, rig, motion)
     rec = dict(mesh=path, vertices=int(rig.verts.shape[0]), faces=int(rig.faces.shape[0]), joints=len(rig.parents),
                frames=0 if motion is None else motion.frames, seconds=round(time.perf_counter() - t0, 4))
-    if a.iou:
+    if rig.fit is not None:
+        rec["fit"] = rig.fit
+    if a.iou or a.psnr:
         cam = dataset_camera(a.source_path)
         if motion is not None:        # the baked frames, carried back from glTF's +Y up into the clip's world
             poses = [(motion, i) for i in range(motion.frames)]
@@ -191,12 +214,18 @@ def main_glb(a):
             trans = model.transl.weight.detach()[a.frame or []]
             full = body.join(pose, rest) if body.rest_width else pose
             poses = [(rg.bake_poses(model._rest_joints, full[i:i + 1], trans[i:i + 1], 1.0, "y"), 0) for i in range(len(a.frame or []))]
-        ious = []
+        ious, psnrs = [], []
         for i, (m, f) in enumerate(poses):
             v = torch.from_numpy(rg.pose_rig(rig, m, f) @ m.up_rotation).float().to(model.device)
-            ious.append(round(silhouette_iou(model, pose[i], trans[i], v, rig.faces, cam[0], cam[1], cam[2],
-                                             None if rest is None else rest[i], actor.pose_mapper)[0], 5))
-        rec["iou"] = ious
+            r = None if rest is None else rest[i]
+            if a.iou:
+                ious.append(round(silhouette_iou(model, pose[i], trans[i], v, rig.faces, cam[0], cam[1], cam[2], r, actor.pose_mapper)[0], 5))
+            if a.psnr:
+                psnrs.append(round(rg.unlit_psnr(model, rig, v, pose[i], trans[i], cam[0], cam[1], cam[2], r, actor.pose_mapper)[0], 4))
+        if a.iou:
+            rec["iou"] = ious
+        if a.psnr:
+            rec["psnr"] = psnrs
     print(json.dumps(rec), flush=True)
     return 0
 
