@@ -36,7 +36,7 @@ class DecoderState:
 
     def __init__(self, S: int, feat_res: int, batch: int, device, c_geom=64, hsize=128, eps=1e-5, momentum=0.1, tensor_cores=True, frames=1):
         self.desc = _lib.GaDecoderDesc(int(S), int(feat_res), int(batch), int(c_geom), int(hsize), float(eps), float(momentum),
-                                       1 if tensor_cores else 0, int(frames))
+                                       _lib.GA_DECODER_TENSOR_CORES if tensor_cores else 0, int(frames))
         nbytes = _lib.lib().ga_decoder_workspace_bytes(ctypes.byref(self.desc))
         if nbytes == 0:
             raise RuntimeError("ga_decoder_workspace_bytes failed: " + _lib.lib().ga_last_error().decode())
