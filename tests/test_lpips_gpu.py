@@ -1,5 +1,7 @@
-"""GPU: the LPIPS kernels (csrc/lpips.cu) launch by launch against fp64, the module against the fp64 oracle, its known answers, and
-the trainer's LPIPS term."""
+"""GPU: the LPIPS network's launches (csrc/lpips.cu: the five convolutions, the two pools, the four data gradients, the two
+un-pools and conv1's image gradient) against fp64 from their own inputs, the module against the fp64 oracle, its known answers,
+and the trainer's LPIPS term.  The head launches (lpips_dist1..5, lpips_sum, lpips_dnorm1..5) are checked element by element from
+their own inputs in test_lpips_head_gpu.py."""
 import ctypes
 
 import numpy as np
