@@ -395,17 +395,25 @@ class AvatarModel:
         plan = getattr(self, "_last_plan", None)
         return True if plan is None else plan.check(wait)
 
-    def _render_batched(self, batch_data, means, scales, colors):
-        from .rasterizer import rasterize_batch
+    def _render_batched(self, batch_data, means, scales, colors, depth=False):
+        """depth: render through rasterize_batch_with_depth and keep its differentiable depth pass [B,2,H,W] in `last_depth`."""
+        from .rasterizer import rasterize_batch, rasterize_batch_with_depth
         B, P = int(means.shape[0]), int(means.shape[1])
         H, W = int(self._scalar_list(batch_data["height"], 1)[0]), int(self._scalar_list(batch_data["width"], 1)[0])
         cams = batch_data["_cams"] if "_cams" in batch_data else self._batch_cameras(batch_data, B, means.device)
         plan = self.raster_plan(B, P, H, W)
         self._last_plan = plan
-        images = rasterize_batch(means, colors, scales, self.fix_rotation, self.fix_opacity, cams, self.background, plan)
+
+        def render():
+            if not depth:
+                return rasterize_batch(means, colors, scales, self.fix_rotation, self.fix_opacity, cams, self.background, plan)
+            images, self.last_depth = rasterize_batch_with_depth(means, colors, scales, self.fix_rotation, self.fix_opacity, cams,
+                                                                 self.background, plan)
+            return images
+        images = render()
         if (not torch.is_grad_enabled() and not torch.cuda.is_current_stream_capturing() and not getattr(self, "defer_raster_check", False)
                 and not plan.check(wait=True)):          # inference: make the result right before returning it (unless the caller checks later)
-            images = rasterize_batch(means, colors, scales, self.fix_rotation, self.fix_opacity, cams, self.background, plan)
+            images = render()
             if not plan.check(wait=True):
                 raise RuntimeError("batched rasterizer: binning buffer overflowed twice in a row")
         return images
@@ -414,9 +422,12 @@ class AvatarModel:
         h, w = self._scalar_list(batch_data["height"], B), self._scalar_list(batch_data["width"], B)
         return len(set(h)) == 1 and len(set(w)) == 1
 
-    def _render_frames(self, batch_data, means, scales, colors):
+    def _render_frames(self, batch_data, means, scales, colors, depth=False):
         if means.is_cuda and means.shape[0] <= MAX_FRAMES_PER_CALL and self._uniform_frames(batch_data, means.shape[0]):
-            return self._render_batched(batch_data, means, scales, colors)
+            return self._render_batched(batch_data, means, scales, colors, depth)
+        if depth:
+            raise RuntimeError(f"training against depth maps needs the batched rasterizer: at most {MAX_FRAMES_PER_CALL} CUDA frames of one "
+                               "size per batch (the one-frame-at-a-time path renders no depth)")
         return self._render_frames_one_by_one(batch_data, means, scales, colors)
 
     def _render_frames_one_by_one(self, batch_data, means, scales, colors):
@@ -447,7 +458,8 @@ class AvatarModel:
         return torch.stack(images, dim=0)
 
     def train_stage1(self, batch_data, iteration):
-        """model/avatar_model.py:272-367: returns (images [B,3,H,W], full_pred [B,N,3], offset_loss, geo_loss, scale_loss)."""
+        """model/avatar_model.py:272-367: returns (images [B,3,H,W], full_pred [B,N,3], offset_loss, geo_loss, scale_loss).  A batch
+        with `depth` (ModelParams.depth_maps) also leaves the differentiable depth pass [B,2,H,W] in `last_depth`."""
         idx = batch_data["pose_idx"]
         means, scales, colors, dec = self._posed_gaussians(idx, iteration, rest_pose=batch_data.get("rest_pose"))
         # regularisers exactly as the reference forms them (avatar_model.py:328-330): mean over ALL S*S pixels of
@@ -456,7 +468,7 @@ class AvatarModel:
         geo_loss = torch.mean(self.geo_feature ** 2)
         scale_loss = torch.mean(scales)
         self._last_gaussians = (means, scales, colors)      # parity tests read the rasterizer's inputs / their gradients here
-        images = self._render_frames(batch_data, means, scales, colors)
+        images = self._render_frames(batch_data, means, scales, colors, depth=batch_data.get("depth") is not None)
         return images, means, offset_loss, geo_loss, scale_loss
 
     def _stage2_gaussians(self, batch_data, pose=None, transl=None, placement=None):
@@ -496,12 +508,13 @@ class AvatarModel:
         return self.pose_mapper(pose, transl)
 
     def train_stage2(self, batch_data, iteration):
-        """model/avatar_model.py:369-463: returns (images [B,3,H,W], full_pred [B,N,3], pose_loss, offset_loss)."""
+        """model/avatar_model.py:369-463: returns (images [B,3,H,W], full_pred [B,N,3], pose_loss, offset_loss); `last_depth` as
+        train_stage1 leaves it."""
         means, scales, colors, dec, pose_featmap = self._stage2_gaussians(batch_data)
         offset_loss = torch.mean((dec[:, :3] * 0.02) ** 2)          # mean over B x S*S x 3 (avatar_model.py:424)
         pose_loss = torch.mean(pose_featmap ** 2)
         self._last_gaussians = (means, scales, colors)
-        images = self._render_frames(batch_data, means, scales, colors)
+        images = self._render_frames(batch_data, means, scales, colors, depth=batch_data.get("depth") is not None)
         return images, means, pose_loss, offset_loss
 
     def render_free_stage1(self, batch_data, iteration):

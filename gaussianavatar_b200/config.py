@@ -32,6 +32,9 @@ class ModelParams:
     # stage 2: build each frame's input position map on the device from its SMPL pose instead of reading inp_map/*.npz
     # (not a reference option; read with getattr(..., False) so the reference's own namespaces keep working)
     inp_posmap_from_pose: bool = False
+    # train against metric depth maps, <split>/depths/<name>.npy (float32 metres) or .png (uint16 millimetres); not a reference
+    # option, read with getattr(..., False)
+    depth_maps: bool = False
 
 
 @dataclass
@@ -63,3 +66,6 @@ class OptimizationParams:
     lr_net: float = 3e-3
     lr_geomfeat: float = 5e-4
     sched_milestones: list = field(default_factory=lambda: [66, 133])
+    # weight of the masked L1 depth loss when the batches carry `depth` (ModelParams.depth_maps); not a reference option, read
+    # with getattr(..., 1.0).  An unmeasured starting point, not a tuned value
+    lambda_depth: float = 1.0

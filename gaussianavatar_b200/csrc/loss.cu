@@ -1,4 +1,4 @@
-// Fused image loss: L1 + SSIM (11x11 Gaussian window, sigma 1.5, zero padding), forward and backward.
+// Fused image loss: L1 + SSIM (11x11 Gaussian window, sigma 1.5, zero padding), forward and backward; the masked L1 depth loss.
 //
 // Replaces `l1_loss_w(image, gt)` and `ssim(image, gt)` (/root/reference utils/loss_utils.py:7-8,23-53; used at
 // train.py:74-75): the reference runs 5 depthwise 11x11 convolutions + ~15 element-wise kernels forward and again
@@ -256,6 +256,161 @@ extern "C" int ga_loss_backward(int32_t B, int32_t H, int32_t W, const float *im
     dim3 grid(cdiv(W, kTX), cdiv(H, kTY), B * 3), block(kTX, kTY);
     { ProfScope _ps("ssim_l1_bwd_kernel", st); ssim_l1_bwd_kernel<<<grid, block, 0, st>>>(H, W, image, gt, maps, maps + n, maps + 2 * n, coef, d_image); }
     GA_CHECK_LAUNCH("ssim_l1_bwd_kernel");
+    return GA_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Masked L1 depth loss on the mean-depth plane: L = lam / N sum |m - d*| over the counted pixels (target d* > 0 and a median, plane 1,
+// that is non-zero, i.e. 1 - T_final >= 0.5), N their number over all B frames; L = 0 and a zero gradient when N = 0.  Every sum
+// has a fixed order (shuffle trees, then one CTA over the per-CTA partials) and N is never read back, so a replayed CUDA graph
+// gives the same loss bit for bit.
+// ---------------------------------------------------------------------------------------------------------------------
+namespace ga {
+namespace {
+constexpr int kDL = 256;            // pixels per CTA of the partial-sum pass
+constexpr int kDLFin = 1024;        // threads of the finalising CTA
+
+__device__ __forceinline__ bool depth_counted(const float *__restrict__ depth, const float *__restrict__ target, size_t HW, size_t i,
+                                              float &diff)
+{
+    const size_t b = i / HW, px = i - b * HW;
+    const float m = depth[b * 2 * HW + px], med = depth[b * 2 * HW + HW + px], t = target[i];
+    diff = m - t;
+    return t > 0.f && med != 0.f;
+}
+
+__global__ void __launch_bounds__(kDL)
+depth_l1_partial_kernel(size_t n, size_t HW, const float *__restrict__ depth, const float *__restrict__ target,
+                        float *__restrict__ part_sum, int32_t *__restrict__ part_cnt)
+{
+    __shared__ float s_sum[kDL / 32];
+    __shared__ int s_cnt[kDL / 32];
+    const size_t i = (size_t)blockIdx.x * kDL + threadIdx.x;
+    float v = 0.f;
+    int c = 0;
+    if (i < n) {
+        float diff;
+        if (depth_counted(depth, target, HW, i, diff)) { v = fabsf(diff); c = 1; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { v += __shfl_xor_sync(0xffffffffu, v, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) { s_sum[warp] = v; s_cnt[warp] = c; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float sv = 0.f;
+        int sc = 0;
+        for (int w = 0; w < kDL / 32; ++w) { sv += s_sum[w]; sc += s_cnt[w]; }
+        part_sum[blockIdx.x] = sv;
+        part_cnt[blockIdx.x] = sc;
+    }
+}
+
+// One CTA: thread t sums partials t, t + 1024, ... in double, then a fixed tree.  out2 = (loss, N); coef = lam / N (0 if N = 0).
+__global__ void __launch_bounds__(kDLFin)
+depth_l1_finalize_kernel(int nblk, float lam, const float *__restrict__ part_sum, const int32_t *__restrict__ part_cnt,
+                         float *__restrict__ out2, float *__restrict__ coef)
+{
+    __shared__ double s_sum[kDLFin];
+    __shared__ long long s_cnt[kDLFin];
+    double v = 0.0;
+    long long c = 0;
+    for (int k = threadIdx.x; k < nblk; k += kDLFin) { v += (double)part_sum[k]; c += part_cnt[k]; }
+    s_sum[threadIdx.x] = v;
+    s_cnt[threadIdx.x] = c;
+    __syncthreads();
+    for (int h = kDLFin / 2; h > 0; h >>= 1) {
+        if ((int)threadIdx.x < h) { s_sum[threadIdx.x] += s_sum[threadIdx.x + h]; s_cnt[threadIdx.x] += s_cnt[threadIdx.x + h]; }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        const long long N = s_cnt[0];
+        out2[0] = N > 0 ? (float)((double)lam * s_sum[0] / (double)N) : 0.f;
+        out2[1] = (float)N;
+        coef[0] = N > 0 ? (float)((double)lam / (double)N) : 0.f;
+    }
+}
+
+// dL/dm = g lam sign(m - d*) / N on counted pixels (sign(0) = 0), 0 elsewhere; g the upstream scalar (NULL: 1).
+__global__ void __launch_bounds__(256)
+depth_l1_bwd_kernel(size_t n, size_t HW, const float *__restrict__ depth, const float *__restrict__ target, const float *__restrict__ coef,
+                    const float *__restrict__ g, float *__restrict__ d_m)
+{
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    float diff;
+    const bool counted = depth_counted(depth, target, HW, i, diff);
+    const float sgn = (diff > 0.f) ? 1.f : ((diff < 0.f) ? -1.f : 0.f);
+    d_m[i] = counted ? (g ? g[0] : 1.f) * coef[0] * sgn : 0.f;
+}
+
+struct DepthLossWs {
+    float *part_sum;
+    int32_t *part_cnt;
+    float *coef;
+    size_t total;
+};
+
+DepthLossWs carve_depth_loss(void *buf, size_t n)
+{
+    Carver c(buf);
+    DepthLossWs w;
+    const size_t nblk = n ? (n + kDL - 1) / kDL : 1;
+    w.part_sum = c.take<float>(nblk);
+    w.part_cnt = c.take<int32_t>(nblk);
+    w.coef = c.take<float>(1);
+    w.total = c.used();
+    return w;
+}
+
+int check_depth_loss(int32_t B, int32_t H, int32_t W)
+{
+    GA_REQUIRE(B > 0 && H > 0 && W > 0, "bad depth loss dims B=%d H=%d W=%d", B, H, W);
+    GA_REQUIRE((long long)B * H * W < (1ll << 31) * kDL, "depth loss too large");
+    return GA_OK;
+}
+}  // namespace
+}  // namespace ga
+
+extern "C" size_t ga_depth_loss_workspace_bytes(int32_t B, int32_t H, int32_t W)
+{
+    return carve_depth_loss(nullptr, (size_t)(B > 0 ? B : 0) * (size_t)(H > 0 ? H : 0) * (size_t)(W > 0 ? W : 0)).total;
+}
+
+extern "C" int ga_depth_loss_forward(int32_t B, int32_t H, int32_t W, const float *depth, const float *target, float lam, void *workspace,
+                                     size_t workspace_bytes, float *out2, void *stream_)
+{
+    if (int rc = check_depth_loss(B, H, W)) return rc;
+    GA_REQUIRE(depth && target && workspace && out2, "NULL pointer argument");
+    const size_t n = (size_t)B * H * W;
+    const DepthLossWs w = carve_depth_loss(workspace, n);
+    if (w.total > workspace_bytes) {
+        set_error("depth loss workspace too small: need %zu bytes, have %zu", w.total, workspace_bytes);
+        return GA_ERR_CAPACITY;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream_);
+    const int nblk = (int)((n + kDL - 1) / kDL);
+    { ProfScope _ps("depth_l1_partial_kernel", st); depth_l1_partial_kernel<<<nblk, kDL, 0, st>>>(n, (size_t)H * W, depth, target, w.part_sum, w.part_cnt); }
+    GA_CHECK_LAUNCH("depth_l1_partial_kernel");
+    { ProfScope _ps("depth_l1_finalize_kernel", st); depth_l1_finalize_kernel<<<1, kDLFin, 0, st>>>(nblk, lam, w.part_sum, w.part_cnt, out2, w.coef); }
+    GA_CHECK_LAUNCH("depth_l1_finalize_kernel");
+    return GA_OK;
+}
+
+extern "C" int ga_depth_loss_backward(int32_t B, int32_t H, int32_t W, const float *depth, const float *target, const float *grad_out,
+                                      void *workspace, size_t workspace_bytes, float *d_depth, void *stream_)
+{
+    if (int rc = check_depth_loss(B, H, W)) return rc;
+    GA_REQUIRE(depth && target && workspace && d_depth, "NULL pointer argument");
+    const size_t n = (size_t)B * H * W;
+    const DepthLossWs w = carve_depth_loss(workspace, n);
+    if (w.total > workspace_bytes) {
+        set_error("depth loss workspace too small: need %zu bytes, have %zu", w.total, workspace_bytes);
+        return GA_ERR_CAPACITY;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream_);
+    { ProfScope _ps("depth_l1_bwd_kernel", st); depth_l1_bwd_kernel<<<cdiv((long long)n, 256), 256, 0, st>>>(n, (size_t)H * W, depth, target, w.coef, grad_out, d_depth); }
+    GA_CHECK_LAUNCH("depth_l1_bwd_kernel");
     return GA_OK;
 }
 

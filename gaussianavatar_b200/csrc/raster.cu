@@ -140,6 +140,25 @@ BinViews carve_bin(void *buf, int64_t cap, const Dims &d)
     return b;
 }
 
+// The depth state the training forward with depth leaves for the depth backward: each pixel's D = sum w z at the start of every
+// 256-entry segment (laid out as BinViews::ckpt) and at the end of its list (laid out as ImgViews::final_state).
+struct DepthState {
+    float *ckpt;             // [max_segments][256]
+    float *final;            // [B*T][256] tile-major
+    size_t total;
+};
+
+DepthState carve_dstate(void *buf, int64_t cap, const Dims &d)
+{
+    Carver c(buf);
+    DepthState s;
+    const size_t BT = (size_t)d.B * d.T;
+    s.ckpt = c.take<float>(max_segments_for(cap, d) * kBlock);
+    s.final = c.take<float>((BT ? BT : 1) * kBlock);
+    s.total = c.used();
+    return s;
+}
+
 // ---- contraction-proof arithmetic (mirrors oracle/raster_oracle_impl.inc op for op) ----
 __device__ __forceinline__ float mul_(float a, float b) { return __fmul_rn(a, b); }
 __device__ __forceinline__ float add_(float a, float b) { return __fadd_rn(a, b); }
@@ -976,6 +995,8 @@ __device__ __forceinline__ void matte_add(float (&mt)[kMaxSets], const MatteSets
 // plane 1 the median, the z of the entry whose blend takes T from above 0.5 to at most 0.5, 0 where the final T > 0.5.  An
 // entry that is not blended leaves T unchanged, so the T crossing alone selects a blended one; the 1e-4 stop cannot pre-empt
 // the crossing, since alpha <= 0.99 puts T below 0.01 before it can fire.
+// With kDepth and a depth state (d_ckpt, d_final non-NULL: the training forward), it also stores each pixel's running D next to
+// the (T, C) checkpoints and D at the end, the state the depth backward's segments start from.
 template <bool kMattes, bool kDepth>
 __global__ void __launch_bounds__(kBlock)
 render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict__ order, const uint2 *__restrict__ ranges,
@@ -983,7 +1004,8 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
                   const float4 *__restrict__ recA, const float4 *__restrict__ recB, const float4 *__restrict__ recC,
                   const float *__restrict__ bg, float4 *__restrict__ ckpt, float *__restrict__ final_T,
                   uint32_t *__restrict__ n_contrib, float4 *__restrict__ final_state, uint32_t *__restrict__ tile_maxc,
-                  float *__restrict__ out, const MatteSets ms, float *__restrict__ depth)
+                  float *__restrict__ out, const MatteSets ms, float *__restrict__ depth, float *__restrict__ d_ckpt,
+                  float *__restrict__ d_final)
 {
     __shared__ float4 s_a[kBlock / 32][32], s_b[kBlock / 32][32], s_c[kBlock / 32][32];
 
@@ -1013,7 +1035,11 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
 
     bool all_done = __all_sync(0xffffffffu, p.done);          // a sub-tile entirely outside the image
     for (int c = 0; c < nchunks && !all_done; ++c) {
-        if ((c & 7) == 0) ck[(size_t)(c >> 3) * kBlock] = make_float4(p.T, p.C0, p.C1, p.C2);
+        if ((c & 7) == 0) {
+            ck[(size_t)(c >> 3) * kBlock] = make_float4(p.T, p.C0, p.C1, p.C2);
+            if constexpr (kDepth)
+                if (d_ckpt) d_ckpt[((size_t)seg_start[blk] + (c >> 3)) * kBlock + tid] = dsum;
+        }
         const float4 a = fa, bq = fb, cq = fc;
         const int kn = (c + 1) * 32 + lane;          // prefetch the next chunk behind this one's compositing
         if (kn < n) { fa = recA[range.x + kn]; fb = recB[range.x + kn]; fc = recC[range.x + kn]; }
@@ -1074,6 +1100,8 @@ render_fwd_kernel(int H, int W, int gx, int T_tiles, const uint32_t *__restrict_
         }
     }
     final_state[(size_t)blk * kBlock + tid] = make_float4(p.T, p.C0, p.C1, p.C2);
+    if constexpr (kDepth)
+        if (d_final) d_final[(size_t)blk * kBlock + tid] = dsum;
     uint32_t m = p.last;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -1122,7 +1150,12 @@ __device__ __forceinline__ float warp_reduce8(float (&v)[8], int lane)
 // checkpoint, un-premultiplied); a pixel whose last contributor lies inside the segment starts from (T_final, 0) as upstream
 // does.  Per-Gaussian gradients are reduced warp-wide with shuffles (9 for the 8 components GaussianAvatar consumes), across
 // the CTA's eight warps in shared memory, then leave as one vector reduction per (segment entry, array).
-template <bool kOpacity>
+// kDepth: also the gradient of the mean depth m = D / A (plane 0 of depth, A = 1 - T_final) given g = dL_dm per pixel.  The depth
+// is a fourth colour channel of the same recurrence: colour z = recC.w, upstream gradient g / A, and the pixel's own m as its
+// "background" (the normalisation's dA/dalpha term has bg_dot's shape), so dL/dalpha gains (g / A) [T (z - zacc) - m T_final /
+// (1 - alpha)] and each entry's dL/dz = (g / A) alpha T goes to d_z [B,P].  A restarted segment starts from the forward's stored D:
+// zacc = (D_final - D_ckpt) / T_ckpt.
+template <bool kOpacity, bool kDepth = false>
 __global__ void __launch_bounds__(kBlock)
 render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__restrict__ status,
                   const uint32_t *__restrict__ seg_tile, const uint32_t *__restrict__ seg_start,
@@ -1130,10 +1163,12 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
                   const float4 *__restrict__ recA, const float4 *__restrict__ recB, const float4 *__restrict__ recC,
                   const float4 *__restrict__ ckpt, const float *__restrict__ bg, const float4 *__restrict__ final_state,
                   const uint32_t *__restrict__ n_contrib, const float *__restrict__ dL_dout,
-                  float2 *__restrict__ d_mean2D, float4 *__restrict__ d_conic_op, float *__restrict__ d_colors)
+                  float2 *__restrict__ d_mean2D, float4 *__restrict__ d_conic_op, float *__restrict__ d_colors,
+                  const float *__restrict__ dL_dm, const float *__restrict__ depth, const float *__restrict__ d_ckpt,
+                  const float *__restrict__ d_final, float *__restrict__ d_z)
 {
     __shared__ float4 s_a[kSeg], s_b[kSeg], s_c[kSeg];
-    __shared__ float s_acc[9][kSeg + 1];      // + 1: the 8 lanes that own a Gaussian's 8 sums hit 8 different banks
+    __shared__ float s_acc[kDepth ? 10 : 9][kSeg + 1];      // + 1: the 8 lanes that own a Gaussian's 8 sums hit 8 different banks
 
     const int g = blockIdx.x;
     if (g >= status[2]) return;
@@ -1162,7 +1197,7 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
         s_a[tid] = recA[o]; s_b[tid] = recB[o]; s_c[tid] = recC[o];
     }
 #pragma unroll
-    for (int k = 0; k < 9; ++k) s_acc[k][tid] = 0.f;
+    for (int k = 0; k < (kDepth ? 10 : 9); ++k) s_acc[k][tid] = 0.f;
 
     const float4 fs = final_state[(size_t)blk * kBlock + tid];
     const float T_final = inside ? fs.x : 0.f;
@@ -1172,15 +1207,25 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
         const float *d = dL_dout + (size_t)b * 3 * HW + pid;
         dpix0 = d[0]; dpix1 = d[HW]; dpix2 = d[2 * HW];
     }
-    const float bg_dot = bg[0] * dpix0 + bg[1] * dpix1 + bg[2] * dpix2;
-    float T = T_final, acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
+    float bg_dot = bg[0] * dpix0 + bg[1] * dpix1 + bg[2] * dpix2;
+    float gA = 0.f;                                // kDepth: dL/dm / A, 0 where nothing was blended (m = 0, A = 0)
+    if constexpr (kDepth) {
+        if (last_contributor) {
+            const float m = depth[(size_t)b * 2 * HW + pid];
+            gA = dL_dm[(size_t)b * HW + pid] / __fsub_rn(1.f, T_final);
+            bg_dot += m * gA;
+        }
+    }
+    float T = T_final, acc0 = 0.f, acc1 = 0.f, acc2 = 0.f, accz = 0.f;
     if (last_contributor > lo + kSeg) {            // blended entries continue behind this segment
-        const float4 ck = ckpt[((size_t)seg_start[blk] + seg + 1) * kBlock + tid];
+        const size_t ci = ((size_t)seg_start[blk] + seg + 1) * kBlock + tid;
+        const float4 ck = ckpt[ci];
         const float inv = 1.f / ck.x;
         T = ck.x;
         acc0 = (fs.y - ck.y) * inv; acc1 = (fs.z - ck.z) * inv; acc2 = (fs.w - ck.w) * inv;
+        if constexpr (kDepth) accz = (d_final[(size_t)blk * kBlock + tid] - d_ckpt[ci]) * inv;
     }
-    float lc0 = 0.f, lc1 = 0.f, lc2 = 0.f, last_alpha = 0.f;
+    float lc0 = 0.f, lc1 = 0.f, lc2 = 0.f, lcz = 0.f, last_alpha = 0.f;
     const float ddelx_dx = 0.5f * (float)W, ddely_dy = 0.5f * (float)H;
     const int vidx = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);   // component this lane ends up owning
     __syncthreads();
@@ -1211,7 +1256,7 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
             float v[8];
 #pragma unroll
             for (int k = 0; k < 8; ++k) v[k] = 0.f;
-            float vo = 0.f;
+            float vo = 0.f, vz = 0.f;
             if (active) {
                 T = T / (1.f - alpha);
                 const float dchannel_dcolor = alpha * T;
@@ -1220,6 +1265,11 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
                 acc1 = last_alpha * lc1 + (1.f - last_alpha) * acc1; lc1 = col.y;
                 acc2 = last_alpha * lc2 + (1.f - last_alpha) * acc2; lc2 = col.z;
                 float dL_dalpha = (col.x - acc0) * dpix0 + (col.y - acc1) * dpix1 + (col.z - acc2) * dpix2;
+                if constexpr (kDepth) {
+                    accz = last_alpha * lcz + (1.f - last_alpha) * accz; lcz = col.w;
+                    dL_dalpha += (col.w - accz) * gA;
+                    vz = dchannel_dcolor * gA;
+                }
                 v[0] = dchannel_dcolor * dpix0; v[1] = dchannel_dcolor * dpix1; v[2] = dchannel_dcolor * dpix2;
                 dL_dalpha *= T;
                 last_alpha = alpha;
@@ -1241,14 +1291,18 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
                 vo = warp_sum(vo);
                 if (lane == 0) atomicAdd(&s_acc[8][j], vo);
             }
+            if constexpr (kDepth) {
+                vz = warp_sum(vz);
+                if (lane == 0) atomicAdd(&s_acc[9][j], vz);
+            }
         }
     }
     __syncthreads();
     if (tid < cnt) {
         const size_t gi = (size_t)b * P + __float_as_uint(s_a[tid].w);
-        float a[9];
+        float a[kDepth ? 10 : 9];
 #pragma unroll
-        for (int k = 0; k < 9; ++k) a[k] = s_acc[k][tid];
+        for (int k = 0; k < (kDepth ? 10 : 9); ++k) a[k] = s_acc[k][tid];
         if (a[0] != 0.f) atomicAdd(&d_colors[3 * gi], a[0]);
         if (a[1] != 0.f) atomicAdd(&d_colors[3 * gi + 1], a[1]);
         if (a[2] != 0.f) atomicAdd(&d_colors[3 * gi + 2], a[2]);
@@ -1257,20 +1311,23 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
             asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(&d_mean2D[gi]), "f"(a[3]), "f"(a[4]) : "memory");
         if (a[5] != 0.f || a[6] != 0.f || a[7] != 0.f || (kOpacity && a[8] != 0.f))
             red_add_v4(&d_conic_op[gi].x, a[5], a[6], a[7], kOpacity ? a[8] : 0.f);
+        if constexpr (kDepth)
+            if (a[9] != 0.f) atomicAdd(&d_z[gi], a[9]);
     }
 }
 
 // Fused K8 (conic -> cov2D -> cov3D / mean) + K9 (mean2D -> mean3D, cov3D -> scale / rotation): one thread per Gaussian.
 // kSH: also the SH colour backward (d_sh, direction term of d_means3D); kCov: dL/dSigma goes to cc.d_cov3D and the scale /
-// rotation chain is skipped (per-frame API only, B = 1).
-template <bool kSH = false, bool kCov = false>
+// rotation chain is skipped (per-frame API only, B = 1).  kZ: d_means3D also gets dL/dz [B,P] (the depth backward's d_z) times
+// the view matrix's z row, the derivative of the view-space z K1 computes.
+template <bool kSH = false, bool kCov = false, bool kZ = false>
 __global__ void __launch_bounds__(256)
 preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *__restrict__ means3D,
                       const float *__restrict__ scales, const float *__restrict__ rots, long long rot_stride,
                       const int32_t *__restrict__ radii, const float *__restrict__ cov3d,
                       const float2 *__restrict__ d_mean2D, const float4 *__restrict__ d_conic_op,
                       float *__restrict__ d_means3D, float *__restrict__ d_scales, float *__restrict__ d_rots,
-                      float *__restrict__ d_opac, float *__restrict__ d_means2D_out, ColorCov cc)
+                      float *__restrict__ d_opac, float *__restrict__ d_means2D_out, ColorCov cc, const float *__restrict__ d_z)
 {
     const int fb = blockIdx.y;
     __shared__ float view[16], proj[16];
@@ -1364,6 +1421,11 @@ preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *_
 #pragma unroll
     for (int k = 0; k < 3; ++k)
         dmean[k] += (proj[4 * k + 0] * m_w - proj[4 * k + 3] * mul1) * g2.x + (proj[4 * k + 1] * m_w - proj[4 * k + 3] * mul2) * g2.y;
+    if constexpr (kZ) {
+        const float dz = d_z[i];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) dmean[k] += view[k * 4 + 2] * dz;
+    }
     if constexpr (kSH) sh_color_bwd(cc, i, px, py, pz, dmean);
     d_means3D[i3] = dmean[0]; d_means3D[i3 + 1] = dmean[1]; d_means3D[i3 + 2] = dmean[2];
     if constexpr (kCov) {
@@ -1455,7 +1517,7 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
 // K3 + K4 + K6 for all frames (a scene: the composite K4, d.P = P + Ps; mattes and / or depth: K6's variant that writes them).
 int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacity, const GeomViews &g, const ImgViews &iv, const BinViews &bv,
                               float *out_color, cudaStream_t stream, const SceneSet *scene = nullptr, const MatteSets *mattes = nullptr,
-                              float *depth = nullptr)
+                              float *depth = nullptr, const DepthState *dstate = nullptr)
 {
     static PerDeviceOnce attr_set;
     if (attr_set.first()) {
@@ -1501,7 +1563,7 @@ int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacit
         ProfScope _ps(name, stream);
         kernel<<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC, a.bg, bv.ckpt,
                                           iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color, mattes ? *mattes : MatteSets{},
-                                          depth);
+                                          depth, dstate ? dstate->ckpt : nullptr, dstate ? dstate->final : nullptr);
     };
     if (mattes && depth) render(render_fwd_kernel<true, true>, "render_fwd_mattes_depth_kernel");
     else if (mattes) render(render_fwd_kernel<true, false>, "render_fwd_mattes_kernel");
@@ -1524,36 +1586,48 @@ size_t bwd_scratch_bytes(size_t BP)
     return align_up(n * sizeof(float2)) + align_up(n * sizeof(float4));
 }
 
-// K7 + fused K8/K9.  cc selects the K8/K9 variant as in launch_preprocess; with SH, K7's d_colors is dL/drgb (cc.d_rgb).
+// The depth backward's scratch: bwd_scratch_bytes' d_mean2D and d_conic_op, then d_z [B*P].
+size_t depth_bwd_scratch_bytes(size_t BP) { return bwd_scratch_bytes(BP) + align_up((BP > 0 ? BP : 1) * sizeof(float)); }
+
+// The inputs of the depth backward: dL/dm [B,H,W], the forward's depth [B,2,H,W] and its depth state.
+struct DepthBwd {
+    const float *dL_dm, *depth;
+    DepthState state;
+};
+
+// K7 + fused K8/K9.  cc selects the K8/K9 variant as in launch_preprocess; with SH, K7's d_colors is dL/drgb (cc.d_rgb).  dz (batched
+// API, no SH / cov3D): the depth variants, with d_z behind d_conic_op in the scratch (depth_bwd_scratch_bytes).
 int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, ColorCov cc, const int32_t *radii, const GeomViews &g,
-                    const ImgViews &iv, const BinViews &bv, void *scratch, cudaStream_t stream)
+                    const ImgViews &iv, const BinViews &bv, void *scratch, cudaStream_t stream, const DepthBwd *dz = nullptr)
 {
     const size_t BP = (size_t)d.B * d.P;
     Carver sc(scratch);
     float2 *d_mean2D = sc.take<float2>(BP);
     float4 *d_conic_op = sc.take<float4>(BP);
-    GA_CHECK_CUDA(cudaMemsetAsync(scratch, 0, bwd_scratch_bytes(BP), stream));
+    float *d_z = dz ? sc.take<float>(BP) : nullptr;
+    GA_CHECK_CUDA(cudaMemsetAsync(scratch, 0, dz ? depth_bwd_scratch_bytes(BP) : bwd_scratch_bytes(BP), stream));
     GA_CHECK_CUDA(cudaMemsetAsync(a.d_colors, 0, sizeof(float) * 3 * BP, stream));
     {
-        ProfScope _ps("render_bwd_kernel", stream);
+        ProfScope _ps(dz ? "render_bwd_depth_kernel" : "render_bwd_kernel", stream);
         const int grid = (int)bv.max_segments;
-        if (a.d_opacities)
-            render_bwd_kernel<true><<<grid, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges,
-                                                                 iv.tile_maxc, bv.recA, bv.recB, bv.recC, bv.ckpt, a.bg, iv.final_state,
-                                                                 iv.n_contrib, a.dL_dout, d_mean2D, d_conic_op, a.d_colors);
-        else
-            render_bwd_kernel<false><<<grid, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges,
-                                                                  iv.tile_maxc, bv.recA, bv.recB, bv.recC, bv.ckpt, a.bg, iv.final_state,
-                                                                  iv.n_contrib, a.dL_dout, d_mean2D, d_conic_op, a.d_colors);
+        auto run = [&](auto kernel) {
+            kernel<<<grid, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges, iv.tile_maxc,
+                                                bv.recA, bv.recB, bv.recC, bv.ckpt, a.bg, iv.final_state, iv.n_contrib, a.dL_dout, d_mean2D,
+                                                d_conic_op, a.d_colors, dz ? dz->dL_dm : nullptr, dz ? dz->depth : nullptr,
+                                                dz ? dz->state.ckpt : nullptr, dz ? dz->state.final : nullptr, d_z);
+        };
+        if (dz) run(a.d_opacities ? render_bwd_kernel<true, true> : render_bwd_kernel<false, true>);
+        else run(a.d_opacities ? render_bwd_kernel<true> : render_bwd_kernel<false>);
     }
     GA_CHECK_LAUNCH("render_bwd_kernel");
     {
         ProfScope _ps("preprocess_bwd_kernel", stream);
         cc.d_rgb = a.d_colors;
-        auto *k89 = cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<true, false>)
+        auto *k89 = dz ? preprocess_bwd_kernel<false, false, true>
+                  : cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<true, false>)
                            : (cc.cov3D ? preprocess_bwd_kernel<false, true> : preprocess_bwd_kernel<>);
         k89<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(d.P, d.H, d.W, cam, a.mod, a.means3D, a.scales, a.rotations, a.rot_stride,
-                 radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D, a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D, cc);
+                 radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D, a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D, cc, d_z);
     }
     GA_CHECK_LAUNCH("preprocess_bwd_kernel");
     return GA_OK;
@@ -1737,7 +1811,7 @@ extern "C" int ga_rasterb_status_to_host(int32_t B, int32_t H, int32_t W, void *
 static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene, const MatteSets *mattes, float *depth,
                          const float *cams, const float *bg, const float *means3D, const float *colors, const float *scales,
                          const float *rotations, const float *opacities, void *geom, void *img, void *binning, int32_t *radii,
-                         float *out_color, cudaStream_t stream)
+                         float *out_color, cudaStream_t stream, const DepthState *dstate = nullptr)
 {
     if (scene == nullptr) {
         GA_REQUIRE(cams && bg && img && binning && out_color, "NULL pointer argument");
@@ -1749,7 +1823,7 @@ static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene
         const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
         const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
         if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
-        return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, nullptr, mattes, depth);
+        return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, nullptr, mattes, depth, dstate);
     }
     GA_REQUIRE(scene->Ps >= 0 && (long long)bd->P + scene->Ps <= 0x7fffffffll, "bad static count Ps=%d (P=%d)", (int)scene->Ps, (int)bd->P);
     const int Pt = bd->P + scene->Ps;
@@ -1862,6 +1936,63 @@ extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cam
                     d_rotations, d_opacities, d_means2D};
     return launch_backward(d, cam, a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P), carve_img(const_cast<void *>(img), d),
                            carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream);
+}
+
+extern "C" size_t ga_rasterb_depth_state_bytes(int32_t B, int32_t H, int32_t W, int64_t capacity)
+{
+    return carve_dstate(nullptr, capacity, make_dims(B, 0, H, W)).total;
+}
+extern "C" size_t ga_rasterb_depth_bwd_scratch_bytes(int32_t B, int32_t P)
+{
+    return depth_bwd_scratch_bytes((size_t)B * (size_t)(P > 0 ? P : 0));
+}
+
+extern "C" int ga_rasterb_forward_depth_train(const GaRasterBatchDesc *bd, float *depth, void *depth_state, size_t depth_state_bytes,
+                                              const float *cams, const float *bg, const float *means3D, const float *colors,
+                                              const float *scales, const float *rotations, const float *opacities, void *geom, void *img,
+                                              void *binning, int32_t *radii, float *out_color, void *stream_)
+{
+    if (int rc = check_batch(bd)) return rc;
+    GA_REQUIRE(depth != nullptr && depth_state != nullptr, "NULL pointer argument");
+    const DepthState ds = carve_dstate(depth_state, bd->capacity, make_dims(bd->B, 0, bd->H, bd->W));
+    if (ds.total > depth_state_bytes) {
+        set_error("depth state too small: need %zu bytes, have %zu", ds.total, depth_state_bytes);
+        return GA_ERR_CAPACITY;
+    }
+    return forward_batch(bd, nullptr, nullptr, depth, cams, bg, means3D, colors, scales, rotations, opacities, geom, img, binning, radii,
+                         out_color, static_cast<cudaStream_t>(stream_), &ds);
+}
+
+extern "C" int ga_rasterb_backward_depth(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,
+                                         const float *colors, const float *scales, const float *rotations, const int32_t *radii,
+                                         const void *geom, const void *img, const void *binning, const float *dL_dout,
+                                         const float *dL_ddepth, const float *depth, const void *depth_state, size_t depth_state_bytes,
+                                         void *scratch, size_t scratch_bytes, float *d_means3D, float *d_colors, float *d_scales,
+                                         float *d_rotations, float *d_opacities, float *d_means2D, void *stream_)
+{
+    if (int rc = check_batch(bd)) return rc;
+    if (bd->P == 0) return GA_OK;
+    GA_REQUIRE(cams && bg && means3D && colors && scales && rotations && radii && geom && img && binning && dL_dout && dL_ddepth && depth &&
+                   depth_state && scratch && d_means3D && d_colors && d_scales,
+               "NULL pointer argument");
+    const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
+    const DepthBwd dz{dL_ddepth, depth, carve_dstate(const_cast<void *>(depth_state), bd->capacity, d)};
+    if (dz.state.total > depth_state_bytes) {
+        set_error("depth state too small: need %zu bytes, have %zu", dz.state.total, depth_state_bytes);
+        return GA_ERR_CAPACITY;
+    }
+    const size_t need = depth_bwd_scratch_bytes((size_t)d.B * d.P);
+    if (need > scratch_bytes) {
+        set_error("depth backward scratch too small: need %zu bytes, have %zu", need, scratch_bytes);
+        return GA_ERR_CAPACITY;
+    }
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
+    const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, bd->rot_stride, bd->scale_modifier, d_means3D, d_colors, d_scales,
+                    d_rotations, d_opacities, d_means2D};
+    return launch_backward(d, cam, a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P),
+                           carve_img(const_cast<void *>(img), d), carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream,
+                           &dz);
 }
 
 extern "C" int ga_raster_views(int32_t B, int32_t P, int32_t H, int32_t W, int64_t capacity, const void *geom, const void *binning,

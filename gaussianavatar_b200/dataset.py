@@ -4,6 +4,8 @@ full_proj_transform camera_center [pose_data transl_data inp_pos_map rest_pose]`
 
     <source_path>/{train,test}/images/<name>.<ext>          RGB frames
                               /masks/<name>.<ext>           foreground masks (>= 128 = subject); absent with no_mask
+                              /depths/<name>.npy | .png     with ModelParams.depth_maps: view-space z [H,W], float32 metres
+                                                            (.npy) or uint16 millimetres (.png); 0 = no measurement
                               /cam_parms.npz                {intrinsic [3,3], extrinsic [4,4]}   (cam_static)
                               /cam_parms/<name>.npz         per-frame cameras                    (not cam_static)
                               /smpl_parms.pth               {beta [1,10], body_pose [F,72], trans [F,3]}  (stage 2: smpl_parms_pred.pth)
@@ -56,6 +58,33 @@ def composite_host(image_u8: np.ndarray, mask_u8: np.ndarray | None) -> torch.Te
     t = torch.from_numpy(np.ascontiguousarray(img)) / 255.0
     t = t.permute(2, 0, 1) if t.dim() == 3 else t.unsqueeze(-1).permute(2, 0, 1)
     return t.clamp(0.0, 1.0)
+
+
+def read_depth(folder: str, name: str, height: int, width: int, mask_u8: np.ndarray | None) -> torch.Tensor:
+    """<folder>/depths/<name>.npy (float32 metres) or .png (uint16 millimetres) as [H,W] float32 metres, zeroed where the mask
+    fails composite_host's >= 128 test (0 = no measurement).  A missing file raises FileNotFoundError, a map whose size is not the
+    image's ValueError, both naming the file."""
+    npy, png = join(folder, "depths", name + ".npy"), join(folder, "depths", name + ".png")
+    if os.path.exists(npy):
+        path, d = npy, np.asarray(np.load(npy), dtype=np.float32)
+    elif os.path.exists(png):
+        from PIL import Image
+        path = png
+        raw = np.array(Image.open(png))
+        if raw.dtype != np.uint16 and raw.dtype != np.int32:
+            raise ValueError(f"{png}: a depth PNG must be 16-bit (millimetres), got {raw.dtype}")
+        d = raw.astype(np.float32) * np.float32(1e-3)
+    else:
+        raise FileNotFoundError(f"depth map not found: {npy} (or {png})")
+    if d.ndim == 3 and d.shape[-1] == 1:
+        d = d[..., 0]
+    if d.shape != (height, width):
+        raise ValueError(f"{path}: depth map is {tuple(d.shape)}, the image is ({height}, {width})")
+    d = np.where(np.isfinite(d), d, 0.0).astype(np.float32)
+    if mask_u8 is not None:
+        m = np.asarray(mask_u8)
+        d = np.where((m if m.ndim == 2 else m[..., 0]) >= 128, d, np.float32(0.0))
+    return torch.from_numpy(np.ascontiguousarray(d, dtype=np.float32))
 
 
 def composite_on_device(image_u8: torch.Tensor, mask_u8: torch.Tensor | None) -> torch.Tensor:
@@ -136,6 +165,8 @@ class _MonoFolder(Dataset):
                 item["mask_u8"] = torch.from_numpy(mask if mask.ndim == 2 else mask[..., 0])
         else:
             item = dict(original_image=composite_host(np.array(image), mask))
+        if getattr(self.dataset_parms, "depth_maps", False):
+            item["depth"] = read_depth(self.data_folder, name, height, width, mask)
         return item, width, height
 
 

@@ -260,7 +260,10 @@ class RasterBatchPlan:
     blocks the enqueueing thread unless asked to.
 
     static_P: the size of a static scene set the plan's forwards composite with (`rasterize_batch_scene`): geom and radii then
-    cover P + static_P Gaussians per frame, and `scene_rgb` [B,static_P,3] receives the scene's per-frame SH colours."""
+    cover P + static_P Gaussians per frame, and `scene_rgb` [B,static_P,3] receives the scene's per-frame SH colours.
+
+    `rasterize_batch_with_depth` also uses `depth_state` (each pixel's depth sums at its checkpoints, sized from `capacity` and
+    re-allocated with the binning buffer) and `depth_scratch`, both allocated on its first call."""
 
     def __init__(self, B, P, H, W, device, capacity=None, static_P=0):
         L = _lib.lib()
@@ -274,6 +277,7 @@ class RasterBatchPlan:
         self.radii = torch.empty(self.B, Pt, dtype=torch.int32, device=device)
         self.scene_rgb = torch.empty(self.B, self.static_P, 3, dtype=torch.float32, device=device) if self.static_P else None
         self.binning = None
+        self.depth_state = self.depth_scratch = None
         self._alloc_binning()
         off = L.ga_rasterb_status(self.B, self.H, self.W, ptr(self.img)) - self.img.data_ptr()
         self.status_dev = self.img[off:off + 64].view(torch.int32)
@@ -289,6 +293,19 @@ class RasterBatchPlan:
         nb = _lib.lib().ga_rasterb_binning_bytes(self.B, self.H, self.W, self.capacity)
         self.binning = None
         self.binning = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        if self.depth_state is not None:
+            self.depth_state = None
+            self.alloc_depth()
+
+    def alloc_depth(self):
+        """The buffers of `rasterize_batch_with_depth` (kept until the plan is dropped; the state follows `capacity`)."""
+        L = _lib.lib()
+        if self.depth_state is None:
+            nb = L.ga_rasterb_depth_state_bytes(self.B, self.H, self.W, self.capacity)
+            self.depth_state = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        if self.depth_scratch is None:
+            nb = L.ga_rasterb_depth_bwd_scratch_bytes(self.B, self.P)
+            self.depth_scratch = torch.empty(nb, dtype=torch.uint8, device=self.device)
 
     def desc(self, rot_shared=True, opac_shared=True, scale_modifier=1.0):
         return _lib.GaRasterBatchDesc(self.B, self.P, self.H, self.W, self.capacity, 0 if rot_shared else 4 * self.P,
@@ -369,6 +386,56 @@ class _RasterizeBatch(torch.autograd.Function):
 
 def rasterize_batch(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan):
     return _RasterizeBatch.apply(means3D, colors, scales, rotations, opacities, cams, bg, plan)
+
+
+class _RasterizeBatchDepth(torch.autograd.Function):
+    """`_RasterizeBatch` that also returns the depth pass [B,2,H,W]; differentiable in the images and in plane 0 (the mean)."""
+
+    @staticmethod
+    def forward(ctx, means3D, colors, scales, rotations, opacities, cams, bg, plan):
+        if not means3D.is_cuda:
+            raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
+        if plan.static_P:
+            raise ValueError("rasterize_batch_with_depth renders the dynamic set alone: the plan has static_P > 0")
+        L = _lib.lib()
+        means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
+        opacities = _c(opacities).reshape(-1)
+        d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
+        plan.alloc_depth()
+        dev = means3D.device
+        out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=dev)
+        depth = torch.empty(plan.B, 2, plan.H, plan.W, dtype=torch.float32, device=dev)
+        _lib.check(L.ga_rasterb_forward_depth_train(ctypes.byref(d), ptr(depth), ptr(plan.depth_state), plan.depth_state.numel(), ptr(cams),
+                                                    ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(opacities),
+                                                    ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii), ptr(out), _stream()),
+                   "ga_rasterb_forward_depth_train")
+        plan.record_status()
+        ctx.plan, ctx.desc = plan, d
+        ctx.save_for_backward(means3D, colors, scales, rotations, cams, bg, depth)
+        return out, depth
+
+    @staticmethod
+    def backward(ctx, grad_out, grad_depth):
+        means3D, colors, scales, rotations, cams, bg, depth = ctx.saved_tensors
+        plan, d = ctx.plan, ctx.desc
+        if d.capacity != plan.capacity:
+            raise RuntimeError("the batched rasterizer's buffers were re-allocated between forward and backward")
+        grad_out = torch.zeros_like(depth[:, :3]) if grad_out is None else _c(grad_out)
+        g_m = torch.zeros_like(depth[:, 0]) if grad_depth is None else _c(grad_depth[:, 0])
+        d_means3D, d_colors, d_scales = torch.empty_like(means3D), torch.empty_like(colors), torch.empty_like(scales)
+        _lib.check(_lib.lib().ga_rasterb_backward_depth(ctypes.byref(d), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales),
+                                                        ptr(rotations), ptr(plan.radii), ptr(plan.geom), ptr(plan.img), ptr(plan.binning),
+                                                        ptr(grad_out), ptr(g_m), ptr(depth), ptr(plan.depth_state), plan.depth_state.numel(),
+                                                        ptr(plan.depth_scratch), plan.depth_scratch.numel(), ptr(d_means3D), ptr(d_colors),
+                                                        ptr(d_scales), None, None, None, _stream()), "ga_rasterb_backward_depth")
+        return d_means3D, d_colors, d_scales, None, None, None, None, None
+
+
+def rasterize_batch_with_depth(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan):
+    """`rasterize_batch` that also returns the depth pass of `rasterize_batch_depth`: (images [B,3,H,W], depth [B,2,H,W]), both
+    bit for bit that call's.  Differentiable in the images and in plane 0, the mean view-space z D / (1 - T) (plane 1, the median,
+    is not differentiated): its gradient reaches means3D through the blending weights and through each Gaussian's own z."""
+    return _RasterizeBatchDepth.apply(means3D, colors, scales, rotations, opacities, cams, bg, plan)
 
 
 def rasterize_batch_scene(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan, scene):

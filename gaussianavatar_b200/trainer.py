@@ -3,6 +3,8 @@ fused kernels, with optional frame-level data parallelism (one process per GPU; 
 the shared feature-net / geo_feature gradients, SURVEY.md §8e).
 
     loss = lambda_scale * scale_loss + wdecay_rgl * offset_loss + (1-lambda_dssim) * L1 + lambda_dssim * (1-SSIM) + geo_loss
+
+plus, in either stage, lambda_depth * masked L1 of the mean depth when the batch carries target `depth` (ModelParams.depth_maps).
 """
 from __future__ import annotations
 
@@ -11,7 +13,7 @@ import os
 import torch
 import torch.distributed as dist
 
-from .losses import image_loss
+from .losses import depth_loss, image_loss
 from .lpips import LPIPS
 from .optim import FusedAdam
 from .rasterizer import MAX_FRAMES_PER_CALL
@@ -40,7 +42,7 @@ def allreduce_gradients(grads, group=None):
 
 class _StepGraph:
     """One captured forward + loss + backward of a stage-1 step and its static input / output tensors."""
-    __slots__ = ("graph", "idx", "rest", "gt", "cams", "loss", "g_flat", "g_geo", "capacity", "plan", "states", "launches")
+    __slots__ = ("graph", "idx", "rest", "gt", "depth", "cams", "loss", "g_flat", "g_geo", "capacity", "plan", "states", "launches")
 
 
 class Stage1Trainer:
@@ -89,6 +91,8 @@ class Stage1Trainer:
         else:
             image, points, offset_loss, geo_loss, scale_loss = m.train_stage1(batch, iteration)
             loss = o.lambda_scale * scale_loss + wdecay_rgl * offset_loss + image_loss(image, batch["original_image"], o.lambda_dssim) + geo_loss
+        if self._depth_active(batch):
+            loss = loss + depth_loss(m.last_depth, batch["depth"], float(getattr(o, "lambda_depth", 1.0)))
         if epoch > o.lpips_start_iter:                   # train.py:89-91
             if self.perceptual_loss is not None:
                 gt = batch["original_image"]
@@ -105,6 +109,9 @@ class Stage1Trainer:
         return loss, image
 
     epoch_start = 0    # train.py:38-45: 0 unless resuming from a checkpoint
+
+    def _depth_active(self, batch) -> bool:
+        return batch.get("depth") is not None and float(getattr(self.opt, "lambda_depth", 1.0)) > 0
 
     def sync_gradients(self):
         """Data parallelism: ONE all-reduce(sum) per step over a flat bucket [net.flat.grad | geo_feature.grad | overflow flag]
@@ -240,10 +247,15 @@ class Stage1Trainer:
         G = _StepGraph()
         G.idx = batch["pose_idx"].to(dev).clone()
         G.gt = batch["original_image"].float().contiguous().clone()
+        G.depth = None
+        if batch.get("depth") is not None:                 # the target depth is a step input like the image
+            G.depth = torch.as_tensor(batch["depth"]).to(device=dev, dtype=torch.float32).contiguous().clone()
         G.cams = m._batch_cameras(batch, B, dev).clone()
         sb = dict(batch)
         sb.update(pose_idx=G.idx, original_image=G.gt, _cams=G.cams, height=m._scalar_list(batch["height"], B),
                   width=m._scalar_list(batch["width"], B))
+        if G.depth is not None:
+            sb["depth"] = G.depth
         # SMPL-X: the frames' hand / face pose is a step input like pose_idx; a replay must read this step's, not the captured one's
         G.rest = None
         if batch.get("rest_pose") is not None:
@@ -290,7 +302,8 @@ class Stage1Trainer:
         B = batch["original_image"].shape[0]
         wdecay_rgl = adjust_loss_weights(o.lambda_rgl, epoch, mode="decay", start=self.epoch_start, every=20)
         lpips_active = self.perceptual_loss is not None and epoch > o.lpips_start_iter
-        key = (B, tuple(batch["original_image"].shape[-2:]), float(wdecay_rgl), lpips_active)
+        # the last word stays the LPIPS flag (callers read it as k[-1]); the depth flag goes before it
+        key = (B, tuple(batch["original_image"].shape[-2:]), float(wdecay_rgl), batch.get("depth") is not None, lpips_active)
         G = self._graphs.get(key)
         if G is not None and G.capacity != G.plan.capacity:      # the rasterizer's buffers were re-allocated: the graph points at freed memory
             G = None
@@ -303,6 +316,8 @@ class Stage1Trainer:
                 raise ValueError(f"rest_pose {tuple(rest.shape)}: expected {tuple(G.rest.shape)}")
             G.rest.copy_(rest, non_blocking=True)
         G.gt.copy_(batch["original_image"], non_blocking=True)
+        if G.depth is not None:
+            G.depth.copy_(torch.as_tensor(batch["depth"]).reshape(G.depth.shape), non_blocking=True)
         G.cams.copy_(m._batch_cameras(batch, B, m.device))
         G.plan.bump_serial()
         G.plan.pending = True

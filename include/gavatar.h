@@ -203,6 +203,35 @@ int ga_rasterb_forward_depth(const GaRasterBatchDesc *d, const GaRasterScene *sc
                              const float *rotations, const float *opacities, void *geom, void *img, void *binning, int32_t *radii,
                              float *out_color, void *stream);
 
+/* Training against depth maps: ga_rasterb_forward / ga_rasterb_backward with the mean depth differentiable.
+ * ga_rasterb_forward_depth_train is ga_rasterb_forward_depth of the dynamic set alone (no scene, no sets): images, radii, every
+ * buffer and both depth planes are that call's, bit for bit.  It also fills `depth_state` (ga_rasterb_depth_state_bytes(B, H, W,
+ * capacity), caller-owned, to be kept with geom / img / binning until the backward): each pixel's D = sum_i w_i z_i at the start of
+ * every 256-entry segment of its tile's list and at its end, where z_i is the entry's view-space z in world units (the z K1 culls at
+ * 0.2 and sorts by, not the length of the ray) and w_i = alpha_i T_i.  A depth_state smaller than the size query asks is refused
+ * with GA_ERR_CAPACITY; NULL pointers are refused; both before anything launches.
+ *
+ * ga_rasterb_backward_depth is ga_rasterb_backward plus the gradient of dL_ddepth [B,H,W] = dL/dm, m = D / A the mean depth
+ * (plane 0 of that forward's `depth`, passed back unchanged), A = 1 - T_final:
+ *   dL/dz_i     = (g / A) w_i
+ *   dL/dalpha_i += (g / A) [T_i (z_i - zhat_i) - m T_final / (1 - alpha_i)],  zhat_i the depth composited behind entry i
+ * (un-premultiplied; a segment starts from the stored D: zhat = (D_final - D_ckpt) / T_ckpt).  dL/dalpha flows through the
+ * conic / mean2D / opacity chain as the colour's does; dL/dz enters d_means3D through the view matrix's z row.  Plane 1 (the
+ * median) is not differentiated.  scratch: ga_rasterb_depth_bwd_scratch_bytes(B, P) bytes (d_mean2D, d_conic_op as for
+ * ga_rasterb_backward, then dL/dz [B,P]).  Undersized depth_state or scratch and NULL pointers are refused before any launch. */
+size_t ga_rasterb_depth_state_bytes(int32_t B, int32_t H, int32_t W, int64_t capacity);
+size_t ga_rasterb_depth_bwd_scratch_bytes(int32_t B, int32_t P);
+int ga_rasterb_forward_depth_train(const GaRasterBatchDesc *d, float *depth, void *depth_state, size_t depth_state_bytes,
+                                   const float *cams, const float *bg, const float *means3D, const float *colors, const float *scales,
+                                   const float *rotations, const float *opacities, void *geom, void *img, void *binning, int32_t *radii,
+                                   float *out_color, void *stream);
+int ga_rasterb_backward_depth(const GaRasterBatchDesc *d, const float *cams, const float *bg, const float *means3D,
+                              const float *colors, const float *scales, const float *rotations, const int32_t *radii,
+                              const void *geom, const void *img, const void *binning, const float *dL_dout, const float *dL_ddepth,
+                              const float *depth, const void *depth_state, size_t depth_state_bytes, void *scratch,
+                              size_t scratch_bytes, float *d_means3D, float *d_colors, float *d_scales, float *d_rotations,
+                              float *d_opacities, float *d_means2D, void *stream);
+
 /* Debug / parity accessors into the opaque buffers (device pointers; valid after the forward that filled them).  B = 1 and
  * capacity = num_rendered for buffers of the per-frame API. */
 typedef struct GaRasterViews {
@@ -402,6 +431,20 @@ int ga_loss_forward(int32_t B, int32_t H, int32_t W, const float *image, const f
                     void *workspace, float *out3, void *stream);
 int ga_loss_backward(int32_t B, int32_t H, int32_t W, const float *image, const float *gt, float w_l1, float w_ssim,
                      const float *grad_out, void *workspace, float *d_image, void *stream);
+
+/* Masked L1 depth loss on the mean depth of ga_rasterb_forward_depth(_train): depth [B,2,H,W] (plane 0 the mean m, plane 1 the
+ * median), target [B,H,W] metric view-space z in the same world units (0 = no measurement).  A pixel counts when target > 0 and
+ * plane 1 is non-zero (exactly where 1 - T_final >= 0.5, so 1 / A <= 2); N = the counted pixels of all B frames.
+ *   out2[0] = lam / N * sum |m - target| over counted pixels (0 when N = 0),  out2[1] = N   (device floats)
+ * N stays on the device and every sum has a fixed order (no atomics), so replays give the same loss bit for bit.  The backward
+ * writes d_depth [B,H,W] = g lam sign(m - target) / N on counted pixels (sign(0) = 0) and 0 elsewhere, g = *grad_out (NULL = 1),
+ * reading N from the workspace (ga_depth_loss_workspace_bytes) the forward of the same inputs filled.  Undersized workspaces and
+ * NULL pointers are refused before any launch. */
+size_t ga_depth_loss_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int ga_depth_loss_forward(int32_t B, int32_t H, int32_t W, const float *depth, const float *target, float lam, void *workspace,
+                          size_t workspace_bytes, float *out2, void *stream);
+int ga_depth_loss_backward(int32_t B, int32_t H, int32_t W, const float *depth, const float *target, const float *grad_out,
+                           void *workspace, size_t workspace_bytes, float *d_depth, void *stream);
 
 /* torch.optim.Adam step (amsgrad=False, weight_decay=0; model/avatar_model.py:148-155,264-267) on one contiguous buffer.
  * `step` is the 1-based count of this update; grad_scale multiplies the gradient first (1/world_size after an
