@@ -286,6 +286,9 @@ class Ensemble:
                 self._check_clip(a.model, a.clip, k)
             if not torch.equal(a.model.background.to(self.dev), m0.background):
                 raise ValueError(f"actor {k}'s background {a.model.background.tolist()} differs from actor 0's {m0.background.tolist()}")
+            if getattr(a.model, "antialiasing", False) != getattr(m0, "antialiasing", False):
+                raise ValueError(f"actor {k} renders with antialiasing={getattr(a.model, 'antialiasing', False)}, actor 0 with "
+                                 f"antialiasing={getattr(m0, 'antialiasing', False)}: the actors of a cast must share the mode")
             stage = 2 if int(a.model.model_parms.train_stage) == 2 else 1
             mapper = a.pose_mapper if a.pose_mapper is not None else getattr(a.model, "pose_mapper", None)
             if stage == 2 and mapper is None:
@@ -295,6 +298,7 @@ class Ensemble:
         self._models = list({id(a.model): a.model for a in self.actors}.values())
         sizes = [int(a.model._query_points.shape[0]) for a in self.actors]
         self.first = [0] + np.cumsum(sizes).tolist()          # actor k's Gaussians in the concatenated dynamic set
+        self.antialiasing = bool(getattr(m0, "antialiasing", False))    # the actors' (shared) mode; a scene's is its own
         one = len(self.actors) == 1                             # rotations / opacities shared by every frame, concatenated
         self._rot = m0.fix_rotation if one else torch.cat([a.model.fix_rotation for a in self.actors])
         self._opac = m0.fix_opacity if one else torch.cat([a.model.fix_opacity for a in self.actors])
@@ -432,7 +436,7 @@ class Ensemble:
     def _plan(self, b):
         if b not in self._plans:
             self._plans[b] = RasterBatchPlan(b, self.first[-1], self.H, self.W, self.dev, capacity=self.capacity,
-                                             static_P=0 if self.scene is None else len(self.scene))
+                                             static_P=0 if self.scene is None else len(self.scene), antialiasing=self.antialiasing)
         return self._plans[b]
 
     def _render(self, parts, cams, plan):

@@ -57,6 +57,8 @@ class AvatarModel:
         if self.device.type != "cuda":
             raise RuntimeError("AvatarModel runs on CUDA only (no CPU fallback)")
         self.batch_size = model_parms.batch_size if train else 1      # avatar_model.py:31-34
+        # every render of this avatar (training, render_free_*, the depth pass and the tools that take the model) uses the mode
+        self.antialiasing = bool(getattr(model_parms, "antialiasing", False))
         self.body = body_of(model_parms.smpl_type)
         if model_parms.train_stage not in (0, 1, 2):
             raise ValueError(f"train_stage {model_parms.train_stage} is not one of 1, 2")
@@ -348,7 +350,7 @@ class AvatarModel:
                             height=batch_data["height"][b], width=batch_data["width"][b], bg_color=self.background,
                             world_view_transform=batch_data["world_view_transform"][b],
                             full_proj_transform=batch_data["full_proj_transform"][b], active_sh_degree=0,
-                            camera_center=batch_data["camera_center"][b])
+                            camera_center=batch_data["camera_center"][b], antialiasing=self.antialiasing)
 
     # ---- batched rasterization: every frame of the step in one set of launches, no host read-back -------------------------------
     @staticmethod
@@ -387,7 +389,7 @@ class AvatarModel:
         plans = self.__dict__.setdefault("_raster_plans", {})
         key = (int(B), int(P), int(H), int(W))
         if key not in plans:
-            plans[key] = RasterBatchPlan(B, P, H, W, self.device)
+            plans[key] = RasterBatchPlan(B, P, H, W, self.device, antialiasing=self.antialiasing)
         return plans[key]
 
     def raster_ok(self, wait=True) -> bool:

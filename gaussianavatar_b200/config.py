@@ -35,6 +35,10 @@ class ModelParams:
     # train against metric depth maps, <split>/depths/<name>.npy (float32 metres) or .png (uint16 millimetres); not a reference
     # option, read with getattr(..., False)
     depth_maps: bool = False
+    # render with 3DGS's `antialiasing` setting (Mip-Splatting's screen-space filter: each splat's opacity is scaled so that its
+    # footprint does not depend on the 0.3 px^2 dilation) in training and every render of the avatar; not a reference option, read
+    # with getattr(..., False).  A checkpoint does not record it: render an avatar with the mode it was trained with
+    antialiasing: bool = False
 
 
 @dataclass

@@ -352,8 +352,10 @@ __device__ __forceinline__ void sh_color_bwd(const ColorCov &cc, size_t i, float
 
 // Per-Gaussian part of K1; returns the tile rect (zero area if the Gaussian is culled).  kCov: Sigma is read from cov_pre (this
 // Gaussian's six values) instead of being built from scales / rotations / mod; everything after Sigma is the same op sequence.
+// kAA (upstream's `antialiasing`): the stored opacity is o rho, rho = sqrt(max(2.5e-5, det(Sigma2) / det(Sigma2 + 0.3 I))) with
+// Sigma2 the projected covariance before the dilation; every other output is the call without it's, bit for bit.
 // i indexes the outputs, src the rows of means3D / scales.
-template <bool kCov>
+template <bool kCov, bool kAA = false>
 __device__ __forceinline__ ushort4
 preprocess_one(int il, size_t i, size_t src, int H, int W, int gx, int gy, const float *view, const float *proj, float tanfovx, float tanfovy,
                float mod, const float *__restrict__ means3D, const float *__restrict__ scales, const float *__restrict__ rq,
@@ -424,9 +426,10 @@ preprocess_one(int il, size_t i, size_t src, int H, int W, int gx, int gy, const
     const float v10 = fma_(S02, m1[2], fma_(S01, m1[1], mul_(S00, m1[0])));
     const float v11 = fma_(S12, m1[2], fma_(S11, m1[1], mul_(S01, m1[0])));
     const float v12 = fma_(S22, m1[2], fma_(S12, m1[1], mul_(S02, m1[0])));
-    const float ca = add_(fma_(m0[2], v02, fma_(m0[1], v01, mul_(m0[0], v00))), 0.3f);
+    const float ca0 = fma_(m0[2], v02, fma_(m0[1], v01, mul_(m0[0], v00)));
     const float cb = fma_(m0[2], v12, fma_(m0[1], v11, mul_(m0[0], v10)));
-    const float cc = add_(fma_(m1[2], v12, fma_(m1[1], v11, mul_(m1[0], v10))), 0.3f);
+    const float cc0 = fma_(m1[2], v12, fma_(m1[1], v11, mul_(m1[0], v10)));
+    const float ca = add_(ca0, 0.3f), cc = add_(cc0, 0.3f);
 
     const float det = sub_(mul_(ca, cc), mul_(cb, cb));
     if (det == 0.f) return none;
@@ -453,7 +456,12 @@ preprocess_one(int il, size_t i, size_t src, int H, int W, int gx, int gy, const
     depth[i] = tvz;
     radii[i] = radius;
     xy[i] = make_float2(pixx, pixy);
-    conic_o[i] = make_float4(conx, cony, conz, opacity);
+    float o = opacity;
+    if constexpr (kAA) {
+        const float det0 = sub_(mul_(ca0, cc0), mul_(cb, cb));
+        o = mul_(opacity, __fsqrt_rn(fmaxf(2.5e-5f, div_(det0, det))));
+    }
+    conic_o[i] = make_float4(conx, cony, conz, o);
     tiles[i] = (uint32_t)area;
     const ushort4 rc = make_ushort4((unsigned short)rminx, (unsigned short)rminy, (unsigned short)rmaxx, (unsigned short)rmaxy);
     rect[i] = rc;
@@ -518,7 +526,8 @@ __device__ __forceinline__ int tile_slot_find(const uint32_t *s_key, uint32_t ti
 // kSH / kCov (per-frame API only, B = 1): SH colours into cc.rgb / cc.clamped, Sigma from cc.cov3D.
 // kScene (composite forward): frame b holds P + sc.Ps Gaussians, the dynamic P first (per-frame means / scales, strided rotations /
 // opacities, as without it), then the static set; a static Gaussian's SH colour for frame b's camera centre goes to sc.rgb[b].
-template <bool kSH = false, bool kCov = false, bool kScene = false>
+// kAA: antialiased opacities (preprocess_one) for the Gaussians of the dynamic set, kAAStatic for those of the static set (kScene).
+template <bool kSH = false, bool kCov = false, bool kScene = false, bool kAA = false, bool kAAStatic = false>
 __global__ void __launch_bounds__(256)
 preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod, const float *__restrict__ means3D,
                       const float *__restrict__ scales, const float *__restrict__ rots, long long rot_stride,
@@ -539,12 +548,12 @@ preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod
     if constexpr (kScene) {
         const int Pf = P + sc.Ps;
         if (il < P) {
-            rc = preprocess_one<false>(il, (size_t)b * Pf + il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod,
+            rc = preprocess_one<false, kAA>(il, (size_t)b * Pf + il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod,
                                        means3D, scales, rots + (size_t)b * rot_stride + 4 * (size_t)il, nullptr,
                                        opac[(size_t)b * opac_stride + il], depth, xy, conic_o, cov3d, tiles, rect, radii);
         } else if (il < Pf) {
             const size_t j = (size_t)(il - P);
-            rc = preprocess_one<false>(il, (size_t)b * Pf + il, j, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, sc.means3D, sc.scales,
+            rc = preprocess_one<false, kAAStatic>(il, (size_t)b * Pf + il, j, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, sc.means3D, sc.scales,
                                        sc.rotations + 4 * j, nullptr, sc.opacities[j], depth, xy, conic_o, cov3d, tiles, rect, radii);
             float r[3] = {0.f, 0.f, 0.f};
             if (rc.z > rc.x)
@@ -554,7 +563,7 @@ preprocess_fwd_kernel(int P, int H, int W, int gx, int gy, CamSrc cam, float mod
             o[0] = r[0]; o[1] = r[1]; o[2] = r[2];
         }
     } else if (il < P) {
-        rc = preprocess_one<kCov>(il, (size_t)b * P + il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, means3D, scales,
+        rc = preprocess_one<kCov, kAA>(il, (size_t)b * P + il, (size_t)b * P + il, H, W, gx, gy, view, proj, tanfovx, tanfovy, mod, means3D, scales,
                                   rots + (size_t)b * rot_stride + 4 * (size_t)il, cc.cov3D + 6 * (size_t)il,
                                   opac[(size_t)b * opac_stride + il], depth, xy, conic_o, cov3d, tiles, rect, radii);
         if constexpr (kSH)
@@ -1320,14 +1329,18 @@ render_bwd_kernel(int H, int W, int gx, int T_tiles, int P, const int32_t *__res
 // kSH: also the SH colour backward (d_sh, direction term of d_means3D); kCov: dL/dSigma goes to cc.d_cov3D and the scale /
 // rotation chain is skipped (per-frame API only, B = 1).  kZ: d_means3D also gets dL/dz [B,P] (the depth backward's d_z) times
 // the view matrix's z row, the derivative of the view-space z K1 computes.
-template <bool kSH = false, bool kCov = false, bool kZ = false>
+// kAA: the backward of K1's antialiased opacity o rho (preprocess_one).  rho is recomputed here from this kernel's own 2D
+// covariance, o is the stored opacity conic_o.w over it (rho >= 0.005), dL/do = gO rho and, where the clamp is inactive,
+// dL/drho = gO o goes through rho = sqrt(r), r = det0 / det1 into the 2D-covariance gradients.
+template <bool kSH = false, bool kCov = false, bool kZ = false, bool kAA = false>
 __global__ void __launch_bounds__(256)
 preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *__restrict__ means3D,
                       const float *__restrict__ scales, const float *__restrict__ rots, long long rot_stride,
                       const int32_t *__restrict__ radii, const float *__restrict__ cov3d,
                       const float2 *__restrict__ d_mean2D, const float4 *__restrict__ d_conic_op,
                       float *__restrict__ d_means3D, float *__restrict__ d_scales, float *__restrict__ d_rots,
-                      float *__restrict__ d_opac, float *__restrict__ d_means2D_out, ColorCov cc, const float *__restrict__ d_z)
+                      float *__restrict__ d_opac, float *__restrict__ d_means2D_out, ColorCov cc, const float *__restrict__ d_z,
+                      const float4 *__restrict__ conic_o)
 {
     const int fb = blockIdx.y;
     __shared__ float view[16], proj[16];
@@ -1343,7 +1356,7 @@ preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *_
     const size_t i3 = 3 * (size_t)i;
     const float4 gco = d_conic_op[i];
     const float2 g2 = d_mean2D[i];
-    if (d_opac) d_opac[i] = gco.w;
+    if (d_opac && (!kAA || radii[i] <= 0)) d_opac[i] = gco.w;     // kAA: gO rho, written below for a visible Gaussian
     if (d_means2D_out) { d_means2D_out[i3] = g2.x; d_means2D_out[i3 + 1] = g2.y; d_means2D_out[i3 + 2] = 0.f; }
     if (radii[i] <= 0) {
         d_means3D[i3] = d_means3D[i3 + 1] = d_means3D[i3 + 2] = 0.f;
@@ -1392,6 +1405,23 @@ preprocess_bwd_kernel(int P, int H, int W, CamSrc cam, float mod, const float *_
         dL_da = denom2inv * (-c * c * gA + 2.f * b * c * gBh + (denom - a * c) * gC);
         dL_dc = denom2inv * (-a * a * gC + 2.f * a * b * gBh + (denom - a * c) * gA);
         dL_db = denom2inv * 2.f * (b * c * gA - (denom + 2.f * b * b) * gBh + a * b * gC);
+    }
+    if constexpr (kAA) {
+        // r = det0 / det1.  The numerators of dr/d(a0, c0, b) det1^2 are expanded so that no two large terms cancel:
+        // c0 det1 - det0 c = 0.3 (c0^2 + b^2) + 0.09 c0, a0 det1 - det0 a = 0.3 (a0^2 + b^2) + 0.09 a0, det1 - det0 = 0.3 (a0 + c0) + 0.09.
+        const float a0 = m0[0] * v0[0] + m0[1] * v0[1] + m0[2] * v0[2];      // a and c before the dilation
+        const float c0 = m1[0] * v1[0] + m1[1] * v1[1] + m1[2] * v1[2];
+        const float det0 = a0 * c0 - b * b;
+        const float r = det0 / denom;
+        const float rho = sqrtf(fmaxf(2.5e-5f, r));
+        if (d_opac) d_opac[i] = gco.w * rho;
+        if (r > 2.5e-5f) {
+            const float o = conic_o[i].w / rho;
+            const float g = gco.w * o * 0.5f / (rho * denom * denom);     // dL/drho drho/dr / det1^2
+            dL_da += g * (0.3f * (c0 * c0 + b * b) + 0.09f * c0);
+            dL_dc += g * (0.3f * (a0 * a0 + b * b) + 0.09f * a0);
+            dL_db -= g * 2.f * b * (0.3f * (a0 + c0) + 0.09f);
+        }
     }
     float dc[6];
     dc[0] = m0[0] * m0[0] * dL_da + m0[0] * m1[0] * dL_db + m1[0] * m1[0] * dL_dc;
@@ -1487,6 +1517,7 @@ struct FwdArgs {
     const float *means3D, *colors, *scales, *rotations, *opacities, *bg;
     long long rot_stride, opac_stride;
     float mod;
+    bool aa, aa_static;      // antialiased opacities for the dynamic / static (scene) set
 };
 
 // K1 + K2 for all frames.  cc selects the K1 variant (all zero: precomputed colours, Sigma from scales / rotations); a scene
@@ -1498,7 +1529,12 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
     GA_CHECK_CUDA(cudaMemsetAsync(iv.count, 0, sizeof(uint32_t) * BT, stream));
     if (d.P > 0) {
         ProfScope _ps("preprocess_fwd_kernel", stream);
-        auto *k1 = scene ? preprocess_fwd_kernel<false, false, true>
+        auto *k1 = scene ? (a.aa ? (a.aa_static ? preprocess_fwd_kernel<false, false, true, true, true>
+                                                : preprocess_fwd_kernel<false, false, true, true, false>)
+                                 : (a.aa_static ? preprocess_fwd_kernel<false, false, true, false, true>
+                                                : preprocess_fwd_kernel<false, false, true>))
+                 : a.aa ? (cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true, false, true> : preprocess_fwd_kernel<true, false, false, true>)
+                                  : (cc.cov3D ? preprocess_fwd_kernel<false, true, false, true> : preprocess_fwd_kernel<false, false, false, true>))
                  : cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true> : preprocess_fwd_kernel<true, false>)
                           : (cc.cov3D ? preprocess_fwd_kernel<false, true> : preprocess_fwd_kernel<>);
         k1<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(scene ? d.P - scene->Ps : d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D,
@@ -1578,6 +1614,7 @@ struct BwdArgs {
     long long rot_stride;
     float mod;
     float *d_means3D, *d_colors, *d_scales, *d_rotations, *d_opacities, *d_means2D;
+    bool aa;                 // the forward stored antialiased opacities
 };
 
 size_t bwd_scratch_bytes(size_t BP)
@@ -1623,11 +1660,14 @@ int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, ColorCov
     {
         ProfScope _ps("preprocess_bwd_kernel", stream);
         cc.d_rgb = a.d_colors;
-        auto *k89 = dz ? preprocess_bwd_kernel<false, false, true>
+        auto *k89 = dz ? (a.aa ? preprocess_bwd_kernel<false, false, true, true> : preprocess_bwd_kernel<false, false, true>)
+                  : a.aa ? (cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true, false, true> : preprocess_bwd_kernel<true, false, false, true>)
+                                   : (cc.cov3D ? preprocess_bwd_kernel<false, true, false, true> : preprocess_bwd_kernel<false, false, false, true>))
                   : cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<true, false>)
                            : (cc.cov3D ? preprocess_bwd_kernel<false, true> : preprocess_bwd_kernel<>);
         k89<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(d.P, d.H, d.W, cam, a.mod, a.means3D, a.scales, a.rotations, a.rot_stride,
-                 radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D, a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D, cc, d_z);
+                 radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D, a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D, cc, d_z,
+                 g.conic_o);
     }
     GA_CHECK_LAUNCH("preprocess_bwd_kernel");
     return GA_OK;
@@ -1685,7 +1725,7 @@ extern "C" int ga_raster_forward_preprocess_ex(const GaRasterSettings *s, const 
     GeomViews g = carve_geom(geom, (size_t)s->P);
     ImgViews iv = carve_img(img, d);
     const CamSrc cam{viewmatrix, projmatrix, nullptr, 0, s->tanfovx, s->tanfovy};
-    const FwdArgs a{means3D, nullptr, scales, rotations, opacities, nullptr, 0, 0, s->scale_modifier};
+    const FwdArgs a{means3D, nullptr, scales, rotations, opacities, nullptr, 0, 0, s->scale_modifier, s->antialiasing != 0};
     if (int rc = launch_preprocess(d, cam, a, cc, kNoCapacity, g, iv, radii, stream)) return rc;
     int32_t total = 0;
     GA_CHECK_CUDA(cudaMemcpyAsync(&total, iv.status, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
@@ -1744,7 +1784,7 @@ extern "C" int ga_raster_backward_ex(const GaRasterSettings *s, const GaRasterCo
     const Dims d = make_dims(1, s->P, s->H, s->W);
     const CamSrc cam{viewmatrix, projmatrix, nullptr, 0, s->tanfovx, s->tanfovy};
     const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, 0, s->scale_modifier, d_means3D, d_colors, d_scales, d_rotations,
-                    d_opacities, d_means2D};
+                    d_opacities, d_means2D, s->antialiasing != 0};
     return launch_backward(d, cam, a, cc, radii, carve_geom(const_cast<void *>(geom), (size_t)s->P),
                            carve_img(const_cast<void *>(img), d), carve_bin(const_cast<void *>(binning), R, d), scratch, stream);
 }
@@ -1821,7 +1861,8 @@ static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene
         ImgViews iv = carve_img(img, d);
         BinViews bv = carve_bin(binning, bd->capacity, d);
         const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
-        const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
+        const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier,
+                          bd->antialiasing != 0};
         if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
         return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, nullptr, mattes, depth, dstate);
     }
@@ -1846,7 +1887,8 @@ static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene
     ImgViews iv = carve_img(img, d);
     BinViews bv = carve_bin(binning, bd->capacity, d);
     const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
-    const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier};
+    const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier,
+                    bd->antialiasing != 0, scene->antialiasing != 0};
     if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream, &sc)) return rc;
     return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, &sc, mattes, depth);
 }
@@ -1933,7 +1975,7 @@ extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cam
     const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
     const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
     const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, bd->rot_stride, bd->scale_modifier, d_means3D, d_colors, d_scales,
-                    d_rotations, d_opacities, d_means2D};
+                    d_rotations, d_opacities, d_means2D, bd->antialiasing != 0};
     return launch_backward(d, cam, a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P), carve_img(const_cast<void *>(img), d),
                            carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream);
 }
@@ -1989,7 +2031,7 @@ extern "C" int ga_rasterb_backward_depth(const GaRasterBatchDesc *bd, const floa
     cudaStream_t stream = static_cast<cudaStream_t>(stream_);
     const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
     const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, bd->rot_stride, bd->scale_modifier, d_means3D, d_colors, d_scales,
-                    d_rotations, d_opacities, d_means2D};
+                    d_rotations, d_opacities, d_means2D, bd->antialiasing != 0};
     return launch_backward(d, cam, a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P),
                            carve_img(const_cast<void *>(img), d), carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream,
                            &dz);

@@ -164,7 +164,7 @@ def posed_gaussians(model, pose, transl, rest_pose=None, pose_mapper=None):
 
 def render_views(model, means, scales, colors, cams, H: int, W: int):
     """Yields (s, e, images [b,3,H,W], depth [b,2,H,W], final_T [b,H,W]) for the camera rows cams[s:e] in chunks of up to 8, rendered
-    with bg 0 (`rasterize_batch_depth`); a chunk whose binning buffer overflowed is rendered again after it grew.  final_T is a view
+    with bg 0 (`rasterize_batch_depth`) in the model's antialiasing mode; a chunk whose binning buffer overflowed is rendered again after it grew.  final_T is a view
     of the chunk's raster buffers: use it before the next chunk is drawn."""
     dev = means.device
     bg = torch.zeros(3, dtype=torch.float32, device=dev)
@@ -174,7 +174,7 @@ def render_views(model, means, scales, colors, cams, H: int, W: int):
         e = min(cams.shape[0], s + MAX_FRAMES_PER_CALL)
         b = e - s
         if b not in plans:
-            plans[b] = RasterBatchPlan(b, P, H, W, dev)
+            plans[b] = RasterBatchPlan(b, P, H, W, dev, antialiasing=getattr(model, "antialiasing", False))
         plan = plans[b]
         args = (means.expand(b, -1, -1), colors.expand(b, -1, -1), scales.expand(b, -1, -1), model.fix_rotation, model.fix_opacity,
                 cams[s:e].contiguous(), bg, plan)

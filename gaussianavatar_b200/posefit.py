@@ -106,7 +106,8 @@ class PoseFitter:
     def _plan(self, b, H, W):
         key = (b, H, W)
         if key not in self._plans:
-            self._plans[key] = RasterBatchPlan(b, int(self.model._query_points.shape[0]), H, W, self.dev, capacity=self.capacity)
+            self._plans[key] = RasterBatchPlan(b, int(self.model._query_points.shape[0]), H, W, self.dev, capacity=self.capacity,
+                                                  antialiasing=getattr(self.model, "antialiasing", False))
         return self._plans[key]
 
     def _fit_group(self, items, objective):

@@ -1,7 +1,8 @@
 """`diff_gaussian_rasterization`-compatible Python surface over the sm_90a rasterizer.
 
 Mirrors the API generation the reference binds at /root/reference gaussian_renderer/__init__.py:6,21-48:
-``GaussianRasterizationSettings`` (12-field NamedTuple), ``GaussianRasterizer(raster_settings)(means3D=, means2D=, shs=,
+``GaussianRasterizationSettings`` (12-field NamedTuple, plus upstream's later 13th field ``antialiasing`` after ``debug``,
+default False, so the 12-field positional form still works), ``GaussianRasterizer(raster_settings)(means3D=, means2D=, shs=,
 colors_precomp=, opacities=, scales=, rotations=, cov3D_precomp=) -> (color[3,H,W], radii[P])``, gradients returned in
 input order.  Validation behaviour follows [UPSTREAM] (SURVEY.md §8b): exactly one of shs / colors_precomp and exactly
 one of (scales+rotations) / cov3D_precomp, else ``Exception``.
@@ -11,6 +12,10 @@ with ``raster_settings.sh_degree`` D in 0..3, (D+1)^2 <= M, seen from ``raster_s
 ``scales`` + ``rotations`` (times ``scale_modifier``) or given as ``cov3D_precomp`` [P, 6] = (xx, xy, xz, yy, yz, zz).
 GaussianAvatar itself passes precomputed colours with scales + rotations (shs=None at model/avatar_model.py:350,
 cov3D_precomp=None at gaussian_renderer/__init__.py:37); the batched training path supports only that combination.
+
+``antialiasing`` (per call here, ``RasterBatchPlan(antialiasing=)`` for the batched path, ``GaussianScene.antialiasing`` for a
+scene) is upstream's screen-space filter: each splat's opacity is scaled by sqrt(det Sigma2 / det(Sigma2 + 0.3 I)) so that its
+footprint no longer depends on the 0.3 px^2 dilation (include/gavatar.h, DESIGN.md §4).
 """
 from __future__ import annotations
 
@@ -37,6 +42,7 @@ class GaussianRasterizationSettings(NamedTuple):
     campos: torch.Tensor
     prefiltered: bool
     debug: bool
+    antialiasing: bool = False
 
 
 def _c(t: torch.Tensor) -> torch.Tensor:
@@ -154,6 +160,11 @@ def _color_cov(P, dev, rs, shs, cov3D_precomp):
     return cc, tuple(keep), rgb, clamped
 
 
+def _aa(obj) -> int:
+    """The C ABI's antialiasing flag of a settings tuple or scene (objects without the field: off, as upstream's 12-field form)."""
+    return int(bool(getattr(obj, "antialiasing", False)))
+
+
 def rasterize_forward(means3D, colors, opacities, scales, rotations, rs: GaussianRasterizationSettings, *, shs=None,
                       cov3D_precomp=None):
     """K1..K6 on the current CUDA stream.  Returns (color [3,H,W], radii [P] int32, RasterContext).
@@ -164,7 +175,7 @@ def rasterize_forward(means3D, colors, opacities, scales, rotations, rs: Gaussia
     L = _lib.lib()
     dev = means3D.device
     P, H, W = int(means3D.shape[0]), int(rs.image_height), int(rs.image_width)
-    s = GaRasterSettings(P, H, W, float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier))
+    s = GaRasterSettings(P, H, W, float(rs.tanfovx), float(rs.tanfovy), float(rs.scale_modifier), _aa(rs))
     cc, keep, rgb, clamped = _color_cov(P, dev, rs, shs, cov3D_precomp)
     opt = lambda t: None if t is None else _c(t)
     means3D, colors, scales, rotations = _c(means3D), opt(colors), opt(scales), opt(rotations)
@@ -263,11 +274,15 @@ class RasterBatchPlan:
     cover P + static_P Gaussians per frame, and `scene_rgb` [B,static_P,3] receives the scene's per-frame SH colours.
 
     `rasterize_batch_with_depth` also uses `depth_state` (each pixel's depth sums at its checkpoints, sized from `capacity` and
-    re-allocated with the binning buffer) and `depth_scratch`, both allocated on its first call."""
+    re-allocated with the binning buffer) and `depth_scratch`, both allocated on its first call.
 
-    def __init__(self, B, P, H, W, device, capacity=None, static_P=0):
+    antialiasing: every forward and backward through the plan renders its dynamic set with antialiased opacities (`desc()`
+    carries the flag; a scene's static set follows its own `GaussianScene.antialiasing`)."""
+
+    def __init__(self, B, P, H, W, device, capacity=None, static_P=0, antialiasing=False):
         L = _lib.lib()
         self.B, self.P, self.H, self.W, self.device = int(B), int(P), int(H), int(W), device
+        self.antialiasing = bool(antialiasing)
         self.static_P = int(static_P)
         Pt = self.P + self.static_P
         self.capacity = int(capacity) if capacity else max(1 << 16, 6 * self.B * Pt)
@@ -309,7 +324,7 @@ class RasterBatchPlan:
 
     def desc(self, rot_shared=True, opac_shared=True, scale_modifier=1.0):
         return _lib.GaRasterBatchDesc(self.B, self.P, self.H, self.W, self.capacity, 0 if rot_shared else 4 * self.P,
-                                      0 if opac_shared else self.P, float(scale_modifier))
+                                      0 if opac_shared else self.P, float(scale_modifier), int(self.antialiasing))
 
     def bump_serial(self):
         """Number the forward that is about to run (eager code; a captured graph cannot change it, so whoever replays a graph
@@ -457,7 +472,7 @@ def rasterize_batch_scene(means3D, colors, scales, rotations, opacities, cams, b
     opacities = _c(opacities).reshape(-1)
     d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
     sc = _lib.GaRasterScene(Ps, int(scene.sh_degree), int(scene.shs.shape[1]), ptr(scene.means3D), ptr(scene.scales), ptr(scene.rotations),
-                            ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb))
+                            ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb), _aa(scene))
     out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=means3D.device)
     _lib.check(L.ga_rasterb_forward_scene(ctypes.byref(d), ctypes.byref(sc), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales),
                                           ptr(rotations), ptr(opacities), ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii),
@@ -513,7 +528,7 @@ def _forward_passes(name, means3D, colors, scales, rotations, opacities, cams, b
     if scene is not None:
         _on_device(dev, scene_means3D=scene.means3D, scene_shs=scene.shs, cams=cams)
         sc = _lib.GaRasterScene(Ps, int(scene.sh_degree), int(scene.shs.shape[1]), ptr(scene.means3D), ptr(scene.scales),
-                                ptr(scene.rotations), ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb))
+                                ptr(scene.rotations), ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb), _aa(scene))
     out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=dev)
     mattes = sets = dmap = None
     if first is not None:

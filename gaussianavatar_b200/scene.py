@@ -73,23 +73,28 @@ def _read_ply_vertices(path):
 @dataclass
 class GaussianScene:
     """Ps static Gaussians, activated: means3D [Ps,3], scales [Ps,3], rotations [Ps,4] (w, x, y, z, unit), opacities [Ps], and SH
-    coefficients shs [Ps,M,3] (k = 0 the DC term, M = (sh_degree + 1)^2), all fp32 and contiguous."""
+    coefficients shs [Ps,M,3] (k = 0 the DC term, M = (sh_degree + 1)^2), all fp32 and contiguous.
+
+    antialiasing: the scene was trained with 3DGS's `antialiasing` setting (Mip-Splatting's screen-space filter) and renders
+    with it.  A PLY does not record this, so it is the caller's to say (the player's `--scene_antialiasing`)."""
     means3D: torch.Tensor
     scales: torch.Tensor
     rotations: torch.Tensor
     opacities: torch.Tensor
     shs: torch.Tensor
     sh_degree: int
+    antialiasing: bool = False
 
     def __len__(self) -> int:
         return int(self.means3D.shape[0])
 
     def to(self, device) -> "GaussianScene":
         f = lambda t: t.to(device=device, dtype=torch.float32).contiguous()
-        return GaussianScene(f(self.means3D), f(self.scales), f(self.rotations), f(self.opacities).reshape(-1), f(self.shs), int(self.sh_degree))
+        return GaussianScene(f(self.means3D), f(self.scales), f(self.rotations), f(self.opacities).reshape(-1), f(self.shs), int(self.sh_degree),
+                             bool(self.antialiasing))
 
     @classmethod
-    def load_ply(cls, path) -> "GaussianScene":
+    def load_ply(cls, path, antialiasing: bool = False) -> "GaussianScene":
         """The `point_cloud.ply` of 3DGS's `GaussianModel.save_ply`: binary little-endian, element `vertex` with x y z, f_dc_0..2,
         f_rest_0..K-1 (channel-major: f_rest_{c (M-1) + k}), opacity, scale_0..2, rot_0..3 (w first).  Properties are read by name
         and others (nx ny nz, ...) ignored; K + 3 = 3M fixes the degree.  opacity -> sigmoid, scale -> exp, rot -> normalised."""
@@ -118,7 +123,7 @@ class GaussianScene:
         rot = rot / np.maximum(np.linalg.norm(rot, axis=1, keepdims=True), 1e-12)
         t = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float32))
         return cls(t(col("x", "y", "z")), t(np.exp(col("scale_0", "scale_1", "scale_2"))), t(rot),
-                   t(1.0 / (1.0 + np.exp(-np.asarray(v["opacity"], np.float64)))), t(shs), D)
+                   t(1.0 / (1.0 + np.exp(-np.asarray(v["opacity"], np.float64)))), t(shs), D, bool(antialiasing))
 
 
 def _rodrigues(rvec) -> np.ndarray:

@@ -302,8 +302,10 @@ class Stage1Trainer:
         B = batch["original_image"].shape[0]
         wdecay_rgl = adjust_loss_weights(o.lambda_rgl, epoch, mode="decay", start=self.epoch_start, every=20)
         lpips_active = self.perceptual_loss is not None and epoch > o.lpips_start_iter
-        # the last word stays the LPIPS flag (callers read it as k[-1]); the depth flag goes before it
-        key = (B, tuple(batch["original_image"].shape[-2:]), float(wdecay_rgl), batch.get("depth") is not None, lpips_active)
+        # the last word stays the LPIPS flag (callers read it as k[-1]); the depth flag (k[3]) and the model's antialiasing mode go
+        # before it
+        key = (B, tuple(batch["original_image"].shape[-2:]), float(wdecay_rgl), batch.get("depth") is not None,
+               bool(getattr(m, "antialiasing", False)), lpips_active)
         G = self._graphs.get(key)
         if G is not None and G.capacity != G.plan.capacity:      # the rasterizer's buffers were re-allocated: the graph points at freed memory
             G = None

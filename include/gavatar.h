@@ -56,9 +56,19 @@ int ga_profile_report(char *buf, size_t cap);
  * reference's transposed 4x4s (scene/dataset_mono.py:248-250), i.e. flat[col*4+row]; image planar [3,H,W];
  * radii int32 [P].
  * ---------------------------------------------------------------------------------------------------------------- */
+/* Antialiasing (upstream's `antialiasing` setting, Mip-Splatting's screen-space filter), one flag per Gaussian set: 0 renders
+ * with the fixed 0.3 px^2 dilation alone, as upstream without the setting; nonzero also scales each splat's opacity so that its
+ * footprint integrates to what the undilated Gaussian's would.  With Sigma2 = [[a0, b], [b, c0]] the projected 2D covariance
+ * before the dilation, a = a0 + 0.3 and c = c0 + 0.3 (conic, radius and tile rect come from (a, b, c) either way):
+ *   r = (a0 c0 - b^2) / (a c - b^2),   rho = sqrt(max(2.5e-5, r)),   stored opacity (conic_opacity w) = o rho.
+ * Nothing else changes: radii, rects, depths, xy, conics and the binning are the call without it's, bit for bit.  The backwards
+ * return dL/do = gO rho (gO: dL/d of the stored opacity) and, where r > 2.5e-5, add gO o / (2 rho) dr/d(a0, b, c0) to the 2D
+ * covariance gradients; they recover o as the stored opacity over rho recomputed from their own covariance, so a backward must
+ * be given the flag its forward had. */
 typedef struct GaRasterSettings {
     int32_t P, H, W;
     float tanfovx, tanfovy, scale_modifier;
+    int32_t antialiasing;        /* 0: off (zero-initialised settings behave as before), else on; see above     */
 } GaRasterSettings;
 
 size_t ga_raster_geom_bytes(int32_t P);                       /* per-Gaussian state (upstream's geomBuffer)   */
@@ -128,6 +138,7 @@ typedef struct GaRasterBatchDesc {
     int64_t capacity;
     int64_t rot_stride, opac_stride;   /* floats between two frames' rotations / opacities: 4P / P, or 0 = shared */
     float scale_modifier;
+    int32_t antialiasing;              /* of the dynamic set (see GaRasterSettings); a backward takes its forward's */
 } GaRasterBatchDesc;
 size_t ga_rasterb_geom_bytes(int32_t B, int32_t P);
 size_t ga_rasterb_img_bytes(int32_t B, int32_t H, int32_t W);
@@ -162,6 +173,7 @@ typedef struct GaRasterScene {
     const float *opacities;      /* [Ps] activated                                                          */
     const float *shs;            /* [Ps, sh_coeffs, 3]                                                      */
     float *rgb;                  /* [B, Ps, 3] written: frame b's evaluated colours                         */
+    int32_t antialiasing;        /* of the static set (see GaRasterSettings), independent of the dynamic set's */
 } GaRasterScene;
 /* ga_rasterb_forward of the dynamic set (d->P, arrays and strides as there) splatted together with a static scene set in one sort
  * per tile, so that each occludes the other correctly.  Frame b has P + Ps Gaussians, the dynamic P first, then the static set:

@@ -21,10 +21,14 @@ others.  It replaces -s / -m / --motion / --body / --stage: the file is a list o
 fields
     source_path, model_path, epoch, motion                                  (required)
     stage (1), body ("smpl"), clip_fps, speed (1), align_to, place [S RX RY RZ TX TY TZ], smpl_model, smpl_gender ("neutral"),
-    uv_template, query_posmap_size (512), inp_posmap_size (128), nf (32), white_background (true)
+    uv_template, query_posmap_size (512), inp_posmap_size (128), nf (32), white_background (true), antialiasing (false)
 The first actor's dataset gives the cameras; each actor's `place` puts its world into the scene's (without a scene, into the
 first actor's placed world).  The output, camera and scene flags are shared; the playback lasts as long as the longest clip, a
 shorter one holding its last pose.
+--antialiasing renders the avatar with 3DGS's `antialiasing` setting (Mip-Splatting's screen-space filter); give it for an avatar
+trained with ModelParams.antialiasing, so that it looks right at any --size or camera distance.  A cast entry's `antialiasing`
+does the same, and the actors of one cast must share it.  --scene_antialiasing does it for a --scene trained with the setting
+(the PLY does not record it); the avatar's and the scene's modes are independent.
 --mattes DIR writes DIR/{:05d}_{k}.png, actor k's visible matte (8-bit greyscale: the weight its Gaussians add to each pixel),
 with --cast or for the single avatar (its visible mask inside a scene).
 --depth DIR writes DIR/{:05d}.npy, float32 [2,H,W]: plane 0 the mean, plane 1 the median view depth of the composited frame (the
@@ -49,13 +53,13 @@ from gaussianavatar_b200.dataset import camera_item  # noqa: E402
 
 CAST_REQUIRED = ("source_path", "model_path", "epoch", "motion")
 CAST_DEFAULTS = dict(stage=1, body="smpl", clip_fps=None, speed=1.0, align_to=None, place=None, smpl_model=None, smpl_gender="neutral",
-                     uv_template=None, query_posmap_size=512, inp_posmap_size=128, nf=32, white_background=True)
+                     uv_template=None, query_posmap_size=512, inp_posmap_size=128, nf=32, white_background=True, antialiasing=False)
 
 
 def read_cast(path):
     """The actors of a --cast file, each a dict of every field (defaults filled in) with its clip loaded as "clip".  Raises
     ValueError naming the entry: a missing or unknown field, a bad value, a clip that is not of the entry's body, or backgrounds
-    that differ from the first actor's."""
+    or antialiasing modes that differ from the first actor's."""
     with open(path) as f:
         try:
             raw = json.load(f)
@@ -84,6 +88,9 @@ def read_cast(path):
         if bool(d["white_background"]) != bool(out[0]["white_background"] if out else d["white_background"]):
             raise ValueError(f"{where}: white_background {d['white_background']}, actor 0 renders on "
                              f"{'white' if out[0]['white_background'] else 'black'}: the actors must share one background")
+        if out and bool(d["antialiasing"]) != bool(out[0]["antialiasing"]):
+            raise ValueError(f"{where}: antialiasing {bool(d['antialiasing'])}, actor 0 renders with antialiasing "
+                             f"{bool(out[0]['antialiasing'])}: the actors must share one mode")
         try:
             d["clip"] = MotionClip.load(d["motion"], d["body"], fps=d["clip_fps"])
         except ValueError as err:
@@ -98,7 +105,7 @@ def load_actor(d, project_path, placement):
     mp = ModelParams(source_path=d["source_path"], model_path=d["model_path"], project_path=project_path, smpl_model_path=model_dir,
                      smplx_model_path=model_dir, smpl_gender=d["smpl_gender"], smpl_type=d["body"], train_stage=d["stage"],
                      query_posmap_size=d["query_posmap_size"], inp_posmap_size=d["inp_posmap_size"], batch_size=1,
-                     white_background=bool(d["white_background"]))
+                     white_background=bool(d["white_background"]), antialiasing=bool(d["antialiasing"]))
     model = AvatarModel(mp, NetworkParams(nf=d["nf"]), OptimizationParams(), train=False)
     pose_mapper = None
     if d["stage"] == 1:
@@ -139,6 +146,10 @@ def main(argv=None):
     ap.add_argument("--scene", default=None, help="a 3DGS point_cloud.ply to render the avatar in")
     ap.add_argument("--place", type=float, nargs=7, metavar=("S", "RX", "RY", "RZ", "TX", "TY", "TZ"), default=None,
                     help="the avatar in the scene: x_scene = S R x + T, R from the axis-angle (RX, RY, RZ)")
+    ap.add_argument("--antialiasing", action="store_true",
+                    help="render the avatar with 3DGS's antialiasing setting (for an avatar trained with it)")
+    ap.add_argument("--scene_antialiasing", action="store_true", help="render --scene with 3DGS's antialiasing setting (for a scene "
+                    "trained with it)")
     ap.add_argument("--scene_cameras", default=None, help="cameras.json for --camera scene:K (default: the 3DGS model folder's)")
     ap.add_argument("--size", type=int, nargs=2, metavar=("W", "H"), default=None)
     ap.add_argument("--chunk", type=int, default=None, help="frames per rasterizer call (default 8, with --scene 2)")
@@ -152,7 +163,7 @@ def main(argv=None):
         ap.error("nothing to write: give --png DIR, --raw FILE, --mattes DIR and / or --depth DIR")
     if a.cast is not None:
         given = [f for f, v in (("-s", a.source_path), ("-m", a.model_path), ("--epoch", a.epoch), ("--motion", a.motion), ("--body", a.body),
-                                ("--stage", a.stage)) if v is not None]
+                                ("--stage", a.stage), ("--antialiasing", a.antialiasing or None)) if v is not None]
         if given:
             ap.error(f"--cast replaces {', '.join(given)}: give each actor's in the cast file")
         try:
@@ -164,7 +175,7 @@ def main(argv=None):
         specs = [dict(source_path=a.source_path, model_path=a.model_path, epoch=a.epoch, stage=a.stage, body=a.body, motion=a.motion,
                       clip_fps=a.clip_fps, speed=a.speed, align_to=a.align_to, place=a.place, smpl_model=a.smpl_model,
                       smpl_gender=a.smpl_gender, uv_template=a.uv_template, query_posmap_size=a.query_posmap_size,
-                      inp_posmap_size=a.inp_posmap_size, nf=a.nf, white_background=True)]
+                      inp_posmap_size=a.inp_posmap_size, nf=a.nf, white_background=True, antialiasing=a.antialiasing)]
     scene_cam = None
     if a.camera.startswith("scene:"):
         if a.scene is None:
@@ -175,6 +186,8 @@ def main(argv=None):
             ap.error(f"--camera {a.camera}: K must be an integer")
     elif a.camera not in ("dataset", "orbit"):
         ap.error(f"--camera {a.camera}: dataset, orbit or scene:K")
+    if a.scene_antialiasing and a.scene is None:
+        ap.error("--scene_antialiasing needs --scene")
     if a.place is not None and (a.scene is None or a.cast is not None):
         ap.error("--place needs --scene" if a.cast is None else "--place: give each actor's place in the cast file")
     if a.cast is None and a.stage == 2 and not (a.smpl_model and a.uv_template):
@@ -200,7 +213,7 @@ def main(argv=None):
     scene = None
     if a.scene is not None:
         from gaussianavatar_b200.scene import GaussianScene, load_scene_cameras, scene_cameras_path
-        scene = GaussianScene.load_ply(a.scene)
+        scene = GaussianScene.load_ply(a.scene, antialiasing=a.scene_antialiasing)
         if scene_cam is not None:
             cams = load_scene_cameras(a.scene_cameras or scene_cameras_path(a.scene))
             if not 0 <= scene_cam < len(cams):

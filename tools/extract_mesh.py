@@ -8,7 +8,8 @@ training frame K's pose and writes OUT/frame_{K:05d}.{ply,obj}; --motion CLIP sa
 does, --align_to mapping its first frame onto a training frame) and writes OUT/{:05d}.{ply,obj}, one mesh per output frame.
 --res samples along the grid's longest side, --views fusion views of --size x --size pixels, --trunc the truncation in voxels,
 --min_carve the views that must see through a sample to carve it.  --iou prints each mesh's silhouette IoU against the avatar's own
-(median depth > 0) from the dataset camera.  One JSON line per mesh goes to stdout.
+(median depth > 0) from the dataset camera.  --antialiasing renders the fusion views and every reference render with 3DGS's
+`antialiasing` setting, for an avatar trained with ModelParams.antialiasing.  One JSON line per mesh goes to stdout.
 
     python tools/extract_mesh.py -s DATA -m MODEL --epoch N --format glb --motion walk.npz --fps 30 --out rig
 
@@ -65,6 +66,8 @@ def parse(argv=None):
     ap.add_argument("--format", choices=("ply", "obj", "glb"), default="ply")
     ap.add_argument("--influences", type=int, choices=(4, 8), default=None, help="glb: joints per vertex (default 4)")
     ap.add_argument("--up", choices=("y", "z", "-y"), default=None, help="glb: the clip world's up axis")
+    ap.add_argument("--antialiasing", action="store_true", help="render the avatar's views with 3DGS's antialiasing setting (for an "
+                    "avatar trained with it)")
     ap.add_argument("--out", required=True)
     ap.add_argument("--iou", action="store_true")
     ap.add_argument("--psnr", action="store_true", help="glb: the unlit rig's PSNR against the avatar's render")
@@ -121,7 +124,8 @@ def main(argv=None):
 
     spec = dict(source_path=a.source_path, model_path=a.model_path, epoch=a.epoch, stage=a.stage, body=a.body, clip=None, speed=1.0,
                 align_to=a.align_to, smpl_model=a.smpl_model, smpl_gender=a.smpl_gender, uv_template=a.uv_template,
-                query_posmap_size=a.query_posmap_size, inp_posmap_size=a.inp_posmap_size, nf=a.nf, white_background=True)
+                query_posmap_size=a.query_posmap_size, inp_posmap_size=a.inp_posmap_size, nf=a.nf, white_background=True,
+                antialiasing=a.antialiasing)
     actor = load_actor(spec, a.project_path, None)
     model, body, dev = actor.model, actor.model.body, actor.model.device
     F = int(model.pose.weight.shape[0])
@@ -168,7 +172,8 @@ def main_glb(a):
 
     spec = dict(source_path=a.source_path, model_path=a.model_path, epoch=a.epoch, stage=a.stage, body=a.body, clip=None, speed=1.0,
                 align_to=a.align_to, smpl_model=a.smpl_model, smpl_gender=a.smpl_gender, uv_template=a.uv_template,
-                query_posmap_size=a.query_posmap_size, inp_posmap_size=a.inp_posmap_size, nf=a.nf, white_background=True)
+                query_posmap_size=a.query_posmap_size, inp_posmap_size=a.inp_posmap_size, nf=a.nf, white_background=True,
+                antialiasing=a.antialiasing)
     actor = load_actor(spec, a.project_path, None)
     model, body = actor.model, actor.model.body
     F = int(model.pose.weight.shape[0])

@@ -41,6 +41,7 @@ def parse_args(argv=None):
     ap.add_argument("--inp_posmap_size", type=int, default=128)
     ap.add_argument("--nf", type=int, default=32, help="stage 2: the pose encoder's base width")
     ap.add_argument("--white_background", type=int, choices=(0, 1), default=1)
+    ap.add_argument("--antialiasing", action="store_true", help="render with 3DGS's antialiasing setting (for an avatar trained with it)")
     a = ap.parse_args(argv)
     if a.iters < 0:
         ap.error(f"--iters {a.iters} is negative")
@@ -85,7 +86,7 @@ def main(argv=None):
     mp = ModelParams(source_path=a.source_path, model_path=a.model_path, project_path=a.project_path, smpl_model_path=model_dir,
                      smplx_model_path=model_dir, smpl_gender=a.smpl_gender, smpl_type=a.body, train_stage=a.stage,
                      query_posmap_size=a.query_posmap_size, inp_posmap_size=a.inp_posmap_size, batch_size=1,
-                     white_background=bool(a.white_background))
+                     white_background=bool(a.white_background), antialiasing=bool(a.antialiasing))
     model = AvatarModel(mp, NetworkParams(nf=a.nf), OptimizationParams(), train=False)
     pose_mapper = None
     if a.stage == 1:
