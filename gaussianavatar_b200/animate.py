@@ -547,12 +547,8 @@ class Ensemble:
                     else:
                         parts.append(m._assemble(decs[id(m)], p, t, rest, placement=a.placement))
                 plan = self._plan(1)       # as _render_batched: a frame whose binning buffer overflowed is rendered again after it grew
-                out = self._render(parts, cams_all[i:i + 1], plan)
-                if not plan.check(wait=True):
-                    self.overflows += 1
-                    out = self._render(parts, cams_all[i:i + 1], plan)
-                    if not plan.check(wait=True):
-                        raise RuntimeError("animation: the rasterizer's binning buffer overflowed again after growing")
+                out, again = plan.render_checked(lambda: self._render(parts, cams_all[i:i + 1], plan), "animation")
+                self.overflows += int(again)
                 self._pack(*out, plan, slot, i - s, i - s + 1)
         return render
 

@@ -412,13 +412,9 @@ class AvatarModel:
             images, self.last_depth = rasterize_batch_with_depth(means, colors, scales, self.fix_rotation, self.fix_opacity, cams,
                                                                  self.background, plan)
             return images
-        images = render()
-        if (not torch.is_grad_enabled() and not torch.cuda.is_current_stream_capturing() and not getattr(self, "defer_raster_check", False)
-                and not plan.check(wait=True)):          # inference: make the result right before returning it (unless the caller checks later)
-            images = render()
-            if not plan.check(wait=True):
-                raise RuntimeError("batched rasterizer: binning buffer overflowed twice in a row")
-        return images
+        if torch.is_grad_enabled() or torch.cuda.is_current_stream_capturing() or getattr(self, "defer_raster_check", False):
+            return render()
+        return plan.render_checked(render, "AvatarModel")[0]    # inference: make the result right before returning it
 
     def _uniform_frames(self, batch_data, B):
         h, w = self._scalar_list(batch_data["height"], B), self._scalar_list(batch_data["width"], B)

@@ -26,6 +26,8 @@
 // so radii / ranges / list order are bit-exact against the CPU oracle regardless of nvcc's FMA contraction.
 #include <cub/cub.cuh>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace ga {
@@ -1520,6 +1522,16 @@ struct FwdArgs {
     bool aa, aa_static;      // antialiased opacities for the dynamic / static (scene) set
 };
 
+// f(std::true_type{}) or f(std::false_type{}): nested, it picks a kernel's template instance from run-time flags.
+template <class F>
+auto with_bool(bool b, F f)
+{
+    return b ? f(std::true_type{}) : f(std::false_type{});
+}
+
+// The batched API's cameras: kCamStride floats per frame, tan(fov / 2) read from the array.
+CamSrc batch_cams(const float *cams) { return CamSrc{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f}; }
+
 // K1 + K2 for all frames.  cc selects the K1 variant (all zero: precomputed colours, Sigma from scales / rotations); a scene
 // selects the composite K1, with d.P = P + Ps Gaussians per frame.
 int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const ColorCov &cc, long long capacity, const GeomViews &g,
@@ -1529,14 +1541,12 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
     GA_CHECK_CUDA(cudaMemsetAsync(iv.count, 0, sizeof(uint32_t) * BT, stream));
     if (d.P > 0) {
         ProfScope _ps("preprocess_fwd_kernel", stream);
-        auto *k1 = scene ? (a.aa ? (a.aa_static ? preprocess_fwd_kernel<false, false, true, true, true>
-                                                : preprocess_fwd_kernel<false, false, true, true, false>)
-                                 : (a.aa_static ? preprocess_fwd_kernel<false, false, true, false, true>
-                                                : preprocess_fwd_kernel<false, false, true>))
-                 : a.aa ? (cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true, false, true> : preprocess_fwd_kernel<true, false, false, true>)
-                                  : (cc.cov3D ? preprocess_fwd_kernel<false, true, false, true> : preprocess_fwd_kernel<false, false, false, true>))
-                 : cc.shs ? (cc.cov3D ? preprocess_fwd_kernel<true, true> : preprocess_fwd_kernel<true, false>)
-                          : (cc.cov3D ? preprocess_fwd_kernel<false, true> : preprocess_fwd_kernel<>);
+        auto *k1 = with_bool(a.aa, [&](auto aa) {
+            return scene ? with_bool(a.aa_static, [&](auto aas) { return preprocess_fwd_kernel<false, false, true, aa, aas>; })
+                         : with_bool(cc.shs != nullptr, [&](auto sh) {
+                               return with_bool(cc.cov3D != nullptr, [&](auto cov) { return preprocess_fwd_kernel<sh, cov, false, aa>; });
+                           });
+        });
         k1<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(scene ? d.P - scene->Ps : d.P, d.H, d.W, d.gx, d.gy, cam, a.mod, a.means3D,
                  a.scales, a.rotations, a.rot_stride, a.opacities, a.opac_stride, g.depth, g.xy, g.conic_o, g.cov3d, g.tiles, g.rect, radii,
                  iv.count, cc, scene ? *scene : SceneSet{});
@@ -1550,31 +1560,28 @@ int launch_preprocess(const Dims &d, const CamSrc &cam, const FwdArgs &a, const 
     return GA_OK;
 }
 
+// The tile sort's long-segment (kLong) or short-segment instance for a forward with or without a scene and a depth pass.
+template <bool kLong>
+auto tile_sort_for(bool scene, bool depth)
+{
+    constexpr int threads = kLong ? kSortThreads : kSortSmallThreads, max = kLong ? kSortMax : kSortSmallMax;
+    return with_bool(scene, [&](auto sc) { return with_bool(depth, [&](auto z) { return tile_sort_kernel<threads, max, kLong, sc, z>; }); });
+}
+
 // K3 + K4 + K6 for all frames (a scene: the composite K4, d.P = P + Ps; mattes and / or depth: K6's variant that writes them).
 int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacity, const GeomViews &g, const ImgViews &iv, const BinViews &bv,
                               float *out_color, cudaStream_t stream, const SceneSet *scene = nullptr, const MatteSets *mattes = nullptr,
                               float *depth = nullptr, const DepthState *dstate = nullptr)
 {
     static PerDeviceOnce attr_set;
-    if (attr_set.first()) {
-        GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           kSortMax * (int)sizeof(uint64_t)));
-        GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           kSortMax * (int)sizeof(uint64_t)));
-        GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true, false, true>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, kSortMax * (int)sizeof(uint64_t)));
-        GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_kernel<kSortThreads, kSortMax, true, true, true>,
-                                           cudaFuncAttributeMaxDynamicSharedMemorySize, kSortMax * (int)sizeof(uint64_t)));
-    }
+    if (attr_set.first())
+        for (int k = 0; k < 4; ++k)      // k = (depth, scene)
+            GA_CHECK_CUDA(cudaFuncSetAttribute(tile_sort_for<true>(k & 1, k & 2), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               kSortMax * (int)sizeof(uint64_t)));
     const float *scene_rgb = scene ? scene->rgb : nullptr;
     const int Pd = scene ? d.P - scene->Ps : d.P;
-    auto *sort_long = depth ? (scene ? tile_sort_kernel<kSortThreads, kSortMax, true, true, true>
-                                     : tile_sort_kernel<kSortThreads, kSortMax, true, false, true>)
-                            : (scene ? tile_sort_kernel<kSortThreads, kSortMax, true, true> : tile_sort_kernel<kSortThreads, kSortMax, true>);
-    auto *sort_short = depth ? (scene ? tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, true, true>
-                                      : tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, false, true>)
-                             : (scene ? tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false, true>
-                                      : tile_sort_kernel<kSortSmallThreads, kSortSmallMax, false>);
+    auto *sort_long = tile_sort_for<true>(scene != nullptr, depth != nullptr);
+    auto *sort_short = tile_sort_for<false>(scene != nullptr, depth != nullptr);
     const int BT = d.B * d.T;
     if (d.P > 0) {
         {
@@ -1595,16 +1602,14 @@ int launch_binning_and_render(const Dims &d, const FwdArgs &a, long long capacit
                  bv.recC, bv.seg_tile, iv.tile_maxc, scene_rgb, Pd);
     }
     GA_CHECK_LAUNCH("tile_sort_kernel");
-    auto render = [&](auto kernel, const char *name) {
-        ProfScope _ps(name, stream);
-        kernel<<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC, a.bg, bv.ckpt,
-                                          iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color, mattes ? *mattes : MatteSets{},
-                                          depth, dstate ? dstate->ckpt : nullptr, dstate ? dstate->final : nullptr);
-    };
-    if (mattes && depth) render(render_fwd_kernel<true, true>, "render_fwd_mattes_depth_kernel");
-    else if (mattes) render(render_fwd_kernel<true, false>, "render_fwd_mattes_kernel");
-    else if (depth) render(render_fwd_kernel<false, true>, "render_fwd_depth_kernel");
-    else render(render_fwd_kernel<false, false>, "render_fwd_kernel");
+    {
+        static const char *const names[2][2] = {{"render_fwd_kernel", "render_fwd_depth_kernel"}, {"render_fwd_mattes_kernel", "render_fwd_mattes_depth_kernel"}};
+        ProfScope _ps(names[mattes != nullptr][depth != nullptr], stream);
+        auto *k6 = with_bool(mattes != nullptr, [&](auto m) { return with_bool(depth != nullptr, [&](auto z) { return render_fwd_kernel<m, z>; }); });
+        k6<<<BT, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, iv.order, iv.ranges, iv.seg_start, bv.recA, bv.recB, bv.recC, a.bg, bv.ckpt,
+                                      iv.final_T, iv.n_contrib, iv.final_state, iv.tile_maxc, out_color, mattes ? *mattes : MatteSets{},
+                                      depth, dstate ? dstate->ckpt : nullptr, dstate ? dstate->final : nullptr);
+    }
     GA_CHECK_LAUNCH("render_fwd_kernel");
     return GA_OK;
 }
@@ -1626,10 +1631,12 @@ size_t bwd_scratch_bytes(size_t BP)
 // The depth backward's scratch: bwd_scratch_bytes' d_mean2D and d_conic_op, then d_z [B*P].
 size_t depth_bwd_scratch_bytes(size_t BP) { return bwd_scratch_bytes(BP) + align_up((BP > 0 ? BP : 1) * sizeof(float)); }
 
-// The inputs of the depth backward: dL/dm [B,H,W], the forward's depth [B,2,H,W] and its depth state.
+// The inputs of the depth backward: dL/dm [B,H,W], the forward's depth [B,2,H,W] and its depth state, with the sizes the caller
+// gave for that state and for the backward's scratch.
 struct DepthBwd {
     const float *dL_dm, *depth;
     DepthState state;
+    size_t state_bytes, scratch_bytes;
 };
 
 // K7 + fused K8/K9.  cc selects the K8/K9 variant as in launch_preprocess; with SH, K7's d_colors is dL/drgb (cc.d_rgb).  dz (batched
@@ -1646,25 +1653,22 @@ int launch_backward(const Dims &d, const CamSrc &cam, const BwdArgs &a, ColorCov
     GA_CHECK_CUDA(cudaMemsetAsync(a.d_colors, 0, sizeof(float) * 3 * BP, stream));
     {
         ProfScope _ps(dz ? "render_bwd_depth_kernel" : "render_bwd_kernel", stream);
-        const int grid = (int)bv.max_segments;
-        auto run = [&](auto kernel) {
-            kernel<<<grid, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges, iv.tile_maxc,
-                                                bv.recA, bv.recB, bv.recC, bv.ckpt, a.bg, iv.final_state, iv.n_contrib, a.dL_dout, d_mean2D,
-                                                d_conic_op, a.d_colors, dz ? dz->dL_dm : nullptr, dz ? dz->depth : nullptr,
-                                                dz ? dz->state.ckpt : nullptr, dz ? dz->state.final : nullptr, d_z);
-        };
-        if (dz) run(a.d_opacities ? render_bwd_kernel<true, true> : render_bwd_kernel<false, true>);
-        else run(a.d_opacities ? render_bwd_kernel<true> : render_bwd_kernel<false>);
+        auto *k7 = with_bool(a.d_opacities != nullptr, [&](auto op) { return with_bool(dz != nullptr, [&](auto z) { return render_bwd_kernel<op, z>; }); });
+        k7<<<(int)bv.max_segments, kBlock, 0, stream>>>(d.H, d.W, d.gx, d.T, d.P, iv.status, bv.seg_tile, iv.seg_start, iv.ranges, iv.tile_maxc,
+                                                        bv.recA, bv.recB, bv.recC, bv.ckpt, a.bg, iv.final_state, iv.n_contrib, a.dL_dout,
+                                                        d_mean2D, d_conic_op, a.d_colors, dz ? dz->dL_dm : nullptr, dz ? dz->depth : nullptr,
+                                                        dz ? dz->state.ckpt : nullptr, dz ? dz->state.final : nullptr, d_z);
     }
     GA_CHECK_LAUNCH("render_bwd_kernel");
     {
         ProfScope _ps("preprocess_bwd_kernel", stream);
         cc.d_rgb = a.d_colors;
-        auto *k89 = dz ? (a.aa ? preprocess_bwd_kernel<false, false, true, true> : preprocess_bwd_kernel<false, false, true>)
-                  : a.aa ? (cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true, false, true> : preprocess_bwd_kernel<true, false, false, true>)
-                                   : (cc.cov3D ? preprocess_bwd_kernel<false, true, false, true> : preprocess_bwd_kernel<false, false, false, true>))
-                  : cc.shs ? (cc.cov3D ? preprocess_bwd_kernel<true, true> : preprocess_bwd_kernel<true, false>)
-                           : (cc.cov3D ? preprocess_bwd_kernel<false, true> : preprocess_bwd_kernel<>);
+        auto *k89 = with_bool(a.aa, [&](auto aa) {
+            return dz ? preprocess_bwd_kernel<false, false, true, aa>
+                      : with_bool(cc.shs != nullptr, [&](auto sh) {
+                            return with_bool(cc.cov3D != nullptr, [&](auto cov) { return preprocess_bwd_kernel<sh, cov, false, aa>; });
+                        });
+        });
         k89<<<dim3(cdiv(d.P, 256), d.B), 256, 0, stream>>>(d.P, d.H, d.W, cam, a.mod, a.means3D, a.scales, a.rotations, a.rot_stride,
                  radii, g.cov3d, d_mean2D, d_conic_op, a.d_means3D, a.d_scales, a.d_rotations, a.d_opacities, a.d_means2D, cc, d_z,
                  g.conic_o);
@@ -1853,27 +1857,17 @@ static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene
                          const float *rotations, const float *opacities, void *geom, void *img, void *binning, int32_t *radii,
                          float *out_color, cudaStream_t stream, const DepthState *dstate = nullptr)
 {
-    if (scene == nullptr) {
-        GA_REQUIRE(cams && bg && img && binning && out_color, "NULL pointer argument");
-        GA_REQUIRE(bd->P == 0 || (means3D && colors && scales && rotations && opacities && geom && radii), "NULL pointer argument");
-        const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
-        GeomViews g = carve_geom(geom, (size_t)d.B * d.P);
-        ImgViews iv = carve_img(img, d);
-        BinViews bv = carve_bin(binning, bd->capacity, d);
-        const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
-        const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier,
-                          bd->antialiasing != 0};
-        if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream)) return rc;
-        return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, nullptr, mattes, depth, dstate);
+    int Pt = bd->P;
+    if (scene) {
+        GA_REQUIRE(scene->Ps >= 0 && (long long)bd->P + scene->Ps <= 0x7fffffffll, "bad static count Ps=%d (P=%d)", (int)scene->Ps, (int)bd->P);
+        Pt += scene->Ps;
+        if (int rc = check_dims(bd->B, Pt, bd->H, bd->W)) return rc;
     }
-    GA_REQUIRE(scene->Ps >= 0 && (long long)bd->P + scene->Ps <= 0x7fffffffll, "bad static count Ps=%d (P=%d)", (int)scene->Ps, (int)bd->P);
-    const int Pt = bd->P + scene->Ps;
-    if (int rc = check_dims(bd->B, Pt, bd->H, bd->W)) return rc;
     GA_REQUIRE(cams && bg && img && binning && out_color, "NULL pointer argument");
     GA_REQUIRE(bd->P == 0 || (means3D && colors && scales && rotations && opacities), "NULL pointer argument");
     GA_REQUIRE(Pt == 0 || (geom && radii), "NULL pointer argument");
     SceneSet sc{};
-    if (scene->Ps > 0) {
+    if (scene && scene->Ps > 0) {
         GA_REQUIRE(scene->means3D && scene->scales && scene->rotations && scene->opacities && scene->shs && scene->rgb,
                    "NULL pointer in the scene descriptor");
         GA_REQUIRE(scene->sh_degree >= 0 && scene->sh_degree <= 3, "scene sh_degree %d outside 0..3", (int)scene->sh_degree);
@@ -1882,15 +1876,15 @@ static int forward_batch(const GaRasterBatchDesc *bd, const GaRasterScene *scene
         sc = SceneSet{scene->means3D, scene->scales, scene->rotations, scene->opacities, scene->shs, scene->Ps, scene->sh_degree,
                       scene->sh_coeffs, scene->sh_coeffs % 4 == 0 && reinterpret_cast<uintptr_t>(scene->shs) % 16 == 0, scene->rgb};
     }
+    const SceneSet *set = scene ? &sc : nullptr;
     const Dims d = make_dims(bd->B, Pt, bd->H, bd->W);
     GeomViews g = carve_geom(geom, (size_t)d.B * d.P);
     ImgViews iv = carve_img(img, d);
     BinViews bv = carve_bin(binning, bd->capacity, d);
-    const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
     const FwdArgs a{means3D, colors, scales, rotations, opacities, bg, bd->rot_stride, bd->opac_stride, bd->scale_modifier,
-                    bd->antialiasing != 0, scene->antialiasing != 0};
-    if (int rc = launch_preprocess(d, cam, a, ColorCov{}, bd->capacity, g, iv, radii, stream, &sc)) return rc;
-    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, &sc, mattes, depth);
+                    bd->antialiasing != 0, scene && scene->antialiasing != 0};
+    if (int rc = launch_preprocess(d, batch_cams(cams), a, ColorCov{}, bd->capacity, g, iv, radii, stream, set)) return rc;
+    return launch_binning_and_render(d, a, bd->capacity, g, iv, bv, out_color, stream, set, mattes, depth, dstate);
 }
 
 extern "C" int ga_rasterb_forward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,
@@ -1960,6 +1954,35 @@ extern "C" int ga_rasterb_forward_depth(const GaRasterBatchDesc *bd, const GaRas
                          binning, radii, out_color, static_cast<cudaStream_t>(stream_));
 }
 
+// The batched backward (bd checked and P > 0 by the caller): dz NULL the colour backward alone, otherwise the depth backward, with
+// its state and scratch sizes checked against the batch.  Every check runs before the first launch.
+static int backward_batch(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D, const float *colors,
+                          const float *scales, const float *rotations, const int32_t *radii, const void *geom, const void *img,
+                          const void *binning, const float *dL_dout, void *scratch, float *d_means3D, float *d_colors, float *d_scales,
+                          float *d_rotations, float *d_opacities, float *d_means2D, cudaStream_t stream, const DepthBwd *dz = nullptr)
+{
+    GA_REQUIRE(cams && bg && means3D && colors && scales && rotations && radii && geom && img && binning && dL_dout && scratch &&
+                   d_means3D && d_colors && d_scales,
+               "NULL pointer argument");
+    const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
+    if (dz) {
+        if (dz->state.total > dz->state_bytes) {
+            set_error("depth state too small: need %zu bytes, have %zu", dz->state.total, dz->state_bytes);
+            return GA_ERR_CAPACITY;
+        }
+        const size_t need = depth_bwd_scratch_bytes((size_t)d.B * d.P);
+        if (need > dz->scratch_bytes) {
+            set_error("depth backward scratch too small: need %zu bytes, have %zu", need, dz->scratch_bytes);
+            return GA_ERR_CAPACITY;
+        }
+    }
+    const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, bd->rot_stride, bd->scale_modifier, d_means3D, d_colors, d_scales,
+                    d_rotations, d_opacities, d_means2D, bd->antialiasing != 0};
+    return launch_backward(d, batch_cams(cams), a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P),
+                           carve_img(const_cast<void *>(img), d), carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream,
+                           dz);
+}
+
 extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cams, const float *bg, const float *means3D,
                                    const float *colors, const float *scales, const float *rotations, const int32_t *radii,
                                    const void *geom, const void *img, const void *binning, const float *dL_dout, void *scratch,
@@ -1968,16 +1991,8 @@ extern "C" int ga_rasterb_backward(const GaRasterBatchDesc *bd, const float *cam
 {
     if (int rc = check_batch(bd)) return rc;
     if (bd->P == 0) return GA_OK;
-    GA_REQUIRE(cams && bg && means3D && colors && scales && rotations && radii && geom && img && binning && dL_dout && scratch &&
-                   d_means3D && d_colors && d_scales,
-               "NULL pointer argument");
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
-    const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
-    const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, bd->rot_stride, bd->scale_modifier, d_means3D, d_colors, d_scales,
-                    d_rotations, d_opacities, d_means2D, bd->antialiasing != 0};
-    return launch_backward(d, cam, a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P), carve_img(const_cast<void *>(img), d),
-                           carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream);
+    return backward_batch(bd, cams, bg, means3D, colors, scales, rotations, radii, geom, img, binning, dL_dout, scratch, d_means3D, d_colors,
+                          d_scales, d_rotations, d_opacities, d_means2D, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" size_t ga_rasterb_depth_state_bytes(int32_t B, int32_t H, int32_t W, int64_t capacity)
@@ -2014,27 +2029,11 @@ extern "C" int ga_rasterb_backward_depth(const GaRasterBatchDesc *bd, const floa
 {
     if (int rc = check_batch(bd)) return rc;
     if (bd->P == 0) return GA_OK;
-    GA_REQUIRE(cams && bg && means3D && colors && scales && rotations && radii && geom && img && binning && dL_dout && dL_ddepth && depth &&
-                   depth_state && scratch && d_means3D && d_colors && d_scales,
-               "NULL pointer argument");
-    const Dims d = make_dims(bd->B, bd->P, bd->H, bd->W);
-    const DepthBwd dz{dL_ddepth, depth, carve_dstate(const_cast<void *>(depth_state), bd->capacity, d)};
-    if (dz.state.total > depth_state_bytes) {
-        set_error("depth state too small: need %zu bytes, have %zu", dz.state.total, depth_state_bytes);
-        return GA_ERR_CAPACITY;
-    }
-    const size_t need = depth_bwd_scratch_bytes((size_t)d.B * d.P);
-    if (need > scratch_bytes) {
-        set_error("depth backward scratch too small: need %zu bytes, have %zu", need, scratch_bytes);
-        return GA_ERR_CAPACITY;
-    }
-    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-    const CamSrc cam{cams, cams + 16, cams + 32, kCamStride, 0.f, 0.f};
-    const BwdArgs a{means3D, colors, scales, rotations, bg, dL_dout, bd->rot_stride, bd->scale_modifier, d_means3D, d_colors, d_scales,
-                    d_rotations, d_opacities, d_means2D, bd->antialiasing != 0};
-    return launch_backward(d, cam, a, ColorCov{}, radii, carve_geom(const_cast<void *>(geom), (size_t)d.B * d.P),
-                           carve_img(const_cast<void *>(img), d), carve_bin(const_cast<void *>(binning), bd->capacity, d), scratch, stream,
-                           &dz);
+    GA_REQUIRE(dL_ddepth && depth && depth_state, "NULL pointer argument");
+    const DepthBwd dz{dL_ddepth, depth, carve_dstate(const_cast<void *>(depth_state), bd->capacity, make_dims(bd->B, bd->P, bd->H, bd->W)),
+                      depth_state_bytes, scratch_bytes};
+    return backward_batch(bd, cams, bg, means3D, colors, scales, rotations, radii, geom, img, binning, dL_dout, scratch, d_means3D, d_colors,
+                          d_scales, d_rotations, d_opacities, d_means2D, static_cast<cudaStream_t>(stream_), &dz);
 }
 
 extern "C" int ga_raster_views(int32_t B, int32_t P, int32_t H, int32_t W, int64_t capacity, const void *geom, const void *binning,

@@ -178,11 +178,7 @@ def render_views(model, means, scales, colors, cams, H: int, W: int):
         plan = plans[b]
         args = (means.expand(b, -1, -1), colors.expand(b, -1, -1), scales.expand(b, -1, -1), model.fix_rotation, model.fix_opacity,
                 cams[s:e].contiguous(), bg, plan)
-        img, depth = rasterize_batch_depth(*args)
-        if not plan.check(wait=True):
-            img, depth = rasterize_batch_depth(*args)
-            if not plan.check(wait=True):
-                raise RuntimeError("mesh extraction: the rasterizer's binning buffer overflowed again after growing")
+        (img, depth), _ = plan.render_checked(lambda: rasterize_batch_depth(*args), "mesh extraction")
         yield s, e, img, depth, final_transmittance(plan)
 
 

@@ -355,6 +355,18 @@ class RasterBatchPlan:
         self.grow(int(self.status_host[0]))
         return False
 
+    def render_checked(self, render, label: str):
+        """Runs render(), a call that renders one forward through this plan, and waits for its status.  If the forward overflowed
+        the binning buffer (which `check` has then grown), runs it once more.  Returns (render()'s result, whether it was run
+        again); a second overflow raises RuntimeError starting with `label`."""
+        out = render()
+        if self.check(wait=True):
+            return out, False
+        out = render()
+        if not self.check(wait=True):
+            raise RuntimeError(f"{label}: the rasterizer's binning buffer overflowed again after growing")
+        return out, True
+
     def grow(self, needed: int):
         """Re-allocate the binning buffer for a forward that needed `needed` instances (status word 0), with headroom."""
         self.capacity = int(1.5 * int(needed)) + 1024
@@ -364,93 +376,82 @@ class RasterBatchPlan:
         return _views(self.B, self.P + self.static_P, self.H, self.W, self.capacity, self.geom, self.binning, self.img, self.radii)
 
 
+def _batch_inputs(plan, means3D, colors, scales, rotations, opacities):
+    """Every batched forward's prelude: (descriptor, means3D, colors, scales, rotations, opacities) as the entry points take them,
+    opacities flattened and the rotation / opacity strides read from their shapes."""
+    if not means3D.is_cuda:
+        raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
+    means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
+    opacities = _c(opacities).reshape(-1)
+    d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
+    return d, means3D, colors, scales, rotations, opacities
+
+
+def _batch_forward_tail(plan, cams, bg, means3D, colors, scales, rotations, opacities, out):
+    """The arguments every ga_rasterb_forward* entry point ends with."""
+    return (ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(opacities), ptr(plan.geom), ptr(plan.img),
+            ptr(plan.binning), ptr(plan.radii), ptr(out), _stream())
+
+
 class _RasterizeBatch(torch.autograd.Function):
-    """means3D / colors / scales [B,P,3] -> images [B,3,H,W]; rotations [P,4] and opacities [P,1] shared by the frames."""
+    """means3D / colors / scales [B,P,3] -> images [B,3,H,W]; rotations [P,4] and opacities [P,1] shared by the frames.  With
+    with_depth, (images, depth pass [B,2,H,W]), differentiable in the images and in plane 0 (the mean)."""
 
     @staticmethod
-    def forward(ctx, means3D, colors, scales, rotations, opacities, cams, bg, plan):
-        if not means3D.is_cuda:
-            raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
+    def forward(ctx, means3D, colors, scales, rotations, opacities, cams, bg, plan, with_depth):
+        d, means3D, colors, scales, rotations, opacities = _batch_inputs(plan, means3D, colors, scales, rotations, opacities)
         L = _lib.lib()
-        means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
-        opacities = _c(opacities).reshape(-1)
-        d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
-        out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=means3D.device)
-        _lib.check(L.ga_rasterb_forward(ctypes.byref(d), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations),
-                                        ptr(opacities), ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii), ptr(out),
-                                        _stream()), "ga_rasterb_forward")
-        plan.record_status()
-        ctx.plan, ctx.desc = plan, d
-        ctx.save_for_backward(means3D, colors, scales, rotations, cams, bg)
-        return out
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        means3D, colors, scales, rotations, cams, bg = ctx.saved_tensors
-        plan, d = ctx.plan, ctx.desc
-        if d.capacity != plan.capacity:
-            raise RuntimeError("the batched rasterizer's buffers were re-allocated between forward and backward")
-        grad_out = _c(grad_out)
-        d_means3D, d_colors, d_scales = torch.empty_like(means3D), torch.empty_like(colors), torch.empty_like(scales)
-        _lib.check(_lib.lib().ga_rasterb_backward(ctypes.byref(d), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales),
-                                                  ptr(rotations), ptr(plan.radii), ptr(plan.geom), ptr(plan.img), ptr(plan.binning),
-                                                  ptr(grad_out), ptr(plan.scratch), ptr(d_means3D), ptr(d_colors), ptr(d_scales),
-                                                  None, None, None, _stream()), "ga_rasterb_backward")
-        return d_means3D, d_colors, d_scales, None, None, None, None, None
-
-
-def rasterize_batch(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan):
-    return _RasterizeBatch.apply(means3D, colors, scales, rotations, opacities, cams, bg, plan)
-
-
-class _RasterizeBatchDepth(torch.autograd.Function):
-    """`_RasterizeBatch` that also returns the depth pass [B,2,H,W]; differentiable in the images and in plane 0 (the mean)."""
-
-    @staticmethod
-    def forward(ctx, means3D, colors, scales, rotations, opacities, cams, bg, plan):
-        if not means3D.is_cuda:
-            raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
-        if plan.static_P:
-            raise ValueError("rasterize_batch_with_depth renders the dynamic set alone: the plan has static_P > 0")
-        L = _lib.lib()
-        means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
-        opacities = _c(opacities).reshape(-1)
-        d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
-        plan.alloc_depth()
         dev = means3D.device
+        depth = None
+        if with_depth:
+            if plan.static_P:
+                raise ValueError("rasterize_batch_with_depth renders the dynamic set alone: the plan has static_P > 0")
+            plan.alloc_depth()
         out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=dev)
-        depth = torch.empty(plan.B, 2, plan.H, plan.W, dtype=torch.float32, device=dev)
-        _lib.check(L.ga_rasterb_forward_depth_train(ctypes.byref(d), ptr(depth), ptr(plan.depth_state), plan.depth_state.numel(), ptr(cams),
-                                                    ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(opacities),
-                                                    ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii), ptr(out), _stream()),
-                   "ga_rasterb_forward_depth_train")
+        tail = _batch_forward_tail(plan, cams, bg, means3D, colors, scales, rotations, opacities, out)
+        if with_depth:
+            depth = torch.empty(plan.B, 2, plan.H, plan.W, dtype=torch.float32, device=dev)
+            _lib.check(L.ga_rasterb_forward_depth_train(ctypes.byref(d), ptr(depth), ptr(plan.depth_state), plan.depth_state.numel(), *tail),
+                       "ga_rasterb_forward_depth_train")
+        else:
+            _lib.check(L.ga_rasterb_forward(ctypes.byref(d), *tail), "ga_rasterb_forward")
         plan.record_status()
         ctx.plan, ctx.desc = plan, d
         ctx.save_for_backward(means3D, colors, scales, rotations, cams, bg, depth)
-        return out, depth
+        return out if depth is None else (out, depth)
 
     @staticmethod
-    def backward(ctx, grad_out, grad_depth):
+    def backward(ctx, grad_out, grad_depth=None):
         means3D, colors, scales, rotations, cams, bg, depth = ctx.saved_tensors
         plan, d = ctx.plan, ctx.desc
         if d.capacity != plan.capacity:
             raise RuntimeError("the batched rasterizer's buffers were re-allocated between forward and backward")
-        grad_out = torch.zeros_like(depth[:, :3]) if grad_out is None else _c(grad_out)
-        g_m = torch.zeros_like(depth[:, 0]) if grad_depth is None else _c(grad_depth[:, 0])
+        if depth is not None:
+            grad_out = torch.zeros_like(depth[:, :3]) if grad_out is None else grad_out
+            g_m = torch.zeros_like(depth[:, 0]) if grad_depth is None else _c(grad_depth[:, 0])
+        grad_out = _c(grad_out)
         d_means3D, d_colors, d_scales = torch.empty_like(means3D), torch.empty_like(colors), torch.empty_like(scales)
-        _lib.check(_lib.lib().ga_rasterb_backward_depth(ctypes.byref(d), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales),
-                                                        ptr(rotations), ptr(plan.radii), ptr(plan.geom), ptr(plan.img), ptr(plan.binning),
-                                                        ptr(grad_out), ptr(g_m), ptr(depth), ptr(plan.depth_state), plan.depth_state.numel(),
-                                                        ptr(plan.depth_scratch), plan.depth_scratch.numel(), ptr(d_means3D), ptr(d_colors),
-                                                        ptr(d_scales), None, None, None, _stream()), "ga_rasterb_backward_depth")
-        return d_means3D, d_colors, d_scales, None, None, None, None, None
+        L = _lib.lib()
+        head = (ctypes.byref(d), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(plan.radii), ptr(plan.geom),
+                ptr(plan.img), ptr(plan.binning), ptr(grad_out))
+        tail = (ptr(d_means3D), ptr(d_colors), ptr(d_scales), None, None, None, _stream())
+        if depth is None:
+            _lib.check(L.ga_rasterb_backward(*head, ptr(plan.scratch), *tail), "ga_rasterb_backward")
+        else:
+            _lib.check(L.ga_rasterb_backward_depth(*head, ptr(g_m), ptr(depth), ptr(plan.depth_state), plan.depth_state.numel(),
+                                                   ptr(plan.depth_scratch), plan.depth_scratch.numel(), *tail), "ga_rasterb_backward_depth")
+        return d_means3D, d_colors, d_scales, None, None, None, None, None, None
+
+
+def rasterize_batch(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan):
+    return _RasterizeBatch.apply(means3D, colors, scales, rotations, opacities, cams, bg, plan, False)
 
 
 def rasterize_batch_with_depth(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan):
     """`rasterize_batch` that also returns the depth pass of `rasterize_batch_depth`: (images [B,3,H,W], depth [B,2,H,W]), both
     bit for bit that call's.  Differentiable in the images and in plane 0, the mean view-space z D / (1 - T) (plane 1, the median,
     is not differentiated): its gradient reaches means3D through the blending weights and through each Gaussian's own z."""
-    return _RasterizeBatchDepth.apply(means3D, colors, scales, rotations, opacities, cams, bg, plan)
+    return _RasterizeBatch.apply(means3D, colors, scales, rotations, opacities, cams, bg, plan, True)
 
 
 def rasterize_batch_scene(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan, scene):
@@ -458,26 +459,8 @@ def rasterize_batch_scene(means3D, colors, scales, rotations, opacities, cams, b
     ways); forward only, images [B,3,H,W].  scene: a `scene.GaussianScene` on the device (means3D, scales, rotations, opacities
     [Ps], shs [Ps,M,3], sh_degree), with Ps = plan.static_P; cams rows must carry the camera centre (words 34..36).  Frame b's
     index space is the dynamic P, then the scene's Ps (plan.radii [B,P+Ps]); the scene's colours land in plan.scene_rgb."""
-    if not means3D.is_cuda:
-        raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
-    if torch.is_grad_enabled() and any(t.requires_grad for t in (means3D, colors, scales, rotations, opacities, scene.means3D, scene.shs,
-                                                                  scene.scales, scene.rotations, scene.opacities)):
-        raise RuntimeError("rasterize_batch_scene is forward only: it has no backward (run it under torch.no_grad())")
-    Ps = int(scene.means3D.shape[0])
-    if Ps != plan.static_P:
-        raise ValueError(f"the scene has {Ps} Gaussians, the plan was sized for static_P={plan.static_P}")
-    _on_device(means3D.device, scene_means3D=scene.means3D, scene_shs=scene.shs, cams=cams)
-    L = _lib.lib()
-    means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
-    opacities = _c(opacities).reshape(-1)
-    d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
-    sc = _lib.GaRasterScene(Ps, int(scene.sh_degree), int(scene.shs.shape[1]), ptr(scene.means3D), ptr(scene.scales), ptr(scene.rotations),
-                            ptr(scene.opacities), ptr(scene.shs), ptr(plan.scene_rgb), _aa(scene))
-    out = torch.empty(plan.B, 3, plan.H, plan.W, dtype=torch.float32, device=means3D.device)
-    _lib.check(L.ga_rasterb_forward_scene(ctypes.byref(d), ctypes.byref(sc), ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales),
-                                          ptr(rotations), ptr(opacities), ptr(plan.geom), ptr(plan.img), ptr(plan.binning), ptr(plan.radii),
-                                          ptr(out), _stream()), "ga_rasterb_forward_scene")
-    plan.record_status()
+    out, = _forward_passes("rasterize_batch_scene", "ga_rasterb_forward_scene", means3D, colors, scales, rotations, opacities, cams, bg,
+                           plan, None, scene)
     return out
 
 
@@ -489,7 +472,8 @@ def rasterize_batch_mattes(means3D, colors, scales, rotations, opacities, cams, 
     first: K+1 nondecreasing dynamic indices, first[0] = 0 and first[K] <= plan.P; set k is Gaussians first[k]..first[k+1]-1.
     Returns (images [B,3,H,W], mattes [B,K,H,W]): matte k is the weight set k's Gaussians added to each pixel (sum of alpha T
     over its blended entries), so the mattes sum to 1 - final transmittance where every splatted Gaussian is in a set."""
-    return _forward_passes("rasterize_batch_mattes", means3D, colors, scales, rotations, opacities, cams, bg, plan, first, scene, False)
+    return _forward_passes("rasterize_batch_mattes", "ga_rasterb_forward_mattes", means3D, colors, scales, rotations, opacities, cams, bg,
+                           plan, first, scene)
 
 
 def rasterize_batch_depth(means3D, colors, scales, rotations, opacities, cams, bg, plan: RasterBatchPlan, scene=None, first=None):
@@ -498,14 +482,15 @@ def rasterize_batch_depth(means3D, colors, scales, rotations, opacities, cams, b
     (images, mattes [B,K,H,W], depth) with `first`.  Depths are view-space z in world units over the entries each pixel blends,
     with the weights its colour uses: plane 0 the mean sum(w z) / (1 - T) (0 where nothing was blended), plane 1 the median, the z
     of the first blended entry after which T <= 0.5 (0 where the final T > 0.5).  0 means no surface (z <= 0.2 is culled)."""
-    return _forward_passes("rasterize_batch_depth", means3D, colors, scales, rotations, opacities, cams, bg, plan, first, scene, True)
+    return _forward_passes("rasterize_batch_depth", "ga_rasterb_forward_depth", means3D, colors, scales, rotations, opacities, cams, bg,
+                           plan, first, scene)
 
 
-def _forward_passes(name, means3D, colors, scales, rotations, opacities, cams, bg, plan, first, scene, depth):
-    """The batched forward with mattes (first not None) and / or depth: ga_rasterb_forward_mattes or ga_rasterb_forward_depth."""
-    if not means3D.is_cuda:
-        raise RuntimeError("gaussianavatar_b200 rasterizer needs CUDA tensors (no CPU fallback)")
+def _forward_passes(name, entry, means3D, colors, scales, rotations, opacities, cams, bg, plan, first, scene):
+    """The forward-only batched renders through `entry`: ga_rasterb_forward_scene (images), ga_rasterb_forward_mattes (images and
+    the mattes of `first`) or ga_rasterb_forward_depth (images, the mattes when `first` is given, and depth)."""
     given = [means3D, colors, scales, rotations, opacities]
+    d, means3D, colors, scales, rotations, opacities = _batch_inputs(plan, means3D, colors, scales, rotations, opacities)
     if scene is not None:
         given += [scene.means3D, scene.shs, scene.scales, scene.rotations, scene.opacities]
     if torch.is_grad_enabled() and any(t.requires_grad for t in given):
@@ -521,9 +506,6 @@ def _forward_passes(name, means3D, colors, scales, rotations, opacities, cams, b
         raise ValueError(f"the scene has {Ps} Gaussians, the plan was sized for static_P={plan.static_P}")
     L = _lib.lib()
     dev = means3D.device
-    means3D, colors, scales, rotations = _c(means3D), _c(colors), _c(scales), _c(rotations)
-    opacities = _c(opacities).reshape(-1)
-    d = plan.desc(rot_shared=rotations.dim() == 2, opac_shared=opacities.numel() == plan.P)
     sc = None
     if scene is not None:
         _on_device(dev, scene_means3D=scene.means3D, scene_shs=scene.shs, cams=cams)
@@ -534,15 +516,16 @@ def _forward_passes(name, means3D, colors, scales, rotations, opacities, cams, b
     if first is not None:
         mattes = torch.empty(plan.B, K, plan.H, plan.W, dtype=torch.float32, device=dev)
         sets = _lib.GaRasterSets(K, (ctypes.c_int32 * 9)(*(first + [0] * (9 - len(first)))), ptr(mattes))
-    rest = (ptr(cams), ptr(bg), ptr(means3D), ptr(colors), ptr(scales), ptr(rotations), ptr(opacities), ptr(plan.geom), ptr(plan.img),
-            ptr(plan.binning), ptr(plan.radii), ptr(out), _stream())
     sc = None if sc is None else ctypes.byref(sc)
     sets = None if sets is None else ctypes.byref(sets)
-    if depth:
+    passes = ()
+    if entry == "ga_rasterb_forward_depth":
         dmap = torch.empty(plan.B, 2, plan.H, plan.W, dtype=torch.float32, device=dev)
-        _lib.check(L.ga_rasterb_forward_depth(ctypes.byref(d), sc, sets, ptr(dmap), *rest), "ga_rasterb_forward_depth")
-    else:
-        _lib.check(L.ga_rasterb_forward_mattes(ctypes.byref(d), sc, sets, *rest), "ga_rasterb_forward_mattes")
+        passes = (sets, ptr(dmap))
+    elif entry == "ga_rasterb_forward_mattes":
+        passes = (sets,)
+    tail = _batch_forward_tail(plan, cams, bg, means3D, colors, scales, rotations, opacities, out)
+    _lib.check(getattr(L, entry)(ctypes.byref(d), sc, *passes, *tail), entry)
     plan.record_status()
     return tuple(t for t in (out, mattes, dmap) if t is not None)
 

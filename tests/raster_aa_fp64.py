@@ -9,26 +9,17 @@ before they are pulled back through J W, with o = conic_opacity.w / rho and rho 
 follows preprocess_one's operation order, tracked with the (value, bound) arithmetic of tests/raster_fp64.py.  Every K1 operation is
 round-to-nearest without contraction, and the bound counts each of them.
 
-`preprocess_backward` is raster_fp64.preprocess_backward with the antialiasing terms inserted where the kernel adds them, right after
-dL/d(a, b, c).  It is built from that function's own source, so the restatement of everything around the new terms stays the one the
-existing tests maintain.  Bug switches for the self-checks: no_rho_dopac (dL/do without the rho factor), no_drho (the dL/drho term
-dropped), dilated_num (det1 used as r's numerator), clamp_grad (the rho term also where the clamp is active).
+`preprocess_backward` is raster_fp64.preprocess_backward with the antialiasing terms (its `aa` argument) added where the kernel adds
+them, right after dL/d(a, b, c), so the restatement of everything around the new terms stays the one the existing tests maintain.  Bug
+switches for the self-checks: no_rho_dopac (dL/do without the rho factor), no_drho (the dL/drho term dropped), dilated_num (det1
+used as r's numerator), clamp_grad (the rho term also where the clamp is active).
 """
-import inspect
 import math
 
 import torch
 
 import raster_fp64 as rf
-from raster_fp64 import add, cf32, div, lsum, mul, sqrt_, sub
-
-R_MIN = cf32(2.5e-5)
-C03, C009 = cf32(0.3), cf32(0.09)
-
-
-def _clamp_min(a, t):
-    """fmaxf(t, a) of a tracked value: 1-Lipschitz, so the bound carries over."""
-    return a[0].clamp_min(t), a[1]
+from raster_fp64 import C03, R_MIN, add, cf32, clamp_min, div, lsum, mul, sqrt_, sub
 
 
 def rho_of(a0, b, c0, dilated_num=False):
@@ -37,7 +28,7 @@ def rho_of(a0, b, c0, dilated_num=False):
     det1 = sub(mul(a, c), mul(b, b))
     det0 = det1 if dilated_num else sub(mul(a0, c0), mul(b, b))
     r = div(det0, det1)
-    return r, sqrt_(_clamp_min(r, R_MIN)), det0, det1
+    return r, sqrt_(clamp_min(r, R_MIN)), det0, det1
 
 
 def forward_opacity(cov3d, means, view, tanfovx, tanfovy, H, W, opacities, bug=()):
@@ -72,59 +63,11 @@ def forward_opacity(cov3d, means, view, tanfovx, tanfovy, H, W, opacities, bug=(
     return mul((o, 0.0), rho), dict(a0=a0, b=b, c0=c0, r=r, rho=rho)
 
 
-def _aa_terms(loc, aa):
-    """The kernel's kAA block on the restatement's locals: returns the new dL/d(a, b, c) and records d_opacities and the clamp
-    decisions in aa."""
-    m0, m1, v0, v1, b, denom = loc["m0"], loc["m1"], loc["v0"], loc["v1"], loc["b"], loc["denom"]
-    bug = aa.get("bug", ())
-    gO = (loc["d_conic_op"][:, 3], 0.0)
-    a0 = lsum(*[mul(m0[k], v0[k]) for k in range(3)])
-    c0 = lsum(*[mul(m1[k], v1[k]) for k in range(3)])
-    det0 = denom if "dilated_num" in bug else sub(mul(a0, c0), mul(b, b))
-    r = div(det0, denom)
-    rho = sqrt_(_clamp_min(r, R_MIN))
-    aa["d_opacities"] = gO if "no_rho_dopac" in bug else mul(gO, rho)
-    active = r[0] > R_MIN
-    aa["marg_clamp"] = (r[0] - R_MIN).abs() <= r[1]
-    aa["active"] = active
-    if "clamp_grad" in bug:
-        active = torch.ones_like(active)
-    da, db, dc = loc["dL_da"], loc["dL_db"], loc["dL_dc"]
-    if "no_drho" in bug:
-        return da, db, dc
-    co_w = (torch.as_tensor(aa["co_w"]).to(r[0]).reshape(-1), 0.0)
-    o = div(co_w, rho)
-    g = div(mul(mul(gO, o), 0.5), mul(mul(rho, denom), denom))
-    bb = mul(b, b)
-    ta = mul(g, add(mul(C03, add(mul(c0, c0), bb)), mul(C009, c0)))
-    tc = mul(g, add(mul(C03, add(mul(a0, a0), bb)), mul(C009, a0)))
-    tb = mul(mul(rf.scale(g, 2.0), b), add(mul(C03, add(a0, c0)), C009))
-    # the terms are evaluated for every Gaussian; those of clamped ones (possibly inf) are discarded, not multiplied by 0
-    keep = lambda new, old: (torch.where(active, new[0], old[0]), torch.where(active, new[1], torch.as_tensor(old[1]).to(new[1])))
-    return keep(add(da, ta), da), keep(sub(db, tb), db), keep(add(dc, tc), dc)
-
-
-def _build():
-    src = inspect.getsource(rf.preprocess_backward)
-    sig = "exact32=True, bug=()):"
-    hook_after = "    dL_db = mul(scale(d2i, 2.0), lsum(sub(mul(mul(b, c), gA), mul(add(denom, mul(scale(b, 2.0), b)), gBh)), mul(mul(a, b), gC)))\n"
-    assert src.count(sig) == 1 and src.count(hook_after) == 1, "raster_fp64.preprocess_backward changed: update raster_aa_fp64"
-    src = src.replace(sig, "exact32=True, bug=(), aa=None):")
-    src = src.replace(hook_after, hook_after + "    if aa is not None:\n        dL_da, dL_db, dL_dc = _aa_terms(locals(), aa)\n")
-    ns = dict(vars(rf))
-    ns["_aa_terms"] = _aa_terms
-    exec(compile(src, rf.__file__, "exec"), ns)
-    return ns["preprocess_backward"]
-
-
-_bwd = _build()
-
-
 def preprocess_backward(*, co_w, bug=(), **inp):
     """raster_fp64.preprocess_backward of a frame rendered with the filter: co_w [P] is the stored opacity (geom conic_opacity.w).
     Adds "d_opacities" (value, bound), "marg_clamp" (clamp decisions within the bound) and "active" (r > 2.5e-5) to its dict."""
     aa = dict(co_w=co_w, bug=tuple(bug))
-    out = _bwd(**inp, aa=aa)
+    out = rf.preprocess_backward(**inp, aa=aa)
     vis = out["vis"]
     dv, de = aa["d_opacities"]
     out["d_opacities"] = (torch.where(vis, dv, 0.0), torch.where(vis, de, 0.0) if torch.is_tensor(de) else 0.0 * dv)

@@ -484,13 +484,52 @@ def sh_forward(means, shs, D, campos):
     return (v, e), v.clamp_min(0)
 
 
+R_MIN = cf32(2.5e-5)
+C03, C009 = cf32(0.3), cf32(0.09)
+
+
+def clamp_min(a, t):
+    """fmaxf(t, a) of a tracked value: 1-Lipschitz, so the bound carries over."""
+    return a[0].clamp_min(t), a[1]
+
+
+def _aa_terms(m0, m1, v0, v1, b, denom, gO, dL_da, dL_db, dL_dc, aa):
+    """The kernel's kAA block: returns the new dL/d(a, b, c) and records d_opacities and the clamp decisions in aa (see
+    raster_aa_fp64.preprocess_backward)."""
+    bug = aa.get("bug", ())
+    a0 = lsum(*[mul(m0[k], v0[k]) for k in range(3)])
+    c0 = lsum(*[mul(m1[k], v1[k]) for k in range(3)])
+    det0 = denom if "dilated_num" in bug else sub(mul(a0, c0), mul(b, b))
+    r = div(det0, denom)
+    rho = sqrt_(clamp_min(r, R_MIN))
+    aa["d_opacities"] = gO if "no_rho_dopac" in bug else mul(gO, rho)
+    active = r[0] > R_MIN
+    aa["marg_clamp"] = (r[0] - R_MIN).abs() <= r[1]
+    aa["active"] = active
+    if "clamp_grad" in bug:
+        active = torch.ones_like(active)
+    if "no_drho" in bug:
+        return dL_da, dL_db, dL_dc
+    co_w = (torch.as_tensor(aa["co_w"]).to(r[0]).reshape(-1), 0.0)
+    o = div(co_w, rho)
+    g = div(mul(mul(gO, o), 0.5), mul(mul(rho, denom), denom))
+    bb = mul(b, b)
+    ta = mul(g, add(mul(C03, add(mul(c0, c0), bb)), mul(C009, c0)))
+    tc = mul(g, add(mul(C03, add(mul(a0, a0), bb)), mul(C009, a0)))
+    tb = mul(mul(scale(g, 2.0), b), add(mul(C03, add(a0, c0)), C009))
+    # the terms are evaluated for every Gaussian; those of clamped ones (possibly inf) are discarded, not multiplied by 0
+    keep = lambda new, old: (torch.where(active, new[0], old[0]), torch.where(active, new[1], torch.as_tensor(old[1]).to(new[1])))
+    return keep(add(dL_da, ta), dL_da), keep(sub(dL_db, tb), dL_db), keep(add(dL_dc, tc), dL_dc)
+
+
 def preprocess_backward(means, view, proj, tanfovx, tanfovy, H, W, mod, radii, cov3d, d_mean2D, d_conic_op, scales=None,
-                        rots=None, depth=None, shs=None, D=0, campos=None, clamped=None, d_rgb=None, exact32=True, bug=()):
+                        rots=None, depth=None, shs=None, D=0, campos=None, clamped=None, d_rgb=None, exact32=True, bug=(), aa=None):
     """preprocess_bwd_kernel for one frame's P Gaussians (tensors of fp32 values; any device, computed in float64).  Returns a
     dict of (value, bound) pairs: d_means3D [P,3], d_cov3D [P,6], and without cov mode (scales given) d_scales [P,3] and
     d_rotations [P,4]; with SH d_sh [P,M,3].  Culled Gaussians (radii <= 0) get exact zeros with bound 0.  `vis`, `xgm` / `ygm`
     (the guard-band gates), `tvz` and `marg_overflow` describe the Gaussians.  exact32=False evaluates the exact part in plain
-    fp64 instead (to match the fp64 oracle)."""
+    fp64 instead (to match the fp64 oracle).  aa: a dict (co_w, bug) for a frame rendered with antialiasing, whose terms are added
+    right after dL/d(a, b, c) as the kernel adds them (raster_aa_fp64.preprocess_backward)."""
     dev = means.device
     f = lambda t: torch.as_tensor(t).to(device=dev, dtype=torch.float64)
     means, view, proj = f(means), f(view).reshape(16), f(proj).reshape(16)
@@ -541,6 +580,8 @@ def preprocess_backward(means, view, proj, tanfovx, tanfovy, H, W, mod, radii, c
     dL_da = mul(d2i, lsum(mul(mul(neg(c), c), gA), mul(mul(scale(b, 2.0), c), gBh), mul(sub(denom, ac), gC)))
     dL_dc = mul(d2i, lsum(mul(mul(neg(a), a), gC), mul(mul(scale(a, 2.0), b), gBh), mul(sub(denom, ac), gA)))
     dL_db = mul(scale(d2i, 2.0), lsum(sub(mul(mul(b, c), gA), mul(add(denom, mul(scale(b, 2.0), b)), gBh)), mul(mul(a, b), gC)))
+    if aa is not None:
+        dL_da, dL_db, dL_dc = _aa_terms(m0, m1, v0, v1, b, denom, (d_conic_op[:, 3], 0.0), dL_da, dL_db, dL_dc, aa)
     dc = [None] * 6
     for k, (i, j) in ((0, (0, 0)), (3, (1, 1)), (5, (2, 2))):
         dc[k] = lsum(mul(mul(m0[i], m0[i]), dL_da), mul(mul(m0[i], m1[i]), dL_db), mul(mul(m1[i], m1[i]), dL_dc))
