@@ -105,6 +105,12 @@ class AvatarModel:
         self.pose = torch.nn.Embedding(num_training_frames, pose_dim, _weight=_pose_data.clone().float(), sparse=True).to(dev)
         self.transl = torch.nn.Embedding(num_training_frames, 3, _weight=_transl_data.clone().float(), sparse=True).to(dev)
         self.optimizer_pose = torch.optim.SparseAdam(list(self.pose.parameters()) + list(self.transl.parameters()), 5.0e-3)
+        # per-training-frame colour transform [A | t] (ModelParams.train_exposure), identity at the start; row 0 is the gauge anchor and
+        # never moves (DESIGN.md §4)
+        self.exposure = None
+        self.exposure_optimizer = None
+        if bool(getattr(model_parms, "train_exposure", False)):
+            self.exposure = nn.Parameter(identity_exposure(num_training_frames, dev))
         bg_color = [1, 1, 1] if model_parms.white_background else [0, 0, 0]
         self.background = torch.tensor(bg_color, dtype=torch.float32, device=dev)
         self.optimizer = None
@@ -191,6 +197,47 @@ class AvatarModel:
             self.optimizer = torch.optim.Adam([{"params": self.net.parameters(), "lr": self.opt_parms.lr_net},
                                                {"params": self.geo_feature, "lr": self.opt_parms.lr_geomfeat}])
         self.scheduler = torch.optim.lr_scheduler.MultiStepLR(self.optimizer, self.opt_parms.sched_milestones, gamma=0.1)
+        self.exposure_setup()
+
+    def exposure_schedule_steps(self, world: int = 1) -> int:
+        """Steps of the stage one process takes: epochs x its batches per epoch (the frames split over `world` data-parallel ranks)."""
+        batches = len(self.train_dataset) // max(int(self.batch_size) * max(int(world), 1), 1)
+        return int(getattr(self.opt_parms, "epochs", 1)) * max(batches, 1)
+
+    def exposure_setup(self, world: int = 1):
+        """The exposure table's own Adam (ModelParams.train_exposure): its rate falls log-linearly over the stage's steps
+        (`exposure_schedule_steps`)."""
+        if self.exposure is None:
+            return
+        from .optim import ExposureAdam
+        op = self.opt_parms
+        self.exposure_optimizer = ExposureAdam(self.exposure, self.exposure_schedule_steps(world), float(getattr(op, "exposure_lr_init", 0.01)),
+                                               float(getattr(op, "exposure_lr_final", 0.001)))
+
+    def _exposure_state(self):
+        """Checkpoint entries of the exposure table: {} when the model does not train one."""
+        if self.exposure is None:
+            return {}
+        out = {"exposure": self.exposure.detach().clone()}
+        if self.exposure_optimizer is not None:
+            out["exposure_optimizer"] = self.exposure_optimizer.state_dict()
+        return out
+
+    def _load_exposure(self, saved, optimizer=True):
+        """The checkpoint's exposure table, or identity when it has none (reference checkpoints, ones written without the table)."""
+        if self.exposure is None:
+            return
+        table = saved.get("exposure")
+        with torch.no_grad():
+            if table is None:
+                self.exposure.copy_(identity_exposure(self.exposure.shape[0], self.device))
+            else:
+                table = torch.as_tensor(table).detach().float()
+                if tuple(table.shape) != tuple(self.exposure.shape):
+                    raise ValueError(f"checkpoint exposure {tuple(table.shape)}: expected {tuple(self.exposure.shape)}")
+                self.exposure.copy_(table)
+        if optimizer and self.exposure_optimizer is not None and "exposure_optimizer" in saved:
+            self.exposure_optimizer.load_state_dict(saved["exposure_optimizer"])
 
     def save(self, iteration):
         path = os.path.join(self.model_path, "net/iteration_{}".format(iteration))
@@ -198,11 +245,11 @@ class AvatarModel:
         if self.model_parms.train_stage == 2:                      # avatar_model.py:177-186
             torch.save({"pose_encoder": self.pose_encoder.state_dict(), "geo_feature": self.geo_feature, "pose": self.pose.state_dict(),
                         "transl": self.transl.state_dict(), "net": self.net.state_dict(), "optimizer": self.optimizer.state_dict(),
-                        "scheduler": self.scheduler.state_dict()}, os.path.join(path, "pose_encoder.pth"))
+                        "scheduler": self.scheduler.state_dict(), **self._exposure_state()}, os.path.join(path, "pose_encoder.pth"))
             return
         torch.save({"net": self.net.state_dict(), "geo_feature": self.geo_feature, "pose": self.pose.state_dict(),
                     "transl": self.transl.state_dict(), "optimizer": self.optimizer.state_dict(),
-                    "scheduler": self.scheduler.state_dict()}, os.path.join(path, "net.pth"))
+                    "scheduler": self.scheduler.state_dict(), **self._exposure_state()}, os.path.join(path, "net.pth"))
 
     def load(self, iteration, test=False):
         self._dec_cache = None
@@ -214,6 +261,8 @@ class AvatarModel:
                 self.pose.load_state_dict(saved["pose"], strict=False)
                 self.transl.load_state_dict(saved["transl"], strict=False)
             self.geo_feature.data[...] = saved["geo_feature"].data[...]
+            if not test:
+                self._load_exposure(saved)
         # optimizer state: written either by this implementation (ONE flat net parameter + geo_feature) or by the reference
         # (53 per-tensor Adam states + geo_feature, avatar_model.py:148-155): the latter is re-laid out into the flat buffer
         if self.optimizer is not None and "optimizer" in saved:
@@ -249,6 +298,7 @@ class AvatarModel:
         self.pose.load_state_dict(saved["pose"], strict=False)
         self.transl.load_state_dict(saved["transl"], strict=False)
         self.geo_feature.data[...] = saved["geo_feature"].data[...]
+        self._load_exposure(saved, optimizer=False)      # stage 1's table carries into stage 2; its Adam state does not
 
     def stage2_load(self, epoch):
         """avatar_model.py:223-236: everything a stage-2 run saved (`pose_encoder.pth`)."""
@@ -260,6 +310,7 @@ class AvatarModel:
         self.transl.load_state_dict(saved["transl"], strict=False)
         self.geo_feature.data[...] = saved["geo_feature"].data[...]
         self.pose_encoder.load_state_dict(saved["pose_encoder"], strict=False)
+        self._load_exposure(saved)
         return getattr(self, "novel_view_dataset", None)
 
     def getTrainDataloader(self):
@@ -292,12 +343,16 @@ class AvatarModel:
 
     def zero_grad(self, epoch):
         self.optimizer.zero_grad()
+        if self.exposure is not None:
+            self.exposure.grad = None
         if self.model_parms.train_stage == 1 and epoch > self.opt_parms.pose_op_start_iter:     # avatar_model.py:258-262
             self.optimizer_pose.zero_grad()
 
     def step(self, epoch):
         self.optimizer.step()
         self.scheduler.step()
+        if self.exposure_optimizer is not None:         # from the first step on, not only after pose_op_start_iter
+            self.exposure_optimizer.step()
         if self.model_parms.train_stage == 1 and epoch > self.opt_parms.pose_op_start_iter:     # avatar_model.py:263-270
             self.optimizer_pose.step()
 
@@ -310,15 +365,25 @@ class AvatarModel:
         """[B,J,12] for the body model: SMPL from pose [B,72]; SMPL-X from pose [B,66] and the frames' rest_pose [B,99]."""
         return Cano2Live.apply(self.body, pose_batch, rest_pose, transl_batch, self._rest_joints, self._inv_cano)
 
-    def _assemble(self, dec, pose, transl, rest_pose=None, scale_mul=1.0, per_frame=False, placement=None):
+    def _assemble(self, dec, pose, transl, rest_pose=None, scale_mul=1.0, per_frame=False, placement=None, exposure=None, exposure_idx=None):
         """Decoder output `dec` posed by pose / transl (and SMPL-X's rest_pose): cano2live, then the fused LBS / attribute assembly.
         Returns means3D, scales, colors [B,N,3].  per_frame: `dec` holds one [S*S,8] block per frame (stage 2).  placement: a
-        `scene.Placement` folded into cano2live, its scale into the LBS scale multiplier (the Gaussians are isotropic)."""
+        `scene.Placement` folded into cano2live, its scale into the LBS scale multiplier (the Gaussians are isotropic).  exposure
+        [F,3,4] with exposure_idx [B]: frame b's colours become A c + t, [A | t] = exposure[exposure_idx[b]] (None: identity)."""
         cano2live = self._cano2live(pose, transl, rest_pose)                                              # [B,J,12]
         if placement is not None:
             cano2live = placement.fold(cano2live)
             scale_mul = scale_mul * placement.scale
-        return LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, scale_mul, per_frame)
+        return LbsAssemble.apply(dec, cano2live, self.valid_index, self._query_points, self._query_lbs, scale_mul, per_frame, exposure,
+                                 exposure_idx)
+
+    def _batch_exposure(self, batch_data):
+        """(table [B,3,4], rows [B]) of a batch whose items carry a fitted `exposure` [3,4] (test frames), else (None, None)."""
+        e = batch_data.get("exposure")
+        if e is None:
+            return None, None
+        e = torch.as_tensor(e).to(device=self.device, dtype=torch.float32).reshape(-1, 3, 4).contiguous()
+        return e, torch.arange(e.shape[0], device=self.device, dtype=torch.int32)
 
     def _stage1_decoder(self, batch):
         """Stage 1's frame-invariant decoder output [S*S,8], its BatchNorm statistics taken over `batch` frames.  With `cache_decoder`
@@ -341,7 +406,8 @@ class AvatarModel:
         S = int(self.model_parms.query_posmap_size)
         dec = self.net.forward_packed(self.geo_feature, S, pose_batch.shape[0])                           # [S*S, 8]
         scale_mul = 1e-3 * iteration if (ramp and iteration < 1000) else 1.0                              # avatar_model.py:316-319
-        means, scales, colors = self._assemble(dec, pose_batch, transl_batch, rest_pose, scale_mul)
+        means, scales, colors = self._assemble(dec, pose_batch, transl_batch, rest_pose, scale_mul, exposure=self.exposure,
+                                               exposure_idx=idx if self.exposure is not None else None)
         return means, scales, colors, dec
 
     def _render_one(self, batch_data, means, scales, colors, b):
@@ -469,11 +535,12 @@ class AvatarModel:
         images = self._render_frames(batch_data, means, scales, colors, depth=batch_data.get("depth") is not None)
         return images, means, offset_loss, geo_loss, scale_loss
 
-    def _stage2_gaussians(self, batch_data, pose=None, transl=None, placement=None):
+    def _stage2_gaussians(self, batch_data, pose=None, transl=None, placement=None, exposure=None, exposure_idx=None):
         """Stage 2 (model/avatar_model.py:369-420 / :557-612): the pose encoder turns each frame's posed-body position map into a
         feature map that is ADDED to the geometry features, so the decoder runs per frame (B*S*S rows, BatchNorm statistics over all of
         them); no scale ramp in this stage.  The skeleton is posed with the model's pose / transl rows at `pose_idx`, as the reference
-        does, unless `pose` [B,72|66] and `transl` [B,3] are given (the animation player's sampled poses)."""
+        does, unless `pose` [B,72|66] and `transl` [B,3] are given (the animation player's sampled poses).  exposure / exposure_idx:
+        as `_assemble` takes them."""
         inp = batch_data.get("inp_pos_map")
         inp = self._pose_map(batch_data) if inp is None else inp.to(self.device).float()
         if pose is None:
@@ -482,15 +549,17 @@ class AvatarModel:
         S = int(self.model_parms.query_posmap_size)
         pose_featmap = self.pose_encoder(inp)                                                         # [B,64,h,h]
         dec = self.net.forward_packed_frames(self.geo_feature, pose_featmap, S)                      # [B*S*S, 8]
-        means, scales, colors = self._assemble(dec, pose, transl, batch_data.get("rest_pose"), per_frame=True, placement=placement)
+        means, scales, colors = self._assemble(dec, pose, transl, batch_data.get("rest_pose"), per_frame=True, placement=placement,
+                                               exposure=exposure, exposure_idx=exposure_idx)
         return means, scales, colors, dec, pose_featmap
 
-    def _stage2_from_pose(self, mapper, pose, transl, rest_pose=None, placement=None):
+    def _stage2_from_pose(self, mapper, pose, transl, rest_pose=None, placement=None, exposure=None, exposure_idx=None):
         """`_stage2_gaussians` of explicit poses [B,72|66] / transl [B,3] (and SMPL-X's rest_pose [B,99]): the input position maps are
         built from the same pose by `mapper` (a posmap.PoseMapper / SmplxPoseMapper, differentiable in pose and transl).  placement
         moves the posed Gaussians into a scene (`_assemble`); the position maps stay in the body's own frame."""
         inp = mapper.maps(pose, rest_pose, transl)
-        return self._stage2_gaussians({"inp_pos_map": inp, "rest_pose": rest_pose}, pose=pose, transl=transl, placement=placement)
+        return self._stage2_gaussians({"inp_pos_map": inp, "rest_pose": rest_pose}, pose=pose, transl=transl, placement=placement,
+                                      exposure=exposure, exposure_idx=exposure_idx)
 
     def _pose_map(self, batch_data):
         """Input position maps [B,3,s,s] of a batch that carries none: from its `pose_data` / `transl_data` when it has them (test,
@@ -508,7 +577,11 @@ class AvatarModel:
     def train_stage2(self, batch_data, iteration):
         """model/avatar_model.py:369-463: returns (images [B,3,H,W], full_pred [B,N,3], pose_loss, offset_loss); `last_depth` as
         train_stage1 leaves it."""
-        means, scales, colors, dec, pose_featmap = self._stage2_gaussians(batch_data)
+        if self.exposure is not None:
+            means, scales, colors, dec, pose_featmap = self._stage2_gaussians(batch_data, exposure=self.exposure,
+                                                                              exposure_idx=batch_data["pose_idx"])
+        else:
+            means, scales, colors, dec, pose_featmap = self._stage2_gaussians(batch_data)
         offset_loss = torch.mean((dec[:, :3] * 0.02) ** 2)          # mean over B x S*S x 3 (avatar_model.py:424)
         pose_loss = torch.mean(pose_featmap ** 2)
         self._last_gaussians = (means, scales, colors)
@@ -530,7 +603,9 @@ class AvatarModel:
             pose_batch, transl_batch = self.pose(idx), self.transl(idx)
         dec = self._stage1_decoder(pose_batch.shape[0])
         scale_mul = 1e-3 * iteration if iteration < 1000 else 1.0
-        means, scales, colors = self._assemble(dec, pose_batch, transl_batch, batch_data.get("rest_pose"), scale_mul)
+        table, rows = self._batch_exposure(batch_data)
+        means, scales, colors = self._assemble(dec, pose_batch, transl_batch, batch_data.get("rest_pose"), scale_mul, exposure=table,
+                                               exposure_idx=rows)
         return self._render_frames(batch_data, means, scales, colors)
 
     def invalidate_decoder_cache(self):
@@ -538,8 +613,14 @@ class AvatarModel:
 
     def render_free_stage2(self, batch_data, iteration):
         """model/avatar_model.py:557-649: the stage-2 forward without the losses."""
-        means, scales, colors, _, _ = self._stage2_gaussians(batch_data)
+        table, rows = self._batch_exposure(batch_data)
+        means, scales, colors, _, _ = self._stage2_gaussians(batch_data, exposure=table, exposure_idx=rows)
         return self._render_frames(batch_data, means, scales, colors)
+
+
+def identity_exposure(frames: int, device="cuda") -> torch.Tensor:
+    """[frames,3,4] of [I | 0]: every frame's colours as the decoder makes them."""
+    return torch.eye(3, 4, device=device, dtype=torch.float32).repeat(int(frames), 1, 1).contiguous()
 
 
 @contextlib.contextmanager

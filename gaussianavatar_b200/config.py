@@ -39,6 +39,9 @@ class ModelParams:
     # footprint does not depend on the 0.3 px^2 dilation) in training and every render of the avatar; not a reference option, read
     # with getattr(..., False).  A checkpoint does not record it: render an avatar with the mode it was trained with
     antialiasing: bool = False
+    # learn each training frame's exposure and white balance, c' = A c + t per frame with training frame 0 fixed at [I | 0]
+    # (DESIGN.md §4); not a reference option, read with getattr(..., False)
+    train_exposure: bool = False
 
 
 @dataclass
@@ -73,3 +76,7 @@ class OptimizationParams:
     # weight of the masked L1 depth loss when the batches carry `depth` (ModelParams.depth_maps); not a reference option, read
     # with getattr(..., 1.0).  An unmeasured starting point, not a tuned value
     lambda_depth: float = 1.0
+    # Adam learning rate of the per-frame exposure table (ModelParams.train_exposure), falling log-linearly from init to final over
+    # the stage's steps, as 3DGS's exposure optimiser does; not reference options, read with getattr
+    exposure_lr_init: float = 0.01
+    exposure_lr_final: float = 0.001

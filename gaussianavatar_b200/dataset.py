@@ -193,6 +193,8 @@ class MonoDataset_test(MonoDataset_train):
         item = super().__getitem__(index)
         pose_idx = item["pose_idx"]
         item["pose_data"], item["transl_data"] = self.pose_data[pose_idx], self.transl_data[pose_idx]      # dataset_mono.py:398-399
+        if "exposure" in self.smpl_data:     # a pose file written by tools/fit_poses.py --exposure: the frame's fitted [A | t]
+            item["exposure"] = _as_tensor(self.smpl_data["exposure"])[pose_idx].float().reshape(3, 4)
         return item
 
 

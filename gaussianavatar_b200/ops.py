@@ -70,10 +70,14 @@ class Cano2Live(torch.autograd.Function):
 class LbsAssemble(torch.autograd.Function):
     """dec_out [S*S,8] (stage 1: one output for all frames) or [B*S*S,8] (stage 2: per frame), cano2live [B,J,12] (J = 24 for SMPL,
     55 for SMPL-X), query_lbs [N,ld] (ld = 24, or 56 for SMPL-X: the 55 weights and a zero column)
-    -> means3D, scales, colors [B,N,3] (model/avatar_model.py:308-326 / :407-420)."""
+    -> means3D, scales, colors [B,N,3] (model/avatar_model.py:308-326 / :407-420).
+
+    exposure [F,3,4] (optional, with pose_idx [B]): frame b's colours become A c + t, [A | t] = exposure[pose_idx[b]], inside the
+    same kernel; the table gets a gradient, zero in row 0 (the gauge anchor, DESIGN.md §4).  pose_idx is moved to the device as
+    int32 and read there only."""
 
     @staticmethod
-    def forward(ctx, dec_out, cano2live, valid_index, query_points, query_lbs, scale_mul, per_frame=False):
+    def forward(ctx, dec_out, cano2live, valid_index, query_points, query_lbs, scale_mul, per_frame=False, exposure=None, pose_idx=None):
         _need_cuda(dec_out, "LbsAssemble")
         dec_out, cano2live = _f32c(dec_out), _f32c(cano2live)
         N, B = int(query_points.shape[0]), int(cano2live.shape[0])
@@ -85,16 +89,31 @@ class LbsAssemble(torch.autograd.Function):
         means = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
         scales = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
         colors = torch.empty(B, N, 3, device=dev, dtype=torch.float32)
-        _lib.check(_lib.lib().ga_lbs_forward_ex(N, B, J, ld, float(scale_mul), stride, ptr(dec_out), ptr(valid_index), ptr(query_points),
-                                                ptr(query_lbs), ptr(cano2live), ptr(means), ptr(scales), ptr(colors), _stream()),
-                   "ga_lbs_forward_ex")
-        ctx.save_for_backward(dec_out, cano2live, valid_index, query_points, query_lbs)
+        if exposure is None:
+            _lib.check(_lib.lib().ga_lbs_forward_ex(N, B, J, ld, float(scale_mul), stride, ptr(dec_out), ptr(valid_index), ptr(query_points),
+                                                    ptr(query_lbs), ptr(cano2live), ptr(means), ptr(scales), ptr(colors), _stream()),
+                       "ga_lbs_forward_ex")
+            table = idx = None
+        else:
+            if pose_idx is None:
+                raise ValueError("LbsAssemble: an exposure table needs the pose_idx it is indexed by")
+            if exposure.dim() != 3 or tuple(exposure.shape[1:]) != (3, 4):
+                raise ValueError(f"exposure {tuple(exposure.shape)}: expected [F,3,4]")
+            table = _f32c(exposure.detach())
+            idx = torch.as_tensor(pose_idx).to(device=dev, dtype=torch.int32).reshape(-1).contiguous()
+            if idx.numel() != B:
+                raise ValueError(f"pose_idx has {idx.numel()} entries for {B} frames")
+            _lib.check(_lib.lib().ga_lbs_forward_exposure(N, B, J, ld, float(scale_mul), stride, ptr(dec_out), ptr(valid_index),
+                                                          ptr(query_points), ptr(query_lbs), ptr(cano2live), int(table.shape[0]), ptr(table),
+                                                          ptr(idx), ptr(means), ptr(scales), ptr(colors), _stream()),
+                       "ga_lbs_forward_exposure")
+        ctx.save_for_backward(dec_out, cano2live, valid_index, query_points, query_lbs, table, idx)
         ctx.scale_mul, ctx.stride = float(scale_mul), stride
         return means, scales, colors
 
     @staticmethod
     def backward(ctx, d_means, d_scales, d_colors):
-        dec_out, cano2live, valid_index, query_points, query_lbs = ctx.saved_tensors
+        dec_out, cano2live, valid_index, query_points, query_lbs, table, idx = ctx.saved_tensors
         N, B = int(query_points.shape[0]), int(cano2live.shape[0])
         dev = dec_out.device
         zeros = None
@@ -111,10 +130,20 @@ class LbsAssemble(torch.autograd.Function):
         d_dec = torch.empty_like(dec_out)
         dC = torch.empty_like(cano2live)
         J, ld = int(cano2live.shape[1]), int(query_lbs.shape[1])
-        _lib.check(_lib.lib().ga_lbs_backward_ex(N, B, J, ld, int(dec_out.shape[0]), ctx.scale_mul, ctx.stride, ptr(dec_out), ptr(valid_index),
-                                                 ptr(query_points), ptr(query_lbs), ptr(cano2live), ptr(d_means), ptr(d_scales),
-                                                 ptr(d_colors), ptr(d_dec), ptr(dC), _stream()), "ga_lbs_backward_ex")
-        return d_dec, dC, None, None, None, None, None
+        if table is None:
+            _lib.check(_lib.lib().ga_lbs_backward_ex(N, B, J, ld, int(dec_out.shape[0]), ctx.scale_mul, ctx.stride, ptr(dec_out),
+                                                     ptr(valid_index), ptr(query_points), ptr(query_lbs), ptr(cano2live), ptr(d_means),
+                                                     ptr(d_scales), ptr(d_colors), ptr(d_dec), ptr(dC), _stream()), "ga_lbs_backward_ex")
+            return d_dec, dC, None, None, None, None, None, None, None
+        L = _lib.lib()
+        nbytes = int(L.ga_lbs_exposure_workspace_bytes(N, J))
+        ws = torch.empty(max(nbytes, 4), device=dev, dtype=torch.uint8)
+        d_table = torch.empty_like(table)
+        _lib.check(L.ga_lbs_backward_exposure(N, B, J, ld, int(dec_out.shape[0]), ctx.scale_mul, ctx.stride, ptr(dec_out), ptr(valid_index),
+                                              ptr(query_points), ptr(query_lbs), ptr(cano2live), int(table.shape[0]), ptr(table), ptr(idx),
+                                              ptr(d_means), ptr(d_scales), ptr(d_colors), ptr(d_dec), ptr(dC), ptr(d_table), ptr(ws), nbytes,
+                                              _stream()), "ga_lbs_backward_exposure")
+        return d_dec, dC, None, None, None, None, None, d_table, None
 
 
 class DecoderNet(torch.autograd.Function):

@@ -42,7 +42,7 @@ def allreduce_gradients(grads, group=None):
 
 class _StepGraph:
     """One captured forward + loss + backward of a stage-1 step and its static input / output tensors."""
-    __slots__ = ("graph", "idx", "rest", "gt", "depth", "cams", "loss", "g_flat", "g_geo", "capacity", "plan", "states", "launches")
+    __slots__ = ("graph", "idx", "rest", "gt", "depth", "cams", "loss", "g_flat", "g_geo", "g_exp", "capacity", "plan", "states", "launches")
 
 
 class Stage1Trainer:
@@ -79,6 +79,11 @@ class Stage1Trainer:
                 model.optimizer.load_state_dict(model.translate_optimizer_state(prev_opt))
             if prev_sched is not None and prev_sched.get("last_epoch", 0) > 0:
                 model.scheduler.load_state_dict(prev_sched)
+        if getattr(model, "exposure", None) is not None:
+            if model.exposure_optimizer is None:
+                model.exposure_setup()
+            # each rank takes 1/world of an epoch's batches: the rate schedule spans the steps this process takes
+            model.exposure_optimizer.total_steps = model.exposure_schedule_steps(self.world)
         self._comm_stream = None
 
     def loss(self, batch, iteration: int, epoch: int = 0):
@@ -114,8 +119,8 @@ class Stage1Trainer:
         return batch.get("depth") is not None and float(getattr(self.opt, "lambda_depth", 1.0)) > 0
 
     def sync_gradients(self):
-        """Data parallelism: ONE all-reduce(sum) per step over a flat bucket [net.flat.grad | geo_feature.grad | overflow flag]
-        (6.2 MB), issued asynchronously on NCCL's stream; the compute stream waits for it in-stream (the host does not), the
+        """Data parallelism: ONE all-reduce(sum) per step over a flat bucket [net.flat.grad | geo_feature.grad | exposure.grad (when
+        the model trains one, [F,12]) | overflow flag] (6.2 MB), issued asynchronously on NCCL's stream; the compute stream waits for it in-stream (the host does not), the
         1/world factor is folded into the Adam kernel and the gradients Adam reads are the bucket's views.  The last word
         carries the batched rasterizer's overflow flag, so that every rank skips (and later re-runs) a step any rank could not
         fit.  Pose / transl embedding rows are per-frame and stay rank-local (sparse grads)."""
@@ -124,6 +129,8 @@ class Stage1Trainer:
         m = self.model
         # the parameters every rank shares: stage 1 = feature net + geo_feature, stage 2 = feature net + pose encoder (avatar_model.py:148-161)
         shared = [m.net.flat] + ([m.geo_feature] if getattr(m.model_parms, "train_stage", 1) != 2 else list(m.pose_encoder.parameters()))
+        if getattr(m, "exposure", None) is not None:     # every rank applies the same dense update to its replica of the table
+            shared.append(m.exposure)
         shared = [p for p in shared if p.grad is not None]
         sizes = [p.grad.numel() for p in shared]
         total = sum(sizes)
@@ -198,6 +205,8 @@ class Stage1Trainer:
                 st["step"] = st["step"] - 1
         m.scheduler.last_epoch -= 1
         m.scheduler._step_count -= 1
+        if getattr(m, "exposure_optimizer", None) is not None:
+            m.exposure_optimizer.undo()
         for g, lr in zip(m.optimizer.param_groups, m.scheduler._get_closed_form_lr() if hasattr(m.scheduler, "_get_closed_form_lr") else m.scheduler.get_last_lr()):
             g["lr"] = lr
 
@@ -262,6 +271,7 @@ class Stage1Trainer:
             G.rest = torch.as_tensor(batch["rest_pose"]).to(device=dev, dtype=torch.float32).contiguous().clone()
             sb["rest_pose"] = G.rest
         m._detach_pose = True
+        exposure = getattr(m, "exposure", None)
         run_backup = m.net.bn_running.clone()
         states = [(st, st.num_batches_tracked) for st in m.net._states.values()]
         side = torch.cuda.Stream(device=dev)
@@ -270,11 +280,15 @@ class Stage1Trainer:
             for _ in range(2):
                 loss, _ = self.loss(sb, iteration, epoch)
                 m.optimizer.zero_grad(set_to_none=True)
+                if exposure is not None:
+                    exposure.grad = None
                 loss.backward()
         torch.cuda.current_stream().wait_stream(side)
         if not m.raster_ok(wait=True):                      # the warm-up found the binning buffer too small: it has been grown
             pass
         m.optimizer.zero_grad(set_to_none=True)
+        if exposure is not None:          # the captured backward must write a fresh gradient, not accumulate into an old one
+            exposure.grad = None
         from . import _lib
         G.graph = torch.cuda.CUDAGraph()
         l0 = _lib.launch_count()
@@ -284,6 +298,7 @@ class Stage1Trainer:
         G.launches = _lib.launch_count() - l0
         G.loss = loss.detach()
         G.g_flat, G.g_geo = m.net.flat.grad, m.geo_feature.grad
+        G.g_exp = None if exposure is None else exposure.grad
         G.plan = m._last_plan
         G.capacity = G.plan.capacity
         m.net.bn_running.copy_(run_backup)                  # warm-up and capture must not count as training iterations
@@ -302,10 +317,10 @@ class Stage1Trainer:
         B = batch["original_image"].shape[0]
         wdecay_rgl = adjust_loss_weights(o.lambda_rgl, epoch, mode="decay", start=self.epoch_start, every=20)
         lpips_active = self.perceptual_loss is not None and epoch > o.lpips_start_iter
-        # the last word stays the LPIPS flag (callers read it as k[-1]); the depth flag (k[3]) and the model's antialiasing mode go
-        # before it
+        # the last word stays the LPIPS flag (callers read it as k[-1]); the depth flag (k[3]), the model's antialiasing mode and its
+        # exposure table go before it
         key = (B, tuple(batch["original_image"].shape[-2:]), float(wdecay_rgl), batch.get("depth") is not None,
-               bool(getattr(m, "antialiasing", False)), lpips_active)
+               bool(getattr(m, "antialiasing", False)), getattr(m, "exposure", None) is not None, lpips_active)
         G = self._graphs.get(key)
         if G is not None and G.capacity != G.plan.capacity:      # the rasterizer's buffers were re-allocated: the graph points at freed memory
             G = None
@@ -329,6 +344,8 @@ class Stage1Trainer:
         for st in G.states:
             st.num_batches_tracked += 1
         m.net.flat.grad, m.geo_feature.grad = G.g_flat, G.g_geo
+        if G.g_exp is not None:
+            m.exposure.grad = G.g_exp
         return G.loss
 
     def _step_once(self, batch, iteration: int, epoch: int = 0):
@@ -358,17 +375,26 @@ class Stage1Trainer:
             loss.backward()
         self.sync_gradients()
         self.sync_pose_gradients(epoch)
+        self._prepare_updates()
+        m.step(epoch)
+        return loss
+
+    def _prepare_updates(self):
+        """Each optimiser's 1/world factor (applied once: in the fused kernels or by dividing the gradients) and its skip flag."""
+        m = self.model
+        plan = getattr(m, "_last_plan", None)
+        skip = self._skip if self.world > 1 else (plan.status_dev[1:2] if plan is not None else None)
         if isinstance(m.optimizer, FusedAdam):
             m.optimizer.grad_scale = 1.0 / self.world
-            plan = getattr(m, "_last_plan", None)
-            m.optimizer.skip_flag = self._skip if self.world > 1 else (plan.status_dev[1:2] if plan is not None else None)
+            m.optimizer.skip_flag = skip
         elif self.world > 1:
             for group in m.optimizer.param_groups:
                 for p in group["params"]:
                     if p.grad is not None:
                         p.grad.div_(self.world)
-        m.step(epoch)
-        return loss
+        if getattr(m, "exposure_optimizer", None) is not None:     # an overflowed step leaves the table and its moments alone
+            m.exposure_optimizer.grad_scale = 1.0 / self.world
+            m.exposure_optimizer.skip_flag = skip
 
 
 AvatarTrainer = Stage1Trainer

@@ -367,6 +367,24 @@ int ga_lbs_backward_ex(int32_t N, int32_t B, int32_t num_joints, int32_t lbs_ld,
                        int64_t dec_frame_stride, const float *dec_out, const int32_t *valid_index, const float *query_points,
                        const float *query_lbs, const float *cano2live, const float *d_means3D, const float *d_scales3,
                        const float *d_colors, float *d_dec_out, float *d_cano2live, void *stream);
+/* The same with each training frame's exposure: frame b's colours become c' = A c + t, [A | t] = exposure[pose_idx[b]] (row-major
+ * 3x4 per row, exposure [num_exposures,12], pose_idx [B] int32, both in device memory: nothing is read on the host).  A frame whose
+ * pose_idx is outside [0, num_exposures) gets NaN colours.  Means and scales are those of ga_lbs_forward_ex.  The backward also
+ * writes d_exposure [num_exposures,12]: row f is the sum, over the frames with pose_idx == f in slot order, of
+ * sum_n g_n (x) [c_n, 1] (g the colour gradient, c the decoder colour); rows no frame touches and row 0 (the gauge anchor) are 0.
+ * No atomics reach d_exposure: equal inputs give equal bits.  Its decoder colour gradient is A^T g; d_cano2live is that of
+ * ga_lbs_backward_ex.  workspace: at least ga_lbs_exposure_workspace_bytes(N, num_joints) bytes of device memory. */
+size_t ga_lbs_exposure_workspace_bytes(int32_t N, int32_t num_joints);
+int ga_lbs_forward_exposure(int32_t N, int32_t B, int32_t num_joints, int32_t lbs_ld, float scale_mul, int64_t dec_frame_stride,
+                            const float *dec_out, const int32_t *valid_index, const float *query_points, const float *query_lbs,
+                            const float *cano2live, int32_t num_exposures, const float *exposure, const int32_t *pose_idx,
+                            float *means3D, float *scales3, float *colors, void *stream);
+int ga_lbs_backward_exposure(int32_t N, int32_t B, int32_t num_joints, int32_t lbs_ld, int32_t num_pixels, float scale_mul,
+                             int64_t dec_frame_stride, const float *dec_out, const int32_t *valid_index, const float *query_points,
+                             const float *query_lbs, const float *cano2live, int32_t num_exposures, const float *exposure,
+                             const int32_t *pose_idx, const float *d_means3D, const float *d_scales3, const float *d_colors,
+                             float *d_dec_out, float *d_cano2live, float *d_exposure, void *workspace, size_t workspace_bytes,
+                             void *stream);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Stage-1 feature net (model/network.py:39-83; model/modules.py:114-137,508-582,745-754): geometry convs -> bilinear

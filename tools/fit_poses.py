@@ -8,7 +8,9 @@ DATA / MODEL are the reference's -s / -m folders; stage 1 loads net/iteration_N/
 (`stage2_load`).  The split's poses come from the file its stage's dataset reads (stage 1: smpl_parms.pth, stage 2:
 smpl_parms_pred.pth); stage 2 builds its input maps from the pose being fitted and never reads inp_map/.  Writes
 DATA/<split>/smpl_parms_fit.pth in the input file's format ({beta, body_pose, trans}; SMPL-X's rest columns copied unchanged) and
-DATA/<split>/smpl_parms_fit.json (per-frame initial and fitted loss, best iteration).  The input file is never overwritten.
+DATA/<split>/smpl_parms_fit.json (per-frame initial and fitted loss, best iteration).  --exposure also fits each frame's colour
+transform [A | t] and adds it to the pose file as `exposure` [F,3,4]; the test dataset's items then carry it and render_free_stage1 /
+render_free_stage2 apply it.  The input file is never overwritten.
 """
 import argparse
 import json
@@ -42,6 +44,7 @@ def parse_args(argv=None):
     ap.add_argument("--nf", type=int, default=32, help="stage 2: the pose encoder's base width")
     ap.add_argument("--white_background", type=int, choices=(0, 1), default=1)
     ap.add_argument("--antialiasing", action="store_true", help="render with 3DGS's antialiasing setting (for an avatar trained with it)")
+    ap.add_argument("--exposure", action="store_true", help="also fit each frame's exposure and white balance [A | t]")
     a = ap.parse_args(argv)
     if a.iters < 0:
         ap.error(f"--iters {a.iters} is negative")
@@ -60,9 +63,9 @@ def input_path(a):
     return os.path.join(a.source_path, a.split, "smpl_parms.pth" if a.stage == 1 else "smpl_parms_pred.pth")
 
 
-def write_fit(src, dst, pose, transl):
+def write_fit(src, dst, pose, transl, exposure=None):
     """Copy of the pose file `src` with body_pose[:n, :pose width] and trans[:n] replaced by the fitted rows; every other entry and
-    column (beta, SMPL-X's rest columns, frames past n) unchanged."""
+    column (beta, SMPL-X's rest columns, frames past n) unchanged.  exposure [n,3,4]: stored as `exposure` [F,3,4], identity past n."""
     if os.path.abspath(src) == os.path.abspath(dst):
         raise ValueError(f"{dst}: the fit must not overwrite its input")
     d = dict(torch.load(src, map_location="cpu", weights_only=False))
@@ -72,6 +75,10 @@ def write_fit(src, dst, pose, transl):
     body[:n, :w] = pose.to(body.dtype)
     trans[:n] = transl.to(trans.dtype)
     d["body_pose"], d["trans"] = body, trans
+    if exposure is not None:
+        table = torch.eye(3, 4).repeat(body.shape[0], 1, 1)
+        table[:n] = exposure.float()
+        d["exposure"] = table
     torch.save(d, dst)
 
 
@@ -102,13 +109,13 @@ def main(argv=None):
     dmp = ModelParams(**{**vars(mp), "inp_posmap_from_pose": True})
     dataset = type("SplitDataset", (MonoDataset_test,), {"split": a.split})(dmp)
     frames = [dataset[i] for i in range(len(dataset))]
-    fitter = PoseFitter(model, iters=a.iters, lr=a.lr, pose_mapper=pose_mapper)
-    pose, transl, report = fitter.fit(frames)
+    fitter = PoseFitter(model, iters=a.iters, lr=a.lr, pose_mapper=pose_mapper, exposure=a.exposure)
+    pose, transl, report, *exposure = fitter.fit(frames)
 
     split_dir = os.path.join(a.source_path, a.split)
-    write_fit(input_path(a), os.path.join(split_dir, OUT_NAME), pose, transl)
+    write_fit(input_path(a), os.path.join(split_dir, OUT_NAME), pose, transl, exposure[0] if exposure else None)
     with open(os.path.join(split_dir, REPORT_NAME), "w") as fh:
-        json.dump(dict(stage=a.stage, body=a.body, iters=a.iters, lr=a.lr, frames=report), fh, indent=1)
+        json.dump(dict(stage=a.stage, body=a.body, iters=a.iters, lr=a.lr, exposure=a.exposure, frames=report), fh, indent=1)
     init = sum(r["initial_loss"] for r in report) / max(1, len(report))
     fit = sum(r["fitted_loss"] for r in report) / max(1, len(report))
     print(json.dumps(dict(frames=len(report), mean_initial_loss=round(init, 6), mean_fitted_loss=round(fit, 6),
